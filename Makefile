@@ -1,4 +1,4 @@
-# Build libgoleft_b200.so (sm_100a only), the goleft CLI and the test oracle.
+# Build libgoleft_b200.so (sm_90a only), the goleft CLI and the test oracle.
 #   make            -> lib + cli + oracle
 #   make lib        -> goleft_b200/libgoleft_b200.so
 #   make cli        -> bin/goleft   (C++ host over the C ABI; links the .so)
@@ -6,7 +6,7 @@
 NVCC      ?= nvcc
 CXX       ?= g++
 CC        ?= gcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v --fmad=false
 CXXFLAGS  := -O2 -std=c++17 -fPIC -Wall
 CSRC      := goleft_b200/csrc
@@ -17,7 +17,7 @@ CU_SRCS   := $(wildcard $(CSRC)/*.cu)
 CPP_SRCS  := $(wildcard $(CSRC)/host/*.cpp)
 CU_OBJS   := $(patsubst $(CSRC)/%.cu,$(BUILD)/%.o,$(CU_SRCS))
 CPP_OBJS  := $(patsubst $(CSRC)/host/%.cpp,$(BUILD)/host_%.o,$(CPP_SRCS))
-HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/host/*.h) include/goleft_b200.h
+HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/host/*.h) include/goleft_b200.h Makefile
 
 NCCL_INC  ?= /usr/include
 NCCL_LIB  ?= /usr/lib/x86_64-linux-gnu

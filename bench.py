@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — Mbases/s depth-counted on a synthetic 30x WGS-shaped alignment stream (BASELINE.json).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload wgs|chr20]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload wgs|chr20] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (default, every N): BASELINE configs[2], the 25 primary GRCh38 contigs (3,088,286,401 bp) at 30x / 150 bp
@@ -18,6 +18,9 @@ e2e   : the drop-in call, per contig: gl_depth_bed_contig — decoder-native int
         of the text are inside the timed region, every step.  Two gl_ctx lanes per GPU (one host thread each) take the
         rank's contigs; every call is the synchronous call.  This is the work the reference arm is charged for (per-base
         counting + window/class walk + BED text).
+--dump-outputs DIR: after the timed steps, rank 0 writes what `value`'s last step computed for its contigs (window sums,
+        class-run starts and classes, per-contig counts) as DIR/*.npy in float64; the inputs are seeded, so two builds compare
+        output for output.
 extras (N=1): chr20 through every path, other shapes of chr20 (5x, maxmeandepth, W=250, W=1, long reads), the CLI on a BAM;
         every N: the 2504-sample indexcov cohort (configs[3]); N>1: the 500 x 6.18 M depthwed matrix (configs[4]).
 roofline / cpu_baseline : DESIGN.md §3.
@@ -58,7 +61,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet, HBM3)"
 
 
 class ClockSampler:
@@ -106,17 +109,6 @@ class ClockSampler:
                     reasons.add(nm)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read+write per launch of `kernel` from the committed ncu --set full captures (profiles/), or None"""
-    for name in ("r02_ncu_full_summary.json", "r01_ncu_full_summary.json"):
-        try:
-            j = json.load(open(os.path.join(ROOT, "profiles", name)))
-            return int(j[kernel]["traffic_bytes"]), name
-        except Exception:
-            continue
-    return None, None
 
 
 def dist_env():
@@ -169,13 +161,11 @@ def run_reference(args):
     total = sum(c[1] for c in contigs)
     nseg = sum(c[2].size for c in contigs)
     log(f"[reference] synth: {nseg} segments over {total} bp in {time.time() - t0:.1f}s; {threads} threads")
-    times, chunks, budget0 = [], 0, time.time()
+    times, chunks = [], 0
     for i in range(args.warmup + args.steps):
         dt, _, chunks = cpu_genome_pass(orc, contigs, threads)
         if i >= args.warmup:
             times.append(dt)
-        if times and time.time() - budget0 > 150:            # bounded: stop after ~2.5 min with at least one timed step
-            break
     t = float(np.mean(times))
     val = total / t / 1e6
     out = {"impl": "reference", "metric": METRIC, "value": val, "unit": "Mbases/s", "n_gpus": args.gpus,
@@ -561,6 +551,30 @@ def cli_wallclock(n_cpus):
         shutil.rmtree(tmp, ignore_errors=True)
 
 
+DUMP_LIMIT = 64 << 20
+
+
+def write_dump(d, dumped):
+    """dumped: per contig (int64 window sums, int32 run starts, uint8 run classes) -> d/*.npy, float64 (exact for these
+    integers), contigs concatenated in the rank's order; contig_windows / contig_runs delimit them.  Window sums beyond
+    DUMP_LIMIT are replaced by a fixed, seeded sample of windows plus its indices (window_index.npy)."""
+    os.makedirs(d, exist_ok=True)
+    out = {"contig_windows": np.array([x[0].size for x in dumped], np.float64),
+           "contig_runs": np.array([x[1].size for x in dumped], np.float64),
+           "run_starts": np.concatenate([x[1] for x in dumped]).astype(np.float64),
+           "run_classes": np.concatenate([x[2] for x in dumped]).astype(np.float64)}
+    sums = np.concatenate([x[0] for x in dumped]).astype(np.float64)
+    room = DUMP_LIMIT - (1 << 12) - sum(a.nbytes for a in out.values())      # 4 KiB for the .npy headers
+    if sums.nbytes > room:
+        k = room // 16
+        idx = np.sort(np.random.default_rng(0).choice(sums.size, k, replace=False))
+        out["window_index"], sums = idx.astype(np.float64), sums[idx]
+    out["window_sums"] = sums
+    for name, a in out.items():
+        np.save(os.path.join(d, name + ".npy"), a)
+    log(f"[dump] {sum(a.nbytes for a in out.values())} bytes of outputs in {len(out)} arrays -> {d}")
+
+
 # ------------------------------------------------------------------------------------------------ GPU arm
 def main():
     ap = argparse.ArgumentParser()
@@ -571,7 +585,12 @@ def main():
     ap.add_argument("--workload", default=os.environ.get("GL_BENCH_WORKLOAD", "wgs"), choices=["wgs", "chr20"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the per-path extras (int32 / general path / packed e2e variants)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl != "b200":
+        ap.error("--dump-outputs dumps the GPU arm's results")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     if args.impl == "reference":
@@ -636,11 +655,14 @@ def main():
         if dist is not None:
             dist.barrier()
 
+    def resident(w):
+        ctx.depth_begin(0, w["L"])
+        ctx.depth_add_segments_packed8_device(w["d_a"], w["d_d"], w["d_l"], w["nb"])
+        ctx.depth_reduce(W, MINCOV, MAXMEAN, STEP)
+
     def step_resident():
         for w in work:
-            ctx.depth_begin(0, w["L"])
-            ctx.depth_add_segments_packed8_device(w["d_a"], w["d_d"], w["d_l"], w["nb"])
-            ctx.depth_reduce(W, MINCOV, MAXMEAN, STEP)
+            resident(w)
 
     text_bytes = [0, 0]
     tr = {"h2d": 0, "pack_s": 0.0, "escaped": 0, "paths": set(), "kinds": set()}
@@ -687,9 +709,7 @@ def main():
         step_resident()
     n_runs = 0
     for w in work:
-        ctx.depth_begin(0, w["L"])
-        ctx.depth_add_segments_packed8_device(w["d_a"], w["d_d"], w["d_l"], w["nb"])
-        ctx.depth_reduce(W, MINCOV, MAXMEAN, STEP)
+        resident(w)
         w["n_runs"] = ctx.depth_result_sizes()[1]
         n_runs += w["n_runs"]
     for _ in range(args.warmup):
@@ -731,11 +751,19 @@ def main():
     barrier()
     l0 = ctx.launch_count()
     ms = 0.0
-    for _ in range(args.steps):
+    dumped = []             # --dump-outputs: per contig of the last timed step, (window sums, run starts, run classes)
+    for i in range(args.steps):
         ctx.flush_l2()
-        ctx.timer_start()
-        step_resident()
-        ms += ctx.timer_stop_ms()
+        if args.dump_outputs and rank == 0 and i == args.steps - 1:
+            for w in work:  # contig by contig: each contig's results leave between its timed window and the next
+                ctx.timer_start()
+                resident(w)
+                ms += ctx.timer_stop_ms()
+                dumped.append((ctx.depth_get_windows(),) + ctx.depth_get_runs())
+        else:
+            ctx.timer_start()
+            step_resident()
+            ms += ctx.timer_stop_ms()
     launches = ctx.launch_count() - l0
     barrier()
 
@@ -929,7 +957,6 @@ def main():
         n_launch = max(1, k_n.get(dom, 1))
         dom_ms_launch = k_ms[dom] / n_launch
         achieved = survey_bytes / n_launch / (dom_ms_launch * 1e-3) / 1e9
-        traffic, traffic_src = ncu_traffic(dom)
         out = {"metric": METRIC, "value": val, "unit": "Mbases/s", "n_gpus": world, "steps": args.steps,
                "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
                "scaling": "strong" if args.workload == "wgs" else "weak",
@@ -968,9 +995,8 @@ def main():
                             "own": {"alg_bytes_per_launch": own.get(dom, 0) / n_launch,
                                     "achieved": own.get(dom, 0) / n_launch / (dom_ms_launch * 1e-3) / 1e9,
                                     "frac": own.get(dom, 0) / n_launch / (dom_ms_launch * 1e-3) / 1e9 / peak,
-                                    "note": "packed words in + 8 B/window + 5 B/run out: the 8 B/base difference array never exists in HBM; "
-                                            "the kernel is issue-bound, not HBM-bound (profiles/)"},
-                            "traffic": traffic, "traffic_source": traffic_src, "kernel_ms": k_ms,
+                                    "note": "packed words in + 8 B/window + 5 B/run out: the 8 B/base difference array never exists in HBM"},
+                            "kernel_ms": k_ms,
                             "step": {"survey_alg_bytes": survey_bytes, "achieved": survey_bytes / (ms_step * 1e-3) / 1e9,
                                      "frac": survey_bytes / (ms_step * 1e-3) / 1e9 / peak}},
                "clocks": clocks}
@@ -997,6 +1023,8 @@ def main():
                                    "sample": f"{reps_c} x the whole workload ({chunks} chunks of 10 Mb, one worker per chunk = the reference's unit of "
                                              "parallelism, all host threads): per-base counting + window/class walk + BED text; "
                                              "BGZF inflate and samtools text print/parse excluded"}
+        if dumped:
+            write_dump(args.dump_outputs, dumped)
         print(json.dumps(out), flush=True)
 
     lane_pool.shutdown()

@@ -1,6 +1,6 @@
-// goleft — C++ host for the B200 engine, keeping the `goleft depth|indexcov|covstats|depthwed` command-line
+// goleft — C++ host for the H100 engine, keeping the `goleft depth|indexcov|covstats|depthwed` command-line
 // and BED/TSV output surface of brentp/goleft v0.2.6 (cmd/goleft/goleft.go:24-69).  Every number it prints is
-// computed by libgoleft_b200.so (CUDA, sm_100a) through the C ABI in include/goleft_b200.h; there is no CPU
+// computed by libgoleft_b200.so (CUDA, sm_90a) through the C ABI in include/goleft_b200.h; there is no CPU
 // fallback: without a GPU the subcommands fail with the library's error.
 //
 // Out of scope here (SURVEY.md §2): HTML/PNG plots, PCA columns of the .ped, --stats GC columns.  .crai input needs --fai.
@@ -1478,7 +1478,7 @@ static int cmd_indexsplit(int argc, char** argv) {
 }
 
 static void print_progs() {                                                          // cmd/goleft/goleft.go:33-53
-    fprintf(stderr, "goleft Version: %s (B200 engine: %s)\n\n", kVersion, gl_version());
+    fprintf(stderr, "goleft Version: %s (GPU engine: %s)\n\n", kVersion, gl_version());
     fprintf(stderr, "covstats    : coverage and insert-size statistics on bams by sampling\n");
     fprintf(stderr, "depth       : parallelize calls to samtools in user-defined windows\n");
     fprintf(stderr, "depthwed    : matricize output from depth to n-sites * n-samples\n");

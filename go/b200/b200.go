@@ -1,4 +1,4 @@
-// Package b200 binds libgoleft_b200.so (CUDA, sm_100a) for goleft's windowed-depth path.
+// Package b200 binds libgoleft_b200.so (CUDA, sm_90a) for goleft's windowed-depth path.
 //
 // SOURCE ONLY: the build image of this repository has no Go toolchain (`go: command not found`), so this file has never
 // been compiled there; the same C ABI (include/goleft_b200.h) is exercised by the C++ CLI (cli/goleft.cpp) and by the

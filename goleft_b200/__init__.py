@@ -1,4 +1,4 @@
-"""goleft_b200 — B200 (sm_100a) engine for goleft's windowed-depth hot path.
+"""goleft_b200 — H100 (sm_90a) engine for goleft's windowed-depth hot path.
 
 The product is the C ABI in include/goleft_b200.h (libgoleft_b200.so) plus the C++ `goleft`
 CLI; this package is the thin ctypes binding the tests and bench.py use.

@@ -1,4 +1,4 @@
-// depth.cu — the `goleft depth` hot path on sm_100a.
+// depth.cu — the `goleft depth` hot path on sm_90a.
 //
 // Work per region [rs,re) of one contig, replacing the `samtools depth` child + per-line Go callback
 // (depth/depth.go:45,238-364):   segments (start,end) -> per-base depth -> per-window sums (+min)
@@ -15,8 +15,8 @@
 //              index span of the cells that can reach the tile (look-back of max-length), tile core.
 //              A tile whose index span is far larger than its segment count (input not in BAM order)
 //              raises a flag and the host reruns the region on the general path.
-//              No difference array in HBM at all: shared-memory atomics run at ~2.7 T/s on B200,
-//              global reds at 0.17 T/s (tools/microbench/atomics_bench.cu).
+//              No difference array in HBM at all: shared-memory atomics run an order of magnitude faster
+//              than global reds (tools/microbench/atomics_bench.cu measures both).
 //  GENERAL path (any order; the fallback):
 //     memset -> [K_scatter] int32 red.global onto a difference array in HBM + warp-aggregated per-tile
 //     net sums -> [K_super] 64-tile sums -> [K_scan] per tile: coalesced load, carry from the two-level
@@ -1060,9 +1060,8 @@ constexpr int kF8BlocksPerPass = kF8Threads / 16;   // a block is 16 lanes x 4 s
 // `if (p) atomicAdd(smem, v)` compiles to a divergent region per atomic (BSSY / BRA / address math / ATOMS / BSYNC, ~15
 // instructions; ptxas does the same to a predicated `red.shared`).  Adding ZERO at an always-valid address instead keeps the
 // warp converged: the position is masked into the tile, the value is the predicate (+1 / -1 or 0), the atomic is
-// unconditional — 7 instructions per event, and the eight atomics of a thread interleave freely.  A/B on the B200 (same box,
-// same run): K_fused8 84.3 -> 80.6 us on chr20 30x, 173.9 -> 168.2 us at 5x, 145.9 -> 140.4 us with maxmeandepth.  (The same
-// change made K_fused 2 % slower — a quarter of its 1024 register slots per tile are idle and would add zeros — so it keeps
+// unconditional — 7 instructions per event, and the eight atomics of a thread interleave freely.  (The same
+// change made K_fused slower — a quarter of its 1024 register slots per tile are idle and would add zeros — so it keeps
 // the branches.)
 __device__ __forceinline__ void fused_apply32(int* s_tile, int a, int len, int& carry) {
     const int b = a + len;
@@ -2252,9 +2251,9 @@ int gl_depth_bed_region(gl_ctx* ctx, const char* chrom, int64_t rs, int64_t re, 
     const char* force_env = getenv("GL_BED_PACK");                      // read per call (tests switch it)
     const int force = force_env ? atoi(force_env) : -1;
     if ((force == 16 && n >= 4096) || (force < 0 && n >= (int64_t(1) << 20) && glhost_pool_size() >= 48)) {
-        // The pack is DRAM-bound: 16 threads reach ~80 % of what 64 do.  More is worse on the 2 x 32-core B200 host: when a
+        // The pack is DRAM-bound: 16 threads reach most of what 64 do.  More is worse on a 2 x 32-core host: when a
         // burst of 24+ threads starts streaming out of an idle pool, every memory access of the process (and the GPU's DMA)
-        // stalls for 20-100 ms every few calls (tools/e2e_transport_probe.py; none at 16 threads, none when the pool never idles).
+        // can stall for tens of ms every few calls (tools/e2e_transport_probe.py; none at 16 threads, none when the pool never idles).
         static const int pack_threads_env = [] { const char* e = getenv("GL_BED_PACK_THREADS"); return e ? atoi(e) : 0; }();
         const int pack_threads = threads > 0 ? threads : (pack_threads_env > 0 ? pack_threads_env : std::min(glhost_pool_size(), 16));
         const auto ph0 = std::chrono::steady_clock::now();

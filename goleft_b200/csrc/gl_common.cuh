@@ -1,5 +1,5 @@
 // gl_common.cuh — context object and error plumbing shared by every translation unit of
-// libgoleft_b200.so.  sm_100a only; there is no CPU fallback anywhere in this library.
+// libgoleft_b200.so.  sm_90a only; there is no CPU fallback anywhere in this library.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,7 +28,7 @@ struct gl_ctx {
     cudaStream_t d2h_stream = nullptr;   // streamed packed8 reduce: finished window sums leave while later chunks arrive
     std::string err;
     int64_t launches = 0;
-    int sm_count = 148;
+    int sm_count = 132;
 
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;         // gl_timer_*
     cudaEvent_t ev_copy[2] = {nullptr, nullptr};      // staging ring

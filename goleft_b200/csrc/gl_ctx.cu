@@ -45,7 +45,7 @@ static void buf_free(gl_buf& b) {
 
 extern "C" {
 
-const char* gl_version(void) { return "goleft_b200 0.1.0 sm_100a"; }
+const char* gl_version(void) { return "goleft_b200 0.1.0 sm_90a"; }
 
 int gl_device_count(int* n) {
     if (!n) return gl_fail(nullptr, GL_EINVAL, "null out pointer");
@@ -84,8 +84,8 @@ int gl_ctx_create(int device, gl_ctx** out) {
         e = cudaGetDeviceProperties(&prop, device);
         if (e == cudaSuccess) {
             ctx->sm_count = prop.multiProcessorCount;
-            if (prop.major < 10) {
-                int rc = gl_fail(nullptr, GL_ECUDA, "device %d is sm_%d%d; this library is built for sm_100a only",
+            if (prop.major != 9 || prop.minor != 0) {   // sm_90a SASS only, no PTX: nothing else can load it
+                int rc = gl_fail(nullptr, GL_ECUDA, "device %d is sm_%d%d; this library is built for sm_90a only",
                                  device, prop.major, prop.minor);
                 delete ctx;
                 return rc;
@@ -323,7 +323,7 @@ int gl_profile_read(gl_ctx* ctx, char* buf, int64_t cap, int64_t* needed) {
 
 int gl_flush_l2(gl_ctx* ctx) {
     GL_CHECK(gl_use(ctx));
-    const size_t bytes = size_t(256) << 20;   // 256 MiB > 126 MB L2
+    const size_t bytes = size_t(256) << 20;   // 256 MiB > 50 MB L2
     GL_CHECK(gl_buf_reserve(ctx, ctx->flush, bytes));
     GL_CUDA(ctx, cudaMemsetAsync(ctx->flush.p, 0x5a, bytes, ctx->stream));
     return GL_OK;

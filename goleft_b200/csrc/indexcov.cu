@@ -1,4 +1,4 @@
-// indexcov.cu — `goleft indexcov` arithmetic on sm_100a, plus the small covstats / depthwed kernels.
+// indexcov.cu — `goleft indexcov` arithmetic on sm_90a, plus the small covstats / depthwed kernels.
 //
 //   I1  ic_sizes_kernel     BAI linear-index virtual offsets -> per-tile sizes   (indexcov/types.go:45-82)
 //   I2+I3 ic_cohort_kernel  ONE kernel, one CTA per sample: capped weighted median by two range-adaptive
@@ -168,7 +168,7 @@ __global__ void __launch_bounds__(kCohortThreads) ic_cohort_kernel(const long lo
 
 // ------------------------------------------------------------------------------------------------ I2 + I3, version 2
 // ic_cohort2_kernel: the same two order statistics, but the sample's tiles are streamed TWICE instead of ~17 times and no
-// shared-memory histogram (64-bit shared atomics are a CAS loop on sm_100) is involved:
+// shared-memory histogram (64-bit shared atomics are a CAS loop on sm_90) is involved:
 //   small samples (n <= 8192): all tiles sorted in shared memory (bitonic), Index.init done literally.
 //   large samples: a strided sample of 8192 tiles is sorted in shared memory; it brackets the 98th-percentile element
 //     (n98) and the capped weighted median (med) by VALUE:  [lo98, hi98] around sample rank 0.98 K (+-64 ranks, > 5 sigma)

@@ -1,5 +1,5 @@
 /*
- * goleft_b200.h — C ABI of libgoleft_b200.so, the B200 (sm_100a) engine behind
+ * goleft_b200.h — C ABI of libgoleft_b200.so, the H100 (sm_90a) engine behind
  * goleft's windowed-depth hot path (`depth`, `indexcov`, `covstats`, `depthwed`).
  *
  * The reference (brentp/goleft, pure Go) has no FFI for this path; each entry point
@@ -48,7 +48,7 @@ typedef struct gl_ctx gl_ctx;
 typedef struct gl_bam gl_bam;            /* an open BAM + its index (gl_bam_open) */
 
 /* ---------------------------------------------------------------- context */
-const char* gl_version(void);                       /* "goleft_b200 <semver> sm_100a" */
+const char* gl_version(void);                       /* "goleft_b200 <semver> sm_90a" */
 int  gl_device_count(int* n);
 int  gl_ctx_create(int device, gl_ctx** out);
 int  gl_ctx_destroy(gl_ctx* ctx);

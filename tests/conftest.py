@@ -9,7 +9,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
     # build the product library and the oracle if they are missing (CPU-only cross compile)
     need = [os.path.join(ROOT, "goleft_b200", "libgoleft_b200.so"), os.path.join(ROOT, "oracle", "_build", "liboracle.so")]
     if not all(os.path.exists(p) for p in need):

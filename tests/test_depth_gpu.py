@@ -1,5 +1,5 @@
 """GPU parity: the CUDA depth path, called through the C ABI, against oracle/oracle_depth.c.
-Integer work -> bit-exact.  Every test here needs a B200 (`-m gpu`)."""
+Integer work -> bit-exact.  Every test here needs an H100 (`-m gpu`)."""
 import numpy as np
 import pytest
 

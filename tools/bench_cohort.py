@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Device-resident throughput of the cohort-scale kernels on one B200 (BASELINE configs 3 and 4 at 1-GPU shard size):
+"""Device-resident throughput of the cohort-scale kernels on one H100 (BASELINE configs 3 and 4 at 1-GPU shard size):
   indexcov: S samples x T tiles -> per-sample capped weighted median + normalised depth (ic_cohort_kernel)
   depthwed: S samples x R windows of float64 means -> int matrix, row-major (depthwed_kernel)
 Prints one JSON object; CUDA-event timing on the ctx stream, L2 flushed before every repetition."""
@@ -24,7 +24,7 @@ def main():
     ap.add_argument("--wed-rows", type=int, default=6_176_584)
     ap.add_argument("--reps", type=int, default=5)
     args = ap.parse_args()
-    peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+    peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0
     out = {"peak_gbs": peak}
     ctx = capi.Ctx(0)
 

@@ -40,7 +40,9 @@ __global__ void global_reds(int* arr, unsigned mask, long long n_per_thread){
 int main(){
     int* out; CK(cudaMalloc(&out, 4));
     cudaEvent_t e0,e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    int iters=2048; int grid=148*8;
+    int sms, khz; CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0)); CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0));
+    const double ghz = khz / 1e6;
+    int iters=2048; int grid=sms*8;
     for(int mode=0; mode<2; mode++){
         for(int rep=0;rep<3;rep++){
             cudaEventRecord(e0);
@@ -48,17 +50,17 @@ int main(){
             cudaEventRecord(e1); CK(cudaEventSynchronize(e1));
             float ms; cudaEventElapsedTime(&ms,e0,e1);
             double n = 2.0*grid*256.0*iters;
-            if(rep==2) printf("smem atomics mode %d: %.1f G atomics/s (%.3f ms), per SM per clk @1.9GHz: %.2f\n", mode, n/ms/1e6, ms, n/ms/1e6/148/1.9);
+            if(rep==2) printf("smem atomics mode %d: %.1f G atomics/s (%.3f ms), per SM per clk @%.2fGHz: %.2f\n", mode, n/ms/1e6, ms, ghz, n/ms/1e6/sms/ghz);
         }
     }
     for(int lg=22; lg<=27; lg+=5){   // 16 MB (L2 resident) and 512 MB (HBM)
         size_t n = (size_t)1<<lg; int* arr; CK(cudaMalloc(&arr, n*4)); CK(cudaMemset(arr,0,n*4));
         for(int rep=0;rep<3;rep++){
             cudaEventRecord(e0);
-            global_reds<<<148*16,256>>>(arr,(unsigned)(n-1), 16);
+            global_reds<<<sms*16,256>>>(arr,(unsigned)(n-1), 16);
             cudaEventRecord(e1); CK(cudaEventSynchronize(e1));
             float ms; cudaEventElapsedTime(&ms,e0,e1);
-            double cnt = 2.0*148*16*256*16;
+            double cnt = 2.0*sms*16*256*16;
             if(rep==2) printf("global reds on %zu MB array: %.1f G reds/s (%.3f ms)\n", n*4>>20, cnt/ms/1e6, ms);
         }
         cudaFree(arr);

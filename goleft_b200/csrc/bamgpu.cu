@@ -13,6 +13,7 @@
 // Anything unexpected (a member the inflater rejects, a malformed record) makes the call return GL_ESTATE and the caller
 // uses the host feeder for that reference.
 #include "gl_common.cuh"
+#include "host/bam_cigar.h"
 #include "host/bam_feed.h"
 #include "host/thread_pool.h"
 #include <unistd.h>
@@ -28,9 +29,15 @@ __device__ __forceinline__ unsigned ld32(const unsigned char* p) {          // u
     return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
 }
 
+// glbam::record_cigar out of line, called only for a record whose first op is S of length l_seq: records without the
+// placeholder walk their CIGAR exactly as before
+__device__ __noinline__ void cg_cigar(const unsigned char* r, unsigned bs, const unsigned char** cg, unsigned* n_op) {
+    glbam::record_cigar(r, bs, cg, n_op);
+}
+
 // one thread per unit: records in [unit_pos[u], unit_pos[u+1]) of the inflated stream.  kEmit = false: count the M/=/X blocks of
 // the passing records; kEmit = true: write them at seg_off[u].  Same walk as host/bam_feed.cpp Emitter::record (blocks
-// separated only by I/S/H/P merge; D and N advance without counting).
+// separated only by I/S/H/P merge; D and N advance without counting), on the CIGAR glbam::record_cigar picks (CG tag).
 template <bool kEmit>
 __global__ void __launch_bounds__(128) bam_parse_kernel(const unsigned char* __restrict__ data, const long long* __restrict__ unit_pos, int n_units,
                                                        int tid_want, int min_mapq, long long* __restrict__ seg_cnt, const long long* __restrict__ seg_off,
@@ -57,9 +64,10 @@ __global__ void __launch_bounds__(128) bam_parse_kernel(const unsigned char* __r
         if (32u + l_name + 4u * n_cig > bs) continue;
         n_pass++;
         const unsigned char* cg = r + 36 + l_name;
+        unsigned n_op = n_cig;
         int ref = rpos, b0 = 0, b1 = 0;
-        bool open = false;
-        for (unsigned k = 0; k < n_cig; k++) {
+        bool open = false, checked = false;
+        for (unsigned k = 0; k < n_op; k++) {
             const unsigned v = ld32(cg + 4 * k);
             const unsigned op = v & 15u;
             const int len = (int)(v >> 4);
@@ -72,6 +80,11 @@ __global__ void __launch_bounds__(128) bam_parse_kernel(const unsigned char* __r
                 }
                 ref += len;
             } else if (op == 2 || op == 3) ref += len;
+            else if (op == 4 && k == 0 && !checked && v == ((ld32(r + 20) << 4) | 4u)) {   // S of length l_seq first: maybe the CG placeholder
+                checked = true;
+                cg_cigar(r + 4, bs, &cg, &n_op);
+                k = ~0u;                                                        // walk the CIGAR it chose from its first op
+            }
         }
         if (open && b1 > b0) { if (kEmit) { start[out] = b0; end[out] = b1; out++; } n_seg++; maxlen = max(maxlen, b1 - b0); }
     }

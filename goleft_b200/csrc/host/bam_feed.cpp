@@ -9,6 +9,7 @@
 #include <atomic>
 #include <chrono>
 #include <mutex>
+#include "bam_cigar.h"
 #include "seg_pack.h"
 #include "thread_pool.h"
 
@@ -94,13 +95,13 @@ struct Emitter {
         while (j > 0 && pend[j - 1].first > s) { pend[j] = pend[j - 1]; j--; }
         pend[j] = Piece(s, len);
     }
-    inline void record(int32_t pos, const uint8_t* cg, uint16_t n_cig) {
+    inline void record(int32_t pos, const uint8_t* cg, uint32_t n_cig) {
         if (pos < last_pos) sorted = false;         // not coordinate-sorted: fixed up at the end
         last_pos = pos;
         if (!pend.empty()) flush_upto(pos);
         int32_t ref = pos, bs = 0, be = 0;
         bool open = false;
-        for (uint16_t k = 0; k < n_cig; k++) {
+        for (uint32_t k = 0; k < n_cig; k++) {
             const uint32_t v = rd32(cg + 4 * k);
             const uint32_t op = v & 15, len = v >> 4;
             if (op == 0 || op == 7 || op == 8) {                               // M = X count
@@ -320,7 +321,10 @@ std::string BamFile::decode(int tid, int64_t beg, int64_t end, int min_mapq, int
                 if ((flag & 0x704) != 0 || (int)mapq < min_mapq) continue;      // samtools depth defaults + -Q (depth.go:45)
                 if (32u + l_name + 4u * n_cig > bs) continue;
                 R.n_pass++;
-                em.record(rpos, r + 32 + l_name, n_cig);
+                const uint8_t* cg;
+                uint32_t n_op;
+                glbam::record_cigar(r, bs, &cg, &n_op);                         // the stored CIGAR, or the real one from CG
+                em.record(rpos, cg, n_op);
             }
             R.parse_s += now_s() - tp;
             if (done_reading) break;

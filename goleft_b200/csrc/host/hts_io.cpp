@@ -1,5 +1,6 @@
 // hts_io.cpp — BGZF / BAM / BAI / FAI readers and a BGZF writer (see hts_io.h).
 #include "hts_io.h"
+#include "bam_cigar.h"
 #include "bam_feed.h"
 #include <stdio.h>
 #include <string.h>
@@ -302,12 +303,14 @@ bool seg_record(void* user, const uint8_t* r, uint32_t size) {
     if ((flag & 0x704) != 0 || (int)mapq < c->min_mapq) return true;       // samtools depth defaults + -Q (depth.go:45)
     if (32u + l_name + 4u * n_cig > size) return true;
     o.n_pass++;
-    const uint8_t* cg = r + 32 + l_name;
+    const uint8_t* cg;
+    uint32_t n_op;
+    glbam::record_cigar(r, size, &cg, &n_op);                              // the stored CIGAR, or the real one from CG
     int32_t ref = pos, bs = 0, be = 0;
     bool open = false;
     std::vector<int32_t>& S = o.start[tid];
     std::vector<int32_t>& E = o.end[tid];
-    for (uint16_t k = 0; k < n_cig; k++) {
+    for (uint32_t k = 0; k < n_op; k++) {
         const uint32_t v = rd32(cg + 4 * k);
         const uint32_t op = v & 15, len = v >> 4;
         if (op == 0 || op == 7 || op == 8) {                               // M = X count

@@ -11,7 +11,8 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-from bamutil import make_bai, make_bam, make_bam_indexed  # noqa: E402
+import bamref  # noqa: E402
+from bamutil import cg_mix_records, cigar_lens, make_bai, make_bam, make_bam_indexed  # noqa: E402
 from goleft_b200 import capi  # noqa: E402
 from oracle import loader as orc  # noqa: E402
 
@@ -40,7 +41,9 @@ def test_dispatcher_and_arg_errors():
     assert p.returncode == 255 and "size is required" in p.stderr
 
 
-def _make_bam(tmp_path, seed=0, n=40000, indexed=True):
+def _make_bam(tmp_path, seed=0, n=40000, indexed=True, long_reads=False):
+    """long_reads: a fourth reference holds ultra-long reads stored through CG, 150 bp reads and the CG edge cases
+    (bamutil.cg_mix_records)"""
     rng = np.random.default_rng(seed)
     refs = [("chrM", 16571), ("chr22", 20001), ("HLA-A*01:01:01:01", 3000)]
     recs, mates = [], []
@@ -55,6 +58,11 @@ def _make_bam(tmp_path, seed=0, n=40000, indexed=True):
             recs.append((tid, int(p0), mapq, flag, cigar))
             ins = int(rng.normal(350, 40))
             mates.append((int(p0) + ins - 100, ins) if flag & 1 and not flag & 16 else (max(0, int(p0) - 250), -ins))
+    if long_reads:
+        long_recs, end = cg_mix_records(np.random.default_rng(seed + 100), len(refs), n_long=30, n_short=3000)
+        refs.append(("chrL", end + 2000))
+        recs += long_recs
+        mates += [(-1, 0)] * len(long_recs)
     for _ in range(50):
         recs.append((-1, -1, 0, 4, [(100, "M")])); mates.append((-1, 0))
     bam = tmp_path / "s.bam"
@@ -74,14 +82,14 @@ def _make_bam(tmp_path, seed=0, n=40000, indexed=True):
 @pytest.mark.gpu
 @pytest.mark.parametrize("W", [100, 250, 13, 2001, 1000000000])
 def test_depth_fai_mode(tmp_path, W):
-    bam, ref, refs, _, _ = _make_bam(tmp_path)
+    bam, ref, refs, recs, _ = _make_bam(tmp_path)
     prefix = str(tmp_path / "x")
     run("depth", "-Q", "1", "--ordered", "--windowsize", str(W), "--prefix", prefix, "--reference", ref, bam)
-    seg = capi.bam_segments(bam, 1, 2)
+    seg = bamref.segments(recs, len(refs), 1)
     exp_hd, exp_ca = b"", b""
     for tid, (name, L) in enumerate(refs):
-        s, e = seg["segments"][tid]
-        d = orc.pileup_brute(s, e, 0, L)
+        s, e = seg[tid]
+        d = bamref.pileup(s, e, 0, L)
         for cs, ce in orc.gen_chunks(L, W):
             h, c = orc.walk_chunk(name, cs, ce, W, 4, 0, d[cs:ce])
             exp_hd += h; exp_ca += c
@@ -91,15 +99,66 @@ def test_depth_fai_mode(tmp_path, W):
 
 @pytest.mark.gpu
 def test_depth_unindexed_bam_falls_back_to_whole_file_decode(tmp_path):
-    bam, ref, refs, _, _ = _make_bam(tmp_path, seed=4, indexed=False)
+    bam, ref, refs, recs, _ = _make_bam(tmp_path, seed=4, indexed=False)
     prefix = str(tmp_path / "u")
     p = run("depth", "-Q", "1", "-w", "100", "--prefix", prefix, "--reference", ref, bam)
     assert "decoding the whole file" in p.stderr
-    seg = capi.bam_segments(bam, 1, 2)
+    seg = bamref.segments(recs, len(refs), 1)
     exp_hd, exp_ca = b"", b""
     for tid, (name, L) in enumerate(refs):
-        s, e = seg["segments"][tid]
-        h, c = orc.walk_chunk(name, 0, L, 100, 4, 0, orc.pileup_brute(s, e, 0, L))
+        s, e = seg[tid]
+        h, c = orc.walk_chunk(name, 0, L, 100, 4, 0, bamref.pileup(s, e, 0, L))
+        exp_hd += h; exp_ca += c
+    assert open(prefix + ".depth.bed", "rb").read() == exp_hd
+    assert open(prefix + ".callable.bed", "rb").read() == exp_ca
+
+
+@pytest.mark.gpu
+def test_depth_cg_long_reads(tmp_path):
+    """ultra-long reads whose CIGAR is in the CG tag, among short reads: whole references through the GPU feeder and the
+    host feeder, and BED lines that start and end inside long reads, byte-equal to the oracle's text over bamref depth"""
+    import json
+    bam, ref, refs, recs, _ = _make_bam(tmp_path, seed=6, long_reads=True)
+    seg = bamref.segments(recs, len(refs), 1)
+    depth = {name: bamref.pileup(*seg[tid], 0, L) for tid, (name, L) in enumerate(refs)}
+    assert depth["chrL"].sum() > 1_000_000
+    W = 250
+    exp_hd, exp_ca = b"", b""
+    for name, L in refs:
+        for cs, ce in orc.gen_chunks(L, W):
+            h, c = orc.walk_chunk(name, cs, ce, W, 4, 0, depth[name][cs:ce])
+            exp_hd += h; exp_ca += c
+    for env, fed in (({}, len(refs)), ({"GL_GPU_FEED": "0"}, 0)):
+        prefix = str(tmp_path / ("w%d" % fed))
+        p = run("depth", "--timing", "-Q", "1", "--ordered", "-w", str(W), "--prefix", prefix, "-r", ref, bam, env=env)
+        assert json.loads(p.stderr.strip().splitlines()[-1])["goleft_depth_timing"]["gpu_fed_passes"] == fed
+        assert open(prefix + ".depth.bed", "rb").read() == exp_hd, env
+        assert open(prefix + ".callable.bed", "rb").read() == exp_ca, env
+    longs = [r for r in recs if r[0] == 3 and len(r[4]) > 65535]
+    regions = []
+    for r in longs[::3]:
+        span = cigar_lens(r[4])[1]
+        regions += [("chrL", r[1] + span // 4, r[1] + span // 4 + 3333), ("chrL", r[1] + 17, r[1] + span - 17), ("chrL", max(0, r[1] - 500), r[1] + 900)]
+    regions += [("chrM", 100, 1000), ("chrL", 0, refs[3][1])]
+    bed = tmp_path / "cg.bed"
+    bed.write_text("".join("%s\t%d\t%d\n" % r for r in regions))
+    prefix = str(tmp_path / "b")
+    run("depth", "--bed", str(bed), "-Q", "1", "-w", "100", "--prefix", prefix, "-r", ref, bam)
+    exp_hd, exp_ca = b"", b""
+    for name, rs, re in regions:
+        h, c = orc.walk_chunk(name, rs, re, 100, 4, 0, depth[name][rs:re])
+        exp_hd += h; exp_ca += c
+    assert open(prefix + ".depth.bed", "rb").read() == exp_hd
+    assert open(prefix + ".callable.bed", "rb").read() == exp_ca
+    # the same records without a linear index: the whole-file decode
+    os.makedirs(str(tmp_path / "u"))
+    bam_u, ref_u, _, _, _ = _make_bam(tmp_path / "u", seed=6, indexed=False, long_reads=True)
+    prefix = str(tmp_path / "u" / "x")
+    p = run("depth", "-Q", "1", "-w", str(W), "--prefix", prefix, "-r", ref_u, bam_u)
+    assert "decoding the whole file" in p.stderr
+    exp_hd, exp_ca = b"", b""
+    for name, L in refs:
+        h, c = orc.walk_chunk(name, 0, L, W, 4, 0, depth[name])
         exp_hd += h; exp_ca += c
     assert open(prefix + ".depth.bed", "rb").read() == exp_hd
     assert open(prefix + ".callable.bed", "rb").read() == exp_ca
@@ -171,10 +230,10 @@ def test_depth_synthetic_bam_index_seek_and_gpus(tmp_path):
 
 @pytest.mark.gpu
 def test_depth_chrom_and_flags(tmp_path):
-    bam, ref, refs, _, _ = _make_bam(tmp_path, seed=1)
+    bam, ref, refs, recs, _ = _make_bam(tmp_path, seed=1)
     prefix = str(tmp_path / "y")
     run("depth", "-c", "chr22", "-w", "71", "--mincov", "2", "-m", "9", "--q", "20", "--prefix", prefix, "-r", ref, bam)
-    s, e = capi.bam_segments(bam, 20, 2)["segments"][1]
+    s, e = bamref.segments(recs, len(refs), 20)[1]
     d = orc.pileup_brute(s, e, 0, 20001)
     exp = orc.walk_chunk("chr22", 0, 20001, 71, 2, 9, d)
     assert open(prefix + ".chr22.depth.bed", "rb").read() == exp[0]            # depth.go:378-389 file naming
@@ -185,18 +244,18 @@ def test_depth_chrom_and_flags(tmp_path):
 @pytest.mark.gpu
 @pytest.mark.parametrize("W", [10, 50, 1000000])
 def test_depth_bed_mode(tmp_path, W):
-    bam, ref, refs, _, _ = _make_bam(tmp_path, seed=2)
+    bam, ref, refs, recs, _ = _make_bam(tmp_path, seed=2)
     bed = tmp_path / "w.bed"
     regions = [("chr22", 14250, 15500), ("chr22", 1575, 15800), ("chrM", 100, 1000), ("chrM", 2000, 5000), ("chrM", 1, 3),
                ("chrM", 9, 13), ("chrM", 16, 17), ("chrM", 24, 29), ("chrM", 39, 43)]
     bed.write_text("".join("%s\t%d\t%d\n" % r for r in regions) + "chrM\t50\t60")     # last line unterminated: dropped like Go's ReadBytes loop
     prefix = str(tmp_path / "z")
     run("depth", "--bed", str(bed), "-Q", "1", "--windowsize", str(W), "--prefix", prefix, "--reference", ref, bam)
-    seg = capi.bam_segments(bam, 1, 2)
+    seg = bamref.segments(recs, len(refs), 1)
     tid_of = {n: i for i, (n, _) in enumerate(refs)}
     exp_hd, exp_ca = b"", b""
     for name, rs, re in regions:
-        s, e = seg["segments"][tid_of[name]]
+        s, e = seg[tid_of[name]]
         h, c = orc.walk_chunk(name, rs, re, W, 4, 0, orc.pileup_brute(s, e, rs, re))
         exp_hd += h; exp_ca += c
     assert open(prefix + ".depth.bed", "rb").read() == exp_hd
@@ -208,7 +267,7 @@ def test_depth_bed_mode(tmp_path, W):
 def test_depth_bed_mode_many_regions(tmp_path, W):
     """Batched BED mode (one pass per contig + gl_depth_interval_sums for the clipped edge windows) against the
     per-line walk of the oracle: random, overlapping, unsorted, window-aligned and out-of-contig regions."""
-    bam, ref, refs, _, _ = _make_bam(tmp_path, seed=3)
+    bam, ref, refs, recs, _ = _make_bam(tmp_path, seed=3)
     rng = np.random.default_rng(W)
     regions = []
     for _ in range(300):
@@ -223,7 +282,7 @@ def test_depth_bed_mode_many_regions(tmp_path, W):
     bed.write_text("".join("%s\t%d\t%d\n" % r for r in regions))
     prefix = str(tmp_path / "m")
     run("depth", "--bed", str(bed), "-Q", "1", "--windowsize", str(W), "--prefix", prefix, "--reference", ref, bam)
-    seg = capi.bam_segments(bam, 1, 2)
+    seg = bamref.segments(recs, len(refs), 1)
     tid_of = {n: i for i, (n, _) in enumerate(refs)}
     exp_hd, exp_ca = b"", b""
     for line in regions:
@@ -231,7 +290,7 @@ def test_depth_bed_mode_many_regions(tmp_path, W):
         if re <= rs:
             continue
         if name in tid_of:
-            s, e = seg["segments"][tid_of[name]]
+            s, e = seg[tid_of[name]]
         else:
             s = e = np.zeros(0, np.int32)
         h, c = orc.walk_chunk(name, rs, re, W, 4, 0, orc.pileup_brute(s, e, rs, re))
@@ -256,17 +315,17 @@ def test_depth_stats_columns(tmp_path, W):
     """--stats: GC / CpG / masked columns in fai mode and BED mode (every functional test of the reference passes
     --stats, depth/functional-test.sh; values follow the Faidx.Stats restatement — parity unpinned)."""
     from fautil import make_fasta
-    bam, ref, refs, _, _ = _make_bam(tmp_path, seed=5)
+    bam, ref, refs, bam_recs, _ = _make_bam(tmp_path, seed=5)
     fa, fai, recs = make_fasta(refs, seed=W, line=60)
     open(ref, "wb").write(fa)
     open(ref + ".fai", "w").write(fai)
-    seg = capi.bam_segments(bam, 1, 2)
+    seg = bamref.segments(bam_recs, len(refs), 1)
     prefix = str(tmp_path / "st")
     run("depth", "--stats", "-Q", "1", "--ordered", "--windowsize", str(W), "--prefix", prefix, "--reference", ref, bam)
     exp_hd, exp_ca = b"", b""
     for tid, (name, L) in enumerate(refs):
-        s, e = seg["segments"][tid]
-        d = orc.pileup_brute(s, e, 0, L)
+        s, e = seg[tid]
+        d = bamref.pileup(s, e, 0, L)
         for cs, ce in orc.gen_chunks(L, W):
             h, c = orc.walk_chunk(name, cs, ce, W, 4, 0, d[cs:ce])
             exp_hd += _with_stats(h, fa, recs); exp_ca += c
@@ -282,7 +341,7 @@ def test_depth_stats_columns(tmp_path, W):
     tid_of = {n: i for i, (n, _) in enumerate(refs)}
     exp_hd, exp_ca = b"", b""
     for name, rs, re in regions:
-        s, e = seg["segments"][tid_of[name]] if name in tid_of else (np.zeros(0, np.int32),) * 2
+        s, e = seg[tid_of[name]] if name in tid_of else (np.zeros(0, np.int32),) * 2
         h, c = orc.walk_chunk(name, rs, re, W, 4, 0, orc.pileup_brute(s, e, rs, re))
         exp_hd += _with_stats(h, fa, recs); exp_ca += c
     assert open(prefix + ".depth.bed", "rb").read() == exp_hd

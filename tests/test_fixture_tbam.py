@@ -73,13 +73,16 @@ def test_oracle_w250_row_counts():
 
 
 # ------------------------------------------------------------------ the feeder on a BAM written here
-from bamutil import make_bam as _bam
+import bamref  # noqa: E402
+from bamutil import cg_mix_records, cigar_lens, make_bam as _bam, make_bam_indexed  # noqa: E402
 
 
-def test_feeder_on_synthetic_bam(tmp_path):
+def _feeder_records(cg=False):
+    """(refs, records).  cg: the unplaced reads move to the end (so the BAM can be indexed) and a third reference holds
+    ultra-long reads stored through CG, short reads, and the CG edge cases (bamutil.cg_mix_records)."""
     rng = np.random.default_rng(0)
     refs = [("chrA", 100000), ("HLA-A*01:01:01:01", 5000)]
-    recs, exp = [], {0: ([], []), 1: ([], [])}
+    recs = []
     pos = 0
     for i in range(30000):
         tid = 0 if i < 25000 else 1
@@ -92,31 +95,97 @@ def test_feeder_on_synthetic_bam(tmp_path):
         cigar = [[(100, "M")], [(40, "M"), (5, "D"), (60, "M")], [(30, "M"), (3, "I"), (67, "M")], [(10, "S"), (90, "M")],
                  [(50, "="), (1, "X"), (20, "N"), (49, "M")], [(5, "H"), (20, "M"), (2, "P"), (30, "M"), (1000, "N"), (50, "M")]][kind]
         recs.append((tid if not (flag & 4) else -1, pos, mapq, flag, cigar))
-        if not (flag & 4) and (flag & 0x704) == 0 and mapq >= 1:
-            ref, cur = pos, None
-            for ln, op in cigar:
-                if op in "M=X":
-                    if cur and cur[1] == ref:
-                        cur[1] = ref + ln
-                    else:
-                        if cur:
-                            exp[tid][0].append(cur[0]); exp[tid][1].append(cur[1])
-                        cur = [ref, ref + ln]
-                    ref += ln
-                elif op in "DN":
-                    ref += ln
-            exp[tid][0].append(cur[0]); exp[tid][1].append(cur[1])
+    if cg:
+        long_recs, end = cg_mix_records(np.random.default_rng(7), 2)
+        refs.append(("chrL", end + 1000))
+        recs = [r for r in recs if r[0] >= 0] + long_recs + [r for r in recs if r[0] < 0]
+    return refs, recs
+
+
+def _check_segments(got_s, got_e, exp_s, exp_e, L, what):
+    """the same blocks as bamref (as a multiset) and the same per-base depth"""
+    assert bamref.same_multiset(got_s, got_e, exp_s, exp_e), what
+    assert np.array_equal(bamref.pileup(got_s, got_e, 0, L), bamref.pileup(exp_s, exp_e, 0, L)), what
+
+
+def test_feeder_on_synthetic_bam(tmp_path):
+    refs, recs = _feeder_records()
+    exp = bamref.segments(recs, len(refs), 1)
     p = tmp_path / "x.bam"
     p.write_bytes(_bam(refs, recs))
     for threads in (1, 4):
         r = capi.bam_segments(str(p), 1, threads)
         assert r["refs"] == refs and r["n_records"] == len(recs)
         for tid in (0, 1):
-            assert r["segments"][tid][0].tolist() == exp[tid][0] and r["segments"][tid][1].tolist() == exp[tid][1]
+            assert r["segments"][tid][0].tolist() == exp[tid][0].tolist() and r["segments"][tid][1].tolist() == exp[tid][1].tolist()
     only = capi.bam_segments(str(p), 1, 2, only_tid=1)
-    assert 0 not in only["segments"] and only["segments"][1][0].tolist() == exp[1][0]
+    assert 0 not in only["segments"] and only["segments"][1][0].tolist() == exp[1][0].tolist()
     with pytest.raises(capi.GlError):
         capi.bam_segments(str(tmp_path / "missing.bam"))
+
+
+def _cg_bam(tmp_path):
+    refs, recs = _feeder_records(cg=True)
+    bam_b, bai_b = make_bam_indexed(refs, recs)
+    p = tmp_path / "cg.bam"
+    p.write_bytes(bam_b)
+    (tmp_path / "cg.bam.bai").write_bytes(bai_b)
+    return str(p), refs, recs
+
+
+def test_stream_decoder_cg_reads(tmp_path):
+    """seg_record (the whole-file decoder) on ultra-long reads whose CIGAR is in the CG tag, the CG edge cases and filtered
+    placeholders, against bamref: the real CIGAR's blocks where htslib swaps it in, nothing where the placeholder stays"""
+    p, refs, recs = _cg_bam(tmp_path)
+    for q in (1, 30):
+        exp = bamref.segments(recs, len(refs), q)
+        assert exp[2][0].size > 100_000                               # the long reads do count
+        for threads in (1, 4):
+            r = capi.bam_segments(p, q, threads)
+            assert r["n_records"] == len(recs)
+            assert r["n_pass"] == sum(1 for rec in recs if bamref.passes(rec, q))
+            for tid, (nm, L) in enumerate(refs):
+                s, e = r["segments"].get(tid, (np.zeros(0, np.int32),) * 2)
+                _check_segments(s, e, *exp[tid], L, (q, threads, nm))
+
+
+def test_indexed_feeder_cg_reads(tmp_path):
+    """Emitter::record (the index-guided host feeder) on the same BAM: whole references as packed8 and int32 words on 1, 3
+    and all threads, and region queries whose ends cut through long CG reads"""
+    p, refs, recs = _cg_bam(tmp_path)
+    b = capi.Bam(p)
+    exp = bamref.segments(recs, len(refs), 1)
+    for tid, (nm, L) in enumerate(refs):
+        n_rec = sum(1 for r in recs if r[0] == tid)
+        n_pass = sum(1 for r in recs if r[0] == tid and bamref.passes(r, 1))
+        es, ee = exp[tid]
+        for threads in (1, 3, 0):
+            d = b.decode(tid, threads=threads, want=8)
+            assert d["format"] == 8 and d["n_records"] == n_rec and d["n_pass"] == n_pass
+            us, ue = capi.unpack_segments8(d["anchors"], d["dstart"], d["len"])
+            _check_segments(us, ue, *bamref.split255(es, ee), L, (nm, threads, 8))
+            d = b.decode(tid, threads=threads, want=32)
+            assert d["format"] == 32 and d["n_records"] == n_rec and d["n_pass"] == n_pass
+            _check_segments(d.get("start", es[:0]), d.get("end", ee[:0]), es, ee, L, (nm, threads, 32))
+    L = refs[2][1]
+    longs = [r for r in recs if r[0] == 2 and len(r[4]) > 65535]
+    regions = [(0, 1), (L - 500, L)]
+    for r in longs[::5]:
+        span = cigar_lens(r[4])[1]
+        regions += [(r[1] + span // 3, r[1] + span // 3 + 777), (r[1] - 100, r[1] + span // 2), (r[1] + span - 1000, r[1] + span + 5000)]
+    es, ee = exp[2]
+    for rs, re in regions:
+        rs, re = max(rs, 0), min(re, L)
+        for want in (8, 32):
+            d = b.decode(2, rs, re, want=want)
+            if d["n"] == 0:
+                s = e = np.zeros(0, np.int32)
+            elif want == 8:
+                s, e = capi.unpack_segments8(d["anchors"], d["dstart"], d["len"])
+            else:
+                s, e = d["start"], d["end"]
+            assert np.array_equal(bamref.pileup(s, e, rs, re), bamref.pileup(es, ee, rs, re)), (rs, re, want)
+    b.close()
 
 
 # ------------------------------------------------------------------ GPU: the fixture through the CUDA path

@@ -1335,10 +1335,20 @@ int accumulate_events(gl_ctx* ctx) {
     return GL_OK;
 }
 
-int read_header(gl_ctx* ctx, uint64_t hdr[4]) {
-    GL_CUDA(ctx, cudaMemcpyAsync(hdr, ctx->scratch.p, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+// The reduce's work is queued: send its header home behind it and leave the rest to depth_resolve (ctx->pend is filled in).
+// No wait here, so the next region's work queues up behind this one while the device is still busy.  The slot is
+// overwritten in stream order by the next reduce's header; depth_resolve only reads it after the latest ev_hdr.
+int defer_header(gl_ctx* ctx) {
+    GL_CUDA(ctx, cudaMemcpyAsync(ctx->hdr_host, ctx->scratch.p, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaEventRecord(ctx->ev_hdr, ctx->stream));
+    ctx->pend.active = true;
     return GL_OK;
+}
+
+// the segments changed: the last reduce's results, settled or not, no longer describe them (nothing waits for its work)
+void drop_result(gl_ctx* ctx) {
+    ctx->depth_reduced = false;
+    ctx->pend.active = false;
 }
 
 constexpr int kP8ChunksMax = 32;
@@ -1387,10 +1397,9 @@ int p8_materialize(gl_ctx* ctx) {
 }
 
 // The region's only batch is packed8: K_tileidx8 + K_fused8 + K_gather straight from the packed words.
-// *accepted = false when the anchors turn out unsorted (hand-made input): the caller unpacks and takes the other paths.
+// When the anchors turn out unsorted (hand-made input) the header says so and depth_resolve unpacks and takes the other paths.
 int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break, bool do_windows, bool do_runs,
-                  int32_t* d_depth_out, bool want_min, bool* accepted) {
-    *accepted = false;
+                  int32_t* d_depth_out, bool want_min) {
     const int64_t len = ctx->re - ctx->rs;
     const int64_t tiles = num_tiles_for(len);
     const int64_t w0 = ctx->rs / W;
@@ -1450,144 +1459,130 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
     p.win_sum = static_cast<unsigned long long*>(ctx->win_sum_p);
     p.win_min = (do_windows && want_min) ? static_cast<int*>(ctx->win_min.p) : nullptr;
 
-    for (int attempt = 0; attempt < 2; attempt++) {
-        p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
-        p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
-        long long cap = 0;
-        if (do_runs) {
-            cap = (long long)ctx->run_class.cap;
-            cap = std::min<long long>(cap, (long long)(ctx->run_start.cap / 4));
-            cap = std::min<long long>(cap, (long long)ctx->run_tmp_class.cap);
-            cap = std::min<long long>(cap, (long long)(ctx->run_tmp_start.cap / 4));
+    p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
+    p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
+    long long cap = 0;
+    if (do_runs) {
+        cap = (long long)ctx->run_class.cap;
+        cap = std::min<long long>(cap, (long long)(ctx->run_start.cap / 4));
+        cap = std::min<long long>(cap, (long long)ctx->run_tmp_class.cap);
+        cap = std::min<long long>(cap, (long long)(ctx->run_tmp_start.cap / 4));
+    }
+    p.run_cap = cap;
+    GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
+    if (do_windows && want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)n_windows * 4, ctx->stream));
+    // One pass over everything that is on the device — or, when the upload was deferred, chunk by chunk: the words
+    // are sorted by position, so once a chunk has landed every tile that ends before its last anchor can be reduced
+    // while the next chunk is still on the wire.
+    const int64_t nb = ctx->p8.n_blocks;
+    const bool streamed = ctx->p8.upload_pending;
+    const int n_chunks = streamed ? p8_chunks() : 1;
+    if (streamed) {
+        while ((int)ctx->ev_chunk.size() < 2 * n_chunks) {
+            cudaEvent_t ev;
+            GL_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+            ctx->ev_chunk.push_back(ev);
         }
-        p.run_cap = cap;
-        GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
-        if (do_windows && want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)n_windows * 4, ctx->stream));
-        // One pass over everything that is on the device — or, when the upload was deferred, chunk by chunk: the words
-        // are sorted by position, so once a chunk has landed every tile that ends before its last anchor can be reduced
-        // while the next chunk is still on the wire.
-        const int64_t nb = ctx->p8.n_blocks;
-        const bool streamed = ctx->p8.upload_pending;
-        const int n_chunks = streamed ? p8_chunks() : 1;
-        if (streamed) {
-            while ((int)ctx->ev_chunk.size() < 2 * n_chunks) {
-                cudaEvent_t ev;
-                GL_CUDA(ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-                ctx->ev_chunk.push_back(ev);
-            }
-            GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[0], 0));   // previous consumer done with the staging buffer
+        GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[0], 0));   // previous consumer done with the staging buffer
+    }
+    int64_t b0 = 0, t_prev = 0, w_sent = 0;             // w_sent: window sums already on their way home
+    const bool early_sums = streamed && ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap;
+    for (int c = 0; c < n_chunks; c++) {
+        const bool last = c == n_chunks - 1;
+        const int64_t b1 = p8_chunk_end(nb, c, n_chunks);
+        if (b1 <= b0 && !last) continue;
+        if (streamed && b1 > b0) {
+            const size_t nbk = (size_t)(b1 - b0);
+            GL_CUDA(ctx, cudaMemcpyAsync(const_cast<int*>(ctx->p8.anchors) + b0, ctx->p8.h_anchors + b0, nbk * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+            GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(const_cast<void*>(ctx->p8.ds)) + b0 * 64, static_cast<const char*>(ctx->p8.h_ds) + b0 * 64,
+                                         nbk * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
+            GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(const_cast<void*>(ctx->p8.len)) + b0 * 64, static_cast<const char*>(ctx->p8.h_len) + b0 * 64,
+                                         nbk * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
+            GL_CUDA(ctx, cudaEventRecord(ctx->ev_chunk[c], ctx->copy_stream));
+            GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
         }
-        int64_t b0 = 0, t_prev = 0, w_sent = 0;             // w_sent: window sums already on their way home
-        const bool early_sums = streamed && ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap;
-        for (int c = 0; c < n_chunks; c++) {
-            const bool last = c == n_chunks - 1;
-            const int64_t b1 = p8_chunk_end(nb, c, n_chunks);
-            if (b1 <= b0 && !last) continue;
-            if (streamed && b1 > b0) {
-                const size_t nbk = (size_t)(b1 - b0);
-                GL_CUDA(ctx, cudaMemcpyAsync(const_cast<int*>(ctx->p8.anchors) + b0, ctx->p8.h_anchors + b0, nbk * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-                GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(const_cast<void*>(ctx->p8.ds)) + b0 * 64, static_cast<const char*>(ctx->p8.h_ds) + b0 * 64,
-                                             nbk * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
-                GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(const_cast<void*>(ctx->p8.len)) + b0 * 64, static_cast<const char*>(ctx->p8.h_len) + b0 * 64,
-                                             nbk * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
-                GL_CUDA(ctx, cudaEventRecord(ctx->ev_chunk[c], ctx->copy_stream));
-                GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
-            }
-            // anchor gaps this chunk completes: (a[i], a[i+1]] for i in [b0-1, b1-1), plus the open end after the last anchor
-            p.idx_begin = (int)(b0 - 1);
-            p.idx_end = (int)(last ? nb : b1 - 1);
-            if (p.idx_end > p.idx_begin) {
-                gl_prof_scope prof(ctx, "depth_tileidx8_kernel");
-                depth_tileidx8_kernel<<<(unsigned)((p.idx_end - p.idx_begin + 255) / 256), 256, 0, ctx->stream>>>(p);
-                GL_LAUNCHED(ctx, 1);
-            }
-            // tiles whose end boundary is not beyond the last anchor on the device are complete
-            int64_t t_ready = tiles;
-            if (!last) {
-                const int64_t a_last = streamed ? (int64_t)ctx->p8.h_anchors[b1 - 1] : 0;
-                t_ready = std::min<int64_t>(tiles, std::max<int64_t>(t_prev, (a_last - ctx->rs) >> kTileShift));
-            }
-            if (t_ready > t_prev) {
-                p.tile_begin = (int)t_prev;
-                p.tile_end = (int)t_ready;
-                gl_prof_scope prof(ctx, "depth_fused8_kernel");
-                depth_fused8_kernel<<<(unsigned)std::min<int64_t>(t_ready - t_prev, (int64_t)ctx->sm_count * f8_ctas_per_sm), kF8Threads, 0, ctx->stream>>>(p);
-                GL_LAUNCHED(ctx, 1);
-            }
-            if (early_sums && !last && t_ready > t_prev) {
-                // windows that end at or before the last reduced tile's end are final: send them home on their own stream
-                const int64_t w_done = std::min<int64_t>(n_windows, std::max<int64_t>(w_sent, (ctx->rs + t_ready * kTile) / W - w0));
-                if (w_done > w_sent) {
-                    cudaEvent_t ev = ctx->ev_chunk[(size_t)n_chunks + c];
-                    GL_CUDA(ctx, cudaEventRecord(ev, ctx->stream));
-                    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->d2h_stream, ev, 0));
-                    GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums + w_sent, static_cast<const char*>(ctx->win_sum_p) + w_sent * 8,
-                                                 (size_t)(w_done - w_sent) * 8, cudaMemcpyDeviceToHost, ctx->d2h_stream));
-                    w_sent = w_done;
-                }
-            }
-            t_prev = t_ready;
-            b0 = b1;
-        }
-        ctx->p8.upload_pending = false;
-        GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));      // the packed staging buffer may be overwritten after this
-        if (do_runs) {
-            gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
-            depth_gather_runs_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, ctx->stream>>>(
-                header, chunk_runs, super_cnt, (int)chunks, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
-                static_cast<unsigned char*>(ctx->run_class.p), cap);
+        // anchor gaps this chunk completes: (a[i], a[i+1]] for i in [b0-1, b1-1), plus the open end after the last anchor
+        p.idx_begin = (int)(b0 - 1);
+        p.idx_end = (int)(last ? nb : b1 - 1);
+        if (p.idx_end > p.idx_begin) {
+            gl_prof_scope prof(ctx, "depth_tileidx8_kernel");
+            depth_tileidx8_kernel<<<(unsigned)((p.idx_end - p.idx_begin + 255) / 256), 256, 0, ctx->stream>>>(p);
             GL_LAUNCHED(ctx, 1);
         }
-        ctx->prefetched = false;
-        if (ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap) {   // (the rest of the) sums travel while the header is read
-            if (n_windows > w_sent)
-                GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums + w_sent, static_cast<const char*>(ctx->win_sum_p) + w_sent * 8,
-                                             (size_t)(n_windows - w_sent) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            ctx->prefetched = true;
+        // tiles whose end boundary is not beyond the last anchor on the device are complete
+        int64_t t_ready = tiles;
+        if (!last) {
+            const int64_t a_last = streamed ? (int64_t)ctx->p8.h_anchors[b1 - 1] : 0;
+            t_ready = std::min<int64_t>(tiles, std::max<int64_t>(t_prev, (a_last - ctx->rs) >> kTileShift));
         }
-        ctx->prefetched_runs = 0;
-        if (ctx->prefetch_run_start && ctx->prefetch_run_class && do_runs) {       // ... and so do the first runs (usually all of them)
-            const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)cap);
-            if (k > 0) {
-                GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
-                GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
-                ctx->prefetched_runs = k;
+        if (t_ready > t_prev) {
+            p.tile_begin = (int)t_prev;
+            p.tile_end = (int)t_ready;
+            gl_prof_scope prof(ctx, "depth_fused8_kernel");
+            depth_fused8_kernel<<<(unsigned)std::min<int64_t>(t_ready - t_prev, (int64_t)ctx->sm_count * f8_ctas_per_sm), kF8Threads, 0, ctx->stream>>>(p);
+            GL_LAUNCHED(ctx, 1);
+        }
+        if (early_sums && !last && t_ready > t_prev) {
+            // windows that end at or before the last reduced tile's end are final: send them home on their own stream
+            const int64_t w_done = std::min<int64_t>(n_windows, std::max<int64_t>(w_sent, (ctx->rs + t_ready * kTile) / W - w0));
+            if (w_done > w_sent) {
+                cudaEvent_t ev = ctx->ev_chunk[(size_t)n_chunks + c];
+                GL_CUDA(ctx, cudaEventRecord(ev, ctx->stream));
+                GL_CUDA(ctx, cudaStreamWaitEvent(ctx->d2h_stream, ev, 0));
+                GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums + w_sent, static_cast<const char*>(ctx->win_sum_p) + w_sent * 8,
+                                             (size_t)(w_done - w_sent) * 8, cudaMemcpyDeviceToHost, ctx->d2h_stream));
+                w_sent = w_done;
             }
         }
-        uint64_t hdr[4];
-        GL_CHECK(read_header(ctx, hdr));
-        if (w_sent > 0) GL_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
-        if (hdr[3] != 0) { ctx->prefetched = false; ctx->prefetched_runs = 0; return GL_OK; }        // anchors not sorted: not accepted
-        ctx->n_runs = do_runs ? (int64_t)hdr[0] : 0;
-        ctx->max_depth = (int32_t)hdr[2];
-        if (do_runs && (long long)hdr[0] > cap) {                          // output did not fit: grow and rerun
-            size_t ncap = (size_t)hdr[0] + 1024;
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, ncap * 4));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, ncap));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, ncap * 4));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, ncap));
-            continue;
-        }
-        break;
+        t_prev = t_ready;
+        b0 = b1;
     }
-    ctx->last_path = 3;
-    ctx->idx_flags = nullptr;
-    ctx->idx_cells = nullptr;
-    ctx->red_W = W; ctx->red_mincov = mincov; ctx->red_maxmean = maxmean; ctx->red_break = run_break;
-    ctx->n_windows = do_windows ? n_windows : 0;
-    ctx->depth_reduced = true;
-    *accepted = true;
-    return GL_OK;
+    ctx->p8.upload_pending = false;
+    GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));      // the packed staging buffer may be overwritten after this
+    if (do_runs) {
+        gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
+        depth_gather_runs_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, ctx->stream>>>(
+            header, chunk_runs, super_cnt, (int)chunks, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
+            static_cast<unsigned char*>(ctx->run_class.p), cap);
+        GL_LAUNCHED(ctx, 1);
+    }
+    ctx->prefetched = false;
+    if (ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap) {   // (the rest of the) sums travel while the header is read
+        if (n_windows > w_sent)
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums + w_sent, static_cast<const char*>(ctx->win_sum_p) + w_sent * 8,
+                                         (size_t)(n_windows - w_sent) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->prefetched = true;
+    }
+    ctx->prefetched_runs = 0;
+    if (ctx->prefetch_run_start && ctx->prefetch_run_class && do_runs) {       // ... and so do the first runs (usually all of them)
+        const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)cap);
+        if (k > 0) {
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+            ctx->prefetched_runs = k;
+        }
+    }
+    ctx->pend.path = 3;
+    ctx->pend.run_cap = cap;
+    ctx->pend.n_windows = n_windows;
+    ctx->pend.d2h = w_sent > 0;
+    ctx->pend.flags = nullptr;
+    ctx->pend.cells = nullptr;
+    return defer_header(ctx);
 }
 
-// One fused pass over the region.  Tries the fused (sorted) path first; the device decides eligibility,
-// the host learns it from the header it has to read anyway, and reruns on the general path if needed.
+// Queues one fused pass over the region on the fastest path the input may take: the packed8 kernel, else the fused
+// (sorted) int32 path, else the general path.  The device decides eligibility; depth_resolve learns it from the header and
+// reruns on the next path when needed.  skip = 1: not the packed8 kernel, 2: not the fused int32 path either (such a rerun).
 int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break, bool do_windows,
-               bool do_runs, int32_t* d_depth_out, bool want_min) {
+               bool do_runs, int32_t* d_depth_out, bool want_min, int skip = 0) {
     const int64_t len = ctx->re - ctx->rs;
     const int64_t tiles = num_tiles_for(len);
     const int64_t w0 = ctx->rs / W;
     const int64_t n_windows = (ctx->re - 1) / W - w0 + 1;
+    drop_result(ctx);
+    ctx->pend.W = W; ctx->pend.mincov = mincov; ctx->pend.maxmean = maxmean; ctx->pend.run_break = run_break;
+    ctx->pend.do_windows = do_windows; ctx->pend.do_runs = do_runs; ctx->pend.want_min = want_min; ctx->pend.d_depth_out = d_depth_out;
 
     if (ctx->copies_pending) {        // host segments still streaming into the store on the copy stream
         GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[0], ctx->copy_stream));
@@ -1595,17 +1590,14 @@ int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t 
         ctx->copies_pending = false;
     }
     if (ctx->p8.pending) {
-        if (ctx->force_path == 0 && ctx->batches.size() == 1 && tiles < (int64_t(1) << 30) && ctx->p8.n_blocks < INT32_MAX) {
-            bool accepted = false;
-            GL_CHECK(run_reduce_f8(ctx, W, mincov, maxmean, run_break, do_windows, do_runs, d_depth_out, want_min, &accepted));
-            if (accepted) return GL_OK;
-        }
+        if (skip == 0 && ctx->force_path == 0 && ctx->batches.size() == 1 && tiles < (int64_t(1) << 30) && ctx->p8.n_blocks < INT32_MAX)
+            return run_reduce_f8(ctx, W, mincov, maxmean, run_break, do_windows, do_runs, d_depth_out, want_min);
         GL_CHECK(p8_materialize(ctx));
     }
     if (do_windows && want_min) GL_CHECK(gl_buf_reserve(ctx, ctx->win_min, (size_t)n_windows * 4));
     // One scratch buffer; everything that must start at zero is contiguous so a single memset clears it:
     //   [header u64[8] | super_cnt u32[supers]] [win_sum u64[n_windows]] [flags] [cell_hi|cell_cnt|cell_lo per batch]  | chunk_runs
-    bool try_fused = ctx->force_path != 2 && ctx->force_path != 4 && !ctx->batches.empty() && (int)ctx->batches.size() <= kMaxBatches;
+    bool try_fused = skip < 2 && ctx->force_path != 2 && ctx->force_path != 4 && !ctx->batches.empty() && (int)ctx->batches.size() <= kMaxBatches;
     for (const gl_seg_batch& b : ctx->batches) if (b.n >= INT32_MAX) try_fused = false;
     const int origin = (int)(std::max<int64_t>(0, ctx->rs - kMaxLookback) & ~int64_t((1 << kCellShift) - 1));
     const int ncells = (int)(((ctx->re - 1 - origin) >> kCellShift) + 1);
@@ -1679,90 +1671,73 @@ int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t 
         }
     }
 
-    for (int attempt = 0; attempt < 3; attempt++) {
-        const bool fused = try_fused;
-        const bool hbm_diff = !fused && ctx->force_path == 2;      // the north-star pipeline (HBM difference array), on request only
-        EvLayout evl = {};
-        if (hbm_diff) {
-            GL_CHECK(accumulate_general(ctx));
-            p.diff = static_cast<const int*>(ctx->diff.p);
-            p.tile_sum = tile_sum_ptr(ctx);
-            p.super_sum = super_sum_ptr(ctx);
-        } else if (!fused) {
-            GL_CHECK(accumulate_events(ctx));
-            evl = ev_layout(ctx, tiles);
-        }
-        p.win_sum = static_cast<unsigned long long*>(ctx->win_sum_p);
-        p.win_min = (do_windows && want_min) ? static_cast<int*>(ctx->win_min.p) : nullptr;
-        p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
-        p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
-        long long cap = 0;
-        if (do_runs) {
-            cap = (long long)ctx->run_class.cap;
-            cap = std::min<long long>(cap, (long long)(ctx->run_start.cap / 4));
-            cap = std::min<long long>(cap, (long long)ctx->run_tmp_class.cap);
-            cap = std::min<long long>(cap, (long long)(ctx->run_tmp_start.cap / 4));
-        }
-        p.run_cap = cap;
-
-        if (attempt > 0) GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, head_bytes + win_bytes, ctx->stream));   // header + window sums again
-        if (do_windows && want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)n_windows * 4, ctx->stream));
-        {
-            gl_prof_scope prof(ctx, fused ? "depth_fused_kernel" : (hbm_diff ? "depth_scan_kernel" : "depth_evtile_kernel"));
-            const unsigned fused_grid = (unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4);
-            if (fused) depth_fused_kernel<<<fused_grid, kScanThreads, 0, ctx->stream>>>(p);
-            else if (hbm_diff) depth_scan_kernel<<<(unsigned)tiles, kScanThreads, 0, ctx->stream>>>(p);
-            else depth_evtile_kernel<<<(unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4), kEvThreads, 0, ctx->stream>>>(p, evl.events, evl.bucket_off, evl.carry);
-        }
-        GL_LAUNCHED(ctx, 1);
-        if (do_runs) {
-            // the run table has one entry per warp chunk of the kernel that ran (8 per tile, 4 for the 32-bases-per-thread K_evtile)
-            const int64_t chunks_now = tiles * ((fused || hbm_diff) ? kWarps : kEvWarps);
-            gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
-            depth_gather_runs_kernel<<<(unsigned)((chunks_now + 255) / 256), 256, 0, ctx->stream>>>(
-                header, chunk_runs, super_cnt, (int)chunks_now, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
-                static_cast<unsigned char*>(ctx->run_class.p), cap);
-            GL_LAUNCHED(ctx, 1);
-        }
-
-        ctx->prefetched = false;
-        if (ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap) {   // sums travel while the header is read
-            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums, ctx->win_sum_p, (size_t)n_windows * 8, cudaMemcpyDeviceToHost, ctx->stream));
-            ctx->prefetched = true;
-        }
-        ctx->prefetched_runs = 0;
-        if (ctx->prefetch_run_start && ctx->prefetch_run_class && do_runs) {       // ... and so do the first runs (usually all of them)
-            const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)cap);
-            if (k > 0) {
-                GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
-                GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
-                ctx->prefetched_runs = k;
-            }
-        }
-        uint64_t hdr[4];
-        GL_CHECK(read_header(ctx, hdr));
-        if (fused && hdr[3] != 0) { try_fused = false; ctx->prefetched = false; ctx->prefetched_runs = 0; continue; }        // not in BAM order / segments too long
-        ctx->last_path = fused ? 1 : (hbm_diff ? 2 : 4);
-        ctx->idx_flags = fused ? flags : nullptr;
-        ctx->idx_cells = fused ? cells : nullptr;
-        ctx->idx_origin = origin;
-        ctx->idx_ncells = ncells;
-        ctx->n_runs = do_runs ? (int64_t)hdr[0] : 0;
-        ctx->max_depth = (int32_t)hdr[2];
-        if (do_runs && (long long)hdr[0] > cap) {                          // output did not fit: grow and rerun
-            size_t ncap = (size_t)hdr[0] + 1024;
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, ncap * 4));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, ncap));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, ncap * 4));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, ncap));
-            continue;
-        }
-        break;
+    const bool fused = try_fused;
+    const bool hbm_diff = !fused && ctx->force_path == 2;      // the north-star pipeline (HBM difference array), on request only
+    EvLayout evl = {};
+    if (hbm_diff) {
+        GL_CHECK(accumulate_general(ctx));
+        p.diff = static_cast<const int*>(ctx->diff.p);
+        p.tile_sum = tile_sum_ptr(ctx);
+        p.super_sum = super_sum_ptr(ctx);
+    } else if (!fused) {
+        GL_CHECK(accumulate_events(ctx));
+        evl = ev_layout(ctx, tiles);
     }
-    ctx->red_W = W; ctx->red_mincov = mincov; ctx->red_maxmean = maxmean; ctx->red_break = run_break;
-    ctx->n_windows = do_windows ? n_windows : 0;
-    ctx->depth_reduced = true;
-    return GL_OK;
+    p.win_sum = static_cast<unsigned long long*>(ctx->win_sum_p);
+    p.win_min = (do_windows && want_min) ? static_cast<int*>(ctx->win_min.p) : nullptr;
+    p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
+    p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
+    long long cap = 0;
+    if (do_runs) {
+        cap = (long long)ctx->run_class.cap;
+        cap = std::min<long long>(cap, (long long)(ctx->run_start.cap / 4));
+        cap = std::min<long long>(cap, (long long)ctx->run_tmp_class.cap);
+        cap = std::min<long long>(cap, (long long)(ctx->run_tmp_start.cap / 4));
+    }
+    p.run_cap = cap;
+
+    if (do_windows && want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)n_windows * 4, ctx->stream));
+    {
+        gl_prof_scope prof(ctx, fused ? "depth_fused_kernel" : (hbm_diff ? "depth_scan_kernel" : "depth_evtile_kernel"));
+        const unsigned fused_grid = (unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4);
+        if (fused) depth_fused_kernel<<<fused_grid, kScanThreads, 0, ctx->stream>>>(p);
+        else if (hbm_diff) depth_scan_kernel<<<(unsigned)tiles, kScanThreads, 0, ctx->stream>>>(p);
+        else depth_evtile_kernel<<<(unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4), kEvThreads, 0, ctx->stream>>>(p, evl.events, evl.bucket_off, evl.carry);
+    }
+    GL_LAUNCHED(ctx, 1);
+    if (do_runs) {
+        // the run table has one entry per warp chunk of the kernel that ran (8 per tile, 4 for the 32-bases-per-thread K_evtile)
+        const int64_t chunks_now = tiles * ((fused || hbm_diff) ? kWarps : kEvWarps);
+        gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
+        depth_gather_runs_kernel<<<(unsigned)((chunks_now + 255) / 256), 256, 0, ctx->stream>>>(
+            header, chunk_runs, super_cnt, (int)chunks_now, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
+            static_cast<unsigned char*>(ctx->run_class.p), cap);
+        GL_LAUNCHED(ctx, 1);
+    }
+
+    ctx->prefetched = false;
+    if (ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap) {   // sums travel while the header is read
+        GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums, ctx->win_sum_p, (size_t)n_windows * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->prefetched = true;
+    }
+    ctx->prefetched_runs = 0;
+    if (ctx->prefetch_run_start && ctx->prefetch_run_class && do_runs) {       // ... and so do the first runs (usually all of them)
+        const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)cap);
+        if (k > 0) {
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+            ctx->prefetched_runs = k;
+        }
+    }
+    ctx->pend.path = fused ? 1 : (hbm_diff ? 2 : 4);
+    ctx->pend.run_cap = cap;
+    ctx->pend.n_windows = n_windows;
+    ctx->pend.d2h = false;
+    ctx->pend.flags = fused ? flags : nullptr;
+    ctx->pend.cells = fused ? cells : nullptr;
+    ctx->pend.origin = origin;
+    ctx->pend.ncells = ncells;
+    return defer_header(ctx);
 }
 
 constexpr int64_t kStageSegs = int64_t(1) << 22;      // segments per pinned staging slot (2 x 16 MiB)
@@ -1796,6 +1771,44 @@ int store_reserve(gl_ctx* ctx, int64_t need) {
 
 }  // namespace
 
+int depth_resolve(gl_ctx* ctx) {
+    while (ctx->pend.active) {
+        const auto q = ctx->pend;
+        ctx->pend.active = false;
+        GL_CUDA(ctx, cudaEventSynchronize(ctx->ev_hdr));
+        if (q.d2h) GL_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
+        const uint64_t* hdr = ctx->hdr_host;
+        int rerun = -1;                                                   // run_reduce's skip level for a rerun
+        if ((q.path == 3 || q.path == 1) && hdr[3] != 0) {                // packed8 anchors not sorted / int32 input not in BAM order
+            ctx->prefetched = false;
+            ctx->prefetched_runs = 0;
+            rerun = q.path == 3 ? 1 : 2;
+        } else if (q.do_runs && (long long)hdr[0] > q.run_cap) {          // the runs did not fit: grow and take the same path again
+            const size_t ncap = (size_t)hdr[0] + 1024;
+            GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, ncap * 4));
+            GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, ncap));
+            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, ncap * 4));
+            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, ncap));
+            rerun = q.path == 3 ? 0 : (q.path == 1 ? 1 : 2);
+        }
+        if (rerun >= 0) {
+            GL_CHECK(run_reduce(ctx, q.W, q.mincov, q.maxmean, q.run_break, q.do_windows, q.do_runs, q.d_depth_out, q.want_min, rerun));
+            continue;
+        }
+        ctx->last_path = q.path;
+        ctx->idx_flags = q.flags;
+        ctx->idx_cells = q.cells;
+        ctx->idx_origin = q.origin;
+        ctx->idx_ncells = q.ncells;
+        ctx->n_runs = q.do_runs ? (int64_t)hdr[0] : 0;
+        ctx->max_depth = (int32_t)hdr[2];
+        ctx->red_W = q.W; ctx->red_mincov = q.mincov; ctx->red_maxmean = q.maxmean; ctx->red_break = q.run_break;
+        ctx->n_windows = q.do_windows ? q.n_windows : 0;
+        ctx->depth_reduced = true;
+    }
+    return GL_OK;
+}
+
 extern "C" {
 
 int gl_depth_begin(gl_ctx* ctx, int64_t region_start, int64_t region_end) {
@@ -1814,7 +1827,7 @@ int gl_depth_begin(gl_ctx* ctx, int64_t region_start, int64_t region_end) {
     ctx->g_valid = false;
     ctx->ev_valid = false;
     ctx->depth_active = true;
-    ctx->depth_reduced = false;
+    drop_result(ctx);     // nobody can ask for a pending result any more; its scratch is reused in stream order
     ctx->n_windows = 0;
     ctx->n_runs = 0;
     ctx->max_depth = 0;
@@ -1832,7 +1845,7 @@ int gl_depth_add_segments_device(gl_ctx* ctx, const int32_t* d_start, const int3
     ctx->batches.push_back(b);
     ctx->g_valid = false;
     ctx->ev_valid = false;
-    ctx->depth_reduced = false;
+    drop_result(ctx);
     return GL_OK;
 }
 
@@ -1845,6 +1858,8 @@ int gl_depth_add_segments(gl_ctx* ctx, const int32_t* start, const int32_t* end,
     GL_CHECK(store_reserve(ctx, ctx->store_n + n));
     int32_t* d_s = static_cast<int32_t*>(ctx->store_s.p) + ctx->store_n;
     int32_t* d_e = static_cast<int32_t*>(ctx->store_e.p) + ctx->store_n;
+    // a reduce of the previous region may still be queued and reading the store: the copies go after it
+    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_hdr, 0));
     if (is_pinned_host(start) && is_pinned_host(end)) {
         GL_CUDA(ctx, cudaMemcpyAsync(d_s, start, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
         GL_CUDA(ctx, cudaMemcpyAsync(d_e, end, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
@@ -1886,7 +1901,7 @@ int gl_depth_add_segments(gl_ctx* ctx, const int32_t* start, const int32_t* end,
     ctx->store_n += n;
     ctx->g_valid = false;
     ctx->ev_valid = false;
-    ctx->depth_reduced = false;
+    drop_result(ctx);
     return GL_OK;
 }
 
@@ -1936,7 +1951,7 @@ int gl_depth_add_segments_packed16(gl_ctx* ctx, const int32_t* anchors, const ui
     ctx->store_n += n;
     ctx->g_valid = false;
     ctx->ev_valid = false;
-    ctx->depth_reduced = false;
+    drop_result(ctx);
     return GL_OK;
 }
 
@@ -1954,7 +1969,7 @@ static int p8_register(gl_ctx* ctx, const int* d_anchor, const void* d_ds, const
     if (ctx->batches.size() > 1) GL_CHECK(p8_materialize(ctx));   // not the only batch: the int32 paths take it
     ctx->g_valid = false;
     ctx->ev_valid = false;
-    ctx->depth_reduced = false;
+    drop_result(ctx);
     return GL_OK;
 }
 
@@ -2014,6 +2029,7 @@ int gl_depth_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int
 
 int gl_depth_result_sizes(gl_ctx* ctx, int64_t* n_windows, int64_t* n_runs, int32_t* max_depth) {
     GL_CHECK(gl_use(ctx));
+    GL_CHECK(depth_resolve(ctx));
     if (!ctx->depth_reduced) return gl_fail(ctx, GL_ESTATE, "gl_depth_result_sizes: call gl_depth_reduce first");
     if (n_windows) *n_windows = ctx->n_windows;
     if (n_runs) *n_runs = ctx->n_runs;
@@ -2038,6 +2054,8 @@ int gl_depth_transport_phases(gl_ctx* ctx, double phases_s[3]) {
 
 int gl_depth_last_path(gl_ctx* ctx, int32_t* path) {
     if (!ctx || !path) return gl_fail(ctx, GL_EINVAL, "null argument");
+    GL_CHECK(gl_use(ctx));
+    GL_CHECK(depth_resolve(ctx));
     *path = ctx->last_path;
     return GL_OK;
 }
@@ -2050,6 +2068,7 @@ int gl_depth_set_path(gl_ctx* ctx, int32_t path) {
 
 int gl_depth_get_windows(gl_ctx* ctx, int64_t* sum_out, int64_t cap) {
     GL_CHECK(gl_use(ctx));
+    GL_CHECK(depth_resolve(ctx));
     if (!ctx->depth_reduced || ctx->n_windows == 0) return gl_fail(ctx, GL_ESTATE, "gl_depth_get_windows: no window results");
     if (!sum_out) return gl_fail(ctx, GL_EINVAL, "gl_depth_get_windows: null sum_out");
     if (cap < ctx->n_windows) return gl_fail(ctx, GL_ERANGE, "gl_depth_get_windows: cap %lld < %lld windows", (long long)cap, (long long)ctx->n_windows);
@@ -2060,6 +2079,7 @@ int gl_depth_get_windows(gl_ctx* ctx, int64_t* sum_out, int64_t cap) {
 
 int gl_depth_get_runs(gl_ctx* ctx, int32_t* run_start, int32_t* run_end, uint8_t* run_class, int64_t cap) {
     GL_CHECK(gl_use(ctx));
+    GL_CHECK(depth_resolve(ctx));
     if (!ctx->depth_reduced) return gl_fail(ctx, GL_ESTATE, "gl_depth_get_runs: call gl_depth_reduce first");
     const int64_t n = ctx->n_runs;
     if (cap < n) return gl_fail(ctx, GL_ERANGE, "gl_depth_get_runs: cap %lld < %lld runs", (long long)cap, (long long)n);
@@ -2082,6 +2102,7 @@ int gl_depth_windows(gl_ctx* ctx, int32_t W, int64_t* sum_out, int32_t* min_out,
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_windows: no region open");
     if (W <= 0) return gl_fail(ctx, GL_EINVAL, "gl_depth_windows: W must be > 0");
     GL_CHECK(run_reduce(ctx, W, 0, 0, 0, true, false, nullptr, min_out != nullptr));
+    GL_CHECK(depth_resolve(ctx));
     GL_CHECK(gl_depth_get_windows(ctx, sum_out, n_windows));
     if (min_out) {
         GL_CUDA(ctx, cudaMemcpyAsync(min_out, ctx->win_min.p, (size_t)ctx->n_windows * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2095,6 +2116,7 @@ int gl_depth_classes(gl_ctx* ctx, int32_t mincov, int32_t maxmean, int32_t* run_
     GL_CHECK(gl_use(ctx));
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_classes: no region open");
     GL_CHECK(run_reduce(ctx, 1 << 30, mincov, maxmean, 0, false, true, nullptr, false));
+    GL_CHECK(depth_resolve(ctx));
     if (n_runs) *n_runs = ctx->n_runs;
     return gl_depth_get_runs(ctx, run_start, run_end, run_class, cap);
 }
@@ -2104,6 +2126,7 @@ int gl_depth_interval_sums(gl_ctx* ctx, const int32_t* a, const int32_t* b, int6
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_interval_sums: no region open");
     if (n < 0 || (n > 0 && (!a || !b || !sums))) return gl_fail(ctx, GL_EINVAL, "gl_depth_interval_sums: bad argument");
     if (n == 0) return GL_OK;
+    GL_CHECK(depth_resolve(ctx));                                  // the last reduce's path decides whether its cell index is used
     if (ctx->copies_pending) {
         GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[0], ctx->copy_stream));
         GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[0], 0));
@@ -2161,6 +2184,7 @@ int gl_depth_perbase(gl_ctx* ctx, int32_t* depth_out) {
     const int64_t len = ctx->re - ctx->rs;
     GL_CHECK(gl_buf_reserve(ctx, ctx->misc, (size_t)(len + 4) * 4));
     GL_CHECK(run_reduce(ctx, 1 << 30, 0, 0, 0, false, false, static_cast<int32_t*>(ctx->misc.p), false));
+    GL_CHECK(depth_resolve(ctx));
     GL_CUDA(ctx, cudaMemcpyAsync(depth_out, ctx->misc.p, (size_t)len * 4, cudaMemcpyDeviceToHost, ctx->stream));
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     ctx->depth_reduced = false;
@@ -2329,7 +2353,7 @@ int gl_depth_bed_region(gl_ctx* ctx, const char* chrom, int64_t rs, int64_t re, 
             bt.off = 0; bt.n = done_blocks * 256;
             ctx->batches.push_back(bt);
             ctx->store_n = done_blocks * 256;
-            ctx->g_valid = false; ctx->ev_valid = false; ctx->depth_reduced = false;
+            ctx->g_valid = false; ctx->ev_valid = false; drop_result(ctx);
         }
         const auto ph2 = std::chrono::steady_clock::now();
         ctx->tr_esc = n_esc;
@@ -2407,6 +2431,7 @@ int gl_depth_bed_contig(gl_ctx* ctx, const char* chrom, int64_t contig_len, cons
 
 static int region_fetch(gl_ctx* ctx, int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class,
                         int64_t run_cap, int64_t* n_runs) {
+    GL_CHECK(depth_resolve(ctx));
     const int64_t nw = ctx->n_windows, nr = ctx->n_runs;
     if (n_windows) *n_windows = nw;
     if (n_runs) *n_runs = nr;
@@ -2415,7 +2440,7 @@ static int region_fetch(gl_ctx* ctx, int64_t* sum_out, int64_t win_cap, int64_t*
     const bool have_sums = ctx->prefetched, have_runs = ctx->prefetched_runs >= nr;
     ctx->prefetched = false;
     ctx->prefetched_runs = 0;
-    if (have_sums && have_runs) return GL_OK;                  // everything came home with the header (the reduce has synchronised)
+    if (have_sums && have_runs) return GL_OK;                  // everything came home with the header (depth_resolve waited for it)
     if (!have_sums) GL_CUDA(ctx, cudaMemcpyAsync(sum_out, ctx->win_sum_p, (size_t)nw * 8, cudaMemcpyDeviceToHost, ctx->stream));
     if (nr > 0 && !have_runs) {
         GL_CUDA(ctx, cudaMemcpyAsync(run_start, ctx->run_start.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ctx->stream));

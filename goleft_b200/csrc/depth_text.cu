@@ -292,6 +292,7 @@ extern "C" {
 int gl_depth_text(gl_ctx* ctx, const char* chrom, char* depth_bed, int64_t depth_cap, int64_t* depth_len,
                   char* callable_bed, int64_t callable_cap, int64_t* callable_len) {
     GL_CHECK(gl_use(ctx));
+    GL_CHECK(depth_resolve(ctx));
     if (!ctx->depth_reduced) return gl_fail(ctx, GL_ESTATE, "gl_depth_text: call gl_depth_reduce first");
     if (!depth_len || !callable_len) return gl_fail(ctx, GL_EINVAL, "gl_depth_text: null length pointer");
     const int W = ctx->red_W;

@@ -62,6 +62,16 @@ struct gl_ctx {
     void* win_sum_p = nullptr;   // u64[n_windows], inside `scratch`
     int64_t* prefetch_sums = nullptr; int64_t prefetch_cap = 0; bool prefetched = false;   // one-call entries: window sums go home while the header is read
     int32_t* prefetch_run_start = nullptr; uint8_t* prefetch_run_class = nullptr; int64_t prefetch_run_cap = 0, prefetched_runs = 0;   // and the first runs
+    // gl_depth_reduce only queues its work: the header (runs claimed, max depth, fast path rejected) travels into the pinned
+    // hdr_host behind ev_hdr, and depth_resolve reads it at the first result query, with what accepting or rerunning needs
+    uint64_t* hdr_host = nullptr;         // 4 words, pinned
+    cudaEvent_t ev_hdr = nullptr;
+    struct { bool active = false;
+             int32_t W = 0, mincov = 0, maxmean = 0; int64_t run_break = 0; bool do_windows = false, do_runs = false, want_min = false;
+             int32_t* d_depth_out = nullptr;
+             int path = 0; long long run_cap = 0; int64_t n_windows = 0;   // the path tried (as gl_depth_last_path) and its run capacity
+             bool d2h = false;                                             // window sums also on their way home on d2h_stream
+             const int* flags = nullptr; const unsigned* cells = nullptr; int origin = 0, ncells = 0; } pend;
     gl_buf win_min;       // i32[n_windows]
     gl_buf run_start;     // i32[run_cap]
     gl_buf run_class;     // u8[run_cap]
@@ -98,7 +108,11 @@ struct gl_ctx {
 extern thread_local std::string g_gl_err;
 
 int gl_fail(gl_ctx* ctx, int code, const char* fmt, ...);
+// Grows b.  Freeing the old buffer first synchronises ctx->stream, so no queued work can still be using it.
 int gl_buf_reserve(gl_ctx* ctx, gl_buf& b, size_t bytes);
+// depth.cu: settle the last gl_depth_reduce (wait for its header; accept it, or rerun it on the next path or with room for
+// every run).  Every reader of the reduce's results calls this first; a no-op when nothing is pending.
+int depth_resolve(gl_ctx* ctx);
 
 #define GL_CUDA(ctx, expr)                                                             \
     do {                                                                               \

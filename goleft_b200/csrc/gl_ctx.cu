@@ -79,6 +79,8 @@ int gl_ctx_create(int device, gl_ctx** out) {
         e = cudaEventCreateWithFlags(&ctx->ev_copy[i], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_used[i], cudaEventDisableTiming);
     }
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_hdr, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaHostAlloc(reinterpret_cast<void**>(&ctx->hdr_host), 4 * sizeof(uint64_t), cudaHostAllocDefault);
     if (e == cudaSuccess) {
         cudaDeviceProp prop;
         e = cudaGetDeviceProperties(&prop, device);
@@ -186,6 +188,8 @@ int gl_ctx_destroy(gl_ctx* ctx) {
         if (ctx->ev_used[i]) cudaEventDestroy(ctx->ev_used[i]);
     }
     if (ctx->pack_pinned) cudaFreeHost(ctx->pack_pinned);
+    if (ctx->hdr_host) cudaFreeHost(ctx->hdr_host);
+    if (ctx->ev_hdr) cudaEventDestroy(ctx->ev_hdr);
     free(ctx->esc_buf);
     for (auto& r : ctx->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
     for (auto e : ctx->prof_pool) cudaEventDestroy(e);

@@ -103,8 +103,10 @@ int  gl_depth_begin(gl_ctx* ctx, int64_t region_start, int64_t region_end);
 /* Add n segments [start[i], end[i]) (absolute contig coordinates, end>start; clipped to the region
  * by the kernels; segments outside are ignored).  May be called repeatedly between begin and reduce.
  * Host-pointer variant copies into a ctx-owned device store on a copy stream (pinned sources DMA
- * directly, pageable ones are staged); _device variant references HBM-resident arrays, which must
- * stay valid until the results have been fetched.
+ * directly after the call returns: leave a pinned source unchanged until the region's results have
+ * been read; pageable ones are staged); _device variant references HBM-resident arrays, which must
+ * stay valid until the region's results have been read or the next gl_depth_begin (a reduce whose fast
+ * path the device rejects is rerun from them at the first result query).
  * Any order is accepted.  Coordinate-sorted segments (non-decreasing start, what a BAM yields) of at
  * most 16384 bases take the fused path: each 4096-base tile's difference array is built in shared
  * memory straight from the segments.  Anything else takes the general path (bucketed events, see
@@ -152,7 +154,8 @@ int  gl_pack_segments8_mt(const int32_t* start, const int32_t* end, int64_t n, i
                           uint8_t* len, int64_t cap_blocks, int64_t* n_blocks);
 int  gl_depth_add_segments_packed8(gl_ctx* ctx, const int32_t* anchors, const uint8_t* dstart, const uint8_t* len, int64_t n_blocks);
 /* same with the three arrays already in device memory (caller-owned, 8-byte aligned, must stay valid until the region's
- * last reduce): nothing is copied; a region whose only batch is packed8 is reduced straight from these words. */
+ * results have been read or the next gl_depth_begin): nothing is copied; a region whose only batch is packed8 is reduced
+ * straight from these words. */
 int  gl_depth_add_segments_packed8_device(gl_ctx* ctx, const int32_t* d_anchors, const uint8_t* d_dstart, const uint8_t* d_len,
                                           int64_t n_blocks);
 
@@ -162,10 +165,14 @@ int  gl_depth_add_segments_packed8_device(gl_ctx* ctx, const int32_t* d_anchors,
  *   (b) class run starts: position x starts a run when x==rs, class(x)!=class(x-1), or
  *       run_break>0 and x%run_break==0 (the reference never merges runs across its 10 Mb
  *       chunks, depth/depth.go:132,150: pass run_break=step to reproduce that).
- * mincov/maxmean as depth/depth.go:223-234.  Synchronous; results stay on the device until fetched. */
+ * mincov/maxmean as depth/depth.go:223-234.  Asynchronous: the arguments are checked at once, the work is queued on the
+ * ctx stream and the call returns without waiting for it, so regions reduced back to back keep the device busy.  Errors
+ * in the device work and fallbacks (input the fast path rejects, a run table that has to grow) are settled at the first
+ * result query (gl_depth_result_sizes, gl_depth_last_path, gl_depth_get_*, gl_depth_text, gl_depth_interval_sums); a
+ * result nobody queried is dropped by the next gl_depth_begin or add.  Results stay on the device until fetched. */
 int  gl_depth_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break);
 
-/* Sizes of the results of the last gl_depth_reduce. */
+/* Sizes of the results of the last gl_depth_reduce (waits for it). */
 int  gl_depth_result_sizes(gl_ctx* ctx, int64_t* n_windows, int64_t* n_runs, int32_t* max_depth);
 /* Which path the last reduce took: 1 = fused (nearly sorted int32 segments), 2 = HBM difference array (the north-star
  * pipeline: red.global scatter + scan; on request only), 3 = packed8 (the region's only batch is packed8: read as it is, no

@@ -1477,6 +1477,166 @@ static int cmd_indexsplit(int argc, char** argv) {
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ multidepth
+// multidepth/multidepth.go: blocks of one chromosome where more than --minsamples of the BAMs reach --mincov, with every
+// sample's mean depth.  Two passes over each sample's segments on the GPU (counts, then block sums); the segments are
+// decoded once and kept in their compact form in between (packed8 words, or the GPU feeder's int32 copied to pinned memory).
+// The output is the reference's with -p 1 (chunks in order).
+struct MdSample {
+    glhts::ContigSegs segs;                 // host feeder: packed8 words or sorted int32
+    std::vector<int32_t> s32, e32;          // unindexed BAM: the contig's segments in record order
+    int32_t* pin = nullptr; int64_t pin_n = 0;   // GPU feeder: start | end copied to pinned host memory
+};
+
+static void md_add(gl_ctx* ctx, const MdSample& m) {
+    if (m.pin) { if (m.pin_n > 0) glck(ctx, gl_depth_add_segments(ctx, m.pin, m.pin + m.pin_n, m.pin_n), "gl_depth_add_segments"); return; }
+    if (!m.s32.empty()) { glck(ctx, gl_depth_add_segments(ctx, m.s32.data(), m.e32.data(), (int64_t)m.s32.size()), "gl_depth_add_segments"); return; }
+    if (m.segs.format == 8 && m.segs.n_blocks > 0)
+        glck(ctx, gl_depth_add_segments_packed8(ctx, m.segs.anchors.data(), m.segs.ds.data(), m.segs.len.data(), m.segs.n_blocks), "gl_depth_add_segments_packed8");
+    else if (m.segs.format == 32 && m.segs.n > 0)
+        glck(ctx, gl_depth_add_segments(ctx, m.segs.start.data(), m.segs.end.data(), m.segs.n), "gl_depth_add_segments");
+}
+
+static int cmd_multidepth(int argc, char** argv) {
+    std::string q = "10", chrom, mincov = "7", maxcov = "1000", maxskip = "10", minsize = "15", window = "10000000", procs = "0",
+                minsamples = "0.5";
+    ArgParser ap;
+    ap.prog = "goleft multidepth";
+    ap.add("q", 'Q', &q); ap.add("chrom", 'c', &chrom, true); ap.add("mincov", 0, &mincov); ap.add("maxcov", 0, &maxcov);
+    ap.add("maxskip", 'k', &maxskip); ap.add("minsize", 'm', &minsize); ap.add("window", 'w', &window); ap.add("processes", 'p', &procs);
+    ap.add("minsamples", 0, &minsamples);
+    ap.parse(argc, argv);
+    if (ap.positional.empty()) ap.fail("bams is required");
+    const std::vector<std::string>& bams = ap.positional;
+    const int S = (int)bams.size();
+    const int Q = atoi(q.c_str()), threads = std::max(0, atoi(procs.c_str()));     // --maxcov: accepted, no effect (DESIGN §0)
+    // header: the short name of every BAM (multidepth.go:66-72); the contig length from the first (chromSize, :34-48)
+    std::string hdr = "#chrom\tstart\tend";
+    std::vector<gl_bam> bam((size_t)S);
+    std::vector<int> tid((size_t)S, -1);
+    long long L = -1;
+    for (int i = 0; i < S; i++) {
+        std::string e = bam[(size_t)i].f.open(bams[(size_t)i]);
+        if (!e.empty()) fatal(2, "panic: %s", e.c_str());
+        hdr += "\t" + short_name(bams[(size_t)i], false, &bam[(size_t)i].f.header);
+        const auto& refs = bam[(size_t)i].f.header.refs;
+        for (size_t r = 0; r < refs.size(); r++) if (refs[r].name == chrom) { tid[(size_t)i] = (int)r; if (i == 0) L = refs[r].length; }
+        if (tid[(size_t)i] < 0) fatal(2, "panic: multidepth: chromosome %s not found in %s", chrom.c_str(), bams[(size_t)i].c_str());
+    }
+    gl_ctx* ctx = nullptr;
+    if (gl_ctx_create(0, &ctx) != GL_OK) fatal(1, "goleft multidepth: %s", gl_last_error(nullptr));
+    if (L <= 0) { printf("%s\n", hdr.c_str()); gl_ctx_destroy(ctx); return 0; }
+    glck(ctx, gl_multidepth_begin(ctx, L, S, atoi(mincov.c_str()), atof(minsamples.c_str())), "goleft multidepth");
+    static const bool gpu_feed = [] { const char* e = getenv("GL_GPU_FEED"); return !e || atoi(e) != 0; }();
+    std::vector<MdSample> smp((size_t)S);
+    // host decode of sample i (index-guided, or the whole file when there is no index); runs beside the GPU work of sample i-1
+    auto host_decode = [&](int i) {
+        gl_bam& b = bam[(size_t)i];
+        if (!b.f.has_index) {
+            glhts::SegmentSet set;
+            std::string e = glhts::bam_decode_segments(bams[(size_t)i], Q, threads > 0 ? threads : 8, tid[(size_t)i], set);
+            if (!e.empty()) fatal(1, "%s", e.c_str());
+            smp[(size_t)i].s32.swap(set.start[(size_t)tid[(size_t)i]]);
+            smp[(size_t)i].e32.swap(set.end[(size_t)tid[(size_t)i]]);
+            return;
+        }
+        std::string e = b.f.decode(tid[(size_t)i], 0, L, Q, threads, 0, smp[(size_t)i].segs, nullptr);
+        if (!e.empty()) fatal(1, "%s", e.c_str());
+    };
+    // pass 1
+    std::thread next;
+    bool next_host = false;
+    for (int i = 0; i < S; i++) {
+        MdSample& m = smp[(size_t)i];
+        const int32_t *ds = nullptr, *de = nullptr;
+        int64_t dn = -1;
+        if (next.joinable()) next.join();
+        if (!next_host) {
+            if (gpu_feed && bam[(size_t)i].f.has_index) {
+                gl_bam_segments st;
+                const int rc = gl_bam_decode_device(ctx, &bam[(size_t)i], tid[(size_t)i], Q, &ds, &de, &dn, &st);
+                if (rc != GL_OK) { dn = -1; if (rc != GL_ESTATE) glck(ctx, rc, "gl_bam_decode_device"); }
+            }
+            if (dn < 0) host_decode(i);
+        }
+        // the next sample's host decode overlaps this sample's device work
+        next_host = i + 1 < S && !(gpu_feed && bam[(size_t)i + 1].f.has_index);
+        if (next_host) next = std::thread(host_decode, i + 1);
+        glck(ctx, gl_depth_begin(ctx, 0, L), "gl_depth_begin");
+        if (dn >= 0) {
+            if (dn > 0) glck(ctx, gl_depth_add_segments_device(ctx, ds, de, dn), "gl_depth_add_segments_device");
+            glck(ctx, gl_multidepth_count(ctx), "gl_multidepth_count");
+            void* p = nullptr;
+            glck(ctx, gl_host_alloc_pinned(ctx, std::max<int64_t>(dn, 1) * 8, &p), "gl_host_alloc_pinned");
+            m.pin = static_cast<int32_t*>(p); m.pin_n = dn;
+            if (dn > 0) {
+                glck(ctx, gl_memcpy_d2h(ctx, m.pin, ds, dn * 4), "gl_memcpy_d2h");
+                glck(ctx, gl_memcpy_d2h(ctx, m.pin + dn, de, dn * 4), "gl_memcpy_d2h");
+            }
+        } else {
+            md_add(ctx, m);
+            glck(ctx, gl_multidepth_count(ctx), "gl_multidepth_count");
+        }
+    }
+    if (next.joinable()) next.join();
+    // blocks
+    int64_t nr = 0;
+    glck(ctx, gl_multidepth_sites(ctx, nullptr, nullptr, 0, &nr), "gl_multidepth_sites");
+    std::vector<int32_t> rs((size_t)std::max<int64_t>(nr, 1));
+    std::vector<uint8_t> rc((size_t)std::max<int64_t>(nr, 1));
+    glck(ctx, gl_multidepth_sites(ctx, rs.data(), rc.data(), nr, &nr), "gl_multidepth_sites");
+    const int64_t max_skip = atoll(maxskip.c_str()), min_size = atoll(minsize.c_str()), win = atoll(window.c_str());
+    int64_t nb = 0;
+    if (gl_multidepth_blocks(rs.data(), rc.data(), nr, L, S, 0, max_skip, min_size, win, nullptr, nullptr, nullptr, 0, &nb) != GL_OK)
+        fatal(1, "gl_multidepth_blocks failed");
+    std::vector<int64_t> bs((size_t)std::max<int64_t>(nb, 1)), be(bs.size()), bn(bs.size());
+    if (gl_multidepth_blocks(rs.data(), rc.data(), nr, L, S, 0, max_skip, min_size, win, bs.data(), be.data(), bn.data(), nb, &nb) != GL_OK)
+        fatal(1, "gl_multidepth_blocks failed");
+    glck(ctx, gl_multidepth_set_blocks(ctx, bs.data(), be.data(), bn.data(), nb), "gl_multidepth_set_blocks");
+    // pass 2
+    for (int i = 0; i < S; i++) {
+        glck(ctx, gl_depth_begin(ctx, 0, L), "gl_depth_begin");
+        md_add(ctx, smp[(size_t)i]);
+        glck(ctx, gl_multidepth_sums(ctx, i), "gl_multidepth_sums");
+    }
+    const size_t cells = (size_t)nb * (size_t)S;
+    std::vector<int64_t> qv(std::max<size_t>(cells, 1));
+    std::vector<double> val(qv.size());
+    std::vector<uint8_t> cert(qv.size());
+    glck(ctx, gl_multidepth_result(ctx, nullptr, qv.data(), val.data(), cert.data()), "gl_multidepth_result");
+    char* text = nullptr;
+    int64_t tl = 0;
+    if (gl_multidepth_text(chrom.c_str(), bs.data(), be.data(), nb, S, qv.data(), val.data(), cert.data(), threads, &text, &tl) != GL_OK)
+        fatal(1, "gl_multidepth_text failed");
+    printf("%s\n", hdr.c_str());
+    fwrite(text, 1, (size_t)tl, stdout);
+    gl_free_text(text);
+    for (MdSample& m : smp) if (m.pin) gl_host_free_pinned(ctx, m.pin);
+    gl_ctx_destroy(ctx);
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ samplename
+// samplename/samplename.go: one @RG -> its SM (nothing when empty); several -> the distinct non-empty SMs, here in header
+// order (the reference iterates a Go map).  -e: anything but exactly one sample is an error.
+static int cmd_samplename(int argc, char** argv) {
+    bool err_multi = false;
+    ArgParser ap;
+    ap.prog = "goleft samplename";
+    ap.addb("errormulti", 'e', &err_multi);
+    ap.parse(argc, argv);
+    if (ap.positional.empty()) ap.fail("bam is required");
+    glhts::BamHeader h;
+    std::string e = glhts::bam_read_header(ap.positional[0], h);
+    if (!e.empty()) fatal(2, "panic: %s", e.c_str());
+    const std::vector<std::string> names = h.sample_names();
+    if (err_multi && names.size() != 1) fatal(2, "panic: goleft/samplename: found multiple samples in %s", ap.positional[0].c_str());
+    std::string out;
+    for (size_t i = 0; i < names.size(); i++) out += (i ? "\n" : "") + names[i];
+    printf("%s\n", out.c_str());
+    return 0;
+}
+
 static void print_progs() {                                                          // cmd/goleft/goleft.go:33-53
     fprintf(stderr, "goleft Version: %s (GPU engine: %s)\n\n", kVersion, gl_version());
     fprintf(stderr, "covstats    : coverage and insert-size statistics on bams by sampling\n");
@@ -1484,6 +1644,8 @@ static void print_progs() {                                                     
     fprintf(stderr, "depthwed    : matricize output from depth to n-sites * n-samples\n");
     fprintf(stderr, "indexcov    : quick coverage estimate using only the bam index\n");
     fprintf(stderr, "indexsplit  : create regions of even coverage across bams/crams\n");
+    fprintf(stderr, "samplename  : report samplename(s) from a bam's SM tag\n");
+    fprintf(stderr, "multidepth  : (extension; a separate binary in goleft) blocks of sufficient coverage across many bams\n");
 }
 
 int main(int argc, char** argv) {
@@ -1494,6 +1656,8 @@ int main(int argc, char** argv) {
     if (prog == "covstats") return cmd_covstats(argc - 1, argv + 1);
     if (prog == "depthwed") return cmd_depthwed(argc - 1, argv + 1);
     if (prog == "indexsplit") return cmd_indexsplit(argc - 1, argv + 1);
+    if (prog == "samplename") return cmd_samplename(argc - 1, argv + 1);
+    if (prog == "multidepth") return cmd_multidepth(argc - 1, argv + 1);
     print_progs();
     return 1;
 }

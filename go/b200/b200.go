@@ -219,3 +219,67 @@ func (c *Ctx) IndexcovCohort(sizes []int64, samplePtr []int64) (medians []float6
 		C.int32_t(S), (*C.double)(unsafe.Pointer(&medians[0])), (*C.float)(unsafe.Pointer(&depths[0])))
 	return medians, depths, c.err(rc)
 }
+
+// Multidepth replaces multidepth/multidepth.go:208-283 for one contig of `length` bases: addSegments(i) must add sample i's
+// M/=/X blocks (records with Flags&0x704 == 0 && MapQ >= Q) to the open region with gl_depth_add_segments* — it is called
+// twice per sample, once per pass.  Returns the rows after the header line, exactly as the reference with -p 1.
+func (c *Ctx) Multidepth(chrom string, length, samples, minCov int, minSamples float64, maxSkip, minSize, window int,
+	addSegments func(i int) error) ([]byte, error) {
+	if err := c.err(C.gl_multidepth_begin(c.h, C.int64_t(length), C.int32_t(samples), C.int32_t(minCov), C.double(minSamples))); err != nil {
+		return nil, err
+	}
+	pass := func(f func(i int) C.int) error {
+		for i := 0; i < samples; i++ {
+			if err := c.err(C.gl_depth_begin(c.h, 0, C.int64_t(length))); err != nil {
+				return err
+			}
+			if err := addSegments(i); err != nil {
+				return err
+			}
+			if err := c.err(f(i)); err != nil {
+				return err
+			}
+		}
+		return nil
+	}
+	if err := pass(func(int) C.int { return C.gl_multidepth_count(c.h) }); err != nil {
+		return nil, err
+	}
+	var nr C.int64_t
+	if err := c.err(C.gl_multidepth_sites(c.h, nil, nil, 0, &nr)); err != nil {
+		return nil, err
+	}
+	rs, rc := make([]int32, nr+1), make([]uint8, nr+1)
+	if err := c.err(C.gl_multidepth_sites(c.h, (*C.int32_t)(&rs[0]), (*C.uint8_t)(&rc[0]), nr, &nr)); err != nil {
+		return nil, err
+	}
+	var nb C.int64_t
+	if C.gl_multidepth_blocks((*C.int32_t)(&rs[0]), (*C.uint8_t)(&rc[0]), nr, C.int64_t(length), C.int32_t(samples), 0, C.int64_t(maxSkip),
+		C.int64_t(minSize), C.int64_t(window), nil, nil, nil, 0, &nb) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_multidepth_blocks failed")
+	}
+	bs, be, bn := make([]int64, nb+1), make([]int64, nb+1), make([]int64, nb+1)
+	C.gl_multidepth_blocks((*C.int32_t)(&rs[0]), (*C.uint8_t)(&rc[0]), nr, C.int64_t(length), C.int32_t(samples), 0, C.int64_t(maxSkip),
+		C.int64_t(minSize), C.int64_t(window), (*C.int64_t)(&bs[0]), (*C.int64_t)(&be[0]), (*C.int64_t)(&bn[0]), nb, &nb)
+	if err := c.err(C.gl_multidepth_set_blocks(c.h, (*C.int64_t)(&bs[0]), (*C.int64_t)(&be[0]), (*C.int64_t)(&bn[0]), nb)); err != nil {
+		return nil, err
+	}
+	if err := pass(func(i int) C.int { return C.gl_multidepth_sums(c.h, C.int32_t(i)) }); err != nil {
+		return nil, err
+	}
+	cells := int(nb)*samples + 1
+	q, val, cert := make([]int64, cells), make([]float64, cells), make([]uint8, cells)
+	if err := c.err(C.gl_multidepth_result(c.h, nil, (*C.int64_t)(&q[0]), (*C.double)(&val[0]), (*C.uint8_t)(&cert[0]))); err != nil {
+		return nil, err
+	}
+	cs := C.CString(chrom)
+	defer C.free(unsafe.Pointer(cs))
+	var text *C.char
+	var tl C.int64_t
+	if C.gl_multidepth_text(cs, (*C.int64_t)(&bs[0]), (*C.int64_t)(&be[0]), nb, C.int32_t(samples), (*C.int64_t)(&q[0]), (*C.double)(&val[0]),
+		(*C.uint8_t)(&cert[0]), 0, &text, &tl) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_multidepth_text failed")
+	}
+	defer C.gl_free_text(text)
+	return C.GoBytes(unsafe.Pointer(text), C.int(tl)), nil
+}

@@ -170,6 +170,17 @@ _proto("gl_crai_make_sizes", C.c_int, _vp, _vp, _vp, C.c_int64, _vp, C.c_int64, 
 _proto("gl_depth_format_chunk", C.c_int, C.c_char_p, C.c_int64, C.c_int64, C.c_int32, _vp, C.c_int64, _vp, _vp,
        C.c_int64, C.POINTER(_vp), _i64p, C.POINTER(_vp), _i64p)
 _proto("gl_free_text", None, _vp)
+_proto("gl_multidepth_begin", C.c_int, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_double)
+_proto("gl_multidepth_count", C.c_int, _vp)
+_proto("gl_multidepth_sites", C.c_int, _vp, _vp, _vp, C.c_int64, _i64p)
+_proto("gl_multidepth_blocks", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+       _vp, _vp, _vp, C.c_int64, _i64p)
+_proto("gl_multidepth_set_blocks", C.c_int, _vp, _vp, _vp, _vp, C.c_int64)
+_proto("gl_multidepth_sums", C.c_int, _vp, C.c_int32)
+_proto("gl_multidepth_result", C.c_int, _vp, _vp, _vp, _vp, _vp)
+_proto("gl_multidepth_stats", C.c_int, _vp, _i64p, _i64p, _i64p, _i64p)
+_proto("gl_multidepth_certify", C.c_int, _vp, _vp, _vp, C.c_int64, _vp, _vp)
+_proto("gl_multidepth_text", C.c_int, C.c_char_p, _vp, _vp, C.c_int64, C.c_int32, _vp, _vp, _vp, C.c_int32, C.POINTER(_vp), _i64p)
 
 
 def version() -> str:
@@ -232,6 +243,51 @@ def format_chunk(chrom: str, rs: int, re: int, W: int, win_sum: np.ndarray, run_
     finally:
         lib.gl_free_text(d)
         lib.gl_free_text(c)
+
+
+# ---- multidepth (multidepth/multidepth.go), host-only parts
+MD_DEFAULTS = dict(Q=10, mincov=7, maxcov=1000, min_samples=0.5, min_size=15, max_skip=10, window=10_000_000)
+
+
+def multidepth_blocks(run_start, run_class, contig_len: int, n_samples: int, max_skip: int = 10, min_size: int = 15,
+                      window: int = 10_000_000, chunk: int = 0):
+    """Host-only: the reference's chunk state machine over site-class runs -> (start, end, sufficient sites) arrays."""
+    run_start, run_class = _as(run_start, np.int32), _as(run_class, np.uint8)
+    n = C.c_int64(0)
+    args = (_ptr(run_start), _ptr(run_class), run_start.size, contig_len, n_samples, chunk, max_skip, min_size, window)
+    rc = lib.gl_multidepth_blocks(*args, None, None, None, 0, C.byref(n))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_multidepth_blocks: bad arguments")
+    s, e, k = np.empty(n.value, np.int64), np.empty(n.value, np.int64), np.empty(n.value, np.int64)
+    rc = lib.gl_multidepth_blocks(*args, _ptr(s), _ptr(e), _ptr(k), n.value, C.byref(n))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_multidepth_blocks: bad arguments")
+    return s, e, k
+
+
+def multidepth_certify(sums, n_sites, spans):
+    """Host-only: (q, certified): q = round(100 sum / span) where the "%.2f" of the reference's chain is provably that."""
+    sums, n_sites, spans = _as(sums, np.int64), _as(n_sites, np.int64), _as(spans, np.int64)
+    q, ok = np.empty(sums.size, np.int64), np.empty(sums.size, np.uint8)
+    rc = lib.gl_multidepth_certify(_ptr(sums), _ptr(n_sites), _ptr(spans), sums.size, _ptr(q), _ptr(ok))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_multidepth_certify: bad arguments")
+    return q, ok.astype(bool)
+
+
+def multidepth_text(chrom: str, blk_start, blk_end, S: int, q, val, certified, threads: int = 0) -> bytes:
+    """Host-only: the rows after the header line."""
+    blk_start, blk_end = _as(blk_start, np.int64), _as(blk_end, np.int64)
+    q, val, certified = _as(q, np.int64), _as(val, np.float64), _as(certified, np.uint8)
+    p, n = _vp(), C.c_int64(0)
+    rc = lib.gl_multidepth_text(chrom.encode(), _ptr(blk_start), _ptr(blk_end), blk_start.size, S, _ptr(q), _ptr(val),
+                                _ptr(certified), threads, C.byref(p), C.byref(n))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_multidepth_text: bad arguments")
+    try:
+        return C.string_at(p, n.value)
+    finally:
+        lib.gl_free_text(p)
 
 
 def chunk_rows(rs: int, re: int, W: int, run_start: np.ndarray, run_class: np.ndarray):
@@ -967,6 +1023,60 @@ class Ctx:
 
     def comm_wait(self):
         self._ck(lib.gl_comm_wait(self.h))
+
+    # ---- multidepth
+    def multidepth_begin(self, contig_len: int, n_samples: int, mincov: int = 7, min_samples: float = 0.5):
+        self._ck(lib.gl_multidepth_begin(self.h, contig_len, n_samples, mincov, float(min_samples)))
+
+    def multidepth_count(self):
+        self._ck(lib.gl_multidepth_count(self.h))
+
+    def multidepth_sites(self):
+        n = C.c_int64(0)
+        self._ck(lib.gl_multidepth_sites(self.h, None, None, 0, C.byref(n)))
+        s, c = np.empty(n.value, np.int32), np.empty(n.value, np.uint8)
+        self._ck(lib.gl_multidepth_sites(self.h, _ptr(s), _ptr(c), n.value, C.byref(n)))
+        return s, c
+
+    def multidepth_set_blocks(self, blk_start, blk_end, blk_sites):
+        blk_start, blk_end, blk_sites = _as(blk_start, np.int64), _as(blk_end, np.int64), _as(blk_sites, np.int64)
+        self._ck(lib.gl_multidepth_set_blocks(self.h, _ptr(blk_start), _ptr(blk_end), _ptr(blk_sites), blk_start.size))
+
+    def multidepth_sums(self, sample: int):
+        self._ck(lib.gl_multidepth_sums(self.h, sample))
+
+    def multidepth_result(self, n_blocks: int, S: int):
+        """(sums, q, val, certified), each n_blocks x S"""
+        sums, q = np.empty((n_blocks, S), np.uint64), np.empty((n_blocks, S), np.int64)
+        val, ok = np.empty((n_blocks, S), np.float64), np.empty((n_blocks, S), np.uint8)
+        self._ck(lib.gl_multidepth_result(self.h, _ptr(sums), _ptr(q), _ptr(val), _ptr(ok)))
+        return sums, q, val, ok.astype(bool)
+
+    def multidepth_stats(self):
+        """{blocks, walked, certified, min_samples}"""
+        v = [C.c_int64(0) for _ in range(4)]
+        self._ck(lib.gl_multidepth_stats(self.h, *[C.byref(x) for x in v]))
+        return dict(zip(("blocks", "walked", "certified", "min_samples"), (x.value for x in v)))
+
+    def multidepth(self, chrom: str, contig_len: int, adders, mincov: int = 7, min_samples: float = 0.5, max_skip: int = 10,
+                   min_size: int = 15, window: int = 10_000_000, chunk: int = 0) -> bytes:
+        """The whole tool for one contig: adders[i](ctx) adds sample i's segments to the open region (it is called twice, once
+        per pass).  Returns the rows after the header line."""
+        S = len(adders)
+        self.multidepth_begin(contig_len, S, mincov, min_samples)
+        for add in adders:
+            self.depth_begin(0, contig_len)
+            add(self)
+            self.multidepth_count()
+        rs, rc = self.multidepth_sites()
+        bs, be, bn = multidepth_blocks(rs, rc, contig_len, S, max_skip, min_size, window, chunk)
+        self.multidepth_set_blocks(bs, be, bn)
+        for i, add in enumerate(adders):
+            self.depth_begin(0, contig_len)
+            add(self)
+            self.multidepth_sums(i)
+        _, q, val, ok = self.multidepth_result(bs.size, S)
+        return multidepth_text(chrom, bs, be, S, q, val, ok)
 
     # ---- multi-GPU
     def comm_init(self, id128: bytes, rank: int, world: int):

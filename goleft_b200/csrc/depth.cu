@@ -340,6 +340,7 @@ struct ScanParams {
     unsigned W_inv;               // floor(2^32 / W): window index by multiplication (fast window path, W >= 16)
     int tile_begin, tile_end;     // K_fused8 processes these tiles (a streamed upload launches it once per arrived chunk)
     int idx_begin, idx_end;       // K_tileidx8 handles the anchor gaps i in [idx_begin, idx_end), i = -1 .. nb-1
+    gl_md_ep md;                  // multidepth epilogue (mode 0: none)
 };
 
 __device__ __forceinline__ int cov_class(int d, int mincov, int maxmean) {
@@ -357,7 +358,7 @@ __device__ __forceinline__ void flush_max(const ScanParams& p, int acc_max) {
 
 // BPT bases per thread (16 or 32), WARPS warps per CTA, BPT * 32 * WARPS == kTile.  32 bases per thread halves the work
 // that is paid per thread and tile (warp scan, class check, window loop, run claim, barrier) — K_fused8 uses <32, 4>.
-template <int BPT, int WARPS, bool kZeroAfterRead>
+template <int BPT, int WARPS, bool kZeroAfterRead, bool kMD = false>
 __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__ s_tile, int* __restrict__ s_depth,
                                           const int* s_carry, int tile, int& acc_max) {
     static_assert(BPT * 32 * WARPS == kTile, "tile shape");
@@ -432,6 +433,50 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
                 if (idx < p.len) p.depth_out[idx] = GL_D(4 * j);
                 if (idx + 1 < p.len) p.depth_out[idx + 1] = GL_D(4 * j + 1);
                 if (idx + 2 < p.len) p.depth_out[idx + 2] = GL_D(4 * j + 2);
+            }
+        }
+    }
+    // ---- multidepth epilogues (multidepth.cu).  Both only overwrite, so a rerun after a rejected fused pass is harmless.
+    if (kMD && p.md.mode == 1) {
+        // pass 1: this sample's (d >= mincov) and (d > 0) bits, 16 bases per halfword
+        const int nv = max(0, min(BPT, p.len - idx0));
+        unsigned ge = 0, pos = 0;
+#pragma unroll
+        for (int k = 0; k < BPT; k++) {
+            const int d = GL_D(k);
+            if (k < nv) {
+                ge |= (d >= p.md.mincov ? 1u : 0u) << k;
+                pos |= (d > 0 ? 1u : 0u) << k;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < BPT / 16; j++) {
+            p.md.ge16[idx0 / 16 + j] = (unsigned short)(ge >> (16 * j));
+            p.md.pos16[idx0 / 16 + j] = (unsigned short)(pos >> (16 * j));
+        }
+    } else if (kMD && p.md.mode == 2) {
+        // pass 2: Σ d over the sufficient sites of every block that meets this warp's bases, one slot per (pair, 512-base chunk)
+        const unsigned sw32 = p.md.suf[idx0 >> 5];
+        const unsigned sm = BPT == 32 ? sw32 : ((sw32 >> (idx0 & 31)) & 0xffffu);
+        const int q0 = p.md.pair_ptr[tile], q1 = p.md.pair_ptr[tile + 1];
+        for (int q = q0; q < q1; q++) {
+            const int b = p.md.pair_blk[q];
+            const int bs = p.md.blk_start[b], be = p.md.blk_end[b];
+            unsigned long long part = 0;
+            if (bs < warp_base + kWElems && be > warp_base) {          // warp-uniform
+                const int lo = min(max(bs - idx0, 0), BPT), hi = min(max(be - idx0, 0), BPT);
+                const unsigned rng = (hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u)) & ~(lo >= 32 ? 0xffffffffu : ((1u << lo) - 1u));
+                const unsigned m = sm & rng;
+#pragma unroll
+                for (int k = 0; k < BPT; k++)
+                    if ((m >> k) & 1u) part += (unsigned long long)(unsigned)GL_D(k);
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(kFull, part, o);
+            }
+            // slots are per 512-base chunk, so every path (8 warps x 16 bases/thread or 4 x 32) rewrites all eight of them
+            if (lane == 0) {
+#pragma unroll
+                for (int h = 0; h < BPT / 16; h++) p.md.slots[(size_t)q * 8 + warp * (BPT / 16) + h] = h ? 0ull : part;
             }
         }
     }
@@ -616,6 +661,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
 #undef GL_D
 
 // GENERAL path, K_scan: coalesced load of the tile's differences -> swizzled smem -> tile core.
+template <bool kMD>
 __global__ void __launch_bounds__(kScanThreads, 4) depth_scan_kernel(const ScanParams p) {
     __shared__ __align__(16) int s_tile[kTile];
     __shared__ __align__(16) int s_depth[kTile];
@@ -639,7 +685,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) depth_scan_kernel(const ScanP
     for (int r = 0; r < 4; r++) reinterpret_cast<int4*>(s_tile)[swz_chunk(warp * 128 + r * 32 + lane)] = v[r];
     __syncwarp();                                                       // a warp only re-reads its own 128 chunks
     int acc_max = 0;
-    tile_core<16, kWarps, false>(p, s_tile, s_depth, s_carry, tile, acc_max);
+    tile_core<16, kWarps, false, kMD>(p, s_tile, s_depth, s_carry, tile, acc_max);
     flush_max(p, acc_max);
 }
 
@@ -805,6 +851,7 @@ __device__ __forceinline__ EvRegs evtile_load(const unsigned short* __restrict__
     return r;
 }
 
+template <bool kMD>
 __global__ void __launch_bounds__(kEvThreads, 4) depth_evtile_kernel(const ScanParams p, const unsigned short* __restrict__ events,
                                                                      const unsigned* __restrict__ bucket_off, const int* __restrict__ carry) {
     __shared__ __align__(16) int s_tile[kTile];
@@ -841,7 +888,7 @@ __global__ void __launch_bounds__(kEvThreads, 4) depth_evtile_kernel(const ScanP
         regs = evtile_load(events, lo, hi);                 // next tile's events: in flight during the core
         lo2 = hi2 = 0; cin2 = 0;
         if (tile + 2 * G < T) { lo2 = bucket_off[tile + 2 * G]; hi2 = bucket_off[tile + 2 * G + 1]; cin2 = carry[tile + 2 * G]; }
-        tile_core<16, kEvWarps, true>(p, s_tile, s_depth, s_carry, tile, acc_max);
+        tile_core<16, kEvWarps, true, kMD>(p, s_tile, s_depth, s_carry, tile, acc_max);
     }
     flush_max(p, acc_max);
 }
@@ -902,6 +949,7 @@ __device__ __forceinline__ void fused_apply(int* s_tile, int t0, int t1, bool fi
     }
 }
 
+template <bool kMD>
 __global__ void __launch_bounds__(kScanThreads, 4) depth_fused_kernel(const ScanParams p) {
     __shared__ __align__(16) int s_tile[kTile];
     __shared__ __align__(16) int s_depth[kTile];
@@ -990,7 +1038,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) depth_fused_kernel(const Scan
             se[j] = ok ? be[i] : 0;
         }
         cells = fused_load_cells(p, b0, tile + 2 * G, maxlen);          // and the tile after that one's cell entries
-        tile_core<16, kWarps, true>(p, s_tile, s_depth, s_carry, tile, acc_max);
+        tile_core<16, kWarps, true, kMD>(p, s_tile, s_depth, s_carry, tile, acc_max);
     }
     flush_max(p, acc_max);
 }
@@ -1105,6 +1153,7 @@ __device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t
 
 // K_fused8: persistent, software-pipelined like K_fused: while tile n runs its core, the packed words of tile n+1 (two
 // passes = 16 blocks, what a 30x tile needs) and the block range of tile n+2 are in flight.
+template <bool kMD>
 __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanParams p) {
     __shared__ __align__(16) int s_tile[kTile];
     __shared__ __align__(16) int s_depth[kTile];
@@ -1139,7 +1188,7 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
         regs1 = fused8_load(p, lo, hi, 1);
         lo2 = hi2 = 0;
         if (tile + 2 * G < p.tile_end) { lo2 = max(0, p.tile_lo[tile + 2 * G] - 1); hi2 = min(nb, p.tile_hi[tile + 2 * G + 1]); }
-        tile_core<kF8BPT, kF8Warps, true>(p, s_tile, s_depth, s_carry, tile, acc_max);
+        tile_core<kF8BPT, kF8Warps, true, kMD>(p, s_tile, s_depth, s_carry, tile, acc_max);
     }
     flush_max(p, acc_max);
 }
@@ -1416,7 +1465,7 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
     static int f8_ctas_per_sm = 0;                            // persistent grid: what fits on an SM (registers decide)
     if (f8_ctas_per_sm == 0) {
         int nblk = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, depth_fused8_kernel, kF8Threads, 0) != cudaSuccess || nblk < 1) { cudaGetLastError(); nblk = 4; }
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, depth_fused8_kernel<false>, kF8Threads, 0) != cudaSuccess || nblk < 1) { cudaGetLastError(); nblk = 4; }
         f8_ctas_per_sm = nblk;
     }
     if (do_runs && ctx->run_start.cap == 0) {
@@ -1450,6 +1499,7 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
     p.num_tiles = (int)tiles;
     p.do_windows = do_windows ? 1 : 0;
     p.do_runs = do_runs ? 1 : 0;
+    p.md = ctx->md_ep;
     p.p8_anchors = ctx->p8.anchors;
     p.p8_ds = static_cast<const unsigned*>(ctx->p8.ds);
     p.p8_len = static_cast<const unsigned*>(ctx->p8.len);
@@ -1519,7 +1569,8 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
             p.tile_begin = (int)t_prev;
             p.tile_end = (int)t_ready;
             gl_prof_scope prof(ctx, "depth_fused8_kernel");
-            depth_fused8_kernel<<<(unsigned)std::min<int64_t>(t_ready - t_prev, (int64_t)ctx->sm_count * f8_ctas_per_sm), kF8Threads, 0, ctx->stream>>>(p);
+            auto k8 = p.md.mode ? depth_fused8_kernel<true> : depth_fused8_kernel<false>;   // the multidepth epilogue, or none
+            k8<<<(unsigned)std::min<int64_t>(t_ready - t_prev, (int64_t)ctx->sm_count * f8_ctas_per_sm), kF8Threads, 0, ctx->stream>>>(p);
             GL_LAUNCHED(ctx, 1);
         }
         if (early_sums && !last && t_ready > t_prev) {
@@ -1645,6 +1696,7 @@ int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t 
     p.num_tiles = (int)tiles;
     p.do_windows = do_windows ? 1 : 0;
     p.do_runs = do_runs ? 1 : 0;
+    p.md = ctx->md_ep;
 
     // ---- fused path set-up: index every batch (the device decides eligibility)
     if (try_fused) {
@@ -1700,9 +1752,10 @@ int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t 
     {
         gl_prof_scope prof(ctx, fused ? "depth_fused_kernel" : (hbm_diff ? "depth_scan_kernel" : "depth_evtile_kernel"));
         const unsigned fused_grid = (unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4);
-        if (fused) depth_fused_kernel<<<fused_grid, kScanThreads, 0, ctx->stream>>>(p);
-        else if (hbm_diff) depth_scan_kernel<<<(unsigned)tiles, kScanThreads, 0, ctx->stream>>>(p);
-        else depth_evtile_kernel<<<(unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4), kEvThreads, 0, ctx->stream>>>(p, evl.events, evl.bucket_off, evl.carry);
+        const bool md = p.md.mode != 0;                       // the multidepth epilogue, or none
+        if (fused) (md ? depth_fused_kernel<true> : depth_fused_kernel<false>)<<<fused_grid, kScanThreads, 0, ctx->stream>>>(p);
+        else if (hbm_diff) (md ? depth_scan_kernel<true> : depth_scan_kernel<false>)<<<(unsigned)tiles, kScanThreads, 0, ctx->stream>>>(p);
+        else (md ? depth_evtile_kernel<true> : depth_evtile_kernel<false>)<<<(unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4), kEvThreads, 0, ctx->stream>>>(p, evl.events, evl.bucket_off, evl.carry);
     }
     GL_LAUNCHED(ctx, 1);
     if (do_runs) {
@@ -1807,6 +1860,13 @@ int depth_resolve(gl_ctx* ctx) {
         ctx->depth_reduced = true;
     }
     return GL_OK;
+}
+
+int depth_reduce_epilogue(gl_ctx* ctx, int32_t* d_depth_out) {
+    if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "multidepth: no region open (call gl_depth_begin)");
+    const int32_t W = (int32_t)std::min<int64_t>(ctx->re, INT32_MAX);      // one window; windows are not computed
+    GL_CHECK(run_reduce(ctx, W, 1, 0, 0, false, false, d_depth_out, false));
+    return depth_resolve(ctx);
 }
 
 extern "C" {

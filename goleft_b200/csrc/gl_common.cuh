@@ -21,6 +21,22 @@ struct gl_seg_batch {      // one gl_depth_add_segments* call
     int64_t n = 0;
 };
 
+// multidepth.cu: a second epilogue of the depth tile core (depth.cu).  It only ever OVERWRITES what it writes, so a pass the
+// device rejects part way (fused paths) and depth_resolve reruns leaves no trace; multidepth.cu folds the outputs in after the
+// result has been settled.
+struct gl_md_ep {
+    int mode = 0;                       // 0 = off (gl_depth_reduce), 1 = count, 2 = block sums
+    int mincov = 0;                     // mode 1: bit (d >= mincov) -> ge16, bit (d > 0) -> pos16 (16 bases per halfword)
+    unsigned short* ge16 = nullptr;
+    unsigned short* pos16 = nullptr;
+    const unsigned* suf = nullptr;      // mode 2: sufficient-site bitmask (32 bases per word)
+    const int* pair_ptr = nullptr;      // [tiles+1] CSR: the (tile, block) pairs of each 4096-base tile
+    const int* pair_blk = nullptr;      // block of each pair
+    const int* blk_start = nullptr;     // region-relative [start, end) of every block
+    const int* blk_end = nullptr;
+    unsigned long long* slots = nullptr;   // [pairs * 8]: slot (pair, c) = Σ d over the block's sufficient sites in the tile's c-th 512 bases
+};
+
 struct gl_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;       // compute stream
@@ -51,6 +67,8 @@ struct gl_ctx {
     // index tables of the last fused reduce (valid until the next reduce): used by gl_depth_interval_sums
     const int* idx_flags = nullptr; const unsigned* idx_cells = nullptr; int idx_origin = 0, idx_ncells = 0, idx_maxlen = -1;
     int force_path = 0;                     // 0 = auto, 1 = no packed8 kernel (int32 fused, else general), 2 = always general
+    gl_md_ep md_ep;                         // the tile core's multidepth epilogue for the next reduce (mode 0: none)
+    void* md = nullptr;                     // multidepth.cu state (gl_multidepth_begin)
     // a packed8 batch that is the region's only batch stays packed: K_fused8 reads it as it is (last_path 3); it is
     // unpacked into the store (its batch descriptor already points there) only when something needs int32 arrays
     struct { const int* anchors = nullptr; const void* ds = nullptr; const void* len = nullptr; int64_t n_blocks = 0, store_off = 0;
@@ -113,6 +131,11 @@ int gl_buf_reserve(gl_ctx* ctx, gl_buf& b, size_t bytes);
 // depth.cu: settle the last gl_depth_reduce (wait for its header; accept it, or rerun it on the next path or with room for
 // every run).  Every reader of the reduce's results calls this first; a no-op when nothing is pending.
 int depth_resolve(gl_ctx* ctx);
+// depth.cu: one pass of the tile core over the open region with ctx->md_ep as its epilogue (no windows, no runs), settled
+// before it returns; d_depth_out (may be null) also receives the per-base depth.
+int depth_reduce_epilogue(gl_ctx* ctx, int32_t* d_depth_out);
+// multidepth.cu: release ctx->md (gl_ctx_destroy)
+void md_free(gl_ctx* ctx);
 
 #define GL_CUDA(ctx, expr)                                                             \
     do {                                                                               \

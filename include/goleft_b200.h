@@ -424,6 +424,44 @@ int  gl_indexsplit_chunks(const double* tile_sum, const int64_t* out_ptr, int32_
                           const int32_t* ref_ids, int32_t n_refs, int32_t N, const int32_t* prob_ref, const int64_t* prob_start,
                           const int64_t* prob_end, int64_t n_prob, char** text, int64_t* text_len);
 
+/* ---------------------------------------------------------------- multidepth
+ * Replaces multidepth/multidepth.go: the `samtools depth -Q q -r chrom:k*C+1` child over all BAMs of one chunk (:208-221),
+ * sufficientDepth (:158-166), the chunk state machine of aggregate (:222-266), splitBlocks (:183-200) and means (:268-283).
+ * One contig [0, L), S samples, L < 2^30, 1 <= S <= 65535.  Device memory is O(L) plus the blocks x S outputs.
+ *   gl_multidepth_begin   : minSamples = int(0.5 + min_samples * S) (:64); zeroes the per-base counters.
+ *   pass 1, per sample    : gl_depth_begin(ctx, 0, L), gl_depth_add_segments* (any form), gl_multidepth_count.  The depth tile
+ *                           core (any path, same eligibility checks and fallbacks as gl_depth_reduce) counts, per base, the
+ *                           samples with d >= mincov and whether any sample has d > 0 (a `samtools depth` line).
+ *   gl_multidepth_sites   : class runs of the contig, in position order: class 0 = no sample covers the base (no line),
+ *                           1 = insufficient site, 2 = sufficient site (more than minSamples samples with d >= mincov).
+ *                           Pass NULL arrays to get *n_runs only; GL_ERANGE when cap is too small.
+ *   gl_multidepth_blocks  : host-only, no GPU needed: the chunk state machine over the runs (chunk = 0: 5e6 bases, / 5 when
+ *                           S > 50, :60-62,121).  Blocks (start, end, sufficient sites) in chunk order: the reference's
+ *                           output with -p 1, duplicate blocks of overlapping chunks included.  NULL outputs: count only.
+ *   gl_multidepth_set_blocks : uploads the blocks.
+ *   pass 2, per sample    : gl_depth_begin(ctx, 0, L), the same segments again, gl_multidepth_sums(ctx, sample): exact Σd over
+ *                           each block's sufficient sites.  A cell whose "%.2f" follows from the integers (gl_multidepth_certify)
+ *                           gets q = round(100 Σd / l); the others take the reference's float64 chain on the device (val).
+ *   gl_multidepth_result  : blocks x S arrays, row-major by block (any may be NULL).
+ *   gl_multidepth_stats   : blocks, cells that took the float64 chain, cells certified, minSamples.
+ *   gl_multidepth_text    : host-only: the rows after the header ("chrom\tstart\tend" + "\t%.2f" per sample), certified cells
+ *                           printed from q, the others from val; made on `threads` of the host pool (0 = all).  gl_free_text. */
+int  gl_multidepth_begin(gl_ctx* ctx, int64_t contig_len, int32_t n_samples, int32_t mincov, double min_samples);
+int  gl_multidepth_count(gl_ctx* ctx);
+int  gl_multidepth_sites(gl_ctx* ctx, int32_t* run_start, uint8_t* run_class, int64_t cap, int64_t* n_runs);
+int  gl_multidepth_blocks(const int32_t* run_start, const uint8_t* run_class, int64_t n_runs, int64_t contig_len, int32_t n_samples,
+                          int64_t chunk, int64_t max_skip, int64_t min_size, int64_t window, int64_t* blk_start, int64_t* blk_end,
+                          int64_t* blk_sites, int64_t cap, int64_t* n_blocks);
+int  gl_multidepth_set_blocks(gl_ctx* ctx, const int64_t* blk_start, const int64_t* blk_end, const int64_t* blk_sites, int64_t n_blocks);
+int  gl_multidepth_sums(gl_ctx* ctx, int32_t sample);
+int  gl_multidepth_result(gl_ctx* ctx, uint64_t* sums, int64_t* q, double* val, uint8_t* certified);
+int  gl_multidepth_stats(gl_ctx* ctx, int64_t* n_blocks, int64_t* n_walked, int64_t* n_certified, int64_t* min_samples);
+/* host-only: certified[i] = 1 and q[i] = round(100 sum / span) when the reference's "%.2f" of its float64 chain over n_sites
+ * terms is provably those digits (host/md_cert.h) */
+int  gl_multidepth_certify(const int64_t* sum, const int64_t* n_sites, const int64_t* span, int64_t n, int64_t* q, uint8_t* certified);
+int  gl_multidepth_text(const char* chrom, const int64_t* blk_start, const int64_t* blk_end, int64_t n_blocks, int32_t S, const int64_t* q,
+                        const double* val, const uint8_t* certified, int32_t threads, char** text, int64_t* text_len);
+
 /* ---------------------------------------------------------------- covstats
  * V2: histogram of int32 values in [lo,hi) -> hist[v-lo].  `goleft covstats` builds it over the sampled insert sizes,
  * template lengths and read lengths and reads every order statistic of covstats/covstats.go:57-76,175-199 off its running

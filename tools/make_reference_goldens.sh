@@ -8,6 +8,7 @@
 #   tests/golden/ref_empty_<W>.{depth,callable}.bed      goleft depth  -w W        on a BAM without reads on the contig
 #   tests/golden/ref_indexcov_sample27.{bed,roc,ped}     goleft indexcov           on indexcov/test-data/sample_issue_27.bam(.bai)
 #   tests/golden/ref_depthwed.tsv                        goleft depthwed -s 1000   on two of the depth.bed files above
+#   tests/golden/ref_multidepth_t_<chrom>.txt            multidepth -Q 1 --minsamples 0 -c chrom on t.bam (contigs with reads)
 #
 # This image has neither toolchain (`go version`, `samtools --version`: command not found), so the files cannot be made
 # here; until they exist every report says "bit-exact vs the restated oracle, parity unpinned".  tests/test_reference_goldens.py
@@ -64,5 +65,10 @@ if [[ -e "$IC/sample_issue_27_0001.bam" ]]; then
   cut -f1-6,10- "$TMP/ic27/ic27-indexcov.ped" > "$OUT/ref_indexcov_sample27.ped" || cp "$TMP/ic27/ic27-indexcov.ped" "$OUT/ref_indexcov_sample27.ped"
 fi
 "$G" depthwed -s 1000 "$OUT/ref_t_100.depth.bed" "$OUT/ref_t_55.depth.bed" > "$OUT/ref_depthwed.tsv" || true
+# multidepth is a separate binary of the reference (multidepth/multidepth.go); -Q 1 matches the committed decoded fixture
+( cd "$REF" && CGO_ENABLED=0 go build -o "$TMP/multidepth" ./multidepth )
+samtools idxstats "$T/t.bam" | awk -F'\t' '$3 > 0 {print $1}' | while read -r c; do
+  "$TMP/multidepth" -Q 1 -p 1 --minsamples 0 -c "$c" "$T/t.bam" > "$OUT/ref_multidepth_t_$c.txt"
+done
 samtools --version | head -1 > "$OUT/ref_PROVENANCE.txt"; go version >> "$OUT/ref_PROVENANCE.txt"; (cd "$REF" && git rev-parse HEAD 2>/dev/null || true) >> "$OUT/ref_PROVENANCE.txt"
 echo "wrote $(ls "$OUT"/ref_* | wc -l) files to $OUT"

@@ -153,15 +153,7 @@ int gl_bam_decode_device(gl_ctx* ctx, gl_bam* b, int32_t tid, int32_t min_mapq, 
     const int64_t c0 = (int64_t)(vbeg >> 16);
     int64_t c1 = std::min<int64_t>(F.file_size(), (int64_t)(vend >> 16) + 65536 + 64);
     const size_t nbytes = (size_t)(c1 - c0);
-    if (ctx->pack_pinned_bytes < nbytes + 256) {
-        GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
-        if (ctx->pack_pinned) cudaFreeHost(ctx->pack_pinned);
-        ctx->pack_pinned = nullptr; ctx->pack_pinned_bytes = 0;
-        const size_t want = nbytes + nbytes / 8 + (size_t(1) << 20);
-        cudaError_t e = cudaHostAlloc(&ctx->pack_pinned, want, cudaHostAllocDefault);
-        if (e != cudaSuccess) { ctx->pack_pinned = nullptr; cudaGetLastError(); return gl_fail(ctx, GL_ENOMEM, "cudaHostAlloc(%zu): %s", want, cudaGetErrorString(e)); }
-        ctx->pack_pinned_bytes = want;
-    }
+    GL_CHECK(gl_pinned_reserve(ctx, nbytes + 256, nbytes + nbytes / 8 + (size_t(1) << 20)));
     uint8_t* h = static_cast<uint8_t*>(ctx->pack_pinned);
     const double t_read = now_s();
     {

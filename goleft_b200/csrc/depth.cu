@@ -5,24 +5,16 @@
 //                                                                      -> coverage-class run starts
 // Per-base depth never exists in HBM: it is produced and consumed inside one 4096-base tile per CTA.
 //
-// Two ways to build a tile's difference array (+1 at a segment start, -1 at its end):
+// A reduce takes the fastest of four paths the region's segments allow (DESIGN §1.0-1.2; the numbers are those of
+// gl_depth_last_path):
+//   3 packed8          the region's only batch is packed8, read as it is   K_tileidx8 -> K_fused8 -> K_gather
+//   1 fused int32      segments in BAM order, at most 16384 bases          K_index -> K_fused -> K_gather
+//   4 bucketed events  the general path: any order, any length             K_evcount -> K_evscan -> K_evscatter -> K_evtile -> K_gather
+//   2 HBM diff. array  on request only (gl_depth_set_path)                 memset -> K_scatter -> K_super -> K_scan -> K_gather
+// The device checks a fast path's eligibility itself and says so in the reduce's header; depth_resolve then reruns the
+// region on the next path down.
 //
-//  FUSED path (segments in BAM order: reads sorted by position, so segment starts are sorted up to the
-//  span of one read):                                              [K_index] -> [K_fused] -> [K_gather]
-//     K_index  one streaming pass over the segments: max segment length, and per 256-base cell the
-//              lowest / highest segment index that starts in it plus their count (run-aggregated atomics).
-//     K_fused  per tile: zero 16 KB of shared memory, shared-memory atomics for the ~800 segments in the
-//              index span of the cells that can reach the tile (look-back of max-length), tile core.
-//              A tile whose index span is far larger than its segment count (input not in BAM order)
-//              raises a flag and the host reruns the region on the general path.
-//              No difference array in HBM at all: shared-memory atomics run an order of magnitude faster
-//              than global reds (tools/microbench/atomics_bench.cu measures both).
-//  GENERAL path (any order; the fallback):
-//     memset -> [K_scatter] int32 red.global onto a difference array in HBM + warp-aggregated per-tile
-//     net sums -> [K_super] 64-tile sums -> [K_scan] per tile: coalesced load, carry from the two-level
-//     sums (no look-back chain, no inter-CTA dependency), tile core -> [K_gather].
-//
-// Tile core (both paths): 16 consecutive bases per thread (swizzled smem transpose), one thread-local
+// Tile core (every path, DESIGN §1.3): 16 or 32 consecutive bases per thread (swizzled smem transpose), one thread-local
 // + one warp scan, REDUX-based window sums from registers, class runs detected on warp min/max with a
 // per-base slow path, runs claimed per tile with one atomic and put in position order by K_gather.
 // All arithmetic is integer; results are bit-exact against oracle/oracle_depth.c.
@@ -1283,12 +1275,62 @@ inline size_t tile_entries_for(int64_t len) { return ((size_t)num_tiles_for(len)
 inline size_t super_entries_for(int64_t len) { return (((size_t)num_tiles_for(len) >> kSuperShift) + 2 + 3) & ~size_t(3); }
 inline int* tile_sum_ptr(gl_ctx* ctx) { return static_cast<int*>(ctx->diff.p) + diff_entries_for(ctx->re - ctx->rs); }
 inline int* super_sum_ptr(gl_ctx* ctx) { return tile_sum_ptr(ctx) + tile_entries_for(ctx->re - ctx->rs); }
+inline size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 
 inline const int32_t* batch_start(gl_ctx* ctx, const gl_seg_batch& b) {
     return b.s ? b.s : static_cast<const int32_t*>(ctx->store_s.p) + b.off;
 }
 inline const int32_t* batch_end(gl_ctx* ctx, const gl_seg_batch& b) {
     return b.e ? b.e : static_cast<const int32_t*>(ctx->store_e.p) + b.off;
+}
+
+// a new reduce is queued: the last one's results, settled or not, are not asked for any more (nothing waits for its work)
+void drop_result(gl_ctx* ctx) {
+    ctx->depth_reduced = false;
+    ctx->pend.active = false;
+}
+
+// the segments changed: neither the last reduce's results nor what ctx->diff holds describe them any more
+void segments_changed(gl_ctx* ctx) {
+    ctx->diff_holds = kPathNone;
+    drop_result(ctx);
+}
+
+// n segments were written at the end of the store: consecutive host adds extend one contiguous batch
+void store_append(gl_ctx* ctx, int64_t n) {
+    if (!ctx->batches.empty() && ctx->batches.back().s == nullptr &&
+        ctx->batches.back().off + ctx->batches.back().n == ctx->store_n) {
+        ctx->batches.back().n += n;
+    } else {
+        gl_seg_batch b;
+        b.off = ctx->store_n; b.n = n;
+        ctx->batches.push_back(b);
+    }
+    ctx->store_n += n;
+    segments_changed(ctx);
+}
+
+// Queues the upload of packed blocks [b0, b1) on copy_stream: the anchors (4 B per block), then the start deltas or
+// offsets and the lengths (block_bytes per block each: 64 for packed8, 512 for packed16).  Records `done` behind them and
+// makes the compute stream wait for it.
+int upload_blocks(gl_ctx* ctx, void* d_anchor, void* d_ds, void* d_len, const void* h_anchor, const void* h_ds, const void* h_len,
+                  int64_t b0, int64_t b1, size_t block_bytes, cudaEvent_t done) {
+    const size_t nb = (size_t)(b1 - b0), a0 = (size_t)b0 * 4, o0 = (size_t)b0 * block_bytes;
+    GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(d_anchor) + a0, static_cast<const char*>(h_anchor) + a0, nb * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
+    GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(d_ds) + o0, static_cast<const char*>(h_ds) + o0, nb * block_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
+    GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(d_len) + o0, static_cast<const char*>(h_len) + o0, nb * block_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
+    GL_CUDA(ctx, cudaEventRecord(done, ctx->copy_stream));
+    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, done, 0));
+    return GL_OK;
+}
+
+// host segments may still be streaming into the store on the copy stream: the compute stream waits for them
+int join_copies(gl_ctx* ctx) {
+    if (!ctx->copies_pending) return GL_OK;
+    GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[0], ctx->copy_stream));
+    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[0], 0));
+    ctx->copies_pending = false;
+    return GL_OK;
 }
 
 int launch_scatter(gl_ctx* ctx, const int32_t* d_start, const int32_t* d_end, int64_t n) {
@@ -1309,10 +1351,10 @@ int launch_scatter(gl_ctx* ctx, const int32_t* d_start, const int32_t* d_end, in
     return GL_OK;
 }
 
-// general path: (re)build the HBM difference array from every batch
+// HBM difference-array path: (re)build the difference array from every batch
 int accumulate_general(gl_ctx* ctx) {
-    if (ctx->g_valid) return GL_OK;
-    ctx->ev_valid = false;                     // the two general paths share ctx->diff
+    if (ctx->diff_holds == kPathHbmDiff) return GL_OK;
+    ctx->diff_holds = kPathNone;                 // the two general paths share ctx->diff
     const int64_t len = ctx->re - ctx->rs;
     const size_t entries = diff_entries_for(len) + tile_entries_for(len) + super_entries_for(len);
     GL_CHECK(gl_buf_reserve(ctx, ctx->diff, entries * 4));
@@ -1328,7 +1370,7 @@ int accumulate_general(gl_ctx* ctx) {
         depth_super_sum_kernel<<<(unsigned)((n_super + 7) / 8), 256, 0, ctx->stream>>>(tile_sum_ptr(ctx), super_sum_ptr(ctx), (int)tiles);
     }
     GL_LAUNCHED(ctx, 1);
-    ctx->g_valid = true;
+    ctx->diff_holds = kPathHbmDiff;
     return GL_OK;
 }
 
@@ -1350,8 +1392,8 @@ EvLayout ev_layout(gl_ctx* ctx, int64_t tiles) {
 }
 
 int accumulate_events(gl_ctx* ctx) {
-    if (ctx->ev_valid) return GL_OK;
-    ctx->g_valid = false;                      // the two general paths share ctx->diff
+    if (ctx->diff_holds == kPathEvents) return GL_OK;
+    ctx->diff_holds = kPathNone;                 // the two general paths share ctx->diff
     const int64_t len = ctx->re - ctx->rs;
     const int64_t tiles = num_tiles_for(len);
     int64_t n_total = 0;
@@ -1380,7 +1422,7 @@ int accumulate_events(gl_ctx* ctx) {
             GL_LAUNCHED(ctx, 1);
         }
     }
-    ctx->ev_valid = true;
+    ctx->diff_holds = kPathEvents;
     return GL_OK;
 }
 
@@ -1392,12 +1434,6 @@ int defer_header(gl_ctx* ctx) {
     GL_CUDA(ctx, cudaEventRecord(ctx->ev_hdr, ctx->stream));
     ctx->pend.active = true;
     return GL_OK;
-}
-
-// the segments changed: the last reduce's results, settled or not, no longer describe them (nothing waits for its work)
-void drop_result(gl_ctx* ctx) {
-    ctx->depth_reduced = false;
-    ctx->pend.active = false;
 }
 
 constexpr int kP8ChunksMax = 32;
@@ -1418,13 +1454,9 @@ static int64_t p8_chunk_end(int64_t nb, int c, int K) {
 // a packed8 batch whose upload was deferred (gl_depth_region_packed8): copy all of it now, in one piece
 int p8_finish_upload(gl_ctx* ctx) {
     if (!ctx->p8.upload_pending) return GL_OK;
-    const size_t nb = (size_t)ctx->p8.n_blocks;
     GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[0], 0));
-    GL_CUDA(ctx, cudaMemcpyAsync(const_cast<int*>(ctx->p8.anchors), ctx->p8.h_anchors, nb * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaMemcpyAsync(const_cast<void*>(ctx->p8.ds), ctx->p8.h_ds, nb * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaMemcpyAsync(const_cast<void*>(ctx->p8.len), ctx->p8.h_len, nb * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[1], ctx->copy_stream));
-    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[1], 0));
+    GL_CHECK(upload_blocks(ctx, const_cast<int*>(ctx->p8.anchors), const_cast<void*>(ctx->p8.ds), const_cast<void*>(ctx->p8.len),
+                           ctx->p8.h_anchors, ctx->p8.h_ds, ctx->p8.h_len, 0, ctx->p8.n_blocks, 64, ctx->ev_copy[1]));
     ctx->p8.upload_pending = false;
     return GL_OK;
 }
@@ -1445,86 +1477,141 @@ int p8_materialize(gl_ctx* ctx) {
     return GL_OK;
 }
 
-// The region's only batch is packed8: K_tileidx8 + K_fused8 + K_gather straight from the packed words.
-// When the anchors turn out unsorted (hand-made input) the header says so and depth_resolve unpacks and takes the other paths.
-int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break, bool do_windows, bool do_runs,
-                  int32_t* d_depth_out, bool want_min) {
+int reserve_runs(gl_ctx* ctx, size_t cap) {
+    GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, cap * 4));
+    GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, cap));
+    GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, cap * 4));
+    GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, cap));
+    return GL_OK;
+}
+
+// One reduce as every path lays it out.  `scratch` holds, with everything that must start at zero in front so one memset
+// clears it:
+//   [header u64[8] | super_cnt u32[supers]] [win_sum u64[n_windows]] [zeroed: the path's own] | chunk_runs u64[chunks] | [tail: the path's own]
+// The run table has one entry per warp chunk of the kernel that runs: chunks = tiles x its warps per tile.
+struct Reduce {
+    ScanParams p;                 // the fields every path shares are filled in
+    int64_t tiles = 0, n_windows = 0, chunks = 0;
+    char* zeroed = nullptr;
+    char* tail = nullptr;
+};
+
+int reduce_begin(gl_ctx* ctx, const ReduceArgs& a, int warps, size_t zeroed_bytes, size_t tail_bytes, Reduce& r) {
     const int64_t len = ctx->re - ctx->rs;
-    const int64_t tiles = num_tiles_for(len);
-    const int64_t w0 = ctx->rs / W;
-    const int64_t n_windows = (ctx->re - 1) / W - w0 + 1;
-    if (do_windows && want_min) GL_CHECK(gl_buf_reserve(ctx, ctx->win_min, (size_t)n_windows * 4));
-    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
-    const int64_t chunks = tiles * kF8Warps;                  // run table: one entry per warp chunk (1024 bases here)
-    const size_t supers = (size_t)(chunks >> kSuperShift) + 2;
-    const size_t head_bytes = al(kHeaderWords * 8 + supers * 4);
-    const size_t win_bytes = al(do_windows ? (size_t)n_windows * 8 : 0);
-    const size_t zero_bytes = head_bytes + win_bytes;
-    const size_t run_bytes = al((size_t)chunks * 8);
-    GL_CHECK(gl_buf_reserve(ctx, ctx->scratch, zero_bytes + run_bytes + 2 * al((size_t)(tiles + 1) * 4)));
+    const int64_t w0 = ctx->rs / a.W;
+    const bool want_min = a.do_windows && a.want_min;
+    r.tiles = num_tiles_for(len);
+    r.n_windows = (ctx->re - 1) / a.W - w0 + 1;
+    r.chunks = r.tiles * warps;
+    if (want_min) GL_CHECK(gl_buf_reserve(ctx, ctx->win_min, (size_t)r.n_windows * 4));
+    const size_t supers = (size_t)(r.chunks >> kSuperShift) + 2;
+    const size_t head_bytes = al256(kHeaderWords * 8 + supers * 4);
+    const size_t win_bytes = al256(a.do_windows ? (size_t)r.n_windows * 8 : 0);
+    const size_t zero_bytes = head_bytes + win_bytes + zeroed_bytes;
+    const size_t run_bytes = al256((size_t)r.chunks * 8);
+    GL_CHECK(gl_buf_reserve(ctx, ctx->scratch, zero_bytes + run_bytes + tail_bytes));
+    if (a.do_runs && ctx->run_start.cap == 0) GL_CHECK(reserve_runs(ctx, (size_t)(len / 16 + 4096)));
+    char* sbase = static_cast<char*>(ctx->scratch.p);
+    ctx->win_sum_p = sbase + head_bytes;
+    r.zeroed = sbase + head_bytes + win_bytes;
+    r.tail = sbase + zero_bytes + run_bytes;
+    GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
+    if (want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)r.n_windows * 4, ctx->stream));
+
+    ScanParams& p = r.p;
+    memset(&p, 0, sizeof p);
+    p.len = (int)len;
+    p.rs = (int)ctx->rs;
+    p.re = (int)ctx->re;
+    p.W = a.W;
+    p.W_inv = a.W >= 2 ? (unsigned)((uint64_t(1) << 32) / (uint64_t)a.W) : 0u;
+    p.w0 = w0;
+    p.mincov = a.mincov;
+    p.maxmean = a.maxmean;
+    p.run_break = (a.run_break >= (int64_t(1) << 32)) ? 0u : (unsigned)a.run_break;
+    p.header = reinterpret_cast<uint64_t*>(sbase);
+    p.chunk_runs = reinterpret_cast<uint64_t*>(sbase + zero_bytes);
+    p.super_cnt = reinterpret_cast<unsigned*>(p.header + kHeaderWords);
+    p.depth_out = a.d_depth_out;
+    p.num_tiles = (int)r.tiles;
+    p.do_windows = a.do_windows ? 1 : 0;
+    p.do_runs = a.do_runs ? 1 : 0;
+    p.md = ctx->md_ep;
+    p.win_sum = static_cast<unsigned long long*>(ctx->win_sum_p);
+    p.win_min = want_min ? static_cast<int*>(ctx->win_min.p) : nullptr;
+    p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
+    p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
+    if (a.do_runs) {
+        p.run_cap = (long long)ctx->run_class.cap;
+        p.run_cap = std::min<long long>(p.run_cap, (long long)(ctx->run_start.cap / 4));
+        p.run_cap = std::min<long long>(p.run_cap, (long long)ctx->run_tmp_class.cap);
+        p.run_cap = std::min<long long>(p.run_cap, (long long)(ctx->run_tmp_start.cap / 4));
+    }
+    return GL_OK;
+}
+
+// The path's kernels are queued: put the claimed runs in position order, send the sums (from window w_sent on: a streamed
+// packed8 reduce has sent the ones before already) and the first runs to a one-call entry's host buffers while the header
+// is read, and leave the rest to depth_resolve.
+int reduce_end(gl_ctx* ctx, const Reduce& r, int path, int64_t w_sent) {
+    const ScanParams& p = r.p;
+    if (p.do_runs) {
+        gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
+        depth_gather_runs_kernel<<<(unsigned)((r.chunks + 255) / 256), 256, 0, ctx->stream>>>(
+            p.header, p.chunk_runs, p.super_cnt, (int)r.chunks, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
+            static_cast<unsigned char*>(ctx->run_class.p), p.run_cap);
+        GL_LAUNCHED(ctx, 1);
+    }
+    ctx->prefetched = false;
+    if (ctx->prefetch_sums && p.do_windows && r.n_windows <= ctx->prefetch_cap) {
+        if (r.n_windows > w_sent)
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums + w_sent, static_cast<const char*>(ctx->win_sum_p) + w_sent * 8,
+                                         (size_t)(r.n_windows - w_sent) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->prefetched = true;
+    }
+    ctx->prefetched_runs = 0;
+    if (ctx->prefetch_run_start && ctx->prefetch_run_class && p.do_runs) {     // usually all of them
+        const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)p.run_cap);
+        if (k > 0) {
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
+            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
+            ctx->prefetched_runs = k;
+        }
+    }
+    ctx->pend.path = path;
+    ctx->pend.run_cap = p.run_cap;
+    ctx->pend.n_windows = r.n_windows;
+    ctx->pend.d2h = w_sent > 0;
+    ctx->pend.flags = p.flags;                 // the fused path's index tables (null on the other paths) start with
+    ctx->pend.cells = p.batch[0].cell_hi;      // batch 0's cell_hi
+    ctx->pend.origin = p.origin;
+    ctx->pend.ncells = p.ncells;
+    return defer_header(ctx);
+}
+
+// The region's only batch is packed8: K_tileidx8 + K_fused8 straight from the packed words.
+// When the anchors turn out unsorted (hand-made input) the header says so and depth_resolve unpacks and takes the other paths.
+int reduce_packed8(gl_ctx* ctx, const ReduceArgs& a) {
+    const size_t tile_tab = al256((size_t)(num_tiles_for(ctx->re - ctx->rs) + 1) * 4);
+    Reduce r;
+    GL_CHECK(reduce_begin(ctx, a, kF8Warps, 0, 2 * tile_tab, r));      // tail: tile_lo | tile_hi
     static int f8_ctas_per_sm = 0;                            // persistent grid: what fits on an SM (registers decide)
     if (f8_ctas_per_sm == 0) {
         int nblk = 0;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, depth_fused8_kernel<false>, kF8Threads, 0) != cudaSuccess || nblk < 1) { cudaGetLastError(); nblk = 4; }
         f8_ctas_per_sm = nblk;
     }
-    if (do_runs && ctx->run_start.cap == 0) {
-        size_t cap = (size_t)(len / 16 + 4096);
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, cap * 4));
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, cap));
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, cap * 4));
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, cap));
-    }
-    char* sbase = static_cast<char*>(ctx->scratch.p);
-    uint64_t* header = reinterpret_cast<uint64_t*>(sbase);
-    unsigned* super_cnt = reinterpret_cast<unsigned*>(header + kHeaderWords);
-    ctx->win_sum_p = sbase + head_bytes;
-    uint64_t* chunk_runs = reinterpret_cast<uint64_t*>(sbase + zero_bytes);
-
-    ScanParams p;
-    memset(&p, 0, sizeof p);
-    p.len = (int)len;
-    p.rs = (int)ctx->rs;
-    p.re = (int)ctx->re;
-    p.W = W;
-    p.W_inv = W >= 2 ? (unsigned)((uint64_t(1) << 32) / (uint64_t)W) : 0u;
-    p.w0 = w0;
-    p.mincov = mincov;
-    p.maxmean = maxmean;
-    p.run_break = (run_break >= (int64_t(1) << 32)) ? 0u : (unsigned)run_break;
-    p.header = header;
-    p.chunk_runs = chunk_runs;
-    p.super_cnt = super_cnt;
-    p.depth_out = d_depth_out;
-    p.num_tiles = (int)tiles;
-    p.do_windows = do_windows ? 1 : 0;
-    p.do_runs = do_runs ? 1 : 0;
-    p.md = ctx->md_ep;
+    ScanParams& p = r.p;
     p.p8_anchors = ctx->p8.anchors;
     p.p8_ds = static_cast<const unsigned*>(ctx->p8.ds);
     p.p8_len = static_cast<const unsigned*>(ctx->p8.len);
     p.p8_nblocks = (int)ctx->p8.n_blocks;
-    p.tile_lo = reinterpret_cast<int*>(sbase + zero_bytes + run_bytes);
-    p.tile_hi = reinterpret_cast<int*>(sbase + zero_bytes + run_bytes + al((size_t)(tiles + 1) * 4));
-    p.win_sum = static_cast<unsigned long long*>(ctx->win_sum_p);
-    p.win_min = (do_windows && want_min) ? static_cast<int*>(ctx->win_min.p) : nullptr;
-
-    p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
-    p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
-    long long cap = 0;
-    if (do_runs) {
-        cap = (long long)ctx->run_class.cap;
-        cap = std::min<long long>(cap, (long long)(ctx->run_start.cap / 4));
-        cap = std::min<long long>(cap, (long long)ctx->run_tmp_class.cap);
-        cap = std::min<long long>(cap, (long long)(ctx->run_tmp_start.cap / 4));
-    }
-    p.run_cap = cap;
-    GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
-    if (do_windows && want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)n_windows * 4, ctx->stream));
+    p.tile_lo = reinterpret_cast<int*>(r.tail);
+    p.tile_hi = reinterpret_cast<int*>(r.tail + tile_tab);
     // One pass over everything that is on the device — or, when the upload was deferred, chunk by chunk: the words
     // are sorted by position, so once a chunk has landed every tile that ends before its last anchor can be reduced
     // while the next chunk is still on the wire.
-    const int64_t nb = ctx->p8.n_blocks;
+    const int64_t nb = ctx->p8.n_blocks, tiles = r.tiles, n_windows = r.n_windows;
     const bool streamed = ctx->p8.upload_pending;
     const int n_chunks = streamed ? p8_chunks() : 1;
     if (streamed) {
@@ -1536,21 +1623,14 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
         GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[0], 0));   // previous consumer done with the staging buffer
     }
     int64_t b0 = 0, t_prev = 0, w_sent = 0;             // w_sent: window sums already on their way home
-    const bool early_sums = streamed && ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap;
+    const bool early_sums = streamed && ctx->prefetch_sums && a.do_windows && n_windows <= ctx->prefetch_cap;
     for (int c = 0; c < n_chunks; c++) {
         const bool last = c == n_chunks - 1;
         const int64_t b1 = p8_chunk_end(nb, c, n_chunks);
         if (b1 <= b0 && !last) continue;
-        if (streamed && b1 > b0) {
-            const size_t nbk = (size_t)(b1 - b0);
-            GL_CUDA(ctx, cudaMemcpyAsync(const_cast<int*>(ctx->p8.anchors) + b0, ctx->p8.h_anchors + b0, nbk * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-            GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(const_cast<void*>(ctx->p8.ds)) + b0 * 64, static_cast<const char*>(ctx->p8.h_ds) + b0 * 64,
-                                         nbk * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
-            GL_CUDA(ctx, cudaMemcpyAsync(static_cast<char*>(const_cast<void*>(ctx->p8.len)) + b0 * 64, static_cast<const char*>(ctx->p8.h_len) + b0 * 64,
-                                         nbk * 64, cudaMemcpyHostToDevice, ctx->copy_stream));
-            GL_CUDA(ctx, cudaEventRecord(ctx->ev_chunk[c], ctx->copy_stream));
-            GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_chunk[c], 0));
-        }
+        if (streamed && b1 > b0)
+            GL_CHECK(upload_blocks(ctx, const_cast<int*>(ctx->p8.anchors), const_cast<void*>(ctx->p8.ds), const_cast<void*>(ctx->p8.len),
+                                   ctx->p8.h_anchors, ctx->p8.h_ds, ctx->p8.h_len, b0, b1, 64, ctx->ev_chunk[c]));
         // anchor gaps this chunk completes: (a[i], a[i+1]] for i in [b0-1, b1-1), plus the open end after the last anchor
         p.idx_begin = (int)(b0 - 1);
         p.idx_end = (int)(last ? nb : b1 - 1);
@@ -1575,7 +1655,7 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
         }
         if (early_sums && !last && t_ready > t_prev) {
             // windows that end at or before the last reduced tile's end are final: send them home on their own stream
-            const int64_t w_done = std::min<int64_t>(n_windows, std::max<int64_t>(w_sent, (ctx->rs + t_ready * kTile) / W - w0));
+            const int64_t w_done = std::min<int64_t>(n_windows, std::max<int64_t>(w_sent, (ctx->rs + t_ready * kTile) / a.W - p.w0));
             if (w_done > w_sent) {
                 cudaEvent_t ev = ctx->ev_chunk[(size_t)n_chunks + c];
                 GL_CUDA(ctx, cudaEventRecord(ev, ctx->stream));
@@ -1590,117 +1670,27 @@ int run_reduce_f8(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64
     }
     ctx->p8.upload_pending = false;
     GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));      // the packed staging buffer may be overwritten after this
-    if (do_runs) {
-        gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
-        depth_gather_runs_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, ctx->stream>>>(
-            header, chunk_runs, super_cnt, (int)chunks, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
-            static_cast<unsigned char*>(ctx->run_class.p), cap);
-        GL_LAUNCHED(ctx, 1);
-    }
-    ctx->prefetched = false;
-    if (ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap) {   // (the rest of the) sums travel while the header is read
-        if (n_windows > w_sent)
-            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums + w_sent, static_cast<const char*>(ctx->win_sum_p) + w_sent * 8,
-                                         (size_t)(n_windows - w_sent) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->prefetched = true;
-    }
-    ctx->prefetched_runs = 0;
-    if (ctx->prefetch_run_start && ctx->prefetch_run_class && do_runs) {       // ... and so do the first runs (usually all of them)
-        const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)cap);
-        if (k > 0) {
-            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
-            ctx->prefetched_runs = k;
-        }
-    }
-    ctx->pend.path = 3;
-    ctx->pend.run_cap = cap;
-    ctx->pend.n_windows = n_windows;
-    ctx->pend.d2h = w_sent > 0;
-    ctx->pend.flags = nullptr;
-    ctx->pend.cells = nullptr;
-    return defer_header(ctx);
+    return reduce_end(ctx, r, kPathPacked8, w_sent);
 }
 
-// Queues one fused pass over the region on the fastest path the input may take: the packed8 kernel, else the fused
-// (sorted) int32 path, else the general path.  The device decides eligibility; depth_resolve learns it from the header and
-// reruns on the next path when needed.  skip = 1: not the packed8 kernel, 2: not the fused int32 path either (such a rerun).
-int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break, bool do_windows,
-               bool do_runs, int32_t* d_depth_out, bool want_min, int skip = 0) {
-    const int64_t len = ctx->re - ctx->rs;
-    const int64_t tiles = num_tiles_for(len);
-    const int64_t w0 = ctx->rs / W;
-    const int64_t n_windows = (ctx->re - 1) / W - w0 + 1;
-    drop_result(ctx);
-    ctx->pend.W = W; ctx->pend.mincov = mincov; ctx->pend.maxmean = maxmean; ctx->pend.run_break = run_break;
-    ctx->pend.do_windows = do_windows; ctx->pend.do_runs = do_runs; ctx->pend.want_min = want_min; ctx->pend.d_depth_out = d_depth_out;
+inline bool general_path(int path) { return path == kPathHbmDiff || path == kPathEvents; }
 
-    if (ctx->copies_pending) {        // host segments still streaming into the store on the copy stream
-        GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[0], ctx->copy_stream));
-        GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[0], 0));
-        ctx->copies_pending = false;
-    }
-    if (ctx->p8.pending) {
-        if (skip == 0 && ctx->force_path == 0 && ctx->batches.size() == 1 && tiles < (int64_t(1) << 30) && ctx->p8.n_blocks < INT32_MAX)
-            return run_reduce_f8(ctx, W, mincov, maxmean, run_break, do_windows, do_runs, d_depth_out, want_min);
-        GL_CHECK(p8_materialize(ctx));
-    }
-    if (do_windows && want_min) GL_CHECK(gl_buf_reserve(ctx, ctx->win_min, (size_t)n_windows * 4));
-    // One scratch buffer; everything that must start at zero is contiguous so a single memset clears it:
-    //   [header u64[8] | super_cnt u32[supers]] [win_sum u64[n_windows]] [flags] [cell_hi|cell_cnt|cell_lo per batch]  | chunk_runs
-    bool try_fused = skip < 2 && ctx->force_path != 2 && ctx->force_path != 4 && !ctx->batches.empty() && (int)ctx->batches.size() <= kMaxBatches;
+// int32 batches: the fused path (K_index per batch + K_fused; the device decides eligibility), else a general path
+// (bucketed events, or the HBM difference array on request).
+int reduce_int32(gl_ctx* ctx, const ReduceArgs& a, int from) {
+    bool try_fused = !general_path(from) && !general_path(ctx->force_path) && !ctx->batches.empty() && (int)ctx->batches.size() <= kMaxBatches;
     for (const gl_seg_batch& b : ctx->batches) if (b.n >= INT32_MAX) try_fused = false;
+    const int path = try_fused ? kPathFused : (ctx->force_path == kPathHbmDiff ? kPathHbmDiff : kPathEvents);
     const int origin = (int)(std::max<int64_t>(0, ctx->rs - kMaxLookback) & ~int64_t((1 << kCellShift) - 1));
     const int ncells = (int)(((ctx->re - 1 - origin) >> kCellShift) + 1);
     const size_t nb = ctx->batches.size();
-    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
-    const int64_t chunks = tiles * kWarps;
-    const size_t supers = (size_t)(chunks >> kSuperShift) + 2;
-    const size_t head_bytes = al(kHeaderWords * 8 + supers * 4);
-    const size_t win_bytes = al(do_windows ? (size_t)n_windows * 8 : 0);
-    const size_t flag_bytes = try_fused ? al(kFlagWords * 4) : 0;
-    const size_t cell_bytes = try_fused ? al((size_t)ncells * 4 * 3 * nb) : 0;
-    const size_t zero_bytes = head_bytes + win_bytes + flag_bytes + cell_bytes;
-    GL_CHECK(gl_buf_reserve(ctx, ctx->scratch, zero_bytes + (size_t)chunks * 8));
-    if (do_runs && ctx->run_start.cap == 0) {
-        size_t cap = (size_t)(len / 16 + 4096);
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, cap * 4));
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, cap));
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, cap * 4));
-        GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, cap));
-    }
-    char* sbase = static_cast<char*>(ctx->scratch.p);
-    uint64_t* header = reinterpret_cast<uint64_t*>(sbase);
-    unsigned* super_cnt = reinterpret_cast<unsigned*>(header + kHeaderWords);
-    ctx->win_sum_p = sbase + head_bytes;
-    int* flags = reinterpret_cast<int*>(sbase + head_bytes + win_bytes);
-    unsigned* cells = reinterpret_cast<unsigned*>(sbase + head_bytes + win_bytes + flag_bytes);
-    uint64_t* chunk_runs = reinterpret_cast<uint64_t*>(sbase + zero_bytes);
-    GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
-
-    ScanParams p;
-    memset(&p, 0, sizeof p);
-    p.len = (int)len;
-    p.rs = (int)ctx->rs;
-    p.re = (int)ctx->re;
-    p.W = W;
-    p.W_inv = W >= 2 ? (unsigned)((uint64_t(1) << 32) / (uint64_t)W) : 0u;
-    p.w0 = w0;
-    p.mincov = mincov;
-    p.maxmean = maxmean;
-    p.run_break = (run_break >= (int64_t(1) << 32)) ? 0u : (unsigned)run_break;
-    p.header = header;
-    p.chunk_runs = chunk_runs;
-    p.super_cnt = super_cnt;
-    p.depth_out = d_depth_out;
-    p.num_tiles = (int)tiles;
-    p.do_windows = do_windows ? 1 : 0;
-    p.do_runs = do_runs ? 1 : 0;
-    p.md = ctx->md_ep;
-
-    // ---- fused path set-up: index every batch (the device decides eligibility)
-    if (try_fused) {
-        unsigned* hi_all = cells;
+    const size_t flag_bytes = al256(kFlagWords * 4);
+    Reduce r;     // zeroed for the fused path: flags | cell_hi | cell_cnt | cell_lo, each cell table [batch][cell]
+    GL_CHECK(reduce_begin(ctx, a, path == kPathEvents ? kEvWarps : kWarps, try_fused ? flag_bytes + al256((size_t)ncells * 4 * 3 * nb) : 0, 0, r));
+    ScanParams& p = r.p;
+    if (path == kPathFused) {
+        int* flags = reinterpret_cast<int*>(r.zeroed);
+        unsigned* hi_all = reinterpret_cast<unsigned*>(r.zeroed + flag_bytes);
         unsigned* cnt_all = hi_all + (size_t)ncells * nb;
         unsigned* lo_all = cnt_all + (size_t)ncells * nb;
         p.flags = flags;
@@ -1722,75 +1712,42 @@ int run_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t 
             GL_LAUNCHED(ctx, 1);
         }
     }
-
-    const bool fused = try_fused;
-    const bool hbm_diff = !fused && ctx->force_path == 2;      // the north-star pipeline (HBM difference array), on request only
     EvLayout evl = {};
-    if (hbm_diff) {
+    if (path == kPathHbmDiff) {
         GL_CHECK(accumulate_general(ctx));
         p.diff = static_cast<const int*>(ctx->diff.p);
         p.tile_sum = tile_sum_ptr(ctx);
         p.super_sum = super_sum_ptr(ctx);
-    } else if (!fused) {
+    } else if (path == kPathEvents) {
         GL_CHECK(accumulate_events(ctx));
-        evl = ev_layout(ctx, tiles);
+        evl = ev_layout(ctx, r.tiles);
     }
-    p.win_sum = static_cast<unsigned long long*>(ctx->win_sum_p);
-    p.win_min = (do_windows && want_min) ? static_cast<int*>(ctx->win_min.p) : nullptr;
-    p.tmp_start = static_cast<int*>(ctx->run_tmp_start.p);
-    p.tmp_class = static_cast<unsigned char*>(ctx->run_tmp_class.p);
-    long long cap = 0;
-    if (do_runs) {
-        cap = (long long)ctx->run_class.cap;
-        cap = std::min<long long>(cap, (long long)(ctx->run_start.cap / 4));
-        cap = std::min<long long>(cap, (long long)ctx->run_tmp_class.cap);
-        cap = std::min<long long>(cap, (long long)(ctx->run_tmp_start.cap / 4));
-    }
-    p.run_cap = cap;
-
-    if (do_windows && want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)n_windows * 4, ctx->stream));
     {
-        gl_prof_scope prof(ctx, fused ? "depth_fused_kernel" : (hbm_diff ? "depth_scan_kernel" : "depth_evtile_kernel"));
-        const unsigned fused_grid = (unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4);
+        gl_prof_scope prof(ctx, path == kPathFused ? "depth_fused_kernel" : (path == kPathHbmDiff ? "depth_scan_kernel" : "depth_evtile_kernel"));
+        const unsigned persistent_grid = (unsigned)std::min<int64_t>(r.tiles, (int64_t)ctx->sm_count * 4);
         const bool md = p.md.mode != 0;                       // the multidepth epilogue, or none
-        if (fused) (md ? depth_fused_kernel<true> : depth_fused_kernel<false>)<<<fused_grid, kScanThreads, 0, ctx->stream>>>(p);
-        else if (hbm_diff) (md ? depth_scan_kernel<true> : depth_scan_kernel<false>)<<<(unsigned)tiles, kScanThreads, 0, ctx->stream>>>(p);
-        else (md ? depth_evtile_kernel<true> : depth_evtile_kernel<false>)<<<(unsigned)std::min<int64_t>(tiles, (int64_t)ctx->sm_count * 4), kEvThreads, 0, ctx->stream>>>(p, evl.events, evl.bucket_off, evl.carry);
+        if (path == kPathFused) (md ? depth_fused_kernel<true> : depth_fused_kernel<false>)<<<persistent_grid, kScanThreads, 0, ctx->stream>>>(p);
+        else if (path == kPathHbmDiff) (md ? depth_scan_kernel<true> : depth_scan_kernel<false>)<<<(unsigned)r.tiles, kScanThreads, 0, ctx->stream>>>(p);
+        else (md ? depth_evtile_kernel<true> : depth_evtile_kernel<false>)<<<persistent_grid, kEvThreads, 0, ctx->stream>>>(p, evl.events, evl.bucket_off, evl.carry);
     }
     GL_LAUNCHED(ctx, 1);
-    if (do_runs) {
-        // the run table has one entry per warp chunk of the kernel that ran (8 per tile, 4 for the 32-bases-per-thread K_evtile)
-        const int64_t chunks_now = tiles * ((fused || hbm_diff) ? kWarps : kEvWarps);
-        gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
-        depth_gather_runs_kernel<<<(unsigned)((chunks_now + 255) / 256), 256, 0, ctx->stream>>>(
-            header, chunk_runs, super_cnt, (int)chunks_now, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
-            static_cast<unsigned char*>(ctx->run_class.p), cap);
-        GL_LAUNCHED(ctx, 1);
-    }
+    return reduce_end(ctx, r, path, 0);
+}
 
-    ctx->prefetched = false;
-    if (ctx->prefetch_sums && do_windows && n_windows <= ctx->prefetch_cap) {   // sums travel while the header is read
-        GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_sums, ctx->win_sum_p, (size_t)n_windows * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->prefetched = true;
+// Queues one pass of the tile core over the region on the fastest path the input may take, starting no faster than
+// `from` (a rerun: depth_resolve) or ctx->force_path: packed8, else fused int32, else a general path.  The device decides
+// a fast path's eligibility; depth_resolve learns it from the header and reruns on the next path when needed.
+int run_reduce(gl_ctx* ctx, const ReduceArgs& a, int from = kPathPacked8) {
+    drop_result(ctx);
+    ctx->pend.args = a;
+    GL_CHECK(join_copies(ctx));
+    if (ctx->p8.pending) {
+        if (from == kPathPacked8 && ctx->force_path == kPathNone && ctx->batches.size() == 1 &&
+            num_tiles_for(ctx->re - ctx->rs) < (int64_t(1) << 30) && ctx->p8.n_blocks < INT32_MAX)
+            return reduce_packed8(ctx, a);
+        GL_CHECK(p8_materialize(ctx));
     }
-    ctx->prefetched_runs = 0;
-    if (ctx->prefetch_run_start && ctx->prefetch_run_class && do_runs) {       // ... and so do the first runs (usually all of them)
-        const int64_t k = std::min<int64_t>(std::min<int64_t>(ctx->prefetch_run_cap, 16384), (int64_t)cap);
-        if (k > 0) {
-            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_start, ctx->run_start.p, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
-            GL_CUDA(ctx, cudaMemcpyAsync(ctx->prefetch_run_class, ctx->run_class.p, (size_t)k, cudaMemcpyDeviceToHost, ctx->stream));
-            ctx->prefetched_runs = k;
-        }
-    }
-    ctx->pend.path = fused ? 1 : (hbm_diff ? 2 : 4);
-    ctx->pend.run_cap = cap;
-    ctx->pend.n_windows = n_windows;
-    ctx->pend.d2h = false;
-    ctx->pend.flags = fused ? flags : nullptr;
-    ctx->pend.cells = fused ? cells : nullptr;
-    ctx->pend.origin = origin;
-    ctx->pend.ncells = ncells;
-    return defer_header(ctx);
+    return reduce_int32(ctx, a, from);
 }
 
 constexpr int64_t kStageSegs = int64_t(1) << 22;      // segments per pinned staging slot (2 x 16 MiB)
@@ -1822,6 +1779,44 @@ int store_reserve(gl_ctx* ctx, int64_t need) {
     return GL_OK;
 }
 
+int region_fetch(gl_ctx* ctx, int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class,
+                 int64_t run_cap, int64_t* n_runs) {
+    GL_CHECK(depth_resolve(ctx));
+    const int64_t nw = ctx->n_windows, nr = ctx->n_runs;
+    if (n_windows) *n_windows = nw;
+    if (n_runs) *n_runs = nr;
+    if (nw > win_cap) return gl_fail(ctx, GL_ERANGE, "gl_depth_region: %lld windows > cap %lld", (long long)nw, (long long)win_cap);
+    if (nr > run_cap) return gl_fail(ctx, GL_ERANGE, "gl_depth_region: %lld runs > cap %lld", (long long)nr, (long long)run_cap);
+    const bool have_sums = ctx->prefetched, have_runs = ctx->prefetched_runs >= nr;
+    ctx->prefetched = false;
+    ctx->prefetched_runs = 0;
+    if (have_sums && have_runs) return GL_OK;                  // everything came home with the header (depth_resolve waited for it)
+    if (!have_sums) GL_CUDA(ctx, cudaMemcpyAsync(sum_out, ctx->win_sum_p, (size_t)nw * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (nr > 0 && !have_runs) {
+        GL_CUDA(ctx, cudaMemcpyAsync(run_start, ctx->run_start.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        GL_CUDA(ctx, cudaMemcpyAsync(run_class, ctx->run_class.p, (size_t)nr, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
+}
+
+// The one-call entries: begin, add (the entry's own form), reduce with the sums and the first runs sent straight to the
+// caller's buffers behind the header, fetch the rest.
+template <class Add>
+int region_one_call(gl_ctx* ctx, int64_t rs, int64_t re, Add add, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break,
+                    int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class, int64_t run_cap,
+                    int64_t* n_runs) {
+    GL_CHECK(gl_depth_begin(ctx, rs, re));
+    GL_CHECK(add());
+    ctx->prefetch_sums = sum_out; ctx->prefetch_cap = sum_out ? win_cap : 0;
+    ctx->prefetch_run_start = run_start; ctx->prefetch_run_class = run_class; ctx->prefetch_run_cap = (run_start && run_class) ? run_cap : 0;
+    const int rc_reduce = gl_depth_reduce(ctx, W, mincov, maxmean, run_break);
+    ctx->prefetch_sums = nullptr; ctx->prefetch_cap = 0;
+    ctx->prefetch_run_start = nullptr; ctx->prefetch_run_class = nullptr; ctx->prefetch_run_cap = 0;
+    GL_CHECK(rc_reduce);
+    return region_fetch(ctx, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
+}
+
 }  // namespace
 
 int depth_resolve(gl_ctx* ctx) {
@@ -1831,21 +1826,15 @@ int depth_resolve(gl_ctx* ctx) {
         GL_CUDA(ctx, cudaEventSynchronize(ctx->ev_hdr));
         if (q.d2h) GL_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
         const uint64_t* hdr = ctx->hdr_host;
-        int rerun = -1;                                                   // run_reduce's skip level for a rerun
-        if ((q.path == 3 || q.path == 1) && hdr[3] != 0) {                // packed8 anchors not sorted / int32 input not in BAM order
+        if ((q.path == kPathPacked8 || q.path == kPathFused) && hdr[3] != 0) {   // packed8 anchors not sorted / int32 input not in BAM order
             ctx->prefetched = false;
             ctx->prefetched_runs = 0;
-            rerun = q.path == 3 ? 1 : 2;
-        } else if (q.do_runs && (long long)hdr[0] > q.run_cap) {          // the runs did not fit: grow and take the same path again
-            const size_t ncap = (size_t)hdr[0] + 1024;
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_start, ncap * 4));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_class, ncap));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_start, ncap * 4));
-            GL_CHECK(gl_buf_reserve(ctx, ctx->run_tmp_class, ncap));
-            rerun = q.path == 3 ? 0 : (q.path == 1 ? 1 : 2);
+            GL_CHECK(run_reduce(ctx, q.args, q.path == kPathPacked8 ? kPathFused : kPathEvents));   // the next path down
+            continue;
         }
-        if (rerun >= 0) {
-            GL_CHECK(run_reduce(ctx, q.W, q.mincov, q.maxmean, q.run_break, q.do_windows, q.do_runs, q.d_depth_out, q.want_min, rerun));
+        if (q.args.do_runs && (long long)hdr[0] > q.run_cap) {                  // the runs did not fit: grow and take the same path again
+            GL_CHECK(reserve_runs(ctx, (size_t)hdr[0] + 1024));
+            GL_CHECK(run_reduce(ctx, q.args, q.path));
             continue;
         }
         ctx->last_path = q.path;
@@ -1853,10 +1842,10 @@ int depth_resolve(gl_ctx* ctx) {
         ctx->idx_cells = q.cells;
         ctx->idx_origin = q.origin;
         ctx->idx_ncells = q.ncells;
-        ctx->n_runs = q.do_runs ? (int64_t)hdr[0] : 0;
+        ctx->n_runs = q.args.do_runs ? (int64_t)hdr[0] : 0;
         ctx->max_depth = (int32_t)hdr[2];
-        ctx->red_W = q.W; ctx->red_mincov = q.mincov; ctx->red_maxmean = q.maxmean; ctx->red_break = q.run_break;
-        ctx->n_windows = q.do_windows ? q.n_windows : 0;
+        ctx->red = q.args;
+        ctx->n_windows = q.args.do_windows ? q.n_windows : 0;
         ctx->depth_reduced = true;
     }
     return GL_OK;
@@ -1864,8 +1853,11 @@ int depth_resolve(gl_ctx* ctx) {
 
 int depth_reduce_epilogue(gl_ctx* ctx, int32_t* d_depth_out) {
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "multidepth: no region open (call gl_depth_begin)");
-    const int32_t W = (int32_t)std::min<int64_t>(ctx->re, INT32_MAX);      // one window; windows are not computed
-    GL_CHECK(run_reduce(ctx, W, 1, 0, 0, false, false, d_depth_out, false));
+    ReduceArgs a;
+    a.W = (int32_t)std::min<int64_t>(ctx->re, INT32_MAX);      // one window; windows are not computed
+    a.mincov = 1;
+    a.d_depth_out = d_depth_out;
+    GL_CHECK(run_reduce(ctx, a));
     return depth_resolve(ctx);
 }
 
@@ -1884,10 +1876,8 @@ int gl_depth_begin(gl_ctx* ctx, int64_t region_start, int64_t region_end) {
     ctx->store_n = 0;
     ctx->p8.pending = false;
     ctx->p8.upload_pending = false;
-    ctx->g_valid = false;
-    ctx->ev_valid = false;
     ctx->depth_active = true;
-    drop_result(ctx);     // nobody can ask for a pending result any more; its scratch is reused in stream order
+    segments_changed(ctx);     // nobody can ask for a pending result any more; its scratch is reused in stream order
     ctx->n_windows = 0;
     ctx->n_runs = 0;
     ctx->max_depth = 0;
@@ -1903,9 +1893,7 @@ int gl_depth_add_segments_device(gl_ctx* ctx, const int32_t* d_start, const int3
     gl_seg_batch b;
     b.s = d_start; b.e = d_end; b.n = n;
     ctx->batches.push_back(b);
-    ctx->g_valid = false;
-    ctx->ev_valid = false;
-    drop_result(ctx);
+    segments_changed(ctx);
     return GL_OK;
 }
 
@@ -1949,19 +1937,7 @@ int gl_depth_add_segments(gl_ctx* ctx, const int32_t* start, const int32_t* end,
         }
     }
     ctx->copies_pending = true;
-    // consecutive host calls extend one contiguous batch in the store
-    if (!ctx->batches.empty() && ctx->batches.back().s == nullptr &&
-        ctx->batches.back().off + ctx->batches.back().n == ctx->store_n) {
-        ctx->batches.back().n += n;
-    } else {
-        gl_seg_batch b;
-        b.off = ctx->store_n; b.n = n;
-        ctx->batches.push_back(b);
-    }
-    ctx->store_n += n;
-    ctx->g_valid = false;
-    ctx->ev_valid = false;
-    drop_result(ctx);
+    store_append(ctx, n);
     return GL_OK;
 }
 
@@ -1975,21 +1951,17 @@ int gl_depth_add_segments_packed16(gl_ctx* ctx, const int32_t* anchors, const ui
     GL_CHECK(store_reserve(ctx, ctx->store_n + n));
     // staging for the packed bytes: anchors | off | len
     const size_t b_anchor = (size_t)n_blocks * 4, b_u16 = (size_t)n * 2;
-    GL_CHECK(gl_buf_reserve(ctx, ctx->packed, ((b_anchor + 255) & ~size_t(255)) + 2 * ((b_u16 + 255) & ~size_t(255))));
+    GL_CHECK(gl_buf_reserve(ctx, ctx->packed, al256(b_anchor) + 2 * al256(b_u16)));
     char* d_anchor = static_cast<char*>(ctx->packed.p);
-    char* d_off = d_anchor + ((b_anchor + 255) & ~size_t(255));
-    char* d_len = d_off + ((b_u16 + 255) & ~size_t(255));
+    char* d_off = d_anchor + al256(b_anchor);
+    char* d_len = d_off + al256(b_u16);
     const bool pinned = is_pinned_host(anchors) && is_pinned_host(off) && is_pinned_host(len);
     if (!pinned) {       // pageable: let the runtime stage it (the fast path is pinned feeder buffers)
         GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
     }
     // the previous unpack must be done with the staging buffer before it is overwritten
     GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[0], 0));
-    GL_CUDA(ctx, cudaMemcpyAsync(d_anchor, anchors, b_anchor, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaMemcpyAsync(d_off, off, b_u16, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaMemcpyAsync(d_len, len, b_u16, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[1], ctx->copy_stream));
-    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[1], 0));
+    GL_CHECK(upload_blocks(ctx, d_anchor, d_off, d_len, anchors, off, len, 0, n_blocks, 512, ctx->ev_copy[1]));
     {
         gl_prof_scope prof(ctx, "depth_unpack16_kernel");
         depth_unpack16_kernel<<<(unsigned)n_blocks, 256, 0, ctx->stream>>>(
@@ -2000,18 +1972,7 @@ int gl_depth_add_segments_packed16(gl_ctx* ctx, const int32_t* anchors, const ui
     GL_LAUNCHED(ctx, 1);
     GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));
     if (!pinned) GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
-    if (!ctx->batches.empty() && ctx->batches.back().s == nullptr &&
-        ctx->batches.back().off + ctx->batches.back().n == ctx->store_n) {
-        ctx->batches.back().n += n;
-    } else {
-        gl_seg_batch b;
-        b.off = ctx->store_n; b.n = n;
-        ctx->batches.push_back(b);
-    }
-    ctx->store_n += n;
-    ctx->g_valid = false;
-    ctx->ev_valid = false;
-    drop_result(ctx);
+    store_append(ctx, n);
     return GL_OK;
 }
 
@@ -2027,9 +1988,7 @@ static int p8_register(gl_ctx* ctx, const int* d_anchor, const void* d_ds, const
     ctx->p8.anchors = d_anchor; ctx->p8.ds = d_ds; ctx->p8.len = d_len; ctx->p8.n_blocks = n_blocks; ctx->p8.store_off = base;
     ctx->p8.pending = true;
     if (ctx->batches.size() > 1) GL_CHECK(p8_materialize(ctx));   // not the only batch: the int32 paths take it
-    ctx->g_valid = false;
-    ctx->ev_valid = false;
-    drop_result(ctx);
+    segments_changed(ctx);
     return GL_OK;
 }
 
@@ -2043,12 +2002,6 @@ int gl_depth_add_segments_packed8_device(gl_ctx* ctx, const int32_t* d_anchors, 
     return p8_register(ctx, d_anchors, d_dstart, d_len, n_blocks);
 }
 
-static int add_packed8_host(gl_ctx* ctx, const int32_t* anchors, const uint8_t* dstart, const uint8_t* len, int64_t n_blocks, bool may_defer);
-
-int gl_depth_add_segments_packed8(gl_ctx* ctx, const int32_t* anchors, const uint8_t* dstart, const uint8_t* len, int64_t n_blocks) {
-    return add_packed8_host(ctx, anchors, dstart, len, n_blocks, false);
-}
-
 static int add_packed8_host(gl_ctx* ctx, const int32_t* anchors, const uint8_t* dstart, const uint8_t* len, int64_t n_blocks, bool may_defer) {
     GL_CHECK(gl_use(ctx));
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_add_segments_packed8: no region open (call gl_depth_begin)");
@@ -2056,12 +2009,12 @@ static int add_packed8_host(gl_ctx* ctx, const int32_t* anchors, const uint8_t* 
     if (n_blocks == 0) return GL_OK;
     GL_CHECK(p8_materialize(ctx));                                  // an earlier packed8 batch still lives in the staging buffer
     const size_t b_anchor = (size_t)n_blocks * 4, b_u8 = (size_t)n_blocks * 64;
-    GL_CHECK(gl_buf_reserve(ctx, ctx->packed, ((b_anchor + 255) & ~size_t(255)) + 2 * ((b_u8 + 255) & ~size_t(255))));
+    GL_CHECK(gl_buf_reserve(ctx, ctx->packed, al256(b_anchor) + 2 * al256(b_u8)));
     char* d_anchor = static_cast<char*>(ctx->packed.p);
-    char* d_ds = d_anchor + ((b_anchor + 255) & ~size_t(255));
-    char* d_len = d_ds + ((b_u8 + 255) & ~size_t(255));
+    char* d_ds = d_anchor + al256(b_anchor);
+    char* d_len = d_ds + al256(b_u8);
     const bool pinned = is_pinned_host(anchors) && is_pinned_host(dstart) && is_pinned_host(len);
-    if (may_defer && pinned && ctx->batches.empty() && ctx->force_path == 0 && n_blocks >= 4096) {
+    if (may_defer && pinned && ctx->batches.empty() && ctx->force_path == kPathNone && n_blocks >= 4096) {
         // one-call entry: the reduce follows at once, so let it stream the words in (chunk k+1 on the wire while chunk k's
         // tiles are reduced)
         GL_CHECK(p8_register(ctx, reinterpret_cast<const int*>(d_anchor), d_ds, d_len, n_blocks));
@@ -2071,20 +2024,26 @@ static int add_packed8_host(gl_ctx* ctx, const int32_t* anchors, const uint8_t* 
     }
     if (!pinned) GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
     GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_used[0], 0));   // previous consumer done with the staging buffer
-    GL_CUDA(ctx, cudaMemcpyAsync(d_anchor, anchors, b_anchor, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaMemcpyAsync(d_ds, dstart, b_u8, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaMemcpyAsync(d_len, len, b_u8, cudaMemcpyHostToDevice, ctx->copy_stream));
-    GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[1], ctx->copy_stream));
-    GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[1], 0));
+    GL_CHECK(upload_blocks(ctx, d_anchor, d_ds, d_len, anchors, dstart, len, 0, n_blocks, 64, ctx->ev_copy[1]));
     if (!pinned) GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
     return p8_register(ctx, reinterpret_cast<const int*>(d_anchor), d_ds, d_len, n_blocks);
+}
+
+int gl_depth_add_segments_packed8(gl_ctx* ctx, const int32_t* anchors, const uint8_t* dstart, const uint8_t* len, int64_t n_blocks) {
+    return add_packed8_host(ctx, anchors, dstart, len, n_blocks, false);
 }
 
 int gl_depth_reduce(gl_ctx* ctx, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break) {
     GL_CHECK(gl_use(ctx));
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_reduce: no region open");
     if (W <= 0 || run_break < 0) return gl_fail(ctx, GL_EINVAL, "gl_depth_reduce: W must be > 0 and run_break >= 0");
-    return run_reduce(ctx, W, mincov, maxmean, run_break, true, true, nullptr, false);
+    ReduceArgs a;
+    a.W = W;
+    a.mincov = mincov;
+    a.maxmean = maxmean;
+    a.run_break = run_break;
+    a.do_windows = a.do_runs = true;
+    return run_reduce(ctx, a);
 }
 
 int gl_depth_result_sizes(gl_ctx* ctx, int64_t* n_windows, int64_t* n_runs, int32_t* max_depth) {
@@ -2121,7 +2080,7 @@ int gl_depth_last_path(gl_ctx* ctx, int32_t* path) {
 }
 
 int gl_depth_set_path(gl_ctx* ctx, int32_t path) {
-    if (!ctx || path < 0 || path > 4 || path == 3) return gl_fail(ctx, GL_EINVAL, "gl_depth_set_path: path must be 0 (auto), 1 (no packed8 kernel), 2 (HBM difference array only) or 4 (bucketed events only)");
+    if (!ctx || (path != kPathNone && path != kPathFused && path != kPathHbmDiff && path != kPathEvents)) return gl_fail(ctx, GL_EINVAL, "gl_depth_set_path: path must be 0 (auto), 1 (no packed8 kernel), 2 (HBM difference array only) or 4 (bucketed events only)");
     ctx->force_path = path;
     return GL_OK;
 }
@@ -2161,7 +2120,11 @@ int gl_depth_windows(gl_ctx* ctx, int32_t W, int64_t* sum_out, int32_t* min_out,
     GL_CHECK(gl_use(ctx));
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_windows: no region open");
     if (W <= 0) return gl_fail(ctx, GL_EINVAL, "gl_depth_windows: W must be > 0");
-    GL_CHECK(run_reduce(ctx, W, 0, 0, 0, true, false, nullptr, min_out != nullptr));
+    ReduceArgs ra;
+    ra.W = W;
+    ra.do_windows = true;
+    ra.want_min = min_out != nullptr;
+    GL_CHECK(run_reduce(ctx, ra));
     GL_CHECK(depth_resolve(ctx));
     GL_CHECK(gl_depth_get_windows(ctx, sum_out, n_windows));
     if (min_out) {
@@ -2175,7 +2138,11 @@ int gl_depth_classes(gl_ctx* ctx, int32_t mincov, int32_t maxmean, int32_t* run_
                      uint8_t* run_class, int64_t cap, int64_t* n_runs) {
     GL_CHECK(gl_use(ctx));
     if (!ctx->depth_active) return gl_fail(ctx, GL_ESTATE, "gl_depth_classes: no region open");
-    GL_CHECK(run_reduce(ctx, 1 << 30, mincov, maxmean, 0, false, true, nullptr, false));
+    ReduceArgs ra;
+    ra.mincov = mincov;
+    ra.maxmean = maxmean;
+    ra.do_runs = true;
+    GL_CHECK(run_reduce(ctx, ra));
     GL_CHECK(depth_resolve(ctx));
     if (n_runs) *n_runs = ctx->n_runs;
     return gl_depth_get_runs(ctx, run_start, run_end, run_class, cap);
@@ -2187,18 +2154,14 @@ int gl_depth_interval_sums(gl_ctx* ctx, const int32_t* a, const int32_t* b, int6
     if (n < 0 || (n > 0 && (!a || !b || !sums))) return gl_fail(ctx, GL_EINVAL, "gl_depth_interval_sums: bad argument");
     if (n == 0) return GL_OK;
     GL_CHECK(depth_resolve(ctx));                                  // the last reduce's path decides whether its cell index is used
-    if (ctx->copies_pending) {
-        GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[0], ctx->copy_stream));
-        GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[0], 0));
-        ctx->copies_pending = false;
-    }
+    GL_CHECK(join_copies(ctx));
     if ((int)ctx->batches.size() > kMaxBatches) return gl_fail(ctx, GL_ERANGE, "gl_depth_interval_sums: more than %d segment batches", kMaxBatches);
     GL_CHECK(p8_materialize(ctx));
     ScanParams p;
     memset(&p, 0, sizeof p);
     p.rs = (int)ctx->rs;
     p.re = (int)ctx->re;
-    const bool use_index = ctx->depth_reduced && ctx->last_path == 1 && ctx->idx_cells != nullptr;
+    const bool use_index = ctx->depth_reduced && ctx->last_path == kPathFused && ctx->idx_cells != nullptr;
     p.n_batches = (int)ctx->batches.size();
     p.flags = ctx->idx_flags;
     p.origin = ctx->idx_origin;
@@ -2209,7 +2172,7 @@ int gl_depth_interval_sums(gl_ctx* ctx, const int32_t* a, const int32_t* b, int6
         p.batch[bi].start = batch_start(ctx, bt);
         p.batch[bi].end = batch_end(ctx, bt);
         p.batch[bi].n = (int)std::min<int64_t>(bt.n, INT32_MAX - 1);
-        if (use_index) {                                           // same layout as run_reduce: hi | cnt | lo
+        if (use_index) {                                           // same layout as reduce_int32: hi | cnt | lo
             const unsigned* hi_all = ctx->idx_cells;
             const unsigned* cnt_all = hi_all + (size_t)ctx->idx_ncells * nb;
             const unsigned* lo_all = cnt_all + (size_t)ctx->idx_ncells * nb;
@@ -2243,7 +2206,9 @@ int gl_depth_perbase(gl_ctx* ctx, int32_t* depth_out) {
     if (!depth_out) return gl_fail(ctx, GL_EINVAL, "gl_depth_perbase: null output");
     const int64_t len = ctx->re - ctx->rs;
     GL_CHECK(gl_buf_reserve(ctx, ctx->misc, (size_t)(len + 4) * 4));
-    GL_CHECK(run_reduce(ctx, 1 << 30, 0, 0, 0, false, false, static_cast<int32_t*>(ctx->misc.p), false));
+    ReduceArgs ra;
+    ra.d_depth_out = static_cast<int32_t*>(ctx->misc.p);
+    GL_CHECK(run_reduce(ctx, ra));
     GL_CHECK(depth_resolve(ctx));
     GL_CUDA(ctx, cudaMemcpyAsync(depth_out, ctx->misc.p, (size_t)len * 4, cudaMemcpyDeviceToHost, ctx->stream));
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -2251,52 +2216,28 @@ int gl_depth_perbase(gl_ctx* ctx, int32_t* depth_out) {
     return GL_OK;
 }
 
-static int region_fetch(gl_ctx* ctx, int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class,
-                        int64_t run_cap, int64_t* n_runs);
-
 int gl_depth_region_packed16(gl_ctx* ctx, int64_t region_start, int64_t region_end, const int32_t* anchors, const uint16_t* off,
                              const uint16_t* len, int64_t n_blocks, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break,
                              int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class,
                              int64_t run_cap, int64_t* n_runs) {
-    GL_CHECK(gl_depth_begin(ctx, region_start, region_end));
-    GL_CHECK(gl_depth_add_segments_packed16(ctx, anchors, off, len, n_blocks));
-    ctx->prefetch_sums = sum_out; ctx->prefetch_cap = sum_out ? win_cap : 0;
-    ctx->prefetch_run_start = run_start; ctx->prefetch_run_class = run_class; ctx->prefetch_run_cap = (run_start && run_class) ? run_cap : 0;
-    const int rc_reduce = gl_depth_reduce(ctx, W, mincov, maxmean, run_break);
-    ctx->prefetch_sums = nullptr; ctx->prefetch_cap = 0;
-    ctx->prefetch_run_start = nullptr; ctx->prefetch_run_class = nullptr; ctx->prefetch_run_cap = 0;
-    GL_CHECK(rc_reduce);
-    return region_fetch(ctx, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
+    return region_one_call(ctx, region_start, region_end, [&] { return gl_depth_add_segments_packed16(ctx, anchors, off, len, n_blocks); },
+                           W, mincov, maxmean, run_break, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
 }
 
 int gl_depth_region_packed8(gl_ctx* ctx, int64_t region_start, int64_t region_end, const int32_t* anchors, const uint8_t* dstart,
                             const uint8_t* len, int64_t n_blocks, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break,
                             int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class,
                             int64_t run_cap, int64_t* n_runs) {
-    GL_CHECK(gl_depth_begin(ctx, region_start, region_end));
-    GL_CHECK(add_packed8_host(ctx, anchors, dstart, len, n_blocks, true));
-    ctx->prefetch_sums = sum_out; ctx->prefetch_cap = sum_out ? win_cap : 0;
-    ctx->prefetch_run_start = run_start; ctx->prefetch_run_class = run_class; ctx->prefetch_run_cap = (run_start && run_class) ? run_cap : 0;
-    const int rc_reduce = gl_depth_reduce(ctx, W, mincov, maxmean, run_break);
-    ctx->prefetch_sums = nullptr; ctx->prefetch_cap = 0;
-    ctx->prefetch_run_start = nullptr; ctx->prefetch_run_class = nullptr; ctx->prefetch_run_cap = 0;
-    GL_CHECK(rc_reduce);
-    return region_fetch(ctx, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
+    return region_one_call(ctx, region_start, region_end, [&] { return add_packed8_host(ctx, anchors, dstart, len, n_blocks, true); },
+                           W, mincov, maxmean, run_break, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
 }
 
 int gl_depth_region(gl_ctx* ctx, int64_t region_start, int64_t region_end, const int32_t* start, const int32_t* end,
                     int64_t n, int32_t W, int32_t mincov, int32_t maxmean, int64_t run_break, int64_t* sum_out,
                     int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class, int64_t run_cap,
                     int64_t* n_runs) {
-    GL_CHECK(gl_depth_begin(ctx, region_start, region_end));
-    GL_CHECK(gl_depth_add_segments(ctx, start, end, n));
-    ctx->prefetch_sums = sum_out; ctx->prefetch_cap = sum_out ? win_cap : 0;
-    ctx->prefetch_run_start = run_start; ctx->prefetch_run_class = run_class; ctx->prefetch_run_cap = (run_start && run_class) ? run_cap : 0;
-    const int rc_reduce = gl_depth_reduce(ctx, W, mincov, maxmean, run_break);
-    ctx->prefetch_sums = nullptr; ctx->prefetch_cap = 0;
-    ctx->prefetch_run_start = nullptr; ctx->prefetch_run_class = nullptr; ctx->prefetch_run_cap = 0;
-    GL_CHECK(rc_reduce);
-    return region_fetch(ctx, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
+    return region_one_call(ctx, region_start, region_end, [&] { return gl_depth_add_segments(ctx, start, end, n); },
+                           W, mincov, maxmean, run_break, sum_out, win_cap, n_windows, run_start, run_class, run_cap, n_runs);
 }
 
 // ---- one region of a contig (whole chunks), segments in, BED text out: depth/depth.go:238-364 for every chunk, in order
@@ -2343,15 +2284,7 @@ int gl_depth_bed_region(gl_ctx* ctx, const char* chrom, int64_t rs, int64_t re, 
         const auto ph0 = std::chrono::steady_clock::now();
         const int64_t nbk = (n + 255) / 256;
         const size_t o_off = ((size_t)nbk * 4 + 255) & ~size_t(255), o_len = o_off + (size_t)nbk * 512, bytes = o_len + (size_t)nbk * 512;
-        if (ctx->pack_pinned_bytes < bytes) {
-            GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
-            if (ctx->pack_pinned) cudaFreeHost(ctx->pack_pinned);
-            ctx->pack_pinned = nullptr; ctx->pack_pinned_bytes = 0;
-            const size_t want = bytes + bytes / 8;
-            cudaError_t e = cudaHostAlloc(&ctx->pack_pinned, want, cudaHostAllocDefault);
-            if (e != cudaSuccess) { ctx->pack_pinned = nullptr; cudaGetLastError(); return gl_fail(ctx, GL_ENOMEM, "cudaHostAlloc(%zu): %s", want, cudaGetErrorString(e)); }
-            ctx->pack_pinned_bytes = want;
-        }
+        GL_CHECK(gl_pinned_reserve(ctx, bytes, bytes + bytes / 8));
         char* hp = static_cast<char*>(ctx->pack_pinned);
         int32_t* A = reinterpret_cast<int32_t*>(hp);
         uint16_t* O = reinterpret_cast<uint16_t*>(hp + o_off);
@@ -2390,11 +2323,7 @@ int gl_depth_bed_region(gl_ctx* ctx, const char* chrom, int64_t rs, int64_t re, 
             ctx->tr_pack_s += std::chrono::duration<double>(std::chrono::steady_clock::now() - tp0).count();
             if (rc == GL_ERANGE) { n_esc = esc_before; fell_back = true; break; }   // (almost) every block escapes: long reads / unsorted input
             if (rc != GL_OK) return gl_fail(ctx, rc, "gl_pack_segments16_fixed_range_mt failed");
-            GL_CUDA(ctx, cudaMemcpyAsync(dp + (size_t)b0 * 4, A + b0, (size_t)(b1 - b0) * 4, cudaMemcpyHostToDevice, ctx->copy_stream));
-            GL_CUDA(ctx, cudaMemcpyAsync(dp + o_off + (size_t)b0 * 512, O + b0 * 256, (size_t)(b1 - b0) * 512, cudaMemcpyHostToDevice, ctx->copy_stream));
-            GL_CUDA(ctx, cudaMemcpyAsync(dp + o_len + (size_t)b0 * 512, Ln + b0 * 256, (size_t)(b1 - b0) * 512, cudaMemcpyHostToDevice, ctx->copy_stream));
-            GL_CUDA(ctx, cudaEventRecord(ctx->ev_copy[1], ctx->copy_stream));
-            GL_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_copy[1], 0));
+            GL_CHECK(upload_blocks(ctx, dp, dp + o_off, dp + o_len, A, O, Ln, b0, b1, 512, ctx->ev_copy[1]));
             {
                 gl_prof_scope prof(ctx, "depth_unpack16_kernel");
                 depth_unpack16_kernel<<<(unsigned)(b1 - b0), 256, 0, ctx->stream>>>(
@@ -2408,13 +2337,7 @@ int gl_depth_bed_region(gl_ctx* ctx, const char* chrom, int64_t rs, int64_t re, 
         }
         GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));
         ctx->copies_pending = true;
-        if (done_blocks > 0) {
-            gl_seg_batch bt;
-            bt.off = 0; bt.n = done_blocks * 256;
-            ctx->batches.push_back(bt);
-            ctx->store_n = done_blocks * 256;
-            ctx->g_valid = false; ctx->ev_valid = false; drop_result(ctx);
-        }
+        if (done_blocks > 0) store_append(ctx, done_blocks * 256);         // the region's first batch: store [0, done_blocks * 256)
         const auto ph2 = std::chrono::steady_clock::now();
         ctx->tr_esc = n_esc;
         ctx->tr_bytes += 8 * n_esc + (fell_back ? 8 * (n - done_blocks * 256) : 0);
@@ -2451,14 +2374,7 @@ int gl_depth_bed_region(gl_ctx* ctx, const char* chrom, int64_t rs, int64_t re, 
     int64_t cap = n / 40 + 1024, nb = 0;
     for (int attempt = 0; attempt < 2; attempt++) {
         const size_t bytes = (size_t)cap * 132 + 256;
-        if (ctx->pack_pinned_bytes < bytes) {
-            GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
-            if (ctx->pack_pinned) cudaFreeHost(ctx->pack_pinned);
-            ctx->pack_pinned = nullptr; ctx->pack_pinned_bytes = 0;
-            cudaError_t e = cudaHostAlloc(&ctx->pack_pinned, bytes, cudaHostAllocDefault);
-            if (e != cudaSuccess) { ctx->pack_pinned = nullptr; cudaGetLastError(); return gl_fail(ctx, GL_ENOMEM, "cudaHostAlloc(%zu): %s", bytes, cudaGetErrorString(e)); }
-            ctx->pack_pinned_bytes = bytes;
-        }
+        GL_CHECK(gl_pinned_reserve(ctx, bytes, bytes));
         const int64_t cap_now = (int64_t)((ctx->pack_pinned_bytes - 256) / 132);
         int32_t* a = static_cast<int32_t*>(ctx->pack_pinned);
         uint8_t* d = reinterpret_cast<uint8_t*>(a + ((cap_now + 3) & ~int64_t(3)));
@@ -2487,27 +2403,6 @@ int gl_depth_bed_contig(gl_ctx* ctx, const char* chrom, int64_t contig_len, cons
                         int64_t* callable_len) {
     return gl_depth_bed_region(ctx, chrom, 0, contig_len, start, end, n, W, mincov, maxmean, step, threads, depth_bed, depth_cap, depth_len,
                                callable_bed, callable_cap, callable_len);
-}
-
-static int region_fetch(gl_ctx* ctx, int64_t* sum_out, int64_t win_cap, int64_t* n_windows, int32_t* run_start, uint8_t* run_class,
-                        int64_t run_cap, int64_t* n_runs) {
-    GL_CHECK(depth_resolve(ctx));
-    const int64_t nw = ctx->n_windows, nr = ctx->n_runs;
-    if (n_windows) *n_windows = nw;
-    if (n_runs) *n_runs = nr;
-    if (nw > win_cap) return gl_fail(ctx, GL_ERANGE, "gl_depth_region: %lld windows > cap %lld", (long long)nw, (long long)win_cap);
-    if (nr > run_cap) return gl_fail(ctx, GL_ERANGE, "gl_depth_region: %lld runs > cap %lld", (long long)nr, (long long)run_cap);
-    const bool have_sums = ctx->prefetched, have_runs = ctx->prefetched_runs >= nr;
-    ctx->prefetched = false;
-    ctx->prefetched_runs = 0;
-    if (have_sums && have_runs) return GL_OK;                  // everything came home with the header (depth_resolve waited for it)
-    if (!have_sums) GL_CUDA(ctx, cudaMemcpyAsync(sum_out, ctx->win_sum_p, (size_t)nw * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    if (nr > 0 && !have_runs) {
-        GL_CUDA(ctx, cudaMemcpyAsync(run_start, ctx->run_start.p, (size_t)nr * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        GL_CUDA(ctx, cudaMemcpyAsync(run_class, ctx->run_class.p, (size_t)nr, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return GL_OK;
 }
 
 }  // extern "C"

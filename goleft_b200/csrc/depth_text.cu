@@ -295,10 +295,10 @@ int gl_depth_text(gl_ctx* ctx, const char* chrom, char* depth_bed, int64_t depth
     GL_CHECK(depth_resolve(ctx));
     if (!ctx->depth_reduced) return gl_fail(ctx, GL_ESTATE, "gl_depth_text: call gl_depth_reduce first");
     if (!depth_len || !callable_len) return gl_fail(ctx, GL_EINVAL, "gl_depth_text: null length pointer");
-    const int W = ctx->red_W;
+    const int W = ctx->red.W;
     if (ctx->n_windows > 0 && ctx->rs % W != 0)
         return gl_fail(ctx, GL_EINVAL, "gl_depth_text: region start %lld is not a multiple of the window size (use gl_depth_format_rows)", (long long)ctx->rs);
-    if (ctx->red_break > 0 && ctx->red_break % W != 0)
+    if (ctx->red.run_break > 0 && ctx->red.run_break % W != 0)
         return gl_fail(ctx, GL_EINVAL, "gl_depth_text: run_break must be a multiple of the window size");
     TextParams pw, pc;
     memset(&pw, 0, sizeof pw);

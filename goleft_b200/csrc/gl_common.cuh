@@ -37,6 +37,24 @@ struct gl_md_ep {
     unsigned long long* slots = nullptr;   // [pairs * 8]: slot (pair, c) = Σ d over the block's sufficient sites in the tile's c-th 512 bases
 };
 
+// depth.cu: the reduce's paths, numbered as gl_depth_last_path reports them (DESIGN §1.0-1.2)
+enum DepthPath : int {
+    kPathNone = 0,          // last_path: nothing reduced yet; force_path: choose automatically
+    kPathFused = 1,         // fused int32 (segments in BAM order)
+    kPathHbmDiff = 2,       // HBM difference array (on request only)
+    kPathPacked8 = 3,       // the region's only batch is packed8, read as it is
+    kPathEvents = 4,        // bucketed events (the general path)
+};
+
+// depth.cu: what one reduce computes.  The defaults ask for nothing: no windows (one window per 2^30 bases), no runs.
+struct ReduceArgs {
+    int32_t W = 1 << 30;
+    int32_t mincov = 0, maxmean = 0;
+    int64_t run_break = 0;
+    bool do_windows = false, do_runs = false, want_min = false;
+    int32_t* d_depth_out = nullptr;     // device per-base depth (may be null)
+};
+
 struct gl_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;       // compute stream
@@ -54,22 +72,25 @@ struct gl_ctx {
     // ---- depth state
     bool depth_active = false, depth_reduced = false;
     int64_t rs = 0, re = 0;
-    int32_t red_W = 0, red_mincov = 0, red_maxmean = 0; int64_t red_break = 0;
+    ReduceArgs red;                         // what the settled result was asked for
     int64_t n_windows = 0, n_runs = 0; int32_t max_depth = 0;
     std::vector<gl_seg_batch> batches;      // segments added since gl_depth_begin
     gl_buf store_s, store_e;                // host-uploaded segments, contiguous
     gl_buf packed;                          // staging for packed16 uploads
     int64_t store_n = 0;
     bool copies_pending = false;            // H2D into the store still in flight on copy_stream
-    bool g_valid = false;                   // the HBM difference array holds every batch (general path)
-    bool ev_valid = false;                  // the per-tile event buckets hold every batch (general path, version 2)
-    int last_path = 0;                      // 1 = fused sorted path, 2 = general scatter path
+    // what `diff` holds, built from every batch: kPathNone (nothing valid), kPathHbmDiff (the difference array) or
+    // kPathEvents (the per-tile event buckets); the two general paths share the buffer
+    int diff_holds = kPathNone;
+    int last_path = kPathNone;              // the path the settled result took (gl_depth_last_path)
     // index tables of the last fused reduce (valid until the next reduce): used by gl_depth_interval_sums
-    const int* idx_flags = nullptr; const unsigned* idx_cells = nullptr; int idx_origin = 0, idx_ncells = 0, idx_maxlen = -1;
-    int force_path = 0;                     // 0 = auto, 1 = no packed8 kernel (int32 fused, else general), 2 = always general
+    const int* idx_flags = nullptr; const unsigned* idx_cells = nullptr; int idx_origin = 0, idx_ncells = 0;
+    // gl_depth_set_path: kPathNone = automatic (packed8, else fused, else bucketed events); kPathFused = never the packed8
+    // kernel; kPathHbmDiff / kPathEvents = always that general path
+    int force_path = kPathNone;
     gl_md_ep md_ep;                         // the tile core's multidepth epilogue for the next reduce (mode 0: none)
     void* md = nullptr;                     // multidepth.cu state (gl_multidepth_begin)
-    // a packed8 batch that is the region's only batch stays packed: K_fused8 reads it as it is (last_path 3); it is
+    // a packed8 batch that is the region's only batch stays packed: K_fused8 reads it as it is (kPathPacked8); it is
     // unpacked into the store (its batch descriptor already points there) only when something needs int32 arrays
     struct { const int* anchors = nullptr; const void* ds = nullptr; const void* len = nullptr; int64_t n_blocks = 0, store_off = 0;
              bool pending = false;
@@ -85,9 +106,8 @@ struct gl_ctx {
     uint64_t* hdr_host = nullptr;         // 4 words, pinned
     cudaEvent_t ev_hdr = nullptr;
     struct { bool active = false;
-             int32_t W = 0, mincov = 0, maxmean = 0; int64_t run_break = 0; bool do_windows = false, do_runs = false, want_min = false;
-             int32_t* d_depth_out = nullptr;
-             int path = 0; long long run_cap = 0; int64_t n_windows = 0;   // the path tried (as gl_depth_last_path) and its run capacity
+             ReduceArgs args;
+             int path = kPathNone; long long run_cap = 0; int64_t n_windows = 0;   // the path tried and its run capacity
              bool d2h = false;                                             // window sums also on their way home on d2h_stream
              const int* flags = nullptr; const unsigned* cells = nullptr; int origin = 0, ncells = 0; } pend;
     gl_buf win_min;       // i32[n_windows]
@@ -96,10 +116,9 @@ struct gl_ctx {
     gl_buf run_tmp_start; // claim-order staging of the runs
     gl_buf run_tmp_class;
     gl_buf scratch;       // header | window sums | index flags + cell tables | per-tile run table
-    gl_buf seg[2];        // device staging for host segments: int32 start|end
     void* pinned[2] = {nullptr, nullptr};
-    size_t pinned_bytes = 0;
-    void* pack_pinned = nullptr; size_t pack_pinned_bytes = 0;   // gl_depth_bed_contig: pinned home of the packed8 words it makes
+    // pinned host staging (gl_pinned_reserve): the packed words gl_depth_bed_region makes, the compressed bytes gl_bam_decode_device reads
+    void* pack_pinned = nullptr; size_t pack_pinned_bytes = 0;
     bool cohort_attr_set = false;                                // ic_cohort2_kernel's dynamic shared-memory limit raised on this ctx's device
     double tr_phase[3] = {0, 0, 0};
     int tr_kind = 0; double tr_pack_s = 0; int64_t tr_bytes = 0, tr_esc = 0;   // gl_depth_transport_stats
@@ -128,6 +147,9 @@ extern thread_local std::string g_gl_err;
 int gl_fail(gl_ctx* ctx, int code, const char* fmt, ...);
 // Grows b.  Freeing the old buffer first synchronises ctx->stream, so no queued work can still be using it.
 int gl_buf_reserve(gl_ctx* ctx, gl_buf& b, size_t bytes);
+// Grows ctx->pack_pinned to `want` bytes when it holds fewer than `bytes`.  Synchronises copy_stream first: the uploads
+// queued out of the old buffer must have left it.  Library-internal: not exported from the .so.
+__attribute__((visibility("hidden"))) int gl_pinned_reserve(gl_ctx* ctx, size_t bytes, size_t want);
 // depth.cu: settle the last gl_depth_reduce (wait for its header; accept it, or rerun it on the next path or with room for
 // every run).  Every reader of the reduce's results calls this first; a no-op when nothing is pending.
 int depth_resolve(gl_ctx* ctx);

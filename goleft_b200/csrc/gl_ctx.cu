@@ -37,6 +37,22 @@ int gl_buf_reserve(gl_ctx* ctx, gl_buf& b, size_t bytes) {
     return GL_OK;
 }
 
+int gl_pinned_reserve(gl_ctx* ctx, size_t bytes, size_t want) {
+    if (ctx->pack_pinned_bytes >= bytes) return GL_OK;
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream));
+    if (ctx->pack_pinned) cudaFreeHost(ctx->pack_pinned);
+    ctx->pack_pinned = nullptr;
+    ctx->pack_pinned_bytes = 0;
+    cudaError_t e = cudaHostAlloc(&ctx->pack_pinned, want, cudaHostAllocDefault);
+    if (e != cudaSuccess) {
+        ctx->pack_pinned = nullptr;
+        cudaGetLastError();
+        return gl_fail(ctx, GL_ENOMEM, "cudaHostAlloc(%zu): %s", want, cudaGetErrorString(e));
+    }
+    ctx->pack_pinned_bytes = want;
+    return GL_OK;
+}
+
 static void buf_free(gl_buf& b) {
     if (b.p) cudaFree(b.p);
     b.p = nullptr;
@@ -180,7 +196,7 @@ int gl_ctx_destroy(gl_ctx* ctx) {
     buf_free(ctx->run_start); buf_free(ctx->run_class); buf_free(ctx->scratch);
     buf_free(ctx->run_tmp_start); buf_free(ctx->run_tmp_class);
     buf_free(ctx->store_s); buf_free(ctx->store_e); buf_free(ctx->packed);
-    buf_free(ctx->seg[0]); buf_free(ctx->seg[1]); buf_free(ctx->flush); buf_free(ctx->misc); buf_free(ctx->fasta);
+    buf_free(ctx->flush); buf_free(ctx->misc); buf_free(ctx->fasta);
     buf_free(ctx->bam_comp); buf_free(ctx->bam_out); buf_free(ctx->bam_seg);
     buf_free(ctx->text_slots); buf_free(ctx->text_blk); buf_free(ctx->text_len); buf_free(ctx->text_out[0]); buf_free(ctx->text_out[1]);
     for (int i = 0; i < 2; i++) {

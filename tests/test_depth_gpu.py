@@ -339,11 +339,17 @@ def test_packed8_path(ctx):
     s, e = synth.segments(synth.reads(L, contig_index=9))
     a, d, ln = capi.pack_segments8(s, e)
     exp = orc.pileup_diff(s, e, 0, L)
-    es, _ = orc.window_sums(exp, 0, L, 500)
+    es, em = orc.window_sums(exp, 0, L, 500)
     ea, ec = orc.class_runs(exp, 0, L, 4, 0, 1_000_000)
     ws, r0, rc = ctx.depth_region_packed8(0, L, a, d, ln, 500, 4, 0, run_break=1_000_000)
     assert ctx.depth_last_path() == 3
     assert np.array_equal(ws, es) and np.array_equal(r0, ea) and np.array_equal(rc, ec)
+    # window sums and minima straight from the packed words (the only batch, queried through gl_depth_windows)
+    ctx.depth_begin(0, L)
+    ctx.depth_add_segments_packed8(a, d, ln)
+    ws, wm = ctx.depth_windows(500, es.size)
+    assert ctx.depth_last_path() == 3
+    assert np.array_equal(ws, es) and np.array_equal(wm, em)
     # an int32 batch of odd length first (the packed8 unpack realigns the store), then packed8 + packed16 batches; clipping
     h = s.size // 3 | 1
     a1, d1, l1 = capi.pack_segments8(s[h:2 * h], e[h:2 * h])
@@ -417,6 +423,22 @@ def test_packed8_streamed_upload(ctx):
     assert ctx.depth_last_path() in (1, 4)                     # unsorted anchors are rejected: the batch is unpacked, the general path takes it
     ea, ec = orc.class_runs(exp, 0, L, 4, 0, 0)
     assert np.array_equal(ws, orc.window_sums(exp, 0, L, 500)[0]) and np.array_equal(r0, ea) and np.array_equal(rc, ec)
+    # more runs than a fresh context's first run table holds (len/16 + 4096): every other base covered, one run per base.
+    # The region is rerun with a larger table from the words the streamed upload left on the device.
+    L3, W3 = 600_000, 500
+    s3 = np.arange(0, L3, 2, dtype=np.int32)
+    e3 = s3 + 1
+    a3, d3, l3 = capi.pack_segments8(s3, e3)
+    assert a3.size >= 4096
+    exp = orc.pileup_diff(s3, e3, 0, L3)
+    ea, ec = orc.class_runs(exp, 0, L3, 4, 0, 0)
+    assert ea.size > L3 // 16 + 4096
+    out = (np.empty((L3 - 1) // W3 + 1, np.int64), np.empty(L3, np.int32), np.empty(L3, np.uint8))
+    with capi.Ctx(0) as c3:
+        h3 = _pinned(c3, a3, d3, l3)
+        ws, r0, rc = c3.depth_region_packed8(0, L3, h3[0], h3[1], h3[2], W3, 4, 0, out=out)
+        assert c3.depth_last_path() == 3
+    assert np.array_equal(ws, orc.window_sums(exp, 0, L3, W3)[0]) and np.array_equal(r0, ea) and np.array_equal(rc, ec)
 
 
 def test_packed8_unsorted_anchors_fall_back(ctx):

@@ -2185,19 +2185,16 @@ int gl_depth_interval_sums(gl_ctx* ctx, const int32_t* a, const int32_t* b, int6
     long long* d_out = static_cast<long long*>(ctx->misc.p);
     int* d_a = reinterpret_cast<int*>(d_out + n);
     int* d_b = d_a + n;
-    int rc = GL_OK;
-    do {
-        if (cudaMemcpyAsync(d_a, a, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(d_b, b, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_depth_interval_sums: H2D failed"); break; }
-        {
-            gl_prof_scope prof(ctx, "depth_interval_sum_kernel");
-            depth_interval_sum_kernel<<<(unsigned)((n + 7) / 8), 256, 0, ctx->stream>>>(p, d_a, d_b, n, use_index ? 1 : 0, d_out);
-        }
-        ctx->launches++;
-        if (cudaMemcpyAsync(sums, d_out, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_depth_interval_sums: %s", cudaGetErrorString(cudaGetLastError())); break; }
-    } while (0);
-    return rc;
+    GL_CUDA(ctx, cudaMemcpyAsync(d_a, a, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    GL_CUDA(ctx, cudaMemcpyAsync(d_b, b, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    {
+        gl_prof_scope prof(ctx, "depth_interval_sum_kernel");
+        depth_interval_sum_kernel<<<(unsigned)((n + 7) / 8), 256, 0, ctx->stream>>>(p, d_a, d_b, n, use_index ? 1 : 0, d_out);
+    }
+    GL_LAUNCHED(ctx, 1);
+    GL_CUDA(ctx, cudaMemcpyAsync(sums, d_out, (size_t)n * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_depth_perbase(gl_ctx* ctx, int32_t* depth_out) {

@@ -89,29 +89,21 @@ int gl_fasta_stats(gl_ctx* ctx, const int64_t* byte_start, const int64_t* byte_e
     const size_t np = pa.size();
     std::vector<unsigned long long> host((size_t)n_rows * 4, 0ull);
     if (np) {
-        gl_buf bp, bc;
-        GL_CHECK(gl_buf_reserve(ctx, bp, np * 20));
-        if (gl_buf_reserve(ctx, bc, (size_t)n_rows * 32) != GL_OK) { cudaFree(bp.p); return GL_ENOMEM; }
-        long long* d_pa = static_cast<long long*>(bp.p);
-        long long* d_pb = d_pa + np;
-        int* d_row = reinterpret_cast<int*>(d_pb + np);
-        int rc = GL_OK;
-        do {
-            if (cudaMemcpyAsync(d_pa, pa.data(), np * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-                cudaMemcpyAsync(d_pb, pb.data(), np * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-                cudaMemcpyAsync(d_row, prow.data(), np * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-                cudaMemsetAsync(bc.p, 0, (size_t)n_rows * 32, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_fasta_stats: H2D failed"); break; }
-            {
-                gl_prof_scope prof(ctx, "fasta_stats_kernel");
-                fasta_stats_kernel<<<(unsigned)((np + 7) / 8), 256, 0, ctx->stream>>>(static_cast<const unsigned char*>(ctx->fasta.p), ctx->fasta_n, d_pa, d_pb,
-                                                                                  d_row, (long long)np, static_cast<unsigned long long*>(bc.p));
-            }
-            ctx->launches++;
-            if (cudaMemcpyAsync(host.data(), bc.p, (size_t)n_rows * 32, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-                cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_fasta_stats: %s", cudaGetErrorString(cudaGetLastError())); break; }
-        } while (0);
-        cudaFree(bp.p); cudaFree(bc.p);
-        if (rc != GL_OK) return rc;
+        gl_scratch tmp(ctx);
+        long long *d_pa, *d_pb; int* d_row; unsigned long long* d_counts;
+        GL_CHECK(tmp.upload(d_pa, pa.data(), np));
+        GL_CHECK(tmp.upload(d_pb, pb.data(), np));
+        GL_CHECK(tmp.upload(d_row, prow.data(), np));
+        GL_CHECK(tmp.alloc(d_counts, (size_t)n_rows * 4));
+        GL_CUDA(ctx, cudaMemsetAsync(d_counts, 0, (size_t)n_rows * 32, ctx->stream));
+        {
+            gl_prof_scope prof(ctx, "fasta_stats_kernel");
+            fasta_stats_kernel<<<(unsigned)((np + 7) / 8), 256, 0, ctx->stream>>>(static_cast<const unsigned char*>(ctx->fasta.p), ctx->fasta_n, d_pa, d_pb,
+                                                                              d_row, (long long)np, d_counts);
+        }
+        GL_LAUNCHED(ctx, 1);
+        GL_CUDA(ctx, cudaMemcpyAsync(host.data(), d_counts, (size_t)n_rows * 32, cudaMemcpyDeviceToHost, ctx->stream));
+        GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
     for (int64_t r = 0; r < n_rows; r++) {
         const unsigned long long gc = host[r * 4], lower = host[r * 4 + 1], tot = host[r * 4 + 2], cpg = host[r * 4 + 3];

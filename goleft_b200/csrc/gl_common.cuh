@@ -196,6 +196,36 @@ struct gl_prof_scope {
     ~gl_prof_scope() { if (b) cudaEventRecord(b, ctx->stream); }
 };
 
+// The device temporaries of one call that takes host arrays: each holds at least 16 bytes, and all are freed when the
+// scratch goes out of scope, so every return path frees them.  alloc fails with GL_ENOMEM, upload's copy with GL_ECUDA.
+// Library-internal: not exported from the .so.
+struct __attribute__((visibility("hidden"))) gl_scratch {
+    static constexpr int kMax = 8;
+    gl_ctx* ctx;
+    void* bufs[kMax] = {};
+    int n_bufs = 0;
+    explicit gl_scratch(gl_ctx* c) : ctx(c) {}
+    gl_scratch(const gl_scratch&) = delete;
+    gl_scratch& operator=(const gl_scratch&) = delete;
+    ~gl_scratch() { for (int i = 0; i < n_bufs; i++) cudaFree(bufs[i]); }
+    // d = room for n elements (null on failure)
+    template <class T> int alloc(T*& d, size_t n) {
+        d = nullptr;
+        if (n_bufs == kMax) return gl_fail(ctx, GL_EINVAL, "gl_scratch: more than %d buffers", kMax);
+        gl_buf b;
+        GL_CHECK(gl_buf_reserve(ctx, b, std::max<size_t>(n * sizeof(T), 16)));
+        bufs[n_bufs++] = b.p;
+        d = static_cast<T*>(b.p);
+        return GL_OK;
+    }
+    // d = a device copy of h[0..n), queued on ctx->stream
+    template <class T> int upload(T*& d, const T* h, size_t n) {
+        GL_CHECK(alloc(d, n));
+        if (n) GL_CUDA(ctx, cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+        return GL_OK;
+    }
+};
+
 static inline int gl_use(gl_ctx* ctx) {
     if (!ctx) return gl_fail(nullptr, GL_EINVAL, "null ctx");
     cudaError_t e = cudaSetDevice(ctx->device);

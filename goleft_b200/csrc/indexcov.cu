@@ -1,8 +1,10 @@
 // indexcov.cu — `goleft indexcov` arithmetic on sm_90a, plus the small covstats / depthwed kernels.
 //
-//   I1  ic_sizes_kernel     BAI linear-index virtual offsets -> per-tile sizes   (indexcov/types.go:45-82)
-//   I2+I3 ic_cohort_kernel  ONE kernel, one CTA per sample: capped weighted median by two range-adaptive
-//                           histogram selects over the sample's tiles (no sort), then normalised depth
+//   I1  ic_sizes_batch_kernel  BAI linear-index virtual offsets -> per-tile sizes, one warp per (sample, reference)
+//                                                                                      (indexcov/types.go:45-82)
+//   I2+I3 ic_cohort2_kernel ONE kernel, a CTA per sample: the 98th percentile and the capped weighted median, exactly, from
+//                           the brackets a sorted strided sample gives and one pass over the tiles (small samples: a full
+//                           sort; brackets that fail: a range-adaptive histogram select), then normalised depth
 //                                                                                      (indexcov.go:83-151)
 //   I4+I5 ic_counts_kernel  per (sample, chromosome) segment: 70-slot histogram + in/out/hi/low counters
 //                                                                            (indexcov.go:170-177,1050-1078)
@@ -22,27 +24,10 @@ namespace {
 
 constexpr unsigned kFull = 0xffffffffu;
 
-// ------------------------------------------------------------------------------------------------ I1
-__global__ void __launch_bounds__(256) ic_sizes_kernel(const unsigned long long* __restrict__ voff,
-                                                      const long long* __restrict__ ref_ptr,
-                                                      const long long* __restrict__ size_ptr, int n_refs,
-                                                      long long* __restrict__ sizes, int* __restrict__ neg_flag) {
-    const int r = blockIdx.x;
-    if (r >= n_refs) return;
-    const long long a = ref_ptr[r], b = ref_ptr[r + 1], o = size_ptr[r];
-    for (long long k = threadIdx.x; k + 1 < b - a; k += blockDim.x) {
-        const long long d = (long long)voff[a + k + 1] - (long long)voff[a + k];   // vOffset = File<<16|Block = raw u64
-        if (d < 0) *neg_flag = 1;
-        sizes[o + k] = d;
-    }
-}
-
 // ------------------------------------------------------------------------------------------------ I2 + I3
-constexpr int kCohortThreads = 512;
-
-// Selection without a sort.  Both selects of Index.init are "smallest value v with F(v) > target", where
-// F(v) = sum over x <= v of w(x):  w = 1 gives the k-th smallest (target = k), w = min(x, cap) gives the capped
-// weighted median (target = total/2).  The answer is bracketed by [lo,hi]; each level histograms the candidates
+// Selection without a sort: ic_cohort2_kernel's exact fallback.  Both selects of Index.init are "smallest value v with
+// F(v) > target", where F(v) = sum over x <= v of w(x):  w = 1 gives the k-th smallest (target = k), w = min(x, cap)
+// gives the capped weighted median (target = total/2).  The answer is bracketed by [lo,hi]; each level histograms the candidates
 // into kSelBins equal-width bins over the CURRENT range (not over radix digits: tile sizes of one sample share
 // their leading bytes, a digit histogram would put every shared-memory atomic on one bin), picks the bin where
 // the running weight crosses the target, and shrinks [lo,hi] to the min/max of that bin's members.  The width
@@ -113,62 +98,13 @@ __device__ long long block_select(const long long* __restrict__ v, long long n, 
         if (nlo > nhi) return lo;                          // cannot happen when F(max) > target; keeps the loop finite
         lo = nlo;
         hi = nhi;
-        if (kWeighted && lo < hi) {
-            // zero-weight members (x == 0) never move the running weight: with lo == 0 the crossing value is > 0
-        }
     }
     return lo;
 }
 
-__global__ void __launch_bounds__(kCohortThreads) ic_cohort_kernel(const long long* __restrict__ sizes,
-                                                                   const long long* __restrict__ sample_ptr, int S,
-                                                                   double* __restrict__ medians, float* __restrict__ depth_out) {
-    __shared__ SelSmem sm;
-    __shared__ long long s_red[kCohortThreads / 32];
-    const int smp = blockIdx.x;
-    if (smp >= S) return;
-    const long long a = sample_ptr[smp], n = sample_ptr[smp + 1] - a;
-    const long long* v = sizes + a;
-    if (n <= 0) { if (threadIdx.x == 0) medians[smp] = 0.0; return; }
-
-    long long vmin, vmax;
-    block_minmax(v, n, -0x7fffffffffffffffll - 1, 0x7fffffffffffffffll, 0, 0.0, -1, sm, vmin, vmax);
-
-    // n98 = sorted[int(0.98*n)]                                              (indexcov.go:111)
-    const long long k98 = (long long)(0.98 * (double)n);
-    const long long n98 = block_select<false>(v, n, 0, k98, vmin, vmax, sm);
-
-    // total = sum min(s, n98)                                                (:112-118)
-    long long part = 0;
-    for (long long i = threadIdx.x; i < n; i += blockDim.x) part += min(v[i], n98);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(kFull, part, o);
-    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = part;
-    __syncthreads();
-    long long total = 0;
-    for (int w = 0; w < kCohortThreads / 32; w++) total += s_red[w];
-    __syncthreads();
-
-    // first sorted position whose capped cumulative sum exceeds total/2      (:119-124).  When total == 0 the
-    // cumsum never exceeds 0: sort.Search returns len and the clamp picks the largest element.
-    const long long med = (total == 0) ? vmax : block_select<true>(v, n, n98, total / 2, vmin, vmax, sm);
-    const double dm = (double)med;
-    if (threadIdx.x == 0) medians[smp] = dm;
-
-    // depth = float32(float64(o)/median), capped at 50000                    (:129-151)
-    if (depth_out) {
-        float* out = depth_out + a;
-        for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-            float d = (med == 0) ? 0.0f : __double2float_rn(__ddiv_rn((double)v[i], dm));
-            if (d > 50000.0f) d = 50000.0f;
-            out[i] = d;
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------ I2 + I3, version 2
-// ic_cohort2_kernel: the same two order statistics, but the sample's tiles are streamed TWICE instead of ~17 times and no
-// shared-memory histogram (64-bit shared atomics are a CAS loop on sm_90) is involved:
+// ic_cohort2_kernel: the two order statistics of Index.init (indexcov.go:111-124).  The sample's tiles are streamed TWICE
+// instead of the ~17 times of the selects above, and no shared-memory histogram (64-bit shared atomics are a CAS loop on
+// sm_90) is involved:
 //   small samples (n <= 8192): all tiles sorted in shared memory (bitonic), Index.init done literally.
 //   large samples: a strided sample of 8192 tiles is sorted in shared memory; it brackets the 98th-percentile element
 //     (n98) and the capped weighted median (med) by VALUE:  [lo98, hi98] around sample rank 0.98 K (+-64 ranks, > 5 sigma)
@@ -898,9 +834,6 @@ __global__ void __launch_bounds__(256) indexsplit_sum_kernel(const long long* __
     out[out_ptr[r] + j] = acc;
 }
 
-// small helper: a scratch device buffer per call site
-int dev_tmp(gl_ctx* ctx, gl_buf& b, size_t bytes) { return gl_buf_reserve(ctx, b, bytes ? bytes : 16); }
-
 }  // namespace
 
 extern "C" {
@@ -909,41 +842,30 @@ int gl_indexcov_sizes(gl_ctx* ctx, const uint64_t* voff, const int64_t* ref_ptr,
                       int64_t* size_ptr) {
     GL_CHECK(gl_use(ctx));
     if (n_refs < 0 || !ref_ptr || !size_ptr || (n_refs > 0 && !voff)) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_sizes: bad argument");
+    std::vector<int64_t> voff_off, size_off;                       // one gl_indexcov_sizes_batch_device descriptor per
+    std::vector<int32_t> n_intv;                                   // reference with >= 2 entries
     size_ptr[0] = 0;
     for (int32_t r = 0; r < n_refs; r++) {
         const int64_t ni = ref_ptr[r + 1] - ref_ptr[r];
         if (ni < 0) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_sizes: ref_ptr not monotone");
+        if (ni > INT32_MAX) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_sizes: reference %d has more than %d entries", r, INT32_MAX);
         size_ptr[r + 1] = size_ptr[r] + (ni >= 2 ? ni - 1 : 0);     // types.go:68-72
+        if (ni >= 2) { voff_off.push_back(ref_ptr[r]); n_intv.push_back((int32_t)ni); size_off.push_back(size_ptr[r]); }
     }
     const int64_t total_v = ref_ptr[n_refs], total_s = size_ptr[n_refs];
     if (total_s == 0) return GL_OK;
     if (!sizes) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_sizes: null sizes");
-    gl_buf bv, bp, bs, bo;
-    const size_t pb = (size_t)(n_refs + 1) * 8;
-    GL_CHECK(dev_tmp(ctx, bv, (size_t)total_v * 8));
-    GL_CHECK(dev_tmp(ctx, bp, pb * 2 + 16));
-    GL_CHECK(dev_tmp(ctx, bs, (size_t)total_s * 8));
-    (void)bo;
-    char* dp = static_cast<char*>(bp.p);
-    int rc = GL_OK;
-    do {
-        if (cudaMemcpyAsync(bv.p, voff, (size_t)total_v * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(dp, ref_ptr, pb, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(dp + pb, size_ptr, pb, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemsetAsync(dp + 2 * pb, 0, 16, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_sizes: copy failed"); break; }
-        ic_sizes_kernel<<<(unsigned)n_refs, 256, 0, ctx->stream>>>(static_cast<const unsigned long long*>(bv.p),
-                                                                   reinterpret_cast<const long long*>(dp),
-                                                                   reinterpret_cast<const long long*>(dp + pb), n_refs,
-                                                                   static_cast<long long*>(bs.p), reinterpret_cast<int*>(dp + 2 * pb));
-        ctx->launches++;
-        int neg = 0;
-        if (cudaMemcpyAsync(sizes, bs.p, (size_t)total_s * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(&neg, dp + 2 * pb, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_sizes: %s", cudaGetErrorString(cudaGetLastError())); break; }
-        if (neg) rc = gl_fail(ctx, GL_ERANGE, "gl_indexcov_sizes: expected positive change in vOffset");   // types.go:75-77
-    } while (0);
-    cudaFree(bv.p); cudaFree(bp.p); cudaFree(bs.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    uint64_t* d_voff; int64_t *d_voff_off, *d_size_off, *d_sizes; int32_t* d_n_intv;
+    GL_CHECK(tmp.upload(d_voff, voff, (size_t)total_v));
+    GL_CHECK(tmp.upload(d_voff_off, voff_off.data(), voff_off.size()));
+    GL_CHECK(tmp.upload(d_n_intv, n_intv.data(), n_intv.size()));
+    GL_CHECK(tmp.upload(d_size_off, size_off.data(), size_off.size()));
+    GL_CHECK(tmp.alloc(d_sizes, (size_t)total_s));
+    GL_CHECK(gl_indexcov_sizes_batch_device(ctx, d_voff, d_voff_off, d_n_intv, d_size_off, (int64_t)n_intv.size(), d_sizes));
+    GL_CUDA(ctx, cudaMemcpyAsync(sizes, d_sizes, (size_t)total_s * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_indexcov_cohort_device(gl_ctx* ctx, const int64_t* d_sizes, const int64_t* d_sample_ptr, int32_t S,
@@ -951,19 +873,13 @@ int gl_indexcov_cohort_device(gl_ctx* ctx, const int64_t* d_sizes, const int64_t
     GL_CHECK(gl_use(ctx));
     if (S < 0 || !d_sizes || !d_sample_ptr || !d_medians) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_cohort_device: bad argument");
     if (S == 0) return GL_OK;
-    static const bool use_v1 = [] { const char* e = getenv("GL_COHORT_V1"); return e && atoi(e) != 0; }();
-    if (use_v1) {
-        gl_prof_scope prof(ctx, "ic_cohort_kernel");
-        ic_cohort_kernel<<<(unsigned)S, kCohortThreads, 0, ctx->stream>>>(reinterpret_cast<const long long*>(d_sizes),
-                                                                          reinterpret_cast<const long long*>(d_sample_ptr), S,
-                                                                          d_medians, d_depth_out);
-    } else {
-        if (!ctx->cohort_attr_set) {                          // per device (a function attribute belongs to the device it was set on)
-            GL_CUDA(ctx, cudaFuncSetAttribute(ic_cohort2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C2Smem)));
-            ctx->cohort_attr_set = true;
-        }
-        GL_CHECK(gl_buf_reserve(ctx, ctx->misc, 64));
-        GL_CUDA(ctx, cudaMemsetAsync(ctx->misc.p, 0, 4, ctx->stream));
+    if (!ctx->cohort_attr_set) {                              // per device (a function attribute belongs to the device it was set on)
+        GL_CUDA(ctx, cudaFuncSetAttribute(ic_cohort2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(C2Smem)));
+        ctx->cohort_attr_set = true;
+    }
+    GL_CHECK(gl_buf_reserve(ctx, ctx->misc, 64));
+    GL_CUDA(ctx, cudaMemsetAsync(ctx->misc.p, 0, 4, ctx->stream));
+    {
         gl_prof_scope prof(ctx, "ic_cohort2_kernel");
         const unsigned grid = (unsigned)std::min<int64_t>((int64_t)S, (int64_t)ctx->sm_count);
         ic_cohort2_kernel<<<grid, kC2Threads, sizeof(C2Smem), ctx->stream>>>(reinterpret_cast<const long long*>(d_sizes),
@@ -971,7 +887,7 @@ int gl_indexcov_cohort_device(gl_ctx* ctx, const int64_t* d_sizes, const int64_t
                                                                               d_depth_out, static_cast<unsigned*>(ctx->misc.p));
     }
     GL_LAUNCHED(ctx, 1);
-    if (!use_v1) GL_CUDA(ctx, cudaMemcpyAsync(&ctx->cohort_fallbacks, ctx->misc.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaMemcpyAsync(&ctx->cohort_fallbacks, ctx->misc.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return GL_OK;
 }
@@ -1013,24 +929,17 @@ int gl_indexcov_cohort(gl_ctx* ctx, const int64_t* sizes, const int64_t* sample_
     if (S == 0) return GL_OK;
     const int64_t total = sample_ptr[S];
     if (total > 0 && !sizes) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_cohort: null sizes");
-    gl_buf bs, bp, bm, bd;
-    GL_CHECK(dev_tmp(ctx, bs, (size_t)total * 8));
-    GL_CHECK(dev_tmp(ctx, bp, (size_t)(S + 1) * 8));
-    GL_CHECK(dev_tmp(ctx, bm, (size_t)S * 8));
-    if (depth_out) GL_CHECK(dev_tmp(ctx, bd, (size_t)total * 4));
-    int rc = GL_OK;
-    do {
-        if ((total && cudaMemcpyAsync(bs.p, sizes, (size_t)total * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) ||
-            cudaMemcpyAsync(bp.p, sample_ptr, (size_t)(S + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_cohort: H2D failed"); break; }
-        rc = gl_indexcov_cohort_device(ctx, static_cast<const int64_t*>(bs.p), static_cast<const int64_t*>(bp.p), S,
-                                       static_cast<double*>(bm.p), depth_out ? static_cast<float*>(bd.p) : nullptr);
-        if (rc != GL_OK) break;
-        if (cudaMemcpyAsync(medians, bm.p, (size_t)S * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            (depth_out && total && cudaMemcpyAsync(depth_out, bd.p, (size_t)total * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_cohort: D2H failed"); break; }
-    } while (0);
-    cudaFree(bs.p); cudaFree(bp.p); cudaFree(bm.p); if (bd.p) cudaFree(bd.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    int64_t *d_sizes, *d_ptr; double* d_med; float* d_depth = nullptr;
+    GL_CHECK(tmp.upload(d_sizes, sizes, (size_t)total));
+    GL_CHECK(tmp.upload(d_ptr, sample_ptr, (size_t)S + 1));
+    GL_CHECK(tmp.alloc(d_med, (size_t)S));
+    if (depth_out) GL_CHECK(tmp.alloc(d_depth, (size_t)total));
+    GL_CHECK(gl_indexcov_cohort_device(ctx, d_sizes, d_ptr, S, d_med, d_depth));
+    GL_CUDA(ctx, cudaMemcpyAsync(medians, d_med, (size_t)S * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (depth_out && total) GL_CUDA(ctx, cudaMemcpyAsync(depth_out, d_depth, (size_t)total * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_indexcov_scale(gl_ctx* ctx, const int64_t* sizes, int64_t n, int64_t* median_out) {
@@ -1047,19 +956,18 @@ int gl_indexcov_normalize(gl_ctx* ctx, const int64_t* sizes, int64_t n, double m
     if (n < 0 || (n > 0 && (!sizes || !depth_out))) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_normalize: bad argument");
     if (n == 0) return GL_OK;
     if (median == 0.0) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_normalize: median is 0 (the reference returns no depths, indexcov.go:140-142)");
-    gl_buf bs, bd;
-    GL_CHECK(dev_tmp(ctx, bs, (size_t)n * 8));
-    GL_CHECK(dev_tmp(ctx, bd, (size_t)n * 4));
-    int rc = GL_OK;
-    do {
-        if (cudaMemcpyAsync(bs.p, sizes, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "H2D failed"); break; }
-        ic_normalize_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(static_cast<const long long*>(bs.p), n, median, static_cast<float*>(bd.p));
-        ctx->launches++;
-        if (cudaMemcpyAsync(depth_out, bd.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_normalize: %s", cudaGetErrorString(cudaGetLastError())); break; }
-    } while (0);
-    cudaFree(bs.p); cudaFree(bd.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    int64_t* d_sizes; float* d_depth;
+    GL_CHECK(tmp.upload(d_sizes, sizes, (size_t)n));
+    GL_CHECK(tmp.alloc(d_depth, (size_t)n));
+    {
+        gl_prof_scope prof(ctx, "ic_normalize_kernel");
+        ic_normalize_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(reinterpret_cast<const long long*>(d_sizes), n, median, d_depth);
+    }
+    GL_LAUNCHED(ctx, 1);
+    GL_CUDA(ctx, cudaMemcpyAsync(depth_out, d_depth, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_indexcov_counts_batch_device(gl_ctx* ctx, const float* d_depth, const int64_t* d_seg_ptr, const int64_t* d_longest,
@@ -1102,27 +1010,18 @@ int gl_indexcov_counts_batch(gl_ctx* ctx, const float* depth, const int64_t* seg
     if (n_seg < 0 || !seg_ptr || !counts70 || !bins4) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_counts_batch: bad argument");
     if (n_seg == 0) return GL_OK;
     const int64_t total = seg_ptr[n_seg];
-    gl_buf bd, bp, bl, bc, bb;
-    GL_CHECK(dev_tmp(ctx, bd, (size_t)total * 4));
-    GL_CHECK(dev_tmp(ctx, bp, (size_t)(n_seg + 1) * 8));
-    GL_CHECK(dev_tmp(ctx, bl, (size_t)n_seg * 8));
-    GL_CHECK(dev_tmp(ctx, bc, (size_t)n_seg * GL_INDEXCOV_SLOTS * 4));
-    GL_CHECK(dev_tmp(ctx, bb, (size_t)n_seg * 32));
-    int rc = GL_OK;
-    do {
-        if ((total && cudaMemcpyAsync(bd.p, depth, (size_t)total * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) ||
-            cudaMemcpyAsync(bp.p, seg_ptr, (size_t)(n_seg + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            (longest && cudaMemcpyAsync(bl.p, longest, (size_t)n_seg * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess)) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_counts_batch: H2D failed"); break; }
-        rc = gl_indexcov_counts_batch_device(ctx, static_cast<const float*>(bd.p), static_cast<const int64_t*>(bp.p),
-                                             longest ? static_cast<const int64_t*>(bl.p) : nullptr, n_seg,
-                                             static_cast<int32_t*>(bc.p), static_cast<int64_t*>(bb.p));
-        if (rc != GL_OK) break;
-        if (cudaMemcpyAsync(counts70, bc.p, (size_t)n_seg * GL_INDEXCOV_SLOTS * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(bins4, bb.p, (size_t)n_seg * 32, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_counts_batch: D2H failed"); break; }
-    } while (0);
-    cudaFree(bd.p); cudaFree(bp.p); cudaFree(bl.p); cudaFree(bc.p); cudaFree(bb.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    float* d_depth; int64_t *d_ptr, *d_longest = nullptr, *d_bins; int32_t* d_counts;
+    GL_CHECK(tmp.upload(d_depth, depth, (size_t)total));
+    GL_CHECK(tmp.upload(d_ptr, seg_ptr, (size_t)n_seg + 1));
+    if (longest) GL_CHECK(tmp.upload(d_longest, longest, (size_t)n_seg));
+    GL_CHECK(tmp.alloc(d_counts, (size_t)n_seg * GL_INDEXCOV_SLOTS));
+    GL_CHECK(tmp.alloc(d_bins, (size_t)n_seg * 4));
+    GL_CHECK(gl_indexcov_counts_batch_device(ctx, d_depth, d_ptr, d_longest, n_seg, d_counts, d_bins));
+    GL_CUDA(ctx, cudaMemcpyAsync(counts70, d_counts, (size_t)n_seg * GL_INDEXCOV_SLOTS * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaMemcpyAsync(bins4, d_bins, (size_t)n_seg * 32, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_indexcov_counts(gl_ctx* ctx, const float* depth, int64_t n, int32_t counts[GL_INDEXCOV_SLOTS]) {
@@ -1154,20 +1053,18 @@ int gl_indexcov_xnorm(gl_ctx* ctx, float* depths, const int32_t* lens, int32_t S
         if (lens[i] < 0 || lens[i] > T) return gl_fail(ctx, GL_EINVAL, "gl_indexcov_xnorm: lens[%d] out of range", i);
         if (lens[i] > max_len) max_len = lens[i];
     }
-    gl_buf bd, bl;
-    GL_CHECK(dev_tmp(ctx, bd, (size_t)S * T * 4));
-    GL_CHECK(dev_tmp(ctx, bl, (size_t)S * 4));
-    int rc = GL_OK;
-    do {
-        if (cudaMemcpyAsync(bd.p, depths, (size_t)S * T * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(bl.p, lens, (size_t)S * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_xnorm: H2D failed"); break; }
-        ic_xnorm_kernel<<<1, kXnThreads, 0, ctx->stream>>>(static_cast<float*>(bd.p), static_cast<const int*>(bl.p), S, T, max_len);
-        ctx->launches++;
-        if (cudaMemcpyAsync(depths, bd.p, (size_t)S * T * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexcov_xnorm: %s", cudaGetErrorString(cudaGetLastError())); break; }
-    } while (0);
-    cudaFree(bd.p); cudaFree(bl.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    float* d_depths; int32_t* d_lens;
+    GL_CHECK(tmp.upload(d_depths, depths, (size_t)S * T));
+    GL_CHECK(tmp.upload(d_lens, lens, (size_t)S));
+    {
+        gl_prof_scope prof(ctx, "ic_xnorm_kernel");
+        ic_xnorm_kernel<<<1, kXnThreads, 0, ctx->stream>>>(d_depths, d_lens, S, T, max_len);
+    }
+    GL_LAUNCHED(ctx, 1);
+    GL_CUDA(ctx, cudaMemcpyAsync(depths, d_depths, (size_t)S * T * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_format_g3_device(gl_ctx* ctx, const float* d_vals, int64_t n, uint8_t* d_tokens) {
@@ -1187,19 +1084,14 @@ int gl_format_g3(gl_ctx* ctx, const float* vals, int64_t n, uint8_t* tokens) {
     GL_CHECK(gl_use(ctx));
     if (n < 0 || (n > 0 && (!vals || !tokens))) return gl_fail(ctx, GL_EINVAL, "gl_format_g3: bad argument");
     if (n == 0) return GL_OK;
-    gl_buf bv, bt;
-    GL_CHECK(dev_tmp(ctx, bv, (size_t)n * 4));
-    GL_CHECK(dev_tmp(ctx, bt, (size_t)n * 10));
-    int rc = GL_OK;
-    do {
-        if (cudaMemcpyAsync(bv.p, vals, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_format_g3: H2D failed"); break; }
-        rc = gl_format_g3_device(ctx, static_cast<const float*>(bv.p), n, static_cast<uint8_t*>(bt.p));
-        if (rc != GL_OK) break;
-        if (cudaMemcpyAsync(tokens, bt.p, (size_t)n * 10, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_format_g3: D2H failed"); break; }
-    } while (0);
-    cudaFree(bv.p); cudaFree(bt.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    float* d_vals; uint8_t* d_tokens;
+    GL_CHECK(tmp.upload(d_vals, vals, (size_t)n));
+    GL_CHECK(tmp.alloc(d_tokens, (size_t)n * 10));
+    GL_CHECK(gl_format_g3_device(ctx, d_vals, n, d_tokens));
+    GL_CUDA(ctx, cudaMemcpyAsync(tokens, d_tokens, (size_t)n * 10, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_indexsplit_accumulate(gl_ctx* ctx, const int64_t* sizes, const int64_t* ptr, int32_t S, int32_t R, const int64_t* out_ptr, double* out) {
@@ -1221,49 +1113,44 @@ int gl_indexsplit_accumulate(gl_ctx* ctx, const int64_t* sizes, const int64_t* p
             if (a < 0 || b < a || b > n_in || b - a > out_ptr[r + 1] - out_ptr[r]) return gl_fail(ctx, GL_EINVAL, "gl_indexsplit_accumulate: ptr out of range (sample %d, ref %d)", s, r);
         }
     if (R > 65535) return gl_fail(ctx, GL_ERANGE, "gl_indexsplit_accumulate: more than 65535 references");
-    gl_buf bs, bp, bo, bq;
-    int rc = GL_OK;
-    do {
-        if (dev_tmp(ctx, bs, (size_t)n_in * 8) != GL_OK || dev_tmp(ctx, bp, (size_t)std::max(S, 1) * (R + 1) * 8) != GL_OK ||
-            dev_tmp(ctx, bo, (size_t)n_out * 8) != GL_OK || dev_tmp(ctx, bq, (size_t)(R + 1) * 8) != GL_OK) { rc = GL_ENOMEM; break; }
-        if ((n_in && cudaMemcpyAsync(bs.p, sizes, (size_t)n_in * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) ||
-            (S && cudaMemcpyAsync(bp.p, ptr, (size_t)S * (R + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) ||
-            cudaMemcpyAsync(bq.p, out_ptr, (size_t)(R + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexsplit_accumulate: H2D failed"); break; }
-        {
-            gl_prof_scope prof(ctx, "indexsplit_sum_kernel");
-            indexsplit_sum_kernel<<<dim3((unsigned)((max_len + 255) / 256), (unsigned)R), 256, 0, ctx->stream>>>(
-                static_cast<const long long*>(bs.p), static_cast<const long long*>(bp.p), S, R, static_cast<const long long*>(bq.p), static_cast<double*>(bo.p));
-        }
-        ctx->launches++;
-        if (cudaMemcpyAsync(out, bo.p, (size_t)n_out * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_indexsplit_accumulate: %s", cudaGetErrorString(cudaGetLastError())); break; }
-    } while (0);
-    cudaFree(bs.p); cudaFree(bp.p); cudaFree(bo.p); cudaFree(bq.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    int64_t *d_sizes, *d_ptr, *d_out_ptr; double* d_out;
+    GL_CHECK(tmp.upload(d_sizes, sizes, (size_t)n_in));
+    GL_CHECK(tmp.upload(d_ptr, ptr, (size_t)S * (R + 1)));
+    GL_CHECK(tmp.upload(d_out_ptr, out_ptr, (size_t)R + 1));
+    GL_CHECK(tmp.alloc(d_out, (size_t)n_out));
+    {
+        gl_prof_scope prof(ctx, "indexsplit_sum_kernel");
+        indexsplit_sum_kernel<<<dim3((unsigned)((max_len + 255) / 256), (unsigned)R), 256, 0, ctx->stream>>>(
+            reinterpret_cast<const long long*>(d_sizes), reinterpret_cast<const long long*>(d_ptr), S, R,
+            reinterpret_cast<const long long*>(d_out_ptr), d_out);
+    }
+    GL_LAUNCHED(ctx, 1);
+    GL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)n_out * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 int gl_bincount_i32(gl_ctx* ctx, const int32_t* v, int64_t n, int32_t lo, int32_t hi, uint64_t* hist) {
     GL_CHECK(gl_use(ctx));
     if (n < 0 || hi <= lo || !hist || (n > 0 && !v)) return gl_fail(ctx, GL_EINVAL, "gl_bincount_i32: bad argument");
     const int64_t nb = (int64_t)hi - lo;
-    gl_buf bv, bh;
-    GL_CHECK(dev_tmp(ctx, bv, (size_t)n * 4));
-    GL_CHECK(dev_tmp(ctx, bh, (size_t)nb * 8));
-    int rc = GL_OK;
-    do {
-        if ((n && cudaMemcpyAsync(bv.p, v, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) ||
-            cudaMemsetAsync(bh.p, 0, (size_t)nb * 8, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_bincount_i32: H2D failed"); break; }
-        if (n) {
-            const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
+    gl_scratch tmp(ctx);
+    int32_t* d_v; unsigned long long* d_hist;
+    GL_CHECK(tmp.upload(d_v, v, (size_t)n));
+    GL_CHECK(tmp.alloc(d_hist, (size_t)nb));
+    GL_CUDA(ctx, cudaMemsetAsync(d_hist, 0, (size_t)nb * 8, ctx->stream));
+    if (n) {
+        const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
+        {
             gl_prof_scope prof(ctx, "bincount_kernel");
-            bincount_kernel<<<grid, 256, 0, ctx->stream>>>(static_cast<const int*>(bv.p), n, lo, hi, static_cast<unsigned long long*>(bh.p));
-            ctx->launches++;
+            bincount_kernel<<<grid, 256, 0, ctx->stream>>>(d_v, n, lo, hi, d_hist);
         }
-        if (cudaMemcpyAsync(hist, bh.p, (size_t)nb * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_bincount_i32: %s", cudaGetErrorString(cudaGetLastError())); break; }
-    } while (0);
-    cudaFree(bv.p); cudaFree(bh.p);
-    return rc;
+        GL_LAUNCHED(ctx, 1);
+    }
+    GL_CUDA(ctx, cudaMemcpyAsync(hist, d_hist, (size_t)nb * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 // groups of consecutive rows per output line (depthwed.go:117-157): sequential in the row order, O(R) on the host
@@ -1356,26 +1243,20 @@ int gl_depthwed_aggregate_i32(gl_ctx* ctx, const int32_t* depth, int32_t S, int6
         out_end[g] = ends[grp[g + 1] - 1];
         out_chrom[g] = chrom_id[grp[g]];
     }
-    gl_buf bm, bg, bo, bf;
-    GL_CHECK(dev_tmp(ctx, bm, (size_t)S * R * 4));
-    GL_CHECK(dev_tmp(ctx, bg, (size_t)(ng + 1) * 8));
-    GL_CHECK(dev_tmp(ctx, bo, (size_t)ng * S * 4));
-    GL_CHECK(dev_tmp(ctx, bf, 16));
-    int rc = GL_OK, ovf = 0;
-    do {
-        if (cudaMemcpyAsync(bm.p, depth, (size_t)S * R * 4, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(bg.p, grp.data(), (size_t)(ng + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemsetAsync(bf.p, 0, 4, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_depthwed_aggregate_i32: H2D failed"); break; }
-        rc = gl_depthwed_aggregate_i32_device(ctx, static_cast<const int32_t*>(bm.p), S, R, static_cast<const int64_t*>(bg.p), 0, ng,
-                                              static_cast<int32_t*>(bo.p), static_cast<int32_t*>(bf.p));
-        if (rc != GL_OK) break;
-        if (cudaMemcpyAsync(out, bo.p, (size_t)ng * S * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(&ovf, bf.p, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_depthwed_aggregate_i32: D2H failed"); break; }
-    } while (0);
-    cudaFree(bm.p); cudaFree(bg.p); cudaFree(bo.p); cudaFree(bf.p);
-    if (rc == GL_OK && ovf) { *n_out = -1; return gl_fail(ctx, GL_ERANGE, "gl_depthwed_aggregate_i32: a group sum does not fit int32"); }
-    return rc;
+    gl_scratch tmp(ctx);
+    int32_t *d_depth, *d_out, *d_ovf; int64_t* d_grp;
+    GL_CHECK(tmp.upload(d_depth, depth, (size_t)S * R));
+    GL_CHECK(tmp.upload(d_grp, grp.data(), (size_t)ng + 1));
+    GL_CHECK(tmp.alloc(d_out, (size_t)ng * S));
+    GL_CHECK(tmp.alloc(d_ovf, 1));
+    GL_CUDA(ctx, cudaMemsetAsync(d_ovf, 0, 4, ctx->stream));
+    GL_CHECK(gl_depthwed_aggregate_i32_device(ctx, d_depth, S, R, d_grp, 0, ng, d_out, d_ovf));
+    int ovf = 0;
+    GL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)ng * S * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaMemcpyAsync(&ovf, d_ovf, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (ovf) { *n_out = -1; return gl_fail(ctx, GL_ERANGE, "gl_depthwed_aggregate_i32: a group sum does not fit int32"); }
+    return GL_OK;
 }
 
 int gl_depthwed_aggregate(gl_ctx* ctx, const double* means, int32_t S, int64_t R, const int32_t* starts, const int32_t* ends,
@@ -1394,21 +1275,15 @@ int gl_depthwed_aggregate(gl_ctx* ctx, const double* means, int32_t S, int64_t R
         out_end[g] = ends[grp[g + 1] - 1];
         out_chrom[g] = chrom_id[grp[g]];
     }
-    gl_buf bm, bg, bo;
-    GL_CHECK(dev_tmp(ctx, bm, (size_t)S * R * 8));
-    GL_CHECK(dev_tmp(ctx, bg, (size_t)(ng + 1) * 8));
-    GL_CHECK(dev_tmp(ctx, bo, (size_t)ng * S * 8));
-    int rc = GL_OK;
-    do {
-        if (cudaMemcpyAsync(bm.p, means, (size_t)S * R * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(bg.p, grp.data(), (size_t)(ng + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_depthwed_aggregate: H2D failed"); break; }
-        rc = gl_depthwed_aggregate_device(ctx, static_cast<const double*>(bm.p), S, R, static_cast<const int64_t*>(bg.p), ng, static_cast<int64_t*>(bo.p));
-        if (rc != GL_OK) break;
-        if (cudaMemcpyAsync(out, bo.p, (size_t)ng * S * 8, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
-            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { rc = gl_fail(ctx, GL_ECUDA, "gl_depthwed_aggregate: D2H failed"); break; }
-    } while (0);
-    cudaFree(bm.p); cudaFree(bg.p); cudaFree(bo.p);
-    return rc;
+    gl_scratch tmp(ctx);
+    double* d_means; int64_t *d_grp, *d_out;
+    GL_CHECK(tmp.upload(d_means, means, (size_t)S * R));
+    GL_CHECK(tmp.upload(d_grp, grp.data(), (size_t)ng + 1));
+    GL_CHECK(tmp.alloc(d_out, (size_t)ng * S));
+    GL_CHECK(gl_depthwed_aggregate_device(ctx, d_means, S, R, d_grp, ng, d_out));
+    GL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)ng * S * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
 }
 
 }  // extern "C"

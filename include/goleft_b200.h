@@ -371,7 +371,9 @@ int  gl_indexcov_sizes(gl_ctx* ctx, const uint64_t* voff, const int64_t* ref_ptr
 int  gl_indexcov_scale(gl_ctx* ctx, const int64_t* sizes, int64_t n, int64_t* median_out);
 /* I3: depth[i] = min(float32(float64(sizes[i])/median), 50000). */
 int  gl_indexcov_normalize(gl_ctx* ctx, const int64_t* sizes, int64_t n, double median, float* depth_out);
-/* I2+I3 for a cohort in one kernel (one CTA per sample, radix selects instead of a sort):
+/* I2+I3 for a cohort in one kernel (a CTA per sample): the two order statistics are bracketed by a sorted strided
+ * sample of the tiles and read off the few tiles inside the brackets after one pass (samples of <= 8192 tiles are sorted
+ * whole; when a bracket fails, an exact histogram select takes over), then a second pass writes the depths.
  * S samples, tile sizes in CSR layout (sample_ptr, S+1); medians[S]; depths in the same layout
  * (depth_out may be NULL).  A sample with median 0 gets zero depths (the reference returns none). */
 int  gl_indexcov_cohort(gl_ctx* ctx, const int64_t* sizes, const int64_t* sample_ptr, int32_t S,

@@ -111,8 +111,10 @@ def test_cohort_large_samples_bracketed_path_and_fallbacks(ctx):
 def test_sizes_batch_equals_per_sample(ctx):
     rng = np.random.default_rng(15)
     voffs, voff_off, n_intv, size_off, exp = [], [], [], [], []
+    samples = []                                                # (voff, ref_ptr, sizes, size_ptr) of each sample alone
     at = so = 0
     for s in range(7):
+        first = len(voffs)
         for r in range(int(rng.integers(1, 30))):
             k = int(rng.choice([0, 1, 2, 3, 50, 4000]))
             v = np.cumsum(rng.integers(0, 1 << 30, k)).astype(np.uint64)
@@ -122,8 +124,26 @@ def test_sizes_batch_equals_per_sample(ctx):
                 exp.append(np.diff(v.astype(np.int64)))
                 so += k - 1
             at += k
+        refs = voffs[first:]
+        ref_ptr = np.concatenate([[0], np.cumsum([v.size for v in refs])]).astype(np.int64)
+        size_ptr = np.concatenate([[0], np.cumsum([max(v.size - 1, 0) for v in refs])]).astype(np.int64)
+        samples.append((np.concatenate(refs), ref_ptr, np.concatenate([np.diff(v.astype(np.int64)) for v in refs]), size_ptr))
     got = ctx.indexcov_sizes_batch(np.concatenate(voffs), voff_off, n_intv, size_off, so)
     assert np.array_equal(got, np.concatenate(exp))
+    # the per-sample entry gives the same sizes and offsets
+    for voff, ref_ptr, sizes, size_ptr in samples:
+        got_s, got_p = ctx.indexcov_sizes(voff, ref_ptr)
+        assert np.array_equal(got_s, sizes) and np.array_equal(got_p, size_ptr)
+    # one negative delta inside a middle reference of a many-reference sample: the reference panics (types.go:75-77)
+    voff, ref_ptr, _, _ = max(samples, key=lambda t: t[1].size)
+    mid = [r for r in range(1, ref_ptr.size - 2) if ref_ptr[r + 1] - ref_ptr[r] >= 2]
+    r = mid[len(mid) // 2]
+    k = int(ref_ptr[r] + (ref_ptr[r + 1] - ref_ptr[r]) // 2)    # ref_ptr[r] < k < ref_ptr[r + 1]
+    bad = voff.copy()
+    bad[k - 1] = bad[k] + np.uint64(1)
+    with pytest.raises(capi.GlError) as ei:
+        ctx.indexcov_sizes(bad, ref_ptr)
+    assert ei.value.code == capi.GL_ERANGE
 
 
 def test_counts_batch(ctx):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Device-resident throughput of the cohort-scale kernels on one H100 (BASELINE configs 3 and 4 at 1-GPU shard size):
-  indexcov: S samples x T tiles -> per-sample capped weighted median + normalised depth (ic_cohort_kernel)
+  indexcov: S samples x T tiles -> per-sample capped weighted median + normalised depth (ic_cohort2_kernel)
   depthwed: S samples x R windows of float64 means -> int matrix, row-major (depthwed_kernel)
 Prints one JSON object; CUDA-event timing on the ctx stream, L2 flushed before every repetition."""
 import argparse
@@ -57,8 +57,7 @@ def main():
     out["indexcov_cohort"] = {"samples": S, "tiles": T, "ms": float(np.mean(ms)), "tile_samples_per_s": S * T / (np.mean(ms) * 1e-3),
                               "alg_bytes": alg, "achieved_gbs": alg / (np.mean(ms) * 1e-3) / 1e9,
                               "frac_of_measured_peak": alg / (np.mean(ms) * 1e-3) / 1e9 / peak,
-                              "kernel": "ic_cohort_kernel (v1: range-adaptive histogram selects, ~17 passes)" if os.environ.get("GL_COHORT_V1") else
-                                        "ic_cohort2_kernel (sorted-sample brackets: one counting/collecting pass + one normalise pass)",
+                              "kernel": "ic_cohort2_kernel (sorted-sample brackets: one counting/collecting pass + one normalise pass)",
                               "fallback_samples": fallbacks,
                               "cpu_port_ms_per_sample_1thread": cpu_per_sample * 1e3}
     for b in (d_sizes, d_ptr, d_med, d_dep):

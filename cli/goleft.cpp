@@ -155,6 +155,128 @@ static bool chrom_start_end(const std::string& line, std::string& chrom, long lo
     return false;
 }
 
+// ------------------------------------------------------------------------------------------------ shared by the subcommands
+static gl_ctx* open_ctx(int device, const char* prog) {
+    gl_ctx* ctx = nullptr;
+    if (gl_ctx_create(device, &ctx) != GL_OK) fatal(1, "%s: %s", prog, gl_last_error(nullptr));
+    return ctx;
+}
+
+// --gpus: 0, or more than the visible devices, means one worker per device.  GL_OVERSUBSCRIBE (a testing aid) keeps the
+// asked-for count on fewer devices: worker g runs on device g % n_dev.  There are never more workers than units of work.
+struct GpuPlan { int G, n_dev; };
+static GpuPlan resolve_gpus(const std::string& flag, size_t units, const char* prog) {
+    int n_dev = 0;
+    if (gl_device_count(&n_dev) != GL_OK || n_dev < 1) fatal(1, "%s: %s", prog, gl_last_error(nullptr));
+    int G = atoi(flag.c_str());
+    if (G <= 0 || (G > n_dev && !getenv("GL_OVERSUBSCRIBE"))) G = n_dev;
+    G = (int)std::min<size_t>((size_t)G, std::max<size_t>(units, 1));
+    return {G, n_dev};
+}
+
+// One host thread per worker, running fn(g).  With several GPUs each thread is bound to the NUMA node of its device; the
+// host pool is created first, so that it keeps every core.
+static std::vector<std::thread> start_workers(const GpuPlan& p, const std::function<void(int)>& fn) {
+    glhost_pool_warm();
+    std::vector<std::thread> th;
+    for (int g = 0; g < p.G; g++)
+        th.emplace_back([p, fn, g] {
+            int node = -1, ncpu = 0;
+            if (p.G > 1) gl_bind_numa_for_device(g % p.n_dev, 0, 1, &node, &ncpu);
+            fn(g);
+        });
+    return th;
+}
+
+// the index of an input (indexcov.go:500-510): x.bam.bai, else x.bai; a .bai names itself
+static std::string bai_path(const std::string& b) {
+    std::string p = ends_with(b, ".bai") ? b : b + ".bai";
+    if (!file_exists(p)) p = b.substr(0, b.size() - 4) + (ends_with(b, ".bai") ? "" : ".bai");
+    return p;
+}
+
+// CRAM pseudo-tile sizes of every reference of a .crai (crai.go:56-127), concatenated; ref_ptr[r] is where reference r's begin
+static void crai_sizes(const std::vector<glhts::CraiSlices>& cr, std::vector<int64_t>& sizes, std::vector<int64_t>& ref_ptr) {
+    sizes.clear();
+    ref_ptr.assign(cr.size() + 1, 0);
+    for (size_t r = 0; r < cr.size(); r++) {
+        std::vector<int64_t> one;
+        if (!glhts::crai_make_sizes(cr[r].start.data(), cr[r].span.data(), cr[r].bytes.data(), (int64_t)cr[r].start.size(), one))
+            fatal(2, "panic: tilewidth logic error");
+        sizes.insert(sizes.end(), one.begin(), one.end());
+        ref_ptr[r + 1] = (int64_t)sizes.size();
+    }
+}
+
+// One reference's segments, in the form they came in: packed8 words or int32 sorted by start from the host feeder (`host`),
+// the GPU feeder's int32 arrays left on the device, or a host int32 view of a whole-file decode (or of any arrays the caller
+// keeps alive).  Every int32 form is (s, e, n); packed8 words are read from `host`.
+struct SegSource {
+    glhts::ContigSegs host;
+    const int32_t* s = nullptr; const int32_t* e = nullptr; int64_t n = 0;
+    bool on_device = false;
+    const glhts::SegmentSet* whole = nullptr;       // set for a BAM without a usable index: fetch views its decode, per tid
+
+    // GL_GPU_FEED=0 keeps every decode on the host feeder
+    static bool gpu_feed() {
+        static const bool on = [] { const char* v = getenv("GL_GPU_FEED"); return !v || atoi(v) != 0; }();
+        return on;
+    }
+
+    void view(const int32_t* vs, const int32_t* ve, int64_t vn) {
+        host = glhts::ContigSegs();
+        s = vs; e = ve; n = vn; on_device = false;
+    }
+
+    // the segments of reference tid (-1: not in the BAM, none) that can overlap [beg,end).  want: 0 auto, 32 int32.
+    // whole_ref = the complete reference is wanted: the GPU feeder (BGZF inflate + record parse on the device, only compressed
+    // bytes over PCIe) takes it when it can and GL_GPU_FEED allows; otherwise the host feeder decodes.  The decode's
+    // statistics are added to *st, and a GPU-fed decode counts in *gpu_fed (both may be null).
+    void fetch(gl_ctx* ctx, gl_bam& bam, int tid, long long beg, long long end, int Q, int threads, int want, bool whole_ref,
+               glhts::DecodeStats* st, int* gpu_fed) {
+        view(nullptr, nullptr, 0);
+        if (tid < 0) return;
+        if (whole) {
+            const std::vector<int32_t>& ws = whole->start[(size_t)tid];
+            view(ws.data(), whole->end[(size_t)tid].data(), (int64_t)ws.size());
+            return;
+        }
+        glhts::DecodeStats one;
+        if (whole_ref && gpu_feed()) {
+            gl_bam_segments g;
+            const int rc = gl_bam_decode_device(ctx, &bam, tid, Q, &s, &e, &n, &g);
+            if (rc == GL_OK) {
+                on_device = true;
+                one.wall_s = g.wall_s; one.inflate_s = g.inflate_s; one.parse_s = g.parse_s;
+                one.n_records = g.n_records; one.bytes_in = g.bytes_in; one.bytes_out = g.bytes_out;
+                if (gpu_fed) ++*gpu_fed;
+            } else {
+                view(nullptr, nullptr, 0);
+                if (rc != GL_ESTATE) glck(ctx, rc, "gl_bam_decode_device");    // GL_ESTATE: not possible on the device for this reference
+            }
+        }
+        if (!on_device) {
+            std::string err = bam.f.decode(tid, beg, end, Q, threads, want, host, &one);
+            if (!err.empty()) fatal(1, "%s", err.c_str());
+            if (host.format == 32) { s = host.start.data(); e = host.end.data(); n = host.n; }
+        }
+        if (st) {
+            st->wall_s += one.wall_s; st->inflate_s += one.inflate_s; st->parse_s += one.parse_s;
+            st->n_records += one.n_records; st->bytes_in += one.bytes_in; st->bytes_out += one.bytes_out;
+        }
+    }
+
+    void add(gl_ctx* ctx) const {
+        if (host.format == 8) {
+            if (host.n_blocks > 0)
+                glck(ctx, gl_depth_add_segments_packed8(ctx, host.anchors.data(), host.ds.data(), host.len.data(), host.n_blocks), "gl_depth_add_segments_packed8");
+        } else if (n > 0) {
+            if (on_device) glck(ctx, gl_depth_add_segments_device(ctx, s, e, n), "gl_depth_add_segments_device");
+            else glck(ctx, gl_depth_add_segments(ctx, s, e, n), "gl_depth_add_segments");
+        }
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ depth
 // `goleft depth`: depth/depth.go:103-159 builds the work list (10 Mb chunks of every .fai contig, or the BED lines), runs one
 // `samtools depth -r` child per entry and concatenates the per-chunk BED files (-o: in order).  Here the unit of work is a
@@ -177,8 +299,8 @@ struct DepthJob {                                   // one contig (.fai mode) or
     long long len = 0;                              // .fai mode: contig length
     std::vector<size_t> lines;                      // BED mode: indices into the region list
     std::string hd, ca;                             // .fai mode output
-    double decode_s = 0, gpu_s = 0, inflate_s = 0, parse_s = 0;
-    long long records = 0, bytes_in = 0, bytes_out = 0;
+    glhts::DecodeStats dec;                         // summed over the job's decodes
+    double gpu_s = 0;
     int gpu_fed = 0;                                // passes whose segments came from the GPU feeder
     bool done = false;
 };
@@ -200,11 +322,9 @@ struct DepthEngine {
     DepthShared& sh;
     const DepthOpts& o;
     gl_ctx* ctx = nullptr;
-    gl_bam gbam;                                            // the library's BAM handle: its BamFile is the host feeder,
-    glhts::BamFile& bam = gbam.f;                           // gl_bam_decode_device runs the feeder on the GPU
+    gl_bam gbam;                                            // the library's BAM handle (host and GPU feeder)
     std::map<std::string, int> tid_of;
-    glhts::ContigSegs segs;
-    const int32_t* dev_s = nullptr; const int32_t* dev_e = nullptr; int64_t dev_n = -1;   // segments left on the device by the GPU feeder (-1: none)
+    SegSource src;
     std::vector<int64_t> sums; std::vector<int32_t> rstart; std::vector<uint8_t> rclass;
     std::vector<char> tbuf_hd, tbuf_ca;
     // --stats state (depth.go:191-200,246-252): chunks of a contig are parked, one gl_fasta_stats launch for all their rows
@@ -213,63 +333,25 @@ struct DepthEngine {
     std::vector<int64_t> row_s, row_e;
 
     DepthEngine(DepthShared& s, int device) : sh(s), o(*s.opt) {
-        if (gl_ctx_create(device, &ctx) != GL_OK) fatal(1, "goleft depth: %s", gl_last_error(nullptr));
-        if (!sh.preload) {
-            std::string e = bam.open(sh.bam_path);
-            if (!e.empty()) fatal(1, "%s", e.c_str());
-            for (size_t i = 0; i < bam.header.refs.size(); i++) tid_of[bam.header.refs[i].name] = (int)i;
+        ctx = open_ctx(device, "goleft depth");
+        if (sh.preload) {
+            src.whole = sh.preload;
         } else {
-            for (size_t i = 0; i < sh.preload->header.refs.size(); i++) tid_of[sh.preload->header.refs[i].name] = (int)i;
+            std::string e = gbam.f.open(sh.bam_path);
+            if (!e.empty()) fatal(1, "%s", e.c_str());
         }
+        const glhts::BamHeader& hdr = sh.preload ? sh.preload->header : gbam.f.header;
+        for (size_t i = 0; i < hdr.refs.size(); i++) tid_of[hdr.refs[i].name] = (int)i;
         rstart.resize(1 << 16); rclass.resize(1 << 16);
     }
     ~DepthEngine() { gl_ctx_destroy(ctx); }
 
-    // segments of [beg,end) of a contig into `segs` (packed8 or sorted int32); want: 0 auto, 32 int32.
-    // whole = the complete reference is wanted: the GPU feeder (BGZF inflate + record parse on the device, only compressed
-    // bytes over PCIe) takes it when it can; GL_GPU_FEED=0 keeps everything on the host feeder.
-    void fetch(const std::string& c, long long beg, long long end, int want, DepthJob* job, bool whole = false) {
-        segs = glhts::ContigSegs();
-        dev_n = -1;
-        auto it = tid_of.find(c);
-        if (it == tid_of.end()) return;
-        static const bool gpu_feed = [] { const char* e = getenv("GL_GPU_FEED"); return !e || atoi(e) != 0; }();
-        if (whole && gpu_feed && !sh.preload) {
-            gl_bam_segments st;
-            const int rc = gl_bam_decode_device(ctx, &gbam, it->second, o.Q, &dev_s, &dev_e, &dev_n, &st);
-            if (rc == GL_OK) {
-                if (job) { job->decode_s += st.wall_s; job->inflate_s += st.inflate_s; job->parse_s += st.parse_s; job->records += st.n_records;
-                           job->bytes_in += st.bytes_in; job->bytes_out += st.bytes_out; job->gpu_fed++; }
-                return;
-            }
-            dev_n = -1;
-            if (rc != GL_ESTATE) glck(ctx, rc, "gl_bam_decode_device");      // GL_ESTATE: not possible on the device for this reference
-        }
-        if (sh.preload) {                                              // unindexed BAM: slices of the preloaded arrays (record order)
-            const std::vector<int32_t>& S = sh.preload->start[(size_t)it->second];
-            const std::vector<int32_t>& E = sh.preload->end[(size_t)it->second];
-            segs.format = S.empty() ? 0 : 32;
-            segs.start = S; segs.end = E; segs.n = (int64_t)S.size();
-            return;
-        }
-        glhts::DecodeStats st;
-        std::string e = bam.decode(it->second, beg, end, o.Q, o.threads, want, segs, &st);
-        if (!e.empty()) fatal(1, "%s", e.c_str());
-        if (job) { job->decode_s += st.wall_s; job->inflate_s += st.inflate_s; job->parse_s += st.parse_s; job->records += st.n_records; job->bytes_in += st.bytes_in; job->bytes_out += st.bytes_out; }
-    }
-
-    void add_segments() {
-        if (dev_n >= 0) { if (dev_n > 0) glck(ctx, gl_depth_add_segments_device(ctx, dev_s, dev_e, dev_n), "gl_depth_add_segments_device"); return; }
-        if (segs.format == 8 && segs.n_blocks > 0)
-            glck(ctx, gl_depth_add_segments_packed8(ctx, segs.anchors.data(), segs.ds.data(), segs.len.data(), segs.n_blocks), "gl_depth_add_segments_packed8");
-        else if (segs.format == 32 && segs.n > 0)
-            glck(ctx, gl_depth_add_segments(ctx, segs.start.data(), segs.end.data(), segs.n), "gl_depth_add_segments");
-    }
+    int tid(const std::string& c) const { auto it = tid_of.find(c); return it == tid_of.end() ? -1 : it->second; }
 
     // window sums + class runs of [rs,re) on the host (the --stats and BED paths)
-    void reduce_to_host(long long rs, long long re, long long run_break, int64_t& nw, int64_t& nr) {
+    void reduce_to_host(const SegSource& segs, long long rs, long long re, long long run_break, int64_t& nw, int64_t& nr) {
         glck(ctx, gl_depth_begin(ctx, rs, re), "gl_depth_begin");
-        add_segments();
+        segs.add(ctx);
         glck(ctx, gl_depth_reduce(ctx, o.W, o.mincov, o.maxmean, run_break), "gl_depth_reduce");
         int32_t md = 0;
         glck(ctx, gl_depth_result_sizes(ctx, &nw, &nr, &md), "gl_depth_result_sizes");
@@ -332,56 +414,52 @@ struct DepthEngine {
         pending.clear(); row_s.clear(); row_e.clear();
     }
 
+    // BED text of [ps,pe) made on the device by call(depth_bed, cap, &len, callable_bed, cap, &len), appended to the job.  The
+    // buffers start at gl_depth_text_bound's size; a call that reports GL_ERANGE has set the lengths it needs and runs once more.
+    template <class Call> void device_text(DepthJob& job, long long ps, long long pe, const char* what, Call call) {
+        const int64_t nwin = (pe - 1) / o.W - ps / o.W + 1;
+        const size_t need_hd = (size_t)gl_depth_text_bound(job.chrom.c_str(), nwin);
+        if (tbuf_hd.size() < need_hd) tbuf_hd.resize(need_hd);
+        if (tbuf_ca.size() < (size_t)(1 << 20)) tbuf_ca.resize(1 << 20);
+        int64_t hl = 0, cl = 0;
+        int rc = call(tbuf_hd.data(), (int64_t)tbuf_hd.size(), &hl, tbuf_ca.data(), (int64_t)tbuf_ca.size(), &cl);
+        if (rc == GL_ERANGE) {
+            tbuf_hd.resize((size_t)hl + 16); tbuf_ca.resize((size_t)cl + 16);
+            rc = call(tbuf_hd.data(), (int64_t)tbuf_hd.size(), &hl, tbuf_ca.data(), (int64_t)tbuf_ca.size(), &cl);
+        }
+        glck(ctx, rc, what);
+        job.hd.append(tbuf_hd.data(), (size_t)hl);
+        job.ca.append(tbuf_ca.data(), (size_t)cl);
+    }
+
     // ---- .fai mode: one contig.  The GPU pass covers at most 2^30-1 bases; longer contigs go in whole-chunk pieces
     //      whose texts concatenate (chunk edges are run breaks anyway).
     void run_contig(DepthJob& job) {
         const long long kMaxPass = ((1LL << 30) - 1) / o.step * o.step;
-        const double t_all = now_s();
+        const char* c = job.chrom.c_str();
         for (long long ps = 0; ps < job.len; ps += kMaxPass) {
             const long long pe = std::min(job.len, ps + kMaxPass);
-            fetch(job.chrom, ps, pe, 0, &job, ps == 0 && pe == job.len);
+            src.fetch(ctx, gbam, tid(job.chrom), ps, pe, o.Q, o.threads, 0, ps == 0 && pe == job.len, &job.dec, &job.gpu_fed);
             const double tg = now_s();
-            const bool device_text = !o.stats && job.chrom.size() <= 64;
-            if (device_text && dev_n >= 0) {                                   // segments already on the device (GPU feeder)
-                const int64_t nwin = (pe - 1) / o.W - ps / o.W + 1;
-                const size_t need_hd = (size_t)gl_depth_text_bound(job.chrom.c_str(), nwin);
-                if (tbuf_hd.size() < need_hd) tbuf_hd.resize(need_hd);
-                if (tbuf_ca.size() < (size_t)(1 << 20)) tbuf_ca.resize(1 << 20);
+            const bool dtext = !o.stats && job.chrom.size() <= 64;
+            if (dtext && src.on_device) {                                      // segments already on the device (GPU feeder)
                 glck(ctx, gl_depth_begin(ctx, ps, pe), "gl_depth_begin");
-                add_segments();
+                src.add(ctx);
                 glck(ctx, gl_depth_reduce(ctx, o.W, o.mincov, o.maxmean, o.step), "gl_depth_reduce");
-                int64_t hl = 0, cl = 0;
-                int rc = gl_depth_text(ctx, job.chrom.c_str(), tbuf_hd.data(), (int64_t)tbuf_hd.size(), &hl, tbuf_ca.data(), (int64_t)tbuf_ca.size(), &cl);
-                if (rc == GL_ERANGE) {
-                    tbuf_hd.resize((size_t)hl + 16); tbuf_ca.resize((size_t)cl + 16);
-                    rc = gl_depth_text(ctx, job.chrom.c_str(), tbuf_hd.data(), (int64_t)tbuf_hd.size(), &hl, tbuf_ca.data(), (int64_t)tbuf_ca.size(), &cl);
-                }
-                glck(ctx, rc, "gl_depth_text");
-                job.hd.append(tbuf_hd.data(), (size_t)hl);
-                job.ca.append(tbuf_ca.data(), (size_t)cl);
-            } else if (device_text) {
-                const int64_t nwin = (pe - 1) / o.W - ps / o.W + 1;
-                const size_t need_hd = (size_t)gl_depth_text_bound(job.chrom.c_str(), nwin);
-                if (tbuf_hd.size() < need_hd) tbuf_hd.resize(need_hd);
-                if (tbuf_ca.size() < (size_t)(1 << 20)) tbuf_ca.resize(1 << 20);
-                int64_t hl = 0, cl = 0;
-                for (int attempt = 0; attempt < 2; attempt++) {
-                    int rc;
-                    if (segs.format == 8)
-                        rc = gl_depth_bed_region_packed8(ctx, job.chrom.c_str(), ps, pe, segs.anchors.data(), segs.ds.data(), segs.len.data(), segs.n_blocks, o.W,
-                                                         o.mincov, o.maxmean, o.step, tbuf_hd.data(), (int64_t)tbuf_hd.size(), &hl, tbuf_ca.data(), (int64_t)tbuf_ca.size(), &cl);
-                    else
-                        rc = gl_depth_bed_region(ctx, job.chrom.c_str(), ps, pe, segs.start.data(), segs.end.data(), segs.n, o.W, o.mincov, o.maxmean, o.step,
-                                                 o.threads, tbuf_hd.data(), (int64_t)tbuf_hd.size(), &hl, tbuf_ca.data(), (int64_t)tbuf_ca.size(), &cl);
-                    if (rc == GL_ERANGE && attempt == 0) { tbuf_hd.resize((size_t)hl + 16); tbuf_ca.resize((size_t)cl + 16); continue; }
-                    glck(ctx, rc, "gl_depth_bed_region");
-                    break;
-                }
-                job.hd.append(tbuf_hd.data(), (size_t)hl);
-                job.ca.append(tbuf_ca.data(), (size_t)cl);
+                device_text(job, ps, pe, "gl_depth_text", [&](char* hd, int64_t hc, int64_t* hl, char* ca, int64_t cc, int64_t* cl) {
+                    return gl_depth_text(ctx, c, hd, hc, hl, ca, cc, cl);
+                });
+            } else if (dtext) {                                                // host segments: the library picks the transport
+                device_text(job, ps, pe, "gl_depth_bed_region", [&](char* hd, int64_t hc, int64_t* hl, char* ca, int64_t cc, int64_t* cl) {
+                    const glhts::ContigSegs& h = src.host;
+                    if (h.format == 8)
+                        return gl_depth_bed_region_packed8(ctx, c, ps, pe, h.anchors.data(), h.ds.data(), h.len.data(), h.n_blocks, o.W, o.mincov,
+                                                           o.maxmean, o.step, hd, hc, hl, ca, cc, cl);
+                    return gl_depth_bed_region(ctx, c, ps, pe, src.s, src.e, src.n, o.W, o.mincov, o.maxmean, o.step, o.threads, hd, hc, hl, ca, cc, cl);
+                });
             } else {
                 int64_t nw = 0, nr = 0;
-                reduce_to_host(ps, pe, o.step, nw, nr);
+                reduce_to_host(src, ps, pe, o.step, nw, nr);
                 for (long long cs = ps; cs < pe; cs += o.step) {
                     const long long ce = std::min(cs + o.step, pe);
                     const int32_t* lo = std::lower_bound(rstart.data(), rstart.data() + nr, (int32_t)cs);
@@ -393,7 +471,6 @@ struct DepthEngine {
             }
             job.gpu_s += now_s() - tg;
         }
-        (void)t_all;
     }
 
     // ---- BED mode: the lines of one contig.  One pass over the span they cover (window sums + class runs, run_break 0),
@@ -406,7 +483,7 @@ struct DepthEngine {
         long long lo = regions[ks[0]].s, hi = regions[ks[0]].e;
         for (size_t k : ks) { lo = std::min(lo, regions[k].s); hi = std::max(hi, regions[k].e); }
         const long long span_s = lo / W * W;
-        fetch(job.chrom, span_s, hi, 32, &job);                               // sorted int32: the interval sums and the per-line slices want arrays
+        src.fetch(ctx, gbam, tid(job.chrom), span_s, hi, o.Q, o.threads, 32, false, &job.dec, &job.gpu_fed);   // int32: the interval sums and the per-line slices want arrays
         const double tg = now_s();
         int64_t nw = 0, nr = 0;
         auto format_one = [&](size_t k, const int64_t* ws, int64_t nw_, const int32_t* rs_, const uint8_t* rc_, int64_t nr_) {
@@ -414,28 +491,24 @@ struct DepthEngine {
         };
         bool batched = ks.size() > 1 && hi - span_s < (1LL << 30) - 2 * (long long)W;
         if (batched) {
-            reduce_to_host(span_s, hi, 0, nw, nr);
+            reduce_to_host(src, span_s, hi, 0, nw, nr);
             int32_t path = 0;
-            batched = gl_depth_last_path(ctx, &path) == GL_OK && (path == 1 || segs.n == 0);   // the interval sums want the fused path's cell index
+            batched = gl_depth_last_path(ctx, &path) == GL_OK && (path == 1 || src.n == 0);   // the interval sums want the fused path's cell index
         }
         if (!batched) {
             // per-line passes over the slice of segments that can reach the line (the arrays are sorted by start)
-            glhts::ContigSegs all;
-            all.start.swap(segs.start); all.end.swap(segs.end); all.n = segs.n; all.format = segs.format; all.max_len = segs.max_len;
-            const int32_t maxlen = std::max<int32_t>(all.max_len, 1);
+            const int32_t maxlen = std::max<int32_t>(src.host.max_len, 1);
             const bool sorted = !sh.preload;                                   // the index-guided decoder sorts; preloaded arrays are in record order
+            SegSource line;
             for (size_t k : ks) {
                 if (regions[k].e - regions[k].s >= (1LL << 30)) fatal(1, "BED region longer than 2^30-1 bases: %s", regions[k].chrom.c_str());
-                size_t a = 0, b = (size_t)all.n;
-                if (sorted && all.n > 0) {
-                    a = (size_t)(std::lower_bound(all.start.begin(), all.start.end(), (int32_t)std::max<long long>(regions[k].s - maxlen, INT32_MIN)) - all.start.begin());
-                    b = (size_t)(std::lower_bound(all.start.begin(), all.start.end(), (int32_t)std::min<long long>(regions[k].e, INT32_MAX)) - all.start.begin());
+                int64_t a = 0, b = src.n;
+                if (sorted && src.n > 0) {
+                    a = std::lower_bound(src.s, src.s + src.n, (int32_t)std::max<long long>(regions[k].s - maxlen, INT32_MIN)) - src.s;
+                    b = std::lower_bound(src.s, src.s + src.n, (int32_t)std::min<long long>(regions[k].e, INT32_MAX)) - src.s;
                 }
-                segs.format = b > a ? 32 : 0;
-                segs.start.assign(all.start.begin() + (long)a, all.start.begin() + (long)b);
-                segs.end.assign(all.end.begin() + (long)a, all.end.begin() + (long)b);
-                segs.n = (int64_t)(b - a);
-                reduce_to_host(regions[k].s, regions[k].e, 0, nw, nr);
+                line.view(src.s + a, src.e + a, b - a);
+                reduce_to_host(line, regions[k].s, regions[k].e, 0, nw, nr);
                 format_one(k, sums.data(), nw, rstart.data(), rclass.data(), nr);
             }
             flush_stats();
@@ -581,32 +654,22 @@ static int cmd_depth(int argc, char** argv) {
     if (!fca || !fhd) fatal(1, "cannot create output files with prefix %s", prefix.c_str());
 
     // ---- GPUs and placement
-    int n_dev = 0;
-    if (gl_device_count(&n_dev) != GL_OK || n_dev < 1) fatal(1, "goleft depth: %s", gl_last_error(nullptr));
-    int G = atoi(gpus.c_str());
-    const bool oversub = getenv("GL_OVERSUBSCRIBE") != nullptr;               // testing aid: --gpus N workers on fewer devices (worker g -> device g % n_dev)
-    if (G <= 0 || (G > n_dev && !oversub)) G = n_dev;
-    G = (int)std::min<size_t>((size_t)G, std::max<size_t>(jobs.size(), 1));
+    const GpuPlan gp = resolve_gpus(gpus, jobs.size(), "goleft depth");
     std::vector<int32_t> gpu_of(jobs.size(), 0);
     {
         std::vector<int64_t> wts(jobs.size());
         for (size_t i = 0; i < jobs.size(); i++) wts[i] = jobs[i].len;
-        if (!jobs.empty() && gl_lpt_assign(wts.data(), (int32_t)jobs.size(), G, gpu_of.data(), nullptr) != GL_OK) fatal(1, "gl_lpt_assign failed");
+        if (!jobs.empty() && gl_lpt_assign(wts.data(), (int32_t)jobs.size(), gp.G, gpu_of.data(), nullptr) != GL_OK) fatal(1, "gl_lpt_assign failed");
     }
-    auto worker = [&](int g) {
-        int node = -1, ncpu = 0;
-        if (G > 1) gl_bind_numa_for_device(g % n_dev, 0, 1, &node, &ncpu);    // this feeder thread next to its GPU (the pool keeps all cores)
-        DepthEngine eng(sh, g % n_dev);
+    std::vector<std::thread> th = start_workers(gp, [&](int g) {
+        DepthEngine eng(sh, g % gp.n_dev);
         for (size_t i = 0; i < jobs.size(); i++) {
             if (gpu_of[i] != g) continue;
             if (bed.empty()) eng.run_contig(jobs[i]); else eng.run_bed_chrom(jobs[i]);
             { std::lock_guard<std::mutex> lk(sh.mu); jobs[i].done = true; }
             sh.cv.notify_all();
         }
-    };
-    glhost_pool_warm();                                                       // create the host pool before the feeder threads narrow their affinity
-    std::vector<std::thread> th;
-    for (int g = 0; g < G; g++) th.emplace_back(worker, g);
+    });
     // ---- ordered output as the jobs finish
     if (bed.empty()) {
         for (size_t i = 0; i < jobs.size(); i++) {
@@ -627,11 +690,14 @@ static int cmd_depth(int argc, char** argv) {
     if (sh.fa_map) munmap(const_cast<uint8_t*>(sh.fa_map), sh.fa_len);
     if (timing) {
         double dec = 0, gpu = 0, inf = 0, par = 0; long long rec = 0, bin = 0, bout = 0; int fed = 0;
-        for (const DepthJob& j : jobs) { fed += j.gpu_fed; dec += j.decode_s; gpu += j.gpu_s; inf += j.inflate_s; par += j.parse_s; rec += j.records; bin += j.bytes_in; bout += j.bytes_out; }
+        for (const DepthJob& j : jobs) {
+            fed += j.gpu_fed; gpu += j.gpu_s;
+            dec += j.dec.wall_s; inf += j.dec.inflate_s; par += j.dec.parse_s; rec += j.dec.n_records; bin += j.dec.bytes_in; bout += j.dec.bytes_out;
+        }
         fprintf(stderr, "{\"goleft_depth_timing\": {\"wall_s\": %.4f, \"gpus\": %d, \"jobs\": %zu, \"decode_wall_s_sum\": %.4f, \"gpu_call_s_sum\": %.4f, "
                         "\"inflate_thread_s_sum\": %.4f, \"parse_thread_s_sum\": %.4f, "
                         "\"records\": %lld, \"bgzf_bytes_in\": %lld, \"bgzf_bytes_out\": %lld, \"host_threads\": %d, \"gpu_fed_passes\": %d}}\n",
-                now_s() - t_start, G, jobs.size(), dec, gpu, inf, par, rec, bin, bout, glhost_pool_size(), fed);
+                now_s() - t_start, gp.G, jobs.size(), dec, gpu, inf, par, rec, bin, bout, glhost_pool_size(), fed);
     }
     return 0;
 }
@@ -692,6 +758,27 @@ template <class T> struct RawBuf {                          // malloc'ed, uninit
     void resize(size_t m) { free(p); p = static_cast<T*>(malloc(std::max<size_t>(m, 1) * sizeof(T))); n = m; if (!p) fatal(1, "out of memory (%zu bytes)", m * sizeof(T)); }
     T* data() { return p; }
     T& operator[](size_t i) { return p[i]; }
+};
+
+// device buffers of one ctx, freed together when the owner goes out of scope
+struct DevBufs {
+    gl_ctx* ctx;
+    std::vector<void*> ptrs;
+    explicit DevBufs(gl_ctx* c = nullptr) : ctx(c) {}
+    DevBufs(const DevBufs&) = delete;
+    DevBufs& operator=(const DevBufs&) = delete;
+    ~DevBufs() { for (void* p : ptrs) gl_dev_free(ctx, p); }
+    template <class T> T* alloc(size_t n) {
+        void* p = nullptr;
+        glck(ctx, gl_dev_alloc(ctx, (int64_t)std::max<size_t>(n * sizeof(T), 16), &p), "gl_dev_alloc");
+        ptrs.push_back(p);
+        return static_cast<T*>(p);
+    }
+    template <class T> T* upload(const T* h, size_t n) {
+        T* d = alloc<T>(n);
+        if (n) glck(ctx, gl_memcpy_h2d(ctx, d, h, (int64_t)(n * sizeof(T))), "gl_memcpy_h2d");
+        return d;
+    }
 };
 
 static int cmd_indexcov(int argc, char** argv) {
@@ -755,9 +842,7 @@ static int cmd_indexcov(int argc, char** argv) {
             names[i] = short_name(b, true, nullptr);
             return;
         }
-        std::string p = ends_with(b, ".bai") ? b : b + ".bai";
-        if (!file_exists(p)) p = b.substr(0, b.size() - 4) + (ends_with(b, ".bai") ? "" : ".bai");
-        read_err[i] = glhts::bai_read(p, idx[i]);
+        read_err[i] = glhts::bai_read(bai_path(b), idx[i]);
         if (!read_err[i].empty()) return;
         if (ends_with(b, ".bai")) names[i] = short_name(b, true, nullptr);
         else { glhts::BamHeader h; read_err[i] = glhts::bam_read_header(b, h); if (read_err[i].empty()) names[i] = short_name(b, false, &h); }
@@ -767,11 +852,8 @@ static int cmd_indexcov(int argc, char** argv) {
     ic_mark("read indexes");
     // ---- GPUs (SURVEY 8(e): samples are independent through I5 -> sample-sharded over the GPUs; the rows need every sample
     //      of a tile, and they are assembled on the host, so the "gather" is each GPU's D2H into its slice of the cohort arrays)
-    int n_dev = 0;
-    if (gl_device_count(&n_dev) != GL_OK || n_dev < 1) fatal(1, "goleft indexcov: %s", gl_last_error(nullptr));
-    int G = atoi(gpus.c_str());
-    const bool oversub = getenv("GL_OVERSUBSCRIBE") != nullptr;               // testing aid: --gpus N shards on fewer devices (shard g -> device g % n_dev)
-    if (G <= 0 || (G > n_dev && !oversub)) G = n_dev;
+    const GpuPlan gp = resolve_gpus(gpus, S, "goleft indexcov");
+    const int G = gp.G;
     fprintf(stderr, "indexcov: running on %zu indexes\n", bams.size());
 
     // ---- I1 for the whole cohort (indexcov/types.go:45-82): every sample's linear-index offsets go up once, one descriptor per
@@ -783,24 +865,14 @@ static int cmd_indexcov(int argc, char** argv) {
     std::vector<int64_t> desc_voff, desc_size;
     std::vector<int32_t> desc_n;
     std::vector<size_t> desc_begin(S + 1, 0), voff_begin(S + 1, 0);         // per sample: its first descriptor / first offset
-    std::vector<std::vector<int64_t>> crai_sizes(S);                        // CRAM samples: the values themselves
+    std::vector<std::vector<int64_t>> crai_tiles(S);                        // CRAM samples: the sizes themselves
     for (size_t i = 0; i < S; i++) {
         const int64_t base = sample_ptr.back();
         desc_begin[i] = desc_n.size(); voff_begin[i] = voff_all.size();
-        if (ends_with(bams[i], ".crai")) {                                  // CRAM: interpolated pseudo-tiles (crai.go:56-127)
-            const size_t nr = crai[i].size();
-            std::vector<int64_t> sp(nr + 1, 0), all;
-            for (size_t r = 0; r < nr; r++) {
-                std::vector<int64_t> one;
-                if (!glhts::crai_make_sizes(crai[i][r].start.data(), crai[i][r].span.data(), crai[i][r].bytes.data(),
-                                            (int64_t)crai[i][r].start.size(), one)) fatal(2, "panic: tilewidth logic error");
-                all.insert(all.end(), one.begin(), one.end());
-                sp[r + 1] = sp[r] + (int64_t)one.size();
-            }
-            if (sp[nr] < 1) fatal(1, "indexcov: no usable chromsomes in bam: %s", bams[i].c_str());
-            sample_ptr.push_back(base + sp[nr]);
-            crai_sizes[i] = std::move(all);
-            size_ptr[i] = sp;
+        if (ends_with(bams[i], ".crai")) {                                  // CRAM: interpolated pseudo-tiles
+            crai_sizes(crai[i], crai_tiles[i], size_ptr[i]);
+            if (size_ptr[i].back() < 1) fatal(1, "indexcov: no usable chromsomes in bam: %s", bams[i].c_str());
+            sample_ptr.push_back(base + size_ptr[i].back());
             continue;
         }
         const size_t nr = idx[i].ioffsets.size();
@@ -820,7 +892,6 @@ static int cmd_indexcov(int argc, char** argv) {
     }
     desc_begin[S] = desc_n.size(); voff_begin[S] = voff_all.size();
     const int64_t total = sample_ptr.back();
-    G = (int)std::min<size_t>((size_t)G, S);
     // contiguous sample ranges with about total/G tiles each
     std::vector<size_t> cut((size_t)G + 1, S);
     cut[0] = 0;
@@ -854,66 +925,61 @@ static int cmd_indexcov(int argc, char** argv) {
 
     std::vector<gl_ctx*> ctxs((size_t)G, nullptr);
     // phase A (per GPU, its samples): I1 + I2 + I3 on the device, medians + depths home; the depths stay resident for phase B
-    struct Shard { int64_t* d_sizes = nullptr; float* d_dep = nullptr; int64_t tiles = 0; };
+    struct Shard { DevBufs resident; float* d_dep = nullptr; int64_t tiles = 0; };
     std::vector<Shard> shard((size_t)G);
+    // a single GPU's work runs on this thread: on a worker thread the row assembly below, which reads what the D2H copies
+    // wrote, took about 0.3 s longer for 313 samples
     auto run_on_gpus = [&](const std::function<void(int)>& fn) {
-        if (G == 1) { fn(0); return; }
-        std::vector<std::thread> th;
-        for (int g = 0; g < G; g++) th.emplace_back([&, g] { int node = -1, ncpu = 0; gl_bind_numa_for_device(g % n_dev, 0, 1, &node, &ncpu); fn(g); });
-        for (auto& t : th) t.join();
+        if (G == 1) fn(0);
+        else for (std::thread& t : start_workers(gp, fn)) t.join();
     };
-    glhost_pool_warm();
     ic_mark("host arrays");
     std::vector<std::array<double, 4>> gpu_t((size_t)G);                     // per GPU: ctx, upload + I1, I2 + I3, D2H
     run_on_gpus([&](int g) {
-        gl_ctx* c = nullptr;
         double tg0 = now_s();
-        if (gl_ctx_create(g % n_dev, &c) != GL_OK) fatal(1, "goleft indexcov: %s", gl_last_error(nullptr));
+        gl_ctx* c = open_ctx(g % gp.n_dev, "goleft indexcov");
         ctxs[(size_t)g] = c;
         gpu_t[(size_t)g] = {now_s() - tg0, 0, 0, 0};
         tg0 = now_s();
         const size_t a = cut[(size_t)g], b = cut[(size_t)g + 1];
         const int64_t t0 = sample_ptr[a], tiles = sample_ptr[b] - t0;
         Shard& sd = shard[(size_t)g];
+        sd.resident.ctx = c;
         sd.tiles = tiles;
         if (b == a) return;
-        auto dalloc = [&](size_t bytes) { void* p = nullptr; glck(c, gl_dev_alloc(c, (int64_t)std::max<size_t>(bytes, 16), &p), "gl_dev_alloc"); return p; };
-        auto up = [&](const void* h, size_t bytes) { void* p = dalloc(bytes); if (bytes) glck(c, gl_memcpy_h2d(c, p, h, (int64_t)bytes), "gl_memcpy_h2d"); return p; };
-        sd.d_sizes = static_cast<int64_t*>(dalloc((size_t)tiles * 8));
+        DevBufs tmp(c);
+        int64_t* d_sizes = tmp.alloc<int64_t>((size_t)tiles);
         const size_t d0 = desc_begin[a], d1 = desc_begin[b], v0 = voff_begin[a], v1 = voff_begin[b];
         if (d1 > d0) {
             std::vector<int64_t> dv(desc_voff.begin() + (long)d0, desc_voff.begin() + (long)d1), ds(desc_size.begin() + (long)d0, desc_size.begin() + (long)d1);
             for (auto& x : dv) x -= (int64_t)v0;
             for (auto& x : ds) x -= t0;
-            void* d_voff = up(voff_all.data() + v0, (v1 - v0) * 8);
-            void* d_dv = up(dv.data(), dv.size() * 8);
-            void* d_dn = up(desc_n.data() + d0, (d1 - d0) * 4);
-            void* d_ds = up(ds.data(), ds.size() * 8);
-            const int rc = gl_indexcov_sizes_batch_device(c, static_cast<const uint64_t*>(d_voff), static_cast<const int64_t*>(d_dv),
-                                                          static_cast<const int32_t*>(d_dn), static_cast<const int64_t*>(d_ds), (int64_t)(d1 - d0), sd.d_sizes);
+            DevBufs in(c);
+            const uint64_t* d_voff = in.upload(voff_all.data() + v0, v1 - v0);
+            const int64_t* d_dv = in.upload(dv.data(), dv.size());
+            const int32_t* d_dn = in.upload(desc_n.data() + d0, d1 - d0);
+            const int64_t* d_ds = in.upload(ds.data(), ds.size());
+            const int rc = gl_indexcov_sizes_batch_device(c, d_voff, d_dv, d_dn, d_ds, (int64_t)(d1 - d0), d_sizes);
             if (rc == GL_ERANGE) fatal(2, "panic: expected positive change in vOffset");                 // types.go:75-77
             glck(c, rc, "gl_indexcov_sizes_batch_device");
-            gl_dev_free(c, d_voff); gl_dev_free(c, d_dv); gl_dev_free(c, d_dn); gl_dev_free(c, d_ds);
         }
         for (size_t i = a; i < b; i++)
-            if (!crai_sizes[i].empty())
-                glck(c, gl_memcpy_h2d(c, sd.d_sizes + (sample_ptr[i] - t0), crai_sizes[i].data(), (int64_t)crai_sizes[i].size() * 8), "gl_memcpy_h2d");
+            if (!crai_tiles[i].empty())
+                glck(c, gl_memcpy_h2d(c, d_sizes + (sample_ptr[i] - t0), crai_tiles[i].data(), (int64_t)crai_tiles[i].size() * 8), "gl_memcpy_h2d");
         glck(c, gl_sync(c), "gl_sync");
         gpu_t[(size_t)g][1] = now_s() - tg0; tg0 = now_s();
         // I2+I3 for the shard in one kernel, on the resident sizes (indexcov.go:83-151)
         std::vector<int64_t> sp(sample_ptr.begin() + (long)a, sample_ptr.begin() + (long)b + 1);
         for (auto& x : sp) x -= t0;
-        void* d_sp = up(sp.data(), sp.size() * 8);
-        double* d_med = static_cast<double*>(dalloc((b - a) * 8));
-        sd.d_dep = static_cast<float*>(dalloc((size_t)tiles * 4));
-        glck(c, gl_indexcov_cohort_device(c, sd.d_sizes, static_cast<const int64_t*>(d_sp), (int32_t)(b - a), d_med, sd.d_dep), "gl_indexcov_cohort_device");
+        const int64_t* d_sp = tmp.upload(sp.data(), sp.size());
+        double* d_med = tmp.alloc<double>(b - a);
+        sd.d_dep = sd.resident.alloc<float>((size_t)tiles);
+        glck(c, gl_indexcov_cohort_device(c, d_sizes, d_sp, (int32_t)(b - a), d_med, sd.d_dep), "gl_indexcov_cohort_device");
         glck(c, gl_sync(c), "gl_sync");
         gpu_t[(size_t)g][2] = now_s() - tg0; tg0 = now_s();
         glck(c, gl_memcpy_d2h(c, med.data() + a, d_med, (int64_t)(b - a) * 8), "gl_memcpy_d2h");
         glck(c, gl_memcpy_d2h(c, dep.data() + t0, sd.d_dep, tiles * 4), "gl_memcpy_d2h");
         gpu_t[(size_t)g][3] = now_s() - tg0;
-        gl_dev_free(c, sd.d_sizes); gl_dev_free(c, d_sp); gl_dev_free(c, d_med);
-        sd.d_sizes = nullptr;
     });
     std::vector<uint64_t>().swap(voff_all);
     if (ic_timing)
@@ -943,12 +1009,12 @@ static int cmd_indexcov(int argc, char** argv) {
             Shard& sd = shard[(size_t)g];
             if (Sg == 0) return;
             const int64_t t0 = sample_ptr[a], tiles = sd.tiles;
-            auto dalloc = [&](size_t bytes) { void* p = nullptr; glck(c, gl_dev_alloc(c, (int64_t)std::max<size_t>(bytes, 16), &p), "gl_dev_alloc"); return p; };
-            auto up = [&](const void* h, size_t bytes) { void* p = dalloc(bytes); if (bytes) glck(c, gl_memcpy_h2d(c, p, h, (int64_t)bytes), "gl_memcpy_h2d"); return p; };
-            uint8_t* d_tok = static_cast<uint8_t*>(dalloc((size_t)tiles * 10));
-            if (tiles) glck(c, gl_format_g3_device(c, sd.d_dep, tiles, d_tok), "gl_format_g3_device");
-            if (tiles) glck(c, gl_memcpy_d2h(c, tok_all.data() + (size_t)t0 * 10, d_tok, tiles * 10), "gl_memcpy_d2h");
-            gl_dev_free(c, d_tok);
+            {
+                DevBufs tmp(c);
+                uint8_t* d_tok = tmp.alloc<uint8_t>((size_t)tiles * 10);
+                if (tiles) glck(c, gl_format_g3_device(c, sd.d_dep, tiles, d_tok), "gl_format_g3_device");
+                if (tiles) glck(c, gl_memcpy_d2h(c, tok_all.data() + (size_t)t0 * 10, d_tok, tiles * 10), "gl_memcpy_d2h");
+            }
             const size_t nseg = nq * Sg;
             if (nseg) {
                 std::vector<int64_t> seg_start(nseg, 0), seg_len(nseg, 0), seg_longest(nseg, 0);
@@ -961,13 +1027,13 @@ static int cmd_indexcov(int argc, char** argv) {
                         }
                         seg_longest[j] = longest_q[q];
                     }
-                void* d_ss = up(seg_start.data(), nseg * 8);
-                void* d_sl = up(seg_len.data(), nseg * 8);
-                void* d_lg = up(seg_longest.data(), nseg * 8);
-                int32_t* d_c = static_cast<int32_t*>(dalloc(nseg * GL_INDEXCOV_SLOTS * 4));
-                int64_t* d_b = static_cast<int64_t*>(dalloc(nseg * 32));
-                glck(c, gl_indexcov_counts_segs_device(c, sd.d_dep, static_cast<const int64_t*>(d_ss), static_cast<const int64_t*>(d_sl),
-                                                       static_cast<const int64_t*>(d_lg), (int32_t)nseg, d_c, d_b), "gl_indexcov_counts_segs_device");
+                DevBufs tmp(c);
+                const int64_t* d_ss = tmp.upload(seg_start.data(), nseg);
+                const int64_t* d_sl = tmp.upload(seg_len.data(), nseg);
+                const int64_t* d_lg = tmp.upload(seg_longest.data(), nseg);
+                int32_t* d_c = tmp.alloc<int32_t>(nseg * GL_INDEXCOV_SLOTS);
+                int64_t* d_b = tmp.alloc<int64_t>(nseg * 4);
+                glck(c, gl_indexcov_counts_segs_device(c, sd.d_dep, d_ss, d_sl, d_lg, (int32_t)nseg, d_c, d_b), "gl_indexcov_counts_segs_device");
                 if (G == 1) {
                     glck(c, gl_memcpy_d2h(c, counts_all.data(), d_c, (int64_t)nseg * GL_INDEXCOV_SLOTS * 4), "gl_memcpy_d2h");
                     glck(c, gl_memcpy_d2h(c, b4_all.data(), d_b, (int64_t)nseg * 32), "gl_memcpy_d2h");
@@ -981,12 +1047,11 @@ static int cmd_indexcov(int argc, char** argv) {
                         memcpy(&b4_all[(q * S + a) * 4], &bb[q * Sg * 4], Sg * 32);
                     }
                 }
-                gl_dev_free(c, d_ss); gl_dev_free(c, d_sl); gl_dev_free(c, d_lg); gl_dev_free(c, d_c); gl_dev_free(c, d_b);
             }
         });
     }
-    for (int g = 0; g < G; g++) if (shard[(size_t)g].d_dep) { gl_dev_free(ctxs[(size_t)g], shard[(size_t)g].d_dep); shard[(size_t)g].d_dep = nullptr; }
-    for (int g = 1; g < G; g++) if (ctxs[(size_t)g]) gl_ctx_destroy(ctxs[(size_t)g]);
+    shard.clear();                                                          // frees the resident depths
+    for (int g = 1; g < G; g++) gl_ctx_destroy(ctxs[(size_t)g]);
     gl_ctx* ctx = ctxs[0];                                                  // -n (I7) runs per reference on GPU 0
     ic_mark("tokens + counts (GPU, + D2H)");
 
@@ -1224,8 +1289,7 @@ static int cmd_covstats(int argc, char** argv) {
     ap.parse(argc, argv);
     if (ap.positional.empty()) ap.fail("bams is required");
     const int N = atoi(nstr.c_str());
-    gl_ctx* ctx = nullptr;
-    if (gl_ctx_create(0, &ctx) != GL_OK) fatal(1, "goleft covstats: %s", gl_last_error(nullptr));
+    gl_ctx* ctx = open_ctx(0, "goleft covstats");
     for (const std::string& bam : ap.positional) {
         glhts::BamHeader hdr;
         glhts::CovstatsSample cs;
@@ -1237,9 +1301,7 @@ static int cmd_covstats(int argc, char** argv) {
         glhts::BaiIndex bai;
         bool have_idx = false;
         if (ends_with(bam, ".bam")) {
-            std::string p = bam + ".bai";
-            if (!file_exists(p)) p = bam.substr(0, bam.size() - 4) + ".bai";
-            std::string be = glhts::bai_read(p, bai);
+            std::string be = glhts::bai_read(bai_path(bam), bai);
             if (!be.empty()) fatal(1, "%s", be.c_str());
             have_idx = true;
         }
@@ -1346,8 +1408,7 @@ static int cmd_depthwed(int argc, char** argv) {
     }
     printf("%s\n", header.c_str());
     if (R == 0) return 0;
-    gl_ctx* ctx = nullptr;
-    if (gl_ctx_create(0, &ctx) != GL_OK) fatal(1, "goleft depthwed: %s", gl_last_error(nullptr));
+    gl_ctx* ctx = open_ctx(0, "goleft depthwed");
     std::vector<int32_t> os(R), oe(R), oc(R);
     std::vector<int64_t> out;
     std::vector<int32_t> out32;
@@ -1378,7 +1439,6 @@ static int cmd_depthwed(int argc, char** argv) {
     return 0;
 }
 
-// ------------------------------------------------------------------------------------------------ dispatcher
 // ------------------------------------------------------------------------------------------------ indexsplit
 // indexsplit/indexsplit.go:24-30,197-216: N regions of about equal amounts of data across the cohort, from the indexes alone
 static int cmd_indexsplit(int argc, char** argv) {
@@ -1409,8 +1469,7 @@ static int cmd_indexsplit(int argc, char** argv) {
     }
     const int32_t R = (int32_t)refs.size();
 
-    gl_ctx* ctx = nullptr;
-    if (gl_ctx_create(0, &ctx) != GL_OK) fatal(1, "goleft indexsplit: %s", gl_last_error(nullptr));
+    gl_ctx* ctx = open_ctx(0, "goleft indexsplit");
     const size_t S = paths.size();
     std::vector<int64_t> all_sizes, ptr(S * (size_t)(R + 1), 0), max_len((size_t)R, 0);
     for (size_t i = 0; i < S; i++) {                                        // indexcov.ReadIndex(path).Sizes(), indexsplit.go:92-93
@@ -1420,18 +1479,10 @@ static int cmd_indexsplit(int argc, char** argv) {
             std::vector<glhts::CraiSlices> cr;
             std::string e = glhts::crai_read(b, cr);
             if (!e.empty()) fatal(1, "%s", e.c_str());
-            sp.assign(cr.size() + 1, 0);
-            for (size_t r = 0; r < cr.size(); r++) {
-                std::vector<int64_t> one;
-                if (!glhts::crai_make_sizes(cr[r].start.data(), cr[r].span.data(), cr[r].bytes.data(), (int64_t)cr[r].start.size(), one)) fatal(2, "panic: tilewidth logic error");
-                sz.insert(sz.end(), one.begin(), one.end());
-                sp[r + 1] = (int64_t)sz.size();
-            }
+            crai_sizes(cr, sz, sp);
         } else {
-            std::string p = ends_with(b, ".bai") ? b : b + ".bai";
-            if (!file_exists(p)) p = b.substr(0, b.size() - 4) + (ends_with(b, ".bai") ? "" : ".bai");
             glhts::BaiIndex bai;
-            std::string e = glhts::bai_read(p, bai);
+            std::string e = glhts::bai_read(bai_path(b), bai);
             if (!e.empty()) fatal(1, "%s", e.c_str());
             const size_t nr = bai.ioffsets.size();
             std::vector<uint64_t> voff;
@@ -1482,21 +1533,6 @@ static int cmd_indexsplit(int argc, char** argv) {
 // sample's mean depth.  Two passes over each sample's segments on the GPU (counts, then block sums); the segments are
 // decoded once and kept in their compact form in between (packed8 words, or the GPU feeder's int32 copied to pinned memory).
 // The output is the reference's with -p 1 (chunks in order).
-struct MdSample {
-    glhts::ContigSegs segs;                 // host feeder: packed8 words or sorted int32
-    std::vector<int32_t> s32, e32;          // unindexed BAM: the contig's segments in record order
-    int32_t* pin = nullptr; int64_t pin_n = 0;   // GPU feeder: start | end copied to pinned host memory
-};
-
-static void md_add(gl_ctx* ctx, const MdSample& m) {
-    if (m.pin) { if (m.pin_n > 0) glck(ctx, gl_depth_add_segments(ctx, m.pin, m.pin + m.pin_n, m.pin_n), "gl_depth_add_segments"); return; }
-    if (!m.s32.empty()) { glck(ctx, gl_depth_add_segments(ctx, m.s32.data(), m.e32.data(), (int64_t)m.s32.size()), "gl_depth_add_segments"); return; }
-    if (m.segs.format == 8 && m.segs.n_blocks > 0)
-        glck(ctx, gl_depth_add_segments_packed8(ctx, m.segs.anchors.data(), m.segs.ds.data(), m.segs.len.data(), m.segs.n_blocks), "gl_depth_add_segments_packed8");
-    else if (m.segs.format == 32 && m.segs.n > 0)
-        glck(ctx, gl_depth_add_segments(ctx, m.segs.start.data(), m.segs.end.data(), m.segs.n), "gl_depth_add_segments");
-}
-
 static int cmd_multidepth(int argc, char** argv) {
     std::string q = "10", chrom, mincov = "7", maxcov = "1000", maxskip = "10", minsize = "15", window = "10000000", procs = "0",
                 minsamples = "0.5";
@@ -1523,59 +1559,47 @@ static int cmd_multidepth(int argc, char** argv) {
         for (size_t r = 0; r < refs.size(); r++) if (refs[r].name == chrom) { tid[(size_t)i] = (int)r; if (i == 0) L = refs[r].length; }
         if (tid[(size_t)i] < 0) fatal(2, "panic: multidepth: chromosome %s not found in %s", chrom.c_str(), bams[(size_t)i].c_str());
     }
-    gl_ctx* ctx = nullptr;
-    if (gl_ctx_create(0, &ctx) != GL_OK) fatal(1, "goleft multidepth: %s", gl_last_error(nullptr));
+    gl_ctx* ctx = open_ctx(0, "goleft multidepth");
     if (L <= 0) { printf("%s\n", hdr.c_str()); gl_ctx_destroy(ctx); return 0; }
     glck(ctx, gl_multidepth_begin(ctx, L, S, atoi(mincov.c_str()), atof(minsamples.c_str())), "goleft multidepth");
-    static const bool gpu_feed = [] { const char* e = getenv("GL_GPU_FEED"); return !e || atoi(e) != 0; }();
-    std::vector<MdSample> smp((size_t)S);
-    // host decode of sample i (index-guided, or the whole file when there is no index); runs beside the GPU work of sample i-1
-    auto host_decode = [&](int i) {
-        gl_bam& b = bam[(size_t)i];
-        if (!b.f.has_index) {
-            glhts::SegmentSet set;
-            std::string e = glhts::bam_decode_segments(bams[(size_t)i], Q, threads > 0 ? threads : 8, tid[(size_t)i], set);
+    std::vector<SegSource> smp((size_t)S);
+    std::vector<glhts::SegmentSet> whole((size_t)S);
+    std::vector<void*> pinned;
+    // sample i's segments of the contig: without an index, a whole-file decode of that one reference; otherwise the GPU feeder
+    // when it can, else the host feeder.  A sample that stays on the host is decoded on a helper thread beside the GPU work
+    // of sample i-1.
+    auto stays_on_host = [&](int i) { return !(SegSource::gpu_feed() && bam[(size_t)i].f.has_index); };
+    auto fetch = [&](int i) {
+        const size_t k = (size_t)i;
+        if (!bam[k].f.has_index) {
+            std::string e = glhts::bam_decode_segments(bams[k], Q, threads > 0 ? threads : 8, tid[k], whole[k]);
             if (!e.empty()) fatal(1, "%s", e.c_str());
-            smp[(size_t)i].s32.swap(set.start[(size_t)tid[(size_t)i]]);
-            smp[(size_t)i].e32.swap(set.end[(size_t)tid[(size_t)i]]);
-            return;
+            smp[k].whole = &whole[k];
         }
-        std::string e = b.f.decode(tid[(size_t)i], 0, L, Q, threads, 0, smp[(size_t)i].segs, nullptr);
-        if (!e.empty()) fatal(1, "%s", e.c_str());
+        smp[k].fetch(ctx, bam[k], tid[k], 0, L, Q, threads, 0, true, nullptr, nullptr);
     };
     // pass 1
     std::thread next;
     bool next_host = false;
     for (int i = 0; i < S; i++) {
-        MdSample& m = smp[(size_t)i];
-        const int32_t *ds = nullptr, *de = nullptr;
-        int64_t dn = -1;
+        SegSource& m = smp[(size_t)i];
         if (next.joinable()) next.join();
-        if (!next_host) {
-            if (gpu_feed && bam[(size_t)i].f.has_index) {
-                gl_bam_segments st;
-                const int rc = gl_bam_decode_device(ctx, &bam[(size_t)i], tid[(size_t)i], Q, &ds, &de, &dn, &st);
-                if (rc != GL_OK) { dn = -1; if (rc != GL_ESTATE) glck(ctx, rc, "gl_bam_decode_device"); }
-            }
-            if (dn < 0) host_decode(i);
-        }
-        // the next sample's host decode overlaps this sample's device work
-        next_host = i + 1 < S && !(gpu_feed && bam[(size_t)i + 1].f.has_index);
-        if (next_host) next = std::thread(host_decode, i + 1);
+        if (!next_host) fetch(i);
+        next_host = i + 1 < S && stays_on_host(i + 1);
+        if (next_host) next = std::thread(fetch, i + 1);
         glck(ctx, gl_depth_begin(ctx, 0, L), "gl_depth_begin");
-        if (dn >= 0) {
-            if (dn > 0) glck(ctx, gl_depth_add_segments_device(ctx, ds, de, dn), "gl_depth_add_segments_device");
-            glck(ctx, gl_multidepth_count(ctx), "gl_multidepth_count");
+        m.add(ctx);
+        glck(ctx, gl_multidepth_count(ctx), "gl_multidepth_count");
+        if (m.on_device) {                          // pass 2 needs the feeder's arrays after the next decode reuses them
             void* p = nullptr;
-            glck(ctx, gl_host_alloc_pinned(ctx, std::max<int64_t>(dn, 1) * 8, &p), "gl_host_alloc_pinned");
-            m.pin = static_cast<int32_t*>(p); m.pin_n = dn;
-            if (dn > 0) {
-                glck(ctx, gl_memcpy_d2h(ctx, m.pin, ds, dn * 4), "gl_memcpy_d2h");
-                glck(ctx, gl_memcpy_d2h(ctx, m.pin + dn, de, dn * 4), "gl_memcpy_d2h");
+            glck(ctx, gl_host_alloc_pinned(ctx, std::max<int64_t>(m.n, 1) * 8, &p), "gl_host_alloc_pinned");
+            pinned.push_back(p);
+            int32_t* pin = static_cast<int32_t*>(p);
+            if (m.n > 0) {
+                glck(ctx, gl_memcpy_d2h(ctx, pin, m.s, m.n * 4), "gl_memcpy_d2h");
+                glck(ctx, gl_memcpy_d2h(ctx, pin + m.n, m.e, m.n * 4), "gl_memcpy_d2h");
             }
-        } else {
-            md_add(ctx, m);
-            glck(ctx, gl_multidepth_count(ctx), "gl_multidepth_count");
+            m.view(pin, pin + m.n, m.n);
         }
     }
     if (next.joinable()) next.join();
@@ -1596,7 +1620,7 @@ static int cmd_multidepth(int argc, char** argv) {
     // pass 2
     for (int i = 0; i < S; i++) {
         glck(ctx, gl_depth_begin(ctx, 0, L), "gl_depth_begin");
-        md_add(ctx, smp[(size_t)i]);
+        smp[(size_t)i].add(ctx);
         glck(ctx, gl_multidepth_sums(ctx, i), "gl_multidepth_sums");
     }
     const size_t cells = (size_t)nb * (size_t)S;
@@ -1611,7 +1635,7 @@ static int cmd_multidepth(int argc, char** argv) {
     printf("%s\n", hdr.c_str());
     fwrite(text, 1, (size_t)tl, stdout);
     gl_free_text(text);
-    for (MdSample& m : smp) if (m.pin) gl_host_free_pinned(ctx, m.pin);
+    for (void* p : pinned) gl_host_free_pinned(ctx, p);
     gl_ctx_destroy(ctx);
     return 0;
 }

@@ -13,6 +13,7 @@
 #include <fcntl.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
+#include <time.h>
 #include <unistd.h>
 #include <algorithm>
 #include <array>
@@ -277,6 +278,55 @@ struct SegSource {
     }
 };
 
+// A FASTA opened for Faidx.Stats (github.com/brentp/faidx, restated in fasta.cu): its .fai records and its bytes, mapped.
+// `depth --stats` and `dcnv` take the GC of their rows through it.
+struct FastaStats {
+    std::vector<glhts::RefInfo> index;
+    const uint8_t* map = nullptr; size_t len = 0;
+    FastaStats() = default;
+    FastaStats(const FastaStats&) = delete;
+    FastaStats& operator=(const FastaStats&) = delete;
+    ~FastaStats() { if (map) munmap(const_cast<uint8_t*>(map), len); }
+    void open(const std::string& path) {
+        std::string e = glhts::fai_read(path + ".fai", index);
+        if (!e.empty()) fatal(1, "%s", e.c_str());
+        int fd = ::open(path.c_str(), O_RDONLY);
+        struct stat st;
+        if (fd < 0 || fstat(fd, &st) != 0) fatal(1, "cannot open %s", path.c_str());
+        len = (size_t)st.st_size;
+        if (len) {
+            void* mm = mmap(nullptr, len, PROT_READ, MAP_PRIVATE, fd, 0);
+            if (mm == MAP_FAILED) fatal(1, "cannot mmap %s", path.c_str());
+            map = static_cast<const uint8_t*>(mm);
+        }
+        close(fd);
+    }
+    const glhts::RefInfo* find(const std::string& c) const {
+        for (const glhts::RefInfo& r : index) if (r.name == c) return &r;
+        return nullptr;
+    }
+    // {GC, CpG, Masked} of the rows [s[i], e[i]) of one record into st3[3 i ..] (one gl_fasta_load, one gl_fasta_stats).
+    // Faidx.Stats panics on a row outside the record (s < 0, e < s or e > length); such a row is clipped to the record
+    // here and counted in the return value, and each caller decides what that means.
+    size_t stats(gl_ctx* ctx, const glhts::RefInfo& ri, const std::vector<int64_t>& s, const std::vector<int64_t>& e, double* st3) const {
+        if (s.empty()) return 0;
+        const int64_t rec_bytes = std::min<int64_t>((int64_t)len - ri.offset, glhts::fasta_position(ri, ri.length) + 1);
+        if (ri.offset < 0 || rec_bytes < 0) fatal(1, "bad .fai entry for %s", ri.name.c_str());
+        glck(ctx, gl_fasta_load(ctx, map + ri.offset, rec_bytes), "gl_fasta_load");
+        std::vector<int64_t> ba(s.size()), bb(s.size());
+        size_t outside = 0;
+        for (size_t i = 0; i < s.size(); i++) {
+            outside += (s[i] < 0 || e[i] < s[i] || e[i] > ri.length);
+            const int64_t a = std::min<int64_t>(std::max<int64_t>(s[i], 0), ri.length), b = std::min<int64_t>(std::max<int64_t>(e[i], a), ri.length);
+            const int64_t ps = glhts::fasta_position(ri, a), pe = glhts::fasta_position(ri, b);
+            ba[i] = std::min(ps, rec_bytes);          // the slice ends one byte past position(end) when that byte exists
+            bb[i] = std::max(ba[i], std::min<int64_t>(pe + ((ri.offset + pe < (int64_t)len) ? 1 : 0), rec_bytes));
+        }
+        glck(ctx, gl_fasta_stats(ctx, ba.data(), bb.data(), (int64_t)ba.size(), nullptr, st3), "gl_fasta_stats");
+        return outside;
+    }
+};
+
 // ------------------------------------------------------------------------------------------------ depth
 // `goleft depth`: depth/depth.go:103-159 builds the work list (10 Mb chunks of every .fai contig, or the BED lines), runs one
 // `samtools depth -r` child per entry and concatenates the per-chunk BED files (-o: in order).  Here the unit of work is a
@@ -312,8 +362,7 @@ struct DepthShared {
     std::vector<DepthRegion>* regions = nullptr;    // BED mode
     std::vector<std::string>* out_hd = nullptr;     // BED mode: per line
     std::vector<std::string>* out_ca = nullptr;
-    std::vector<glhts::RefInfo> fa_index;
-    const uint8_t* fa_map = nullptr; size_t fa_len = 0;
+    FastaStats fa;                                  // --stats
     std::mutex mu; std::condition_variable cv;
 };
 
@@ -385,23 +434,9 @@ struct DepthEngine {
         if (pending.empty()) return;
         const std::string& c = pending[0].chrom;
         std::vector<double> st3(row_s.size() * 3, 0.0);
-        const glhts::RefInfo* ri = nullptr;
-        for (const glhts::RefInfo& r : sh.fa_index) if (r.name == c) { ri = &r; break; }
+        const glhts::RefInfo* ri = sh.fa.find(c);
         if (!ri) fprintf(stderr, "GC: unknown sequence %s\n", c.c_str());                 // faidx error text; zeros are printed (depth.go:195-199)
-        else if (!row_s.empty()) {
-            const int64_t rec_bytes = std::min<int64_t>((int64_t)sh.fa_len - ri->offset, glhts::fasta_position(*ri, ri->length) + 1);
-            if (ri->offset < 0 || rec_bytes < 0) fatal(1, "bad .fai entry for %s", c.c_str());
-            glck(ctx, gl_fasta_load(ctx, sh.fa_map + ri->offset, rec_bytes), "gl_fasta_load");
-            std::vector<int64_t> ba(row_s.size()), bb(row_s.size());
-            for (size_t i = 0; i < row_s.size(); i++) {
-                // faidx panics on coordinates past the contig; rows are clipped to it here instead
-                const int64_t s = std::min<int64_t>(std::max<int64_t>(row_s[i], 0), ri->length), e = std::min<int64_t>(std::max<int64_t>(row_e[i], s), ri->length);
-                const int64_t ps = glhts::fasta_position(*ri, s), pe = glhts::fasta_position(*ri, e);
-                ba[i] = std::min(ps, rec_bytes);
-                bb[i] = std::max(ba[i], std::min<int64_t>(pe + ((ri->offset + pe < (int64_t)sh.fa_len) ? 1 : 0), rec_bytes));
-            }
-            glck(ctx, gl_fasta_stats(ctx, ba.data(), bb.data(), (int64_t)ba.size(), nullptr, st3.data()), "gl_fasta_stats");
-        }
+        else sh.fa.stats(ctx, *ri, row_s, row_e, st3.data());                            // faidx panics past the contig; clipped here instead
         for (const Pending& pc : pending) {
             char *hd = nullptr, *ca = nullptr;
             int64_t hl = 0, cl = 0;
@@ -634,18 +669,7 @@ static int cmd_depth(int argc, char** argv) {
     }
     if (stats) {
         if (reference.empty()) fatal(1, "goleft depth: --stats needs --reference");
-        std::string e2 = glhts::fai_read(reference + ".fai", sh.fa_index);
-        if (!e2.empty()) fatal(1, "%s", e2.c_str());
-        int fd = open(reference.c_str(), O_RDONLY);
-        struct stat st;
-        if (fd < 0 || fstat(fd, &st) != 0) fatal(1, "cannot open %s", reference.c_str());
-        sh.fa_len = (size_t)st.st_size;
-        if (sh.fa_len) {
-            void* mm = mmap(nullptr, sh.fa_len, PROT_READ, MAP_PRIVATE, fd, 0);
-            if (mm == MAP_FAILED) fatal(1, "cannot mmap %s", reference.c_str());
-            sh.fa_map = static_cast<const uint8_t*>(mm);
-        }
-        close(fd);
+        sh.fa.open(reference);
     }
 
     const std::string sfx = chrom.empty() ? "" : "." + chrom;               // depth.go:378-389
@@ -687,7 +711,6 @@ static int cmd_depth(int argc, char** argv) {
         }
     }
     fclose(fca); fclose(fhd);
-    if (sh.fa_map) munmap(const_cast<uint8_t*>(sh.fa_map), sh.fa_len);
     if (timing) {
         double dec = 0, gpu = 0, inf = 0, par = 0; long long rec = 0, bin = 0, bout = 0; int fed = 0;
         for (const DepthJob& j : jobs) {
@@ -1661,6 +1684,254 @@ static int cmd_samplename(int argc, char** argv) {
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ dcnv
+// dcnv/dcnv.go:153-186,323-354 (a separate binary of the reference; `dcnv <matrix> <ref.fa>`, positional only): read the
+// sites x samples matrix depthwed writes (plain, gzip/BGZF or "-"), take each row's GC from the FASTA, argsort the rows by
+// GC as Go does (gl_go_argsort_f64), debias and median-normalise every sample on the GPU (gl_dcnv_normalize, column blocks
+// sized to device memory), and write depth.bed with "%.2f" tokens made on the GPU (gl_format_f2).  The reference's panics
+// are an error message and exit 2.  Parsing and row assembly run on the host pool.
+namespace {
+
+struct DcnvRow { const char* p; size_t n; };                 // one line, without its "\n"
+
+bool go_space(char c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r' || c == '\v' || c == '\f'; }
+
+// strconv.Atoi, then the reference's uint32(); a value outside uint32 (which the reference wraps) is an error here
+bool dcnv_atou32(const char* p, size_t n, int64_t& v) {
+    size_t i = (n && (p[0] == '+' || p[0] == '-')) ? 1 : 0;
+    if (i == n || n - i > 18) return false;
+    int64_t x = 0;
+    for (size_t k = i; k < n; k++) {
+        if (p[k] < '0' || p[k] > '9') return false;
+        x = x * 10 + (p[k] - '0');
+    }
+    v = p[0] == '-' ? -x : x;
+    return v >= 0 && v < (int64_t(1) << 32);
+}
+
+// strconv.ParseFloat of the decimal form (depthwed writes integers: those take the fast path); NaN, Inf, hexadecimal
+// and out-of-range tokens are errors here
+bool dcnv_atof(const char* p, size_t n, double& v) {
+    size_t i = (n && (p[0] == '+' || p[0] == '-')) ? 1 : 0;
+    size_t k = i;
+    while (k < n && p[k] >= '0' && p[k] <= '9') k++;
+    if (k == n && k > i && k - i <= 15) {                       // at most 15 digits: exact in float64
+        int64_t x = 0;
+        for (size_t j = i; j < n; j++) x = x * 10 + (p[j] - '0');
+        v = p[0] == '-' ? -(double)x : (double)x;
+        return true;
+    }
+    const size_t int_digits = k - i;
+    size_t frac_digits = 0;
+    if (k < n && p[k] == '.') { k++; while (k < n && p[k] >= '0' && p[k] <= '9') { k++; frac_digits++; } }
+    if (int_digits + frac_digits == 0) return false;
+    if (k < n && (p[k] == 'e' || p[k] == 'E')) {
+        k++;
+        if (k < n && (p[k] == '+' || p[k] == '-')) k++;
+        const size_t e0 = k;
+        while (k < n && p[k] >= '0' && p[k] <= '9') k++;
+        if (k == e0) return false;
+    }
+    if (k != n) return false;
+    std::string s(p, n);
+    v = strtod(s.c_str(), nullptr);                             // correctly rounded, as ParseFloat
+    return std::isfinite(v);
+}
+
+// Go's log.Println prefix: "2009/11/10 23:00:00 "
+void go_log(const char* msg) {
+    time_t t = time(nullptr);
+    struct tm tm;
+    localtime_r(&t, &tm);
+    fprintf(stderr, "%04d/%02d/%02d %02d:%02d:%02d %s\n", tm.tm_year + 1900, tm.tm_mon + 1, tm.tm_mday, tm.tm_hour, tm.tm_min, tm.tm_sec, msg);
+}
+
+}  // namespace
+
+static int cmd_dcnv(int argc, char** argv) {
+    if (argc < 3) fatal(2, "panic: runtime error: index out of range (usage: goleft dcnv <depthwed matrix> <ref.fa>)");
+    const std::string path = argv[1], fasta = argv[2];
+    const bool timing = getenv("GL_TIMING") != nullptr;        // phase wall clocks on stderr
+    double tp = now_s();
+    auto mark = [&](const char* what) { if (timing) { const double t = now_s(); fprintf(stderr, "[dcnv timing] %-22s %.3f s\n", what, t - tp); tp = t; } };
+    FastaStats fa;
+    fa.open(fasta);
+    glhost_pool_warm();
+
+    // ---- the text: all of it, then its lines (ReadString('\n'): a final line without "\n" is dropped)
+    std::string text;
+    {
+        gzFile f = path == "-" ? gzdopen(dup(0), "rb") : gzopen(path.c_str(), "rb");
+        if (!f) fatal(2, "panic: open %s: %s", path.c_str(), strerror(errno));
+        gzbuffer(f, 1 << 20);
+        std::vector<char> buf((size_t)1 << 22);
+        int n;
+        while ((n = gzread(f, buf.data(), (unsigned)buf.size())) > 0) text.append(buf.data(), (size_t)n);
+        if (n < 0) fatal(2, "panic: read %s", path.c_str());
+        gzclose(f);
+    }
+    std::vector<DcnvRow> rows;
+    std::vector<std::string> samples;
+    bool have_header = false;
+    for (size_t a = 0; a < text.size();) {
+        const char* nl = static_cast<const char*>(memchr(text.data() + a, '\n', text.size() - a));
+        if (!nl) break;
+        const size_t b = (size_t)(nl - text.data());
+        if (rows.empty() && (text[a] == '#' || text.compare(a, 5, "chrom") == 0)) {       // only before the first data line
+            size_t s = a, e = b + 1;
+            while (s < e && go_space(text[s])) s++;
+            while (e > s && go_space(text[e - 1])) e--;
+            std::vector<std::string> f;
+            for (size_t x = s;;) {
+                const size_t t = text.find('\t', x);
+                if (t == std::string::npos || t >= e) { f.push_back(text.substr(x, e - x)); break; }
+                f.push_back(text.substr(x, t - x));
+                x = t + 1;
+            }
+            if (f.size() < 3) fatal(2, "panic: runtime error: slice bounds out of range (header line has %zu fields)", f.size());
+            samples.assign(f.begin() + 3, f.end());
+            have_header = true;
+        } else {
+            rows.push_back({text.data() + a, b - a});
+        }
+        a = b + 1;
+    }
+    if (!have_header) fatal(2, "panic: runtime error: integer divide by zero (no header line: no samples)");
+    const size_t S = samples.size();
+    const size_t R = rows.size();
+    if (S == 0) fatal(2, "panic: runtime error: integer divide by zero (the header names no samples)");
+    std::string label;                                           // ivs.Chrom: set by data lines 0 and 1, so the second wins
+    for (size_t r = 0; r < std::min<size_t>(R, 2); r++) {
+        const void* t = memchr(rows[r].p, '\t', rows[r].n);
+        if (!t) fatal(2, "panic: runtime error: slice bounds out of range [:-1] (data line %zu has no tab)", r + 1);
+        label.assign(rows[r].p, (size_t)(static_cast<const char*>(t) - rows[r].p));
+    }
+    mark("read");
+
+    // ---- rows on the host pool: chrom, clamped start, end, S values
+    std::vector<double> X(R * S);
+    std::vector<int64_t> starts(R), ends(R);
+    std::vector<std::pair<const char*, size_t>> chrom(R);
+    const int64_t per = 4096, tasks = ((int64_t)R + per - 1) / per;
+    std::vector<std::string> errs((size_t)tasks);
+    glhost::ThreadPool::global().run(tasks, [&](int64_t t, int) {
+        for (size_t r = (size_t)t * per; r < std::min(R, (size_t)(t + 1) * per); r++) {
+            const char* p = rows[r].p;
+            const char* end = p + rows[r].n;
+            size_t col = 0;
+            auto fail = [&](const std::string& m) { errs[(size_t)t] = "panic: line " + std::to_string(r + 1) + " of the data: " + m; };
+            for (const char* a = p;; col++) {
+                const char* tab = static_cast<const char*>(memchr(a, '\t', (size_t)(end - a)));
+                const char* b = tab ? tab : end;
+                const char* s = a;
+                if (!tab) {                                                                // only the last field is trimmed
+                    while (s < b && go_space(*s)) s++;
+                    while (b > s && go_space(b[-1])) b--;
+                }
+                if (col == 0) chrom[r] = {s, (size_t)(b - s)};
+                else if (col < 3) {
+                    int64_t v;
+                    if (!dcnv_atou32(s, (size_t)(b - s), v)) { fail("strconv.Atoi: parsing \"" + std::string(s, b) + "\": invalid syntax or outside uint32"); return; }
+                    (col == 1 ? starts[r] : ends[r]) = col == 1 ? std::max<int64_t>(v, 250) : v;      // dcnv.go:83-85
+                } else if (col - 3 < S) {
+                    if (!dcnv_atof(s, (size_t)(b - s), X[r * S + col - 3])) { fail("strconv.ParseFloat: parsing \"" + std::string(s, b) + "\": invalid syntax or out of range"); return; }
+                }
+                if (!tab) break;
+                a = tab + 1;
+            }
+            if (col < 2) { fail("runtime error: index out of range (fewer than 3 columns)"); return; }
+            if (col + 1 != S + 3) { fail(std::to_string(col - 2) + " values but " + std::to_string(S) + " samples in the header"); return; }
+        }
+    });
+    for (const std::string& e : errs) if (!e.empty()) fatal(2, "%s", e.c_str());
+    if (R < 5) fatal(2, "panic: runtime error: index out of range (%zu data rows; the moving median needs 5)", R);
+    mark("parse");
+
+    // ---- GC of every row, a contig at a time: Faidx.Stats(chrom, start - 250, end)
+    gl_ctx* ctx = open_ctx(0, "goleft dcnv");
+    std::vector<double> gc(R, 0.0);
+    {
+        std::map<std::string, std::vector<size_t>> by_chrom;
+        std::string prev;
+        std::vector<size_t>* cur = nullptr;
+        for (size_t r = 0; r < R; r++) {
+            if (!cur || chrom[r].second != prev.size() || memcmp(chrom[r].first, prev.data(), prev.size()) != 0) {
+                prev.assign(chrom[r].first, chrom[r].second);
+                cur = &by_chrom[prev];
+            }
+            cur->push_back(r);
+        }
+        std::vector<int64_t> s, e;
+        std::vector<double> st3;
+        for (auto& kv : by_chrom) {
+            const glhts::RefInfo* ri = fa.find(kv.first);
+            if (!ri) { fprintf(stderr, "GC: unknown sequence %s\n", kv.first.c_str()); continue; }      // the error is printed; GC 0 (dcnv.go:86-89)
+            s.clear(); e.clear();
+            for (size_t r : kv.second) { s.push_back(starts[r] - 250); e.push_back(ends[r]); }
+            st3.assign(s.size() * 3, 0.0);
+            if (fa.stats(ctx, *ri, s, e, st3.data()))
+                for (size_t k = 0; k < s.size(); k++)
+                    if (e[k] < s[k] || e[k] > ri->length)
+                        fatal(2, "panic: faidx: %s:%lld-%lld is outside the sequence (length %lld)", kv.first.c_str(), (long long)s[k], (long long)e[k], (long long)ri->length);
+            for (size_t k = 0; k < s.size(); k++) gc[kv.second[k]] = st3[k * 3];
+        }
+    }
+    mark("gc");
+    std::vector<int64_t> inds(R);
+    glck(ctx, gl_go_argsort_f64(gc.data(), (int64_t)R, inds.data()), "gl_go_argsort_f64");
+    bool changed = false;
+    for (size_t i = 0; i < R && !changed; i++) changed = inds[i] != (int64_t)i;
+    if (!changed) go_log("WARNING: no change after sorting. This usually means .Vals is unset or same as previous run");   // debiaser.go:71-73
+    mark("argsort");
+
+    // ---- debias + normalise on the GPU, in place
+    const char* bc = getenv("GL_DCNV_BLOCK_COLS");
+    std::vector<double> med(S);
+    const int rc = gl_dcnv_normalize(ctx, X.data(), (int64_t)R, (int64_t)S, inds.data(), 0, (int32_t)S, bc ? atoi(bc) : 0, X.data(), (int64_t)S, med.data());
+    if (rc == GL_ERANGE) fatal(2, "panic: runtime error: index out of range: %s", gl_last_error(ctx));
+    glck(ctx, rc, "gl_dcnv_normalize");
+    mark("normalize");
+
+    // ---- depth.bed: "%.2f" tokens from the GPU, rows assembled on the host pool
+    FILE* fo = fopen("depth.bed", "w");
+    if (!fo) fatal(2, "panic: open depth.bed: %s", strerror(errno));
+    std::string head = "#chrom\tstart\tend";
+    for (const std::string& s : samples) head += "\t" + s;
+    head += "\n";
+    fwrite(head.data(), 1, head.size(), fo);
+    const size_t chunk_rows = std::max<size_t>(1, ((size_t)1 << 24) / S);
+    std::vector<uint8_t> tok;
+    const size_t per_text = 2048;
+    std::vector<std::string> parts;
+    for (size_t r0 = 0; r0 < R; r0 += chunk_rows) {
+        const size_t nr = std::min(chunk_rows, R - r0);
+        tok.resize(nr * S * 16);
+        glck(ctx, gl_format_f2(ctx, X.data() + r0 * S, (int64_t)(nr * S), tok.data()), "gl_format_f2");
+        const size_t groups = (nr + per_text - 1) / per_text;
+        parts.assign(groups, std::string());
+        glhost::ThreadPool::global().run((int64_t)groups, [&](int64_t g, int) {
+            std::string& o = parts[(size_t)g];
+            char num[48];
+            for (size_t r = r0 + (size_t)g * per_text; r < std::min(r0 + nr, r0 + ((size_t)g + 1) * per_text); r++) {
+                o += label;
+                o.append(num, (size_t)snprintf(num, sizeof num, "\t%lld\t%lld", (long long)starts[r], (long long)ends[r]));
+                for (size_t c = 0; c < S; c++) {
+                    const char* t = reinterpret_cast<const char*>(tok.data() + ((r - r0) * S + c) * 16);
+                    o += '\t';
+                    if (t[0]) o.append(t, strnlen(t, 16));
+                    else o += go_float("%.2f", X[r * S + c]);                                  // text longer than a token
+                }
+                o += '\n';
+            }
+        });
+        for (const std::string& p : parts) fwrite(p.data(), 1, p.size(), fo);
+    }
+    if (fclose(fo) != 0) fatal(1, "write depth.bed: %s", strerror(errno));
+    mark("format + write");
+    gl_ctx_destroy(ctx);
+    return 0;
+}
+
 static void print_progs() {                                                          // cmd/goleft/goleft.go:33-53
     fprintf(stderr, "goleft Version: %s (GPU engine: %s)\n\n", kVersion, gl_version());
     fprintf(stderr, "covstats    : coverage and insert-size statistics on bams by sampling\n");
@@ -1670,6 +1941,7 @@ static void print_progs() {                                                     
     fprintf(stderr, "indexsplit  : create regions of even coverage across bams/crams\n");
     fprintf(stderr, "samplename  : report samplename(s) from a bam's SM tag\n");
     fprintf(stderr, "multidepth  : (extension; a separate binary in goleft) blocks of sufficient coverage across many bams\n");
+    fprintf(stderr, "dcnv        : (extension; a separate binary in goleft) GC-debias and median-normalise a depthwed matrix\n");
 }
 
 int main(int argc, char** argv) {
@@ -1682,6 +1954,7 @@ int main(int argc, char** argv) {
     if (prog == "indexsplit") return cmd_indexsplit(argc - 1, argv + 1);
     if (prog == "samplename") return cmd_samplename(argc - 1, argv + 1);
     if (prog == "multidepth") return cmd_multidepth(argc - 1, argv + 1);
+    if (prog == "dcnv") return cmd_dcnv(argc - 1, argv + 1);
     print_progs();
     return 1;
 }

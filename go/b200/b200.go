@@ -283,3 +283,28 @@ func (c *Ctx) Multidepth(chrom string, length, samples, minCov int, minSamples f
 	defer C.gl_free_text(text)
 	return C.GoBytes(unsafe.Pointer(text), C.int(tl)), nil
 }
+
+// Dcnv replaces GeneralDebiaser.Sort / Debias / Unsort + NormalizeBySampleMedian of dcnv/dcnv.go:329-337 on the
+// n x S row-major depth matrix `depths` (rows in position order; normalised in place), with gcs the GC fraction of each row.
+// The argsort is Go's own sort.Sort order (gl_go_argsort_f64), so floats.Argsort may equally be used.  Returns the sample
+// medians; fmt.Sprintf("%.2f") of the result is what dcnv writes, or FormatF2 gives the same text as 16-byte tokens.
+func (c *Ctx) Dcnv(depths []float64, gcs []float64, samples int) ([]float64, error) {
+	n := len(gcs)
+	inds := make([]int64, n)
+	if C.gl_go_argsort_f64((*C.double)(&gcs[0]), C.int64_t(n), (*C.int64_t)(&inds[0])) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_go_argsort_f64 failed")
+	}
+	medians := make([]float64, samples)
+	d := (*C.double)(unsafe.Pointer(&depths[0]))
+	rc := C.gl_dcnv_normalize(c.h, d, C.int64_t(n), C.int64_t(samples), (*C.int64_t)(&inds[0]), 0, C.int32_t(samples), 0, d,
+		C.int64_t(samples), (*C.double)(&medians[0]))
+	return medians, c.err(rc)
+}
+
+// FormatF2 is fmt.Sprintf("%.2f", v) of every value, made on the GPU: 16 bytes per value, the text NUL-padded; an empty
+// token means the text is longer and the caller formats that value itself.
+func (c *Ctx) FormatF2(vals []float64) ([]byte, error) {
+	tok := make([]byte, 16*len(vals)+16)
+	rc := C.gl_format_f2(c.h, (*C.double)(&vals[0]), C.int64_t(len(vals)), (*C.uint8_t)(&tok[0]))
+	return tok[:16*len(vals)], c.err(rc)
+}

@@ -181,6 +181,12 @@ _proto("gl_multidepth_result", C.c_int, _vp, _vp, _vp, _vp, _vp)
 _proto("gl_multidepth_stats", C.c_int, _vp, _i64p, _i64p, _i64p, _i64p)
 _proto("gl_multidepth_certify", C.c_int, _vp, _vp, _vp, C.c_int64, _vp, _vp)
 _proto("gl_multidepth_text", C.c_int, C.c_char_p, _vp, _vp, C.c_int64, C.c_int32, _vp, _vp, _vp, C.c_int32, C.POINTER(_vp), _i64p)
+_proto("gl_go_argsort_f64", C.c_int, _vp, C.c_int64, _vp)
+_proto("gl_dcnv_normalize_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int32, _vp, C.c_int64, _vp)
+_proto("gl_dcnv_normalize", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, _vp)
+_proto("gl_format_f2", C.c_int, _vp, _vp, C.c_int64, _vp)
+_proto("gl_format_f2_device", C.c_int, _vp, _vp, C.c_int64, _vp)
+_proto("gl_format_f2_host", C.c_int, _vp, C.c_int64, _vp)
 
 
 def version() -> str:
@@ -288,6 +294,39 @@ def multidepth_text(chrom: str, blk_start, blk_end, S: int, q, val, certified, t
         return C.string_at(p, n.value)
     finally:
         lib.gl_free_text(p)
+
+
+# ---- dcnv (dcnv/dcnv.go), host-only parts
+F2_TOKEN = 16
+
+
+def go_argsort(v) -> np.ndarray:
+    """Host-only: the permutation gonum's floats.Argsort (Go's unstable sort.Sort) gives v."""
+    v = _as(v, np.float64)
+    inds = np.empty(v.size, np.int64)
+    rc = lib.gl_go_argsort_f64(_ptr(v), v.size, _ptr(inds))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_go_argsort_f64: bad arguments")
+    return inds
+
+
+def format_f2_host(vals) -> np.ndarray:
+    """Host-only: n x 16 "%.2f" tokens (text, NUL-padded; an empty token: the caller formats the value)."""
+    vals = _as(vals, np.float64)
+    tok = np.empty((vals.size, F2_TOKEN), np.uint8)
+    rc = lib.gl_format_f2_host(_ptr(vals), vals.size, _ptr(tok))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_format_f2_host: bad arguments")
+    return tok
+
+
+def f2_text(tokens, vals) -> list:
+    """the "%.2f" strings (bytes) of tokens, with Python formatting where a token is empty"""
+    out = []
+    for t, v in zip(np.asarray(tokens, np.uint8).reshape(-1, F2_TOKEN), np.asarray(vals, np.float64).ravel()):
+        b = t.tobytes().rstrip(b"\0")
+        out.append(b if b else b"%.2f" % v)
+    return out
 
 
 def chunk_rows(rs: int, re: int, W: int, run_start: np.ndarray, run_class: np.ndarray):
@@ -1077,6 +1116,31 @@ class Ctx:
             self.multidepth_sums(i)
         _, q, val, ok = self.multidepth_result(bs.size, S)
         return multidepth_text(chrom, bs, be, S, q, val, ok)
+
+    # ---- dcnv
+    def dcnv_normalize(self, x: np.ndarray, inds, c0: int = 0, c1: Optional[int] = None, block_cols: int = 0):
+        """Columns [c0, c1) of the n x S matrix x (rows in position order), inds = the GC argsort -> (normalised n x (c1 - c0),
+        sample medians)"""
+        x = np.ascontiguousarray(x, np.float64)
+        n, S = x.shape
+        c1 = S if c1 is None else c1
+        inds = _as(inds, np.int64)
+        out, med = np.empty((n, c1 - c0), np.float64), np.empty(c1 - c0, np.float64)
+        self._ck(lib.gl_dcnv_normalize(self.h, _ptr(x), n, S, _ptr(inds), c0, c1, block_cols, _ptr(out), c1 - c0, _ptr(med)))
+        return out, med
+
+    def dcnv_normalize_device(self, d_x: DevBuf, n: int, ld: int, d_inds: DevBuf, c0: int, c1: int, d_out: DevBuf, ld_out: int,
+                              d_medians: DevBuf):
+        self._ck(lib.gl_dcnv_normalize_device(self.h, d_x.ptr, n, ld, d_inds.ptr, c0, c1, d_out.ptr, ld_out, d_medians.ptr))
+
+    def format_f2(self, vals: np.ndarray) -> np.ndarray:
+        vals = _as(vals, np.float64)
+        tok = np.empty((vals.size, F2_TOKEN), np.uint8)
+        self._ck(lib.gl_format_f2(self.h, _ptr(vals), vals.size, _ptr(tok)))
+        return tok
+
+    def format_f2_device(self, d_vals: DevBuf, n: int, d_tokens: DevBuf):
+        self._ck(lib.gl_format_f2_device(self.h, d_vals.ptr, n, d_tokens.ptr))
 
     # ---- multi-GPU
     def comm_init(self, id128: bytes, rank: int, world: int):

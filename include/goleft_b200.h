@@ -464,6 +464,33 @@ int  gl_multidepth_certify(const int64_t* sum, const int64_t* n_sites, const int
 int  gl_multidepth_text(const char* chrom, const int64_t* blk_start, const int64_t* blk_end, int64_t n_blocks, int32_t S, const int64_t* q,
                         const double* val, const uint8_t* certified, int32_t threads, char** text, int64_t* text_len);
 
+/* ---------------------------------------------------------------- dcnv
+ * Replaces dcnv/dcnv.go:323-354 (a separate binary of the reference), the step after depthwed: GC-debias and median-normalise
+ * an n-sites x S-samples matrix (DESIGN §1.9).
+ *   gl_go_argsort_f64  : host-only: inds = the permutation gonum's floats.Argsort(v) leaves, i.e. Go's unstable sort.Sort
+ *                        (pdqsort, go 1.21) over (value, index) pairs.  The order inside ties is Go's own.
+ *   gl_dcnv_normalize_device : columns [c0, c1) of the row-major n x ld float64 matrix d_x, rows in position order; d_inds =
+ *                        the GC argsort (a permutation of [0, n), not checked here).  Per column: divide every row by
+ *                        max(1, the moving median of 9 along the GC order, with the reference's window quirks), then by the
+ *                        sample median (sorted[k + int(0.65 (n - k))], k = leading exact zeros, 0 when a value is
+ *                        negative).  Writes the result to columns [0, c1 - c0) of d_out (row stride ld_out; must not overlap
+ *                        d_x) and the sample medians to d_medians[0, c1 - c0).  n >= 5.  An all-zero column (the
+ *                        reference panics) returns GL_ERANGE naming it.
+ *   gl_dcnv_normalize  : the same from host arrays; checks inds, streams blocks of block_cols columns (0: as many as fit in free
+ *                        device memory, 24 bytes per cell).  out may be x itself (out = x + c0, ld_out = ld).
+ *   gl_format_f2[_device] : the exact "%.2f" of every value as a 16-byte token, the text NUL-padded; an empty token means the
+ *                        text does not fit (|v| near or above 1e12) and the caller formats it.  NaN / ±Inf are spelled as Go
+ *                        does.  d_tokens is 16-byte aligned.
+ *   gl_format_f2_host  : host-only mirror of the same tokens. */
+int  gl_go_argsort_f64(const double* v, int64_t n, int64_t* inds);
+int  gl_dcnv_normalize_device(gl_ctx* ctx, const double* d_x, int64_t n, int64_t ld, const int64_t* d_inds, int32_t c0, int32_t c1,
+                              double* d_out, int64_t ld_out, double* d_medians);
+int  gl_dcnv_normalize(gl_ctx* ctx, const double* x, int64_t n, int64_t ld, const int64_t* inds, int32_t c0, int32_t c1, int32_t block_cols,
+                       double* out, int64_t ld_out, double* medians);
+int  gl_format_f2(gl_ctx* ctx, const double* vals, int64_t n, uint8_t* tokens);
+int  gl_format_f2_device(gl_ctx* ctx, const double* d_vals, int64_t n, uint8_t* d_tokens);
+int  gl_format_f2_host(const double* vals, int64_t n, uint8_t* tokens);
+
 /* ---------------------------------------------------------------- covstats
  * V2: histogram of int32 values in [lo,hi) -> hist[v-lo].  `goleft covstats` builds it over the sampled insert sizes,
  * template lengths and read lengths and reads every order statistic of covstats/covstats.go:57-76,175-199 off its running

@@ -9,6 +9,7 @@
 #   tests/golden/ref_indexcov_sample27.{bed,roc,ped}     goleft indexcov           on indexcov/test-data/sample_issue_27.bam(.bai)
 #   tests/golden/ref_depthwed.tsv                        goleft depthwed -s 1000   on two of the depth.bed files above
 #   tests/golden/ref_multidepth_t_<chrom>.txt            multidepth -Q 1 --minsamples 0 -c chrom on t.bam (contigs with reads)
+#   tests/golden/ref_dcnv_{depthwed,ties}.bed            dcnv on ref_depthwed.tsv and on dcnv_ties.tsv, with hg19.fa(.fai)
 #
 # This image has neither toolchain (`go version`, `samtools --version`: command not found), so the files cannot be made
 # here; until they exist every report says "bit-exact vs the restated oracle, parity unpinned".  tests/test_reference_goldens.py
@@ -70,5 +71,18 @@ fi
 samtools idxstats "$T/t.bam" | awk -F'\t' '$3 > 0 {print $1}' | while read -r c; do
   "$TMP/multidepth" -Q 1 -p 1 --minsamples 0 -c "$c" "$T/t.bam" > "$OUT/ref_multidepth_t_$c.txt"
 done
+# dcnv is another separate binary (dcnv/dcnv.go); it writes depth.bed in its working directory.  hg19.fa(.fai) is the
+# reference's own test FASTA, copied as a data fixture.  dcnv_ties.tsv: rows of 40 bases on chrM / chr22 share a few hundred
+# GC values, so the order pdqsort leaves inside ties is pinned.
+( cd "$REF" && CGO_ENABLED=0 go build -o "$TMP/dcnv" ./dcnv )
+if [[ -e "$T/hg19.fa" && -e "$T/hg19.fa.fai" ]]; then
+  cp "$T/hg19.fa" "$T/hg19.fa.fai" "$OUT/"
+  awk -F'\t' 'BEGIN{OFS="\t"; srand(7); printf "#chrom\tstart\tend"; for(i=0;i<7;i++) printf "\ts%d", i; print ""}
+       $1=="chrM" || $1=="chr22" {n=0; for(a=0; a+40<$2 && n<2000; a+=40){n++; printf "%s\t%d\t%d", $1, a, a+40; for(i=0;i<7;i++) printf "\t%d", int(rand()*60); print ""}}' \
+      "$T/hg19.fa.fai" > "$OUT/dcnv_ties.tsv"
+  for c in depthwed:ref_depthwed.tsv ties:dcnv_ties.tsv; do
+    ( cd "$TMP" && "$TMP/dcnv" "$OUT/${c#*:}" "$OUT/hg19.fa" >/dev/null && cp depth.bed "$OUT/ref_dcnv_${c%%:*}.bed" ) || true
+  done
+fi
 samtools --version | head -1 > "$OUT/ref_PROVENANCE.txt"; go version >> "$OUT/ref_PROVENANCE.txt"; (cd "$REF" && git rev-parse HEAD 2>/dev/null || true) >> "$OUT/ref_PROVENANCE.txt"
 echo "wrote $(ls "$OUT"/ref_* | wc -l) files to $OUT"

@@ -1746,6 +1746,102 @@ void go_log(const char* msg) {
     fprintf(stderr, "%04d/%02d/%02d %02d:%02d:%02d %s\n", tm.tm_year + 1900, tm.tm_mon + 1, tm.tm_mday, tm.tm_hour, tm.tm_min, tm.tm_sec, msg);
 }
 
+
+// The sites x samples matrix depthwed writes, read by dcnv and emdepth (dcnv.go:59-104 ReadRegions): plain, gzip/BGZF or "-".
+// ReadString('\n'): a final line without "\n" is dropped.  Header lines ('#' or "chrom") count only before the first data
+// line, and the last one names the samples.  Every reference panic is exit 2.
+struct Matrix {
+    std::string text;
+    std::vector<DcnvRow> rows;                               // data lines, without their "\n"
+    std::vector<std::string> header;                         // the header line's fields (trimmed)
+    std::vector<std::string> samples;                        // header[3:]
+    std::vector<double> X;                                   // matrix_parse: rows x samples, row-major
+    std::vector<int64_t> starts, ends;                       // as parsed (uint32 range)
+    std::vector<std::pair<const char*, size_t>> chrom;       // into text
+};
+
+void matrix_read(const std::string& path, Matrix& m) {
+    {
+        gzFile f = path == "-" ? gzdopen(dup(0), "rb") : gzopen(path.c_str(), "rb");
+        if (!f) fatal(2, "panic: open %s: %s", path.c_str(), strerror(errno));
+        gzbuffer(f, 1 << 20);
+        std::vector<char> buf((size_t)1 << 22);
+        int n;
+        while ((n = gzread(f, buf.data(), (unsigned)buf.size())) > 0) m.text.append(buf.data(), (size_t)n);
+        if (n < 0) fatal(2, "panic: read %s", path.c_str());
+        gzclose(f);
+    }
+    const std::string& text = m.text;
+    bool have_header = false;
+    for (size_t a = 0; a < text.size();) {
+        const char* nl = static_cast<const char*>(memchr(text.data() + a, '\n', text.size() - a));
+        if (!nl) break;
+        const size_t b = (size_t)(nl - text.data());
+        if (m.rows.empty() && (text[a] == '#' || text.compare(a, 5, "chrom") == 0)) {       // only before the first data line
+            size_t s = a, e = b + 1;
+            while (s < e && go_space(text[s])) s++;
+            while (e > s && go_space(text[e - 1])) e--;
+            std::vector<std::string> f;
+            for (size_t x = s;;) {
+                const size_t t = text.find('\t', x);
+                if (t == std::string::npos || t >= e) { f.push_back(text.substr(x, e - x)); break; }
+                f.push_back(text.substr(x, t - x));
+                x = t + 1;
+            }
+            if (f.size() < 3) fatal(2, "panic: runtime error: slice bounds out of range (header line has %zu fields)", f.size());
+            m.samples.assign(f.begin() + 3, f.end());
+            m.header = std::move(f);
+            have_header = true;
+        } else {
+            m.rows.push_back({text.data() + a, b - a});
+        }
+        a = b + 1;
+    }
+    if (!have_header) fatal(2, "panic: runtime error: integer divide by zero (no header line: no samples)");
+    if (m.samples.empty()) fatal(2, "panic: runtime error: integer divide by zero (the header names no samples)");
+}
+
+// chrom, start, end and one value per sample of every data line, on the host pool
+void matrix_parse(Matrix& m) {
+    const size_t R = m.rows.size(), S = m.samples.size();
+    m.X.assign(R * S, 0.0);
+    m.starts.assign(R, 0);
+    m.ends.assign(R, 0);
+    m.chrom.assign(R, {nullptr, 0});
+    const int64_t per = 4096, tasks = ((int64_t)R + per - 1) / per;
+    std::vector<std::string> errs((size_t)tasks);
+    glhost::ThreadPool::global().run(tasks, [&](int64_t t, int) {
+        for (size_t r = (size_t)t * per; r < std::min(R, (size_t)(t + 1) * per); r++) {
+            const char* p = m.rows[r].p;
+            const char* end = p + m.rows[r].n;
+            size_t col = 0;
+            auto fail = [&](const std::string& msg) { errs[(size_t)t] = "panic: line " + std::to_string(r + 1) + " of the data: " + msg; };
+            for (const char* a = p;; col++) {
+                const char* tab = static_cast<const char*>(memchr(a, '\t', (size_t)(end - a)));
+                const char* b = tab ? tab : end;
+                const char* s = a;
+                if (!tab) {                                                                // only the last field is trimmed
+                    while (s < b && go_space(*s)) s++;
+                    while (b > s && go_space(b[-1])) b--;
+                }
+                if (col == 0) m.chrom[r] = {s, (size_t)(b - s)};
+                else if (col < 3) {
+                    int64_t v;
+                    if (!dcnv_atou32(s, (size_t)(b - s), v)) { fail("strconv.Atoi: parsing \"" + std::string(s, b) + "\": invalid syntax or outside uint32"); return; }
+                    (col == 1 ? m.starts[r] : m.ends[r]) = v;
+                } else if (col - 3 < S) {
+                    if (!dcnv_atof(s, (size_t)(b - s), m.X[r * S + col - 3])) { fail("strconv.ParseFloat: parsing \"" + std::string(s, b) + "\": invalid syntax or out of range"); return; }
+                }
+                if (!tab) break;
+                a = tab + 1;
+            }
+            if (col < 2) { fail("runtime error: index out of range (fewer than 3 columns)"); return; }
+            if (col + 1 != S + 3) { fail(std::to_string(col - 2) + " values but " + std::to_string(S) + " samples in the header"); return; }
+        }
+    });
+    for (const std::string& e : errs) if (!e.empty()) fatal(2, "%s", e.c_str());
+}
+
 }  // namespace
 
 static int cmd_dcnv(int argc, char** argv) {
@@ -1758,48 +1854,10 @@ static int cmd_dcnv(int argc, char** argv) {
     fa.open(fasta);
     glhost_pool_warm();
 
-    // ---- the text: all of it, then its lines (ReadString('\n'): a final line without "\n" is dropped)
-    std::string text;
-    {
-        gzFile f = path == "-" ? gzdopen(dup(0), "rb") : gzopen(path.c_str(), "rb");
-        if (!f) fatal(2, "panic: open %s: %s", path.c_str(), strerror(errno));
-        gzbuffer(f, 1 << 20);
-        std::vector<char> buf((size_t)1 << 22);
-        int n;
-        while ((n = gzread(f, buf.data(), (unsigned)buf.size())) > 0) text.append(buf.data(), (size_t)n);
-        if (n < 0) fatal(2, "panic: read %s", path.c_str());
-        gzclose(f);
-    }
-    std::vector<DcnvRow> rows;
-    std::vector<std::string> samples;
-    bool have_header = false;
-    for (size_t a = 0; a < text.size();) {
-        const char* nl = static_cast<const char*>(memchr(text.data() + a, '\n', text.size() - a));
-        if (!nl) break;
-        const size_t b = (size_t)(nl - text.data());
-        if (rows.empty() && (text[a] == '#' || text.compare(a, 5, "chrom") == 0)) {       // only before the first data line
-            size_t s = a, e = b + 1;
-            while (s < e && go_space(text[s])) s++;
-            while (e > s && go_space(text[e - 1])) e--;
-            std::vector<std::string> f;
-            for (size_t x = s;;) {
-                const size_t t = text.find('\t', x);
-                if (t == std::string::npos || t >= e) { f.push_back(text.substr(x, e - x)); break; }
-                f.push_back(text.substr(x, t - x));
-                x = t + 1;
-            }
-            if (f.size() < 3) fatal(2, "panic: runtime error: slice bounds out of range (header line has %zu fields)", f.size());
-            samples.assign(f.begin() + 3, f.end());
-            have_header = true;
-        } else {
-            rows.push_back({text.data() + a, b - a});
-        }
-        a = b + 1;
-    }
-    if (!have_header) fatal(2, "panic: runtime error: integer divide by zero (no header line: no samples)");
-    const size_t S = samples.size();
-    const size_t R = rows.size();
-    if (S == 0) fatal(2, "panic: runtime error: integer divide by zero (the header names no samples)");
+    Matrix mx;
+    matrix_read(path, mx);
+    const std::vector<DcnvRow>& rows = mx.rows;
+    const size_t S = mx.samples.size(), R = rows.size();
     std::string label;                                           // ivs.Chrom: set by data lines 0 and 1, so the second wins
     for (size_t r = 0; r < std::min<size_t>(R, 2); r++) {
         const void* t = memchr(rows[r].p, '\t', rows[r].n);
@@ -1808,42 +1866,13 @@ static int cmd_dcnv(int argc, char** argv) {
     }
     mark("read");
 
-    // ---- rows on the host pool: chrom, clamped start, end, S values
-    std::vector<double> X(R * S);
-    std::vector<int64_t> starts(R), ends(R);
-    std::vector<std::pair<const char*, size_t>> chrom(R);
-    const int64_t per = 4096, tasks = ((int64_t)R + per - 1) / per;
-    std::vector<std::string> errs((size_t)tasks);
-    glhost::ThreadPool::global().run(tasks, [&](int64_t t, int) {
-        for (size_t r = (size_t)t * per; r < std::min(R, (size_t)(t + 1) * per); r++) {
-            const char* p = rows[r].p;
-            const char* end = p + rows[r].n;
-            size_t col = 0;
-            auto fail = [&](const std::string& m) { errs[(size_t)t] = "panic: line " + std::to_string(r + 1) + " of the data: " + m; };
-            for (const char* a = p;; col++) {
-                const char* tab = static_cast<const char*>(memchr(a, '\t', (size_t)(end - a)));
-                const char* b = tab ? tab : end;
-                const char* s = a;
-                if (!tab) {                                                                // only the last field is trimmed
-                    while (s < b && go_space(*s)) s++;
-                    while (b > s && go_space(b[-1])) b--;
-                }
-                if (col == 0) chrom[r] = {s, (size_t)(b - s)};
-                else if (col < 3) {
-                    int64_t v;
-                    if (!dcnv_atou32(s, (size_t)(b - s), v)) { fail("strconv.Atoi: parsing \"" + std::string(s, b) + "\": invalid syntax or outside uint32"); return; }
-                    (col == 1 ? starts[r] : ends[r]) = col == 1 ? std::max<int64_t>(v, 250) : v;      // dcnv.go:83-85
-                } else if (col - 3 < S) {
-                    if (!dcnv_atof(s, (size_t)(b - s), X[r * S + col - 3])) { fail("strconv.ParseFloat: parsing \"" + std::string(s, b) + "\": invalid syntax or out of range"); return; }
-                }
-                if (!tab) break;
-                a = tab + 1;
-            }
-            if (col < 2) { fail("runtime error: index out of range (fewer than 3 columns)"); return; }
-            if (col + 1 != S + 3) { fail(std::to_string(col - 2) + " values but " + std::to_string(S) + " samples in the header"); return; }
-        }
-    });
-    for (const std::string& e : errs) if (!e.empty()) fatal(2, "%s", e.c_str());
+    // ---- rows on the host pool: chrom, start (clamped to 250, dcnv.go:83-85), end, S values
+    matrix_parse(mx);
+    std::vector<double>& X = mx.X;
+    std::vector<int64_t>& starts = mx.starts;
+    const std::vector<int64_t>& ends = mx.ends;
+    const std::vector<std::pair<const char*, size_t>>& chrom = mx.chrom;
+    for (int64_t& v : starts) v = std::max<int64_t>(v, 250);
     if (R < 5) fatal(2, "panic: runtime error: index out of range (%zu data rows; the moving median needs 5)", R);
     mark("parse");
 
@@ -1896,7 +1925,7 @@ static int cmd_dcnv(int argc, char** argv) {
     FILE* fo = fopen("depth.bed", "w");
     if (!fo) fatal(2, "panic: open depth.bed: %s", strerror(errno));
     std::string head = "#chrom\tstart\tend";
-    for (const std::string& s : samples) head += "\t" + s;
+    for (const std::string& s : mx.samples) head += "\t" + s;
     head += "\n";
     fwrite(head.data(), 1, head.size(), fo);
     const size_t chunk_rows = std::max<size_t>(1, ((size_t)1 << 24) / S);
@@ -1932,6 +1961,115 @@ static int cmd_dcnv(int argc, char** argv) {
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ emdepth
+// emdepth/emdepth.go (a library of the reference with no command; DESIGN §1.10): `goleft emdepth [--prefix P] <matrix>` reads
+// the matrix dcnv reads (matrix_read / matrix_parse; no 250 clamp, every row keeps its own chromosome), takes each value as
+// float32(ParseFloat), runs the EM of every row on the GPU (gl_emdepth, row blocks sized to device memory) and walks the
+// reference's Cache on the host (gl_emdepth_cnvs: Clear(nil) at every chromosome change and at the end).  Writes P.cn.bed (the
+// header line, then chrom, start, end and one CN per sample) and P.cnv.bed (#chrom start end sample n cns psize: the first
+// kept row's chromosome and start, the last kept row's end, the rows' CNs comma-joined).  Every error is exit 2.
+static int cmd_emdepth(int argc, char** argv) {
+    std::string prefix = "emdepth";
+    ArgParser ap;
+    ap.prog = "goleft emdepth";
+    ap.add("prefix", 0, &prefix);
+    ap.parse(argc, argv);
+    if (ap.positional.size() != 1) fatal(2, "panic: usage: goleft emdepth [--prefix P] <matrix>");
+    const bool timing = getenv("GL_TIMING") != nullptr;        // phase wall clocks on stderr
+    double tp = now_s();
+    auto mark = [&](const char* what) { if (timing) { const double t = now_s(); fprintf(stderr, "[emdepth timing] %-22s %.3f s\n", what, t - tp); tp = t; } };
+    glhost_pool_warm();
+
+    Matrix mx;
+    matrix_read(ap.positional[0], mx);
+    mark("read");
+    matrix_parse(mx);
+    const size_t S = mx.samples.size(), R = mx.rows.size();
+    if (S == 2) fatal(2, "panic: runtime error: index out of range [2] with length 2 (median32 of 2 samples)");
+    std::vector<float> X((size_t)R * S);                          // float32(strconv.ParseFloat(tok, 64))
+    const int64_t per = 4096, tasks = ((int64_t)R + per - 1) / per;
+    glhost::ThreadPool::global().run(tasks, [&](int64_t t, int) {
+        for (size_t i = (size_t)t * per * S; i < std::min(R, (size_t)(t + 1) * per) * S; i++) X[i] = (float)mx.X[i];
+    });
+    mark("parse");
+
+    gl_ctx* ctx = open_ctx(0, "goleft emdepth");
+    std::vector<uint8_t> cells((size_t)R * S);
+    const char* br = getenv("GL_EMDEPTH_BLOCK_ROWS");
+    const int rc = gl_emdepth(ctx, X.data(), (int64_t)R, (int64_t)S, (int32_t)S, br ? atoll(br) : 0, cells.data(), nullptr);
+    if (rc == GL_EINVAL) fatal(2, "panic: %s", gl_last_error(ctx));
+    glck(ctx, rc, "gl_emdepth");
+    int64_t n_unc = 0;
+    gl_emdepth_stats(ctx, nullptr, &n_unc, nullptr);
+    if (n_unc) fprintf(stderr, "emdepth: %lld cells were decided inside the error band of the reference's CPU-dependent Exp / Log\n", (long long)n_unc);
+    mark("em");
+
+    const std::string cn_path = prefix + ".cn.bed", cnv_path = prefix + ".cnv.bed";
+    FILE* fo = fopen(cn_path.c_str(), "w");
+    if (!fo) fatal(2, "panic: open %s: %s", cn_path.c_str(), strerror(errno));
+    std::string head;
+    for (size_t i = 0; i < mx.header.size(); i++) head += (i ? "\t" : "") + mx.header[i];
+    head += "\n";
+    fwrite(head.data(), 1, head.size(), fo);
+    const size_t per_text = 4096, groups = (R + per_text - 1) / per_text, group_batch = 64;
+    for (size_t g0 = 0; g0 < groups; g0 += group_batch) {
+        const size_t ng = std::min(group_batch, groups - g0);
+        std::vector<std::string> parts(ng);
+        glhost::ThreadPool::global().run((int64_t)ng, [&](int64_t k, int) {
+            std::string& o = parts[(size_t)k];
+            char num[48];
+            const size_t r0 = (g0 + (size_t)k) * per_text;
+            for (size_t r = r0; r < std::min(R, r0 + per_text); r++) {
+                o.append(mx.chrom[r].first, mx.chrom[r].second);
+                o.append(num, (size_t)snprintf(num, sizeof num, "\t%lld\t%lld", (long long)mx.starts[r], (long long)mx.ends[r]));
+                for (size_t c = 0; c < S; c++) {
+                    o += '\t';
+                    o += (char)('0' + (cells[r * S + c] & 15));
+                }
+                o += '\n';
+            }
+        });
+        for (const std::string& p : parts) fwrite(p.data(), 1, p.size(), fo);
+    }
+    if (fclose(fo) != 0) fatal(1, "write %s: %s", cn_path.c_str(), strerror(errno));
+    mark("cn.bed");
+
+    std::vector<int64_t> breaks;                                  // rows where a chromosome starts
+    for (size_t r = 1; r < R; r++)
+        if (mx.chrom[r].second != mx.chrom[r - 1].second || memcmp(mx.chrom[r].first, mx.chrom[r - 1].first, mx.chrom[r].second) != 0)
+            breaks.push_back((int64_t)r);
+    int64_t nc = 0, nr = 0;
+    auto walk = [&](int32_t* smp, int32_t* psz, int64_t* ptr, int64_t* rows) {
+        return gl_emdepth_cnvs(cells.data(), (int64_t)R, (int32_t)S, mx.starts.data(), mx.ends.data(), breaks.data(), (int64_t)breaks.size(),
+                               smp, psz, ptr, nc, &nc, rows, nr, &nr);
+    };
+    if (walk(nullptr, nullptr, nullptr, nullptr) != GL_OK) fatal(1, "gl_emdepth_cnvs: bad arguments");
+    std::vector<int32_t> smp((size_t)nc), psz((size_t)nc);
+    std::vector<int64_t> ptr((size_t)nc + 1), rows((size_t)nr);
+    if (walk(smp.data(), psz.data(), ptr.data(), rows.data()) != GL_OK) fatal(1, "gl_emdepth_cnvs: bad arguments");
+    fo = fopen(cnv_path.c_str(), "w");
+    if (!fo) fatal(2, "panic: open %s: %s", cnv_path.c_str(), strerror(errno));
+    std::string o = "#chrom\tstart\tend\tsample\tn\tcns\tpsize\n";
+    char num[64];
+    for (int64_t i = 0; i < nc; i++) {
+        const int64_t a = rows[(size_t)ptr[(size_t)i]], b = rows[(size_t)ptr[(size_t)i + 1] - 1];
+        o.append(mx.chrom[(size_t)a].first, mx.chrom[(size_t)a].second);
+        o.append(num, (size_t)snprintf(num, sizeof num, "\t%lld\t%lld\t", (long long)mx.starts[(size_t)a], (long long)mx.ends[(size_t)b]));
+        o += mx.samples[(size_t)smp[(size_t)i]];
+        o.append(num, (size_t)snprintf(num, sizeof num, "\t%lld\t", (long long)(ptr[(size_t)i + 1] - ptr[(size_t)i])));
+        for (int64_t k = ptr[(size_t)i]; k < ptr[(size_t)i + 1]; k++) {
+            if (k > ptr[(size_t)i]) o += ',';
+            o += (char)('0' + (cells[(size_t)rows[(size_t)k] * S + (size_t)smp[(size_t)i]] & 15));
+        }
+        o.append(num, (size_t)snprintf(num, sizeof num, "\t%d\n", psz[(size_t)i]));
+    }
+    fwrite(o.data(), 1, o.size(), fo);
+    if (fclose(fo) != 0) fatal(1, "write %s: %s", cnv_path.c_str(), strerror(errno));
+    mark("cnv.bed");
+    gl_ctx_destroy(ctx);
+    return 0;
+}
+
 static void print_progs() {                                                          // cmd/goleft/goleft.go:33-53
     fprintf(stderr, "goleft Version: %s (GPU engine: %s)\n\n", kVersion, gl_version());
     fprintf(stderr, "covstats    : coverage and insert-size statistics on bams by sampling\n");
@@ -1942,6 +2080,7 @@ static void print_progs() {                                                     
     fprintf(stderr, "samplename  : report samplename(s) from a bam's SM tag\n");
     fprintf(stderr, "multidepth  : (extension; a separate binary in goleft) blocks of sufficient coverage across many bams\n");
     fprintf(stderr, "dcnv        : (extension; a separate binary in goleft) GC-debias and median-normalise a depthwed matrix\n");
+    fprintf(stderr, "emdepth     : (extension; a library in goleft) per-sample copy numbers and CNVs from a depth matrix\n");
 }
 
 int main(int argc, char** argv) {
@@ -1955,6 +2094,7 @@ int main(int argc, char** argv) {
     if (prog == "samplename") return cmd_samplename(argc - 1, argv + 1);
     if (prog == "multidepth") return cmd_multidepth(argc - 1, argv + 1);
     if (prog == "dcnv") return cmd_dcnv(argc - 1, argv + 1);
+    if (prog == "emdepth") return cmd_emdepth(argc - 1, argv + 1);
     print_progs();
     return 1;
 }

@@ -308,3 +308,62 @@ func (c *Ctx) FormatF2(vals []float64) ([]byte, error) {
 	rc := C.gl_format_f2(c.h, (*C.double)(&vals[0]), C.int64_t(len(vals)), (*C.uint8_t)(&tok[0]))
 	return tok[:16*len(vals)], c.err(rc)
 }
+
+// Emdepth replaces emdepth.EMDepth + EMD.CN / Log2FC / Same of emdepth/emdepth.go:117-304 on the n x S row-major float32
+// matrix `depths`: one byte per cell (bits 0-3 the CN, bits 4-5 the Same class of Log2FC, bit 6 set when Log2FC is outside
+// (-0.5, 0.3)), and the nine final centres of every row.  Rows are streamed in blocks sized to free device memory.
+func (c *Ctx) Emdepth(depths []float32, samples int) (cells []uint8, lambda []float64, err error) {
+	n := len(depths) / samples
+	cells = make([]uint8, n*samples+1)
+	lambda = make([]float64, n*9+1)
+	rc := C.gl_emdepth(c.h, (*C.float)(&depths[0]), C.int64_t(n), C.int64_t(samples), C.int32_t(samples), 0,
+		(*C.uint8_t)(&cells[0]), (*C.double)(&lambda[0]))
+	return cells[:n*samples], lambda[:n*9], c.err(rc)
+}
+
+// EmdepthStats reports, for the last Emdepth call, the rows done, the cells decided inside the error band of the
+// reference's CPU-dependent Exp / Log, and the bin means summed in sample order.
+func (c *Ctx) EmdepthStats() (rows, uncertified, sequential int64) {
+	var r, u, s C.int64_t
+	C.gl_emdepth_stats(c.h, &r, &u, &s)
+	return int64(r), int64(u), int64(s)
+}
+
+// EmdepthCNV is one emdepth.CNV: the sample, PSize, and the rows it holds (their CNs are cells[row*S+Sample] & 15).
+type EmdepthCNV struct {
+	Sample, PSize int
+	Rows          []int64
+}
+
+// EmdepthCNVs walks emdepth.Cache over the cells in row order (emdepth/emdepth.go:330-398), with Clear(nil) before every
+// row in breaks (the rows where a chromosome starts) and after the last row.  CNVs of one Clear come in sample order.
+func EmdepthCNVs(cells []uint8, samples int, starts, ends, breaks []int64) ([]EmdepthCNV, error) {
+	n := len(starts)
+	var nc, nr C.int64_t
+	pc := (*C.uint8_t)(unsafe.Pointer(nil))
+	if len(cells) > 0 {
+		pc = (*C.uint8_t)(&cells[0])
+	}
+	ps, pe, pb := (*C.int64_t)(unsafe.Pointer(nil)), (*C.int64_t)(unsafe.Pointer(nil)), (*C.int64_t)(unsafe.Pointer(nil))
+	if n > 0 {
+		ps, pe = (*C.int64_t)(&starts[0]), (*C.int64_t)(&ends[0])
+	}
+	if len(breaks) > 0 {
+		pb = (*C.int64_t)(&breaks[0])
+	}
+	if C.gl_emdepth_cnvs(pc, C.int64_t(n), C.int32_t(samples), ps, pe, pb, C.int64_t(len(breaks)), nil, nil, nil, 0, &nc,
+		nil, 0, &nr) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_emdepth_cnvs failed")
+	}
+	smp, psz := make([]int32, nc+1), make([]int32, nc+1)
+	ptr, rows := make([]int64, nc+1), make([]int64, nr+1)
+	if C.gl_emdepth_cnvs(pc, C.int64_t(n), C.int32_t(samples), ps, pe, pb, C.int64_t(len(breaks)), (*C.int32_t)(&smp[0]),
+		(*C.int32_t)(&psz[0]), (*C.int64_t)(&ptr[0]), nc, &nc, (*C.int64_t)(&rows[0]), nr, &nr) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_emdepth_cnvs failed")
+	}
+	out := make([]EmdepthCNV, int(nc))
+	for i := range out {
+		out[i] = EmdepthCNV{Sample: int(smp[i]), PSize: int(psz[i]), Rows: append([]int64(nil), rows[ptr[i]:ptr[i+1]]...)}
+	}
+	return out, nil
+}

@@ -187,6 +187,13 @@ _proto("gl_dcnv_normalize", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_in
 _proto("gl_format_f2", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_f2_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_f2_host", C.c_int, _vp, C.c_int64, _vp)
+_proto("gl_emdepth_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, _vp, _vp)
+_proto("gl_emdepth", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_int64, _vp, _vp)
+_proto("gl_emdepth_stats", C.c_int, _vp, _i64p, _i64p, _i64p)
+_proto("gl_emdepth_factors", C.c_int, _vp)
+_proto("gl_emdepth_cnvs", C.c_int, _vp, C.c_int64, C.c_int32, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_int64, _i64p,
+       _vp, C.c_int64, _i64p)
+_proto("gl_emdepth_sum_host", C.c_int, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_uint8))
 
 
 def version() -> str:
@@ -327,6 +334,46 @@ def f2_text(tokens, vals) -> list:
         b = t.tobytes().rstrip(b"\0")
         out.append(b if b else b"%.2f" % v)
     return out
+
+
+# ---- emdepth (emdepth/emdepth.go), host-only parts
+EM_CN_MASK, EM_OUTSIDE = 0x0F, 0x40
+
+
+def emdepth_factors() -> np.ndarray:
+    """Host-only: math.Pow(i / 2, 1.1), i = 0..8, as the kernel uses them"""
+    f = np.empty(9, np.float64)
+    lib.gl_emdepth_factors(_ptr(f))
+    return f
+
+
+def emdepth_cnvs(cells, starts, ends, breaks=()):
+    """Host-only: the reference's Cache over the cells (n x S) -> [(sample, psize, row indices)], Clear(nil) before every row
+    in breaks and after the last"""
+    cells = _as(cells, np.uint8)
+    n, S = cells.shape
+    starts, ends, breaks = _as(starts, np.int64), _as(ends, np.int64), _as(breaks, np.int64)
+    nc, nr = C.c_int64(0), C.c_int64(0)
+    args = (_ptr(cells), n, S, _ptr(starts), _ptr(ends), _ptr(breaks), breaks.size)
+    rc = lib.gl_emdepth_cnvs(*args, None, None, None, 0, C.byref(nc), None, 0, C.byref(nr))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_emdepth_cnvs: bad arguments")
+    smp, psz, ptr = np.empty(nc.value, np.int32), np.empty(nc.value, np.int32), np.zeros(nc.value + 1, np.int64)
+    rows = np.empty(nr.value, np.int64)
+    rc = lib.gl_emdepth_cnvs(*args, _ptr(smp), _ptr(psz), _ptr(ptr), nc.value, C.byref(nc), _ptr(rows), nr.value, C.byref(nr))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_emdepth_cnvs: bad arguments")
+    return [(int(smp[i]), int(psz[i]), rows[ptr[i]:ptr[i + 1]]) for i in range(nc.value)]
+
+
+def emdepth_sum_host(v):
+    """Host-only: (the kernel's tree-order float64 sum of v, whether its exactness certificate holds)"""
+    v = _as(v, np.float32)
+    s, ok = C.c_double(0), C.c_uint8(0)
+    rc = lib.gl_emdepth_sum_host(_ptr(v), v.size, C.byref(s), C.byref(ok))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_emdepth_sum_host: bad arguments")
+    return s.value, bool(ok.value)
 
 
 def chunk_rows(rs: int, re: int, W: int, run_start: np.ndarray, run_class: np.ndarray):
@@ -1141,6 +1188,26 @@ class Ctx:
 
     def format_f2_device(self, d_vals: DevBuf, n: int, d_tokens: DevBuf):
         self._ck(lib.gl_format_f2_device(self.h, d_vals.ptr, n, d_tokens.ptr))
+
+    # ---- emdepth
+    def emdepth(self, x: np.ndarray, block_rows: int = 0, ld: Optional[int] = None, S: Optional[int] = None, want_lambda: bool = True):
+        """cells (n x S uint8) and the final centres (n x 9, or None) of the float32 rows of x (columns [0, S) of each row)"""
+        x = np.ascontiguousarray(x, np.float32)
+        n, ld = x.shape[0], x.shape[1] if ld is None else ld
+        S = x.shape[1] if S is None else S
+        cells = np.empty((n, S), np.uint8)
+        lam = np.empty((n, 9), np.float64) if want_lambda else None
+        self._ck(lib.gl_emdepth(self.h, _ptr(x), n, ld, S, block_rows, _ptr(cells), _ptr(lam)))
+        return cells, lam
+
+    def emdepth_device(self, d_x: DevBuf, n: int, ld: int, S: int, d_cells: DevBuf, d_lambda: Optional[DevBuf] = None):
+        self._ck(lib.gl_emdepth_device(self.h, d_x.ptr, n, ld, S, d_cells.ptr, d_lambda.ptr if d_lambda else None))
+
+    def emdepth_stats(self):
+        """{rows, uncertified, sequential} of the last emdepth call"""
+        v = [C.c_int64(0) for _ in range(3)]
+        self._ck(lib.gl_emdepth_stats(self.h, *[C.byref(x) for x in v]))
+        return dict(zip(("rows", "uncertified", "sequential"), (x.value for x in v)))
 
     # ---- multi-GPU
     def comm_init(self, id128: bytes, rank: int, world: int):

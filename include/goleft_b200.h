@@ -491,6 +491,38 @@ int  gl_format_f2(gl_ctx* ctx, const double* vals, int64_t n, uint8_t* tokens);
 int  gl_format_f2_device(gl_ctx* ctx, const double* d_vals, int64_t n, uint8_t* d_tokens);
 int  gl_format_f2_host(const double* vals, int64_t n, uint8_t* tokens);
 
+/* ---------------------------------------------------------------- emdepth
+ * Restates emdepth/emdepth.go (a library of the reference with no command): a cn.mops-style EM per row of an n x S depth
+ * matrix, the copy number (CN) of every cell, and the Cache that merges non-CN2 rows into per-sample CNVs (DESIGN §1.10).
+ * Values are used as given (float32, no normalisation); each must be finite, non-negative (sign bit clear) and below 2^62,
+ * else GL_EINVAL naming the row (a policy: the reference panics only for some of these values).  S = 2 is GL_EINVAL (the reference's even median indexes out of range); 1 <= S <= 65535.
+ * One byte per cell, row-major n x S: bits 0-3 the CN (0..9; 9 = above the top centre), bits 4-5 the Same class of
+ * Log2FC = log2(d / lambda[2]) (0: -0.8 < fc < 0.4, 1: fc <= -0.8, 2: fc >= 0.4, 3: NaN), bit 6 set when fc is outside
+ * (-0.5, 0.3).
+ *   gl_emdepth_device : rows of the row-major float32 matrix d_x (row stride ld >= S); d_cells n x S; d_lambda (nullable)
+ *                       n x 9 final centres.
+ *   gl_emdepth        : the same from host arrays, streamed in blocks of block_rows rows (0: as many as fit in free device
+ *                       memory, 5 bytes per cell).
+ *   gl_emdepth_stats  : of the last call: rows, cells whose Poisson test or Log2FC thresholds fell inside the error band of
+ *                       the reference's CPU-dependent Exp / Log (decided by the device's functions: UNPINNED), and bin
+ *                       means that were summed in sample order because a tree sum could round differently.
+ *   gl_emdepth_factors : host-only: the centres' factors math.Pow(i / 2, 1.1), i = 0..8, as the kernel uses them.
+ *   gl_emdepth_cnvs   : host-only: the reference's Cache over the rows in order, Clear(nil) before every row in breaks[]
+ *                       (sorted row indices where a chromosome starts) and after the last row; starts / ends are the rows'
+ *                       uint32 positions.  CNV i is sample cnv_sample[i] with PSize cnv_psize[i]; its rows are
+ *                       rows[cnv_ptr[i], cnv_ptr[i+1]).  Within one Clear, CNVs come in sample order.  NULL outputs count
+ *                       only; GL_ERANGE (with the counts set) when cap or rows_cap is too small.
+ *   gl_emdepth_sum_host : host-only mirror of the kernel's bin sum: the float64 sum of v in a warp's order (32 strided
+ *                       partial sums, then a butterfly) and whether the exactness certificate holds for it. */
+int  gl_emdepth_device(gl_ctx* ctx, const float* d_x, int64_t n, int64_t ld, int32_t S, uint8_t* d_cells, double* d_lambda);
+int  gl_emdepth(gl_ctx* ctx, const float* x, int64_t n, int64_t ld, int32_t S, int64_t block_rows, uint8_t* cells, double* lambda);
+int  gl_emdepth_stats(gl_ctx* ctx, int64_t* n_rows, int64_t* n_uncertified, int64_t* n_sequential);
+int  gl_emdepth_factors(double* f9);
+int  gl_emdepth_cnvs(const uint8_t* cells, int64_t n, int32_t S, const int64_t* starts, const int64_t* ends, const int64_t* breaks,
+                     int64_t n_breaks, int32_t* cnv_sample, int32_t* cnv_psize, int64_t* cnv_ptr, int64_t cap, int64_t* n_cnvs,
+                     int64_t* rows, int64_t rows_cap, int64_t* n_rows);
+int  gl_emdepth_sum_host(const float* v, int64_t n, double* sum, uint8_t* certified);
+
 /* ---------------------------------------------------------------- covstats
  * V2: histogram of int32 values in [lo,hi) -> hist[v-lo].  `goleft covstats` builds it over the sampled insert sizes,
  * template lengths and read lengths and reads every order statistic of covstats/covstats.go:57-76,175-199 off its running

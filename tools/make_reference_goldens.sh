@@ -10,6 +10,11 @@
 #   tests/golden/ref_depthwed.tsv                        goleft depthwed -s 1000   on two of the depth.bed files above
 #   tests/golden/ref_multidepth_t_<chrom>.txt            multidepth -Q 1 --minsamples 0 -c chrom on t.bam (contigs with reads)
 #   tests/golden/ref_dcnv_{depthwed,ties}.bed            dcnv on ref_depthwed.tsv and on dcnv_ties.tsv, with hg19.fa(.fai)
+#   tests/golden/ref_emdepth_pow.txt                     the bits of math.Pow(i/2, 1.1), i = 1, 3..8, as Go computes them
+#   tests/golden/ref_emdepth.{cn,cnv}.bed                our driver over the reference's emdepth package on emdepth_cohort.tsv
+#                                                        (9 samples with planted CN1 / CN3 runs; ref_depthwed.tsv has 2 samples,
+#                                                        where the reference's median32 panics)
+#   tests/golden/ref_emdepth_gotest.txt                  `go test ./emdepth` (its TestBig fails: it expects CN 8, the code gives 9)
 #
 # This image has neither toolchain (`go version`, `samtools --version`: command not found), so the files cannot be made
 # here; until they exist every report says "bit-exact vs the restated oracle, parity unpinned".  tests/test_reference_goldens.py
@@ -84,5 +89,121 @@ if [[ -e "$T/hg19.fa" && -e "$T/hg19.fa.fai" ]]; then
     ( cd "$TMP" && "$TMP/dcnv" "$OUT/${c#*:}" "$OUT/hg19.fa" >/dev/null && cp depth.bed "$OUT/ref_dcnv_${c%%:*}.bed" ) || true
   done
 fi
+# emdepth is a library of the reference with no command.  The driver below (ours, DESIGN §1.10) builds against a copy of
+# the package's non-test sources made here at run time: one Cache over the rows in file order, Clear(nil) at every
+# chromosome change and at the end, the CNVs of one Clear in sample order.  It writes P.cn.bed / P.cnv.bed as
+# `goleft emdepth --prefix P` does, and prints the Pow bits.
+mkdir -p "$TMP/emdrv/emdepth"
+cp "$REF"/emdepth/emdepth.go "$REF"/emdepth/stats.go "$TMP/emdrv/emdepth/"
+printf 'module emdrv\n\ngo 1.12\n' > "$TMP/emdrv/go.mod"
+cat > "$TMP/emdrv/main.go" <<'GO'
+package main
+
+import (
+	"bufio"
+	"fmt"
+	"math"
+	"os"
+	"sort"
+	"strconv"
+	"strings"
+
+	"emdrv/emdepth"
+)
+
+type row struct {
+	chrom      string
+	start, end uint32
+}
+
+func main() {
+	if os.Args[1] == "pow" {
+		for _, i := range []int{1, 3, 4, 5, 6, 7, 8} {
+			fmt.Printf("%x\n", math.Float64bits(math.Pow(float64(i)/2, 1.1)))
+		}
+		return
+	}
+	f, err := os.Open(os.Args[1])
+	if err != nil {
+		panic(err)
+	}
+	prefix := os.Args[2]
+	cn, _ := os.Create(prefix + ".cn.bed")
+	cnv, _ := os.Create(prefix + ".cnv.bed")
+	wcn, wcnv := bufio.NewWriter(cn), bufio.NewWriter(cnv)
+	fmt.Fprintln(wcnv, "#chrom\tstart\tend\tsample\tn\tcns\tpsize")
+	br := bufio.NewReader(f)
+	var samples []string
+	var rows []row
+	var cache emdepth.Cache
+	emit := func(cs []*emdepth.CNV) {
+		sort.Slice(cs, func(a, b int) bool { return cs[a].SampleI < cs[b].SampleI })
+		for _, c := range cs {
+			p0, p1 := c.Position[0], c.Position[len(c.Position)-1]
+			chrom := ""
+			for k := len(rows) - 1; k >= 0; k-- { // the most recent row at the first kept position
+				if rows[k].start == p0.Start && rows[k].end == p0.End {
+					chrom = rows[k].chrom
+					break
+				}
+			}
+			cns := make([]string, len(c.CN))
+			for k, v := range c.CN {
+				cns[k] = strconv.Itoa(v)
+			}
+			fmt.Fprintf(wcnv, "%s\t%d\t%d\t%s\t%d\t%s\t%d\n", chrom, p0.Start, p1.End, samples[c.SampleI], len(c.CN), strings.Join(cns, ","), c.PSize)
+		}
+	}
+	for {
+		line, err := br.ReadString('\n')
+		if err != nil {
+			break
+		}
+		if len(rows) == 0 && (line[0] == '#' || strings.HasPrefix(line, "chrom")) {
+			h := strings.Split(strings.TrimSpace(line), "\t")
+			samples = h[3:]
+			fmt.Fprintln(wcn, strings.Join(h, "\t"))
+			continue
+		}
+		toks := strings.Split(strings.TrimSpace(line), "\t")
+		s, _ := strconv.Atoi(toks[1])
+		e, _ := strconv.Atoi(toks[2])
+		r := row{toks[0], uint32(s), uint32(e)}
+		if len(rows) > 0 && rows[len(rows)-1].chrom != r.chrom {
+			emit(cache.Clear(nil))
+		}
+		rows = append(rows, r)
+		d := make([]float32, len(toks)-3)
+		for k, t := range toks[3:] {
+			v, err := strconv.ParseFloat(t, 64)
+			if err != nil {
+				panic(err)
+			}
+			d[k] = float32(v)
+		}
+		em := emdepth.EMDepth(d, emdepth.Position{Start: r.start, End: r.end})
+		c := em.CN()
+		out := make([]string, len(c))
+		for k, v := range c {
+			out[k] = strconv.Itoa(v)
+		}
+		fmt.Fprintf(wcn, "%s\t%d\t%d\t%s\n", r.chrom, r.start, r.end, strings.Join(out, "\t"))
+		emit(cache.Add(em))
+	}
+	emit(cache.Clear(nil))
+	wcn.Flush()
+	wcnv.Flush()
+	cn.Close()
+	cnv.Close()
+}
+GO
+( cd "$TMP/emdrv" && CGO_ENABLED=0 go build -o "$TMP/emdrv_bin" . )
+"$TMP/emdrv_bin" pow > "$OUT/ref_emdepth_pow.txt"
+awk 'BEGIN{OFS="\t"; srand(11); printf "#chrom\tstart\tend"; for(i=0;i<9;i++) printf "\ts%d", i; print ""
+     for(c=1;c<=2;c++) for(r=0;r<(c==1?2000:1000);r++){printf "chr%d\t%d\t%d", c, r*1000, r*1000+1000
+       for(i=0;i<9;i++){v=30+rand()*10; if(c==1&&i==3&&r>=500&&r<540) v/=2; if(c==2&&i==6&&r>=100&&r<130) v*=1.5; printf "\t%d", int(v)}
+       print ""}}' > "$OUT/emdepth_cohort.tsv"
+"$TMP/emdrv_bin" "$OUT/emdepth_cohort.tsv" "$TMP/em" && cp "$TMP/em.cn.bed" "$OUT/ref_emdepth.cn.bed" && cp "$TMP/em.cnv.bed" "$OUT/ref_emdepth.cnv.bed" || true
+( cd "$REF" && go test ./emdepth 2>&1 || true ) > "$OUT/ref_emdepth_gotest.txt"
 samtools --version | head -1 > "$OUT/ref_PROVENANCE.txt"; go version >> "$OUT/ref_PROVENANCE.txt"; (cd "$REF" && git rev-parse HEAD 2>/dev/null || true) >> "$OUT/ref_PROVENANCE.txt"
 echo "wrote $(ls "$OUT"/ref_* | wc -l) files to $OUT"

@@ -3,7 +3,7 @@
 // computed by libgoleft_b200.so (CUDA, sm_90a) through the C ABI in include/goleft_b200.h; there is no CPU
 // fallback: without a GPU the subcommands fail with the library's error.
 //
-// Out of scope here (SURVEY.md §2): HTML/PNG plots, PCA columns of the .ped, --stats GC columns.  .crai input needs --fai.
+// Out of scope here (SURVEY.md §2): HTML/PNG plots, --stats GC columns.  .crai input needs --fai.
 #include <errno.h>
 #include <math.h>
 #include <stdarg.h>
@@ -31,6 +31,7 @@
 #include "../goleft_b200/csrc/host/hts_io.h"
 #include "../goleft_b200/csrc/host/bam_feed.h"
 #include "../goleft_b200/csrc/host/thread_pool.h"
+#include "../goleft_b200/csrc/host/pca8.h"
 #include "goleft_b200.h"
 
 static const char* kVersion = "0.2.6";          // goleft.go:3 (the surface this build mirrors)
@@ -1082,6 +1083,23 @@ static int cmd_indexcov(int argc, char** argv) {
     std::vector<int64_t> bins(S * 4, 0);
     std::vector<float> slopes(S, 0);
     int n_slopes = 0;
+    // the PCA's byte matrix (indexcov.go:686-705): every kept reference that is not a sex chromosome gives each sample
+    // longest + 1 columns, its clipped values' bytes and then zeros (the range loop leaves i at the last index, or -1)
+    std::vector<int64_t> pca_col(kept.size(), -1);
+    int64_t pca_D = 0;
+    for (size_t q = 0; q < kept.size(); q++) {
+        if (same_chrom(sexes_wanted, kept[q]->name)) continue;
+        int64_t lg = 0;
+        for (size_t k = 0; k < S; k++)
+            if (kept[q]->id + 1 < (int)size_ptr[k].size() && med[k] != 0)
+                lg = std::max(lg, size_ptr[k][kept[q]->id + 1] - size_ptr[k][kept[q]->id]);
+        pca_col[q] = pca_D;
+        pca_D += lg + 1;
+    }
+    const int64_t pca_rank = std::min<int64_t>((int64_t)S, pca_D);          // gonum's min(S, D) components
+    const int64_t pca_ld = (pca_D + 63) / 64 * 64;
+    RawBuf<uint8_t> pca_x;
+    if (pca_rank >= 3) pca_x.resize(S * (size_t)pca_ld);
     for (size_t q = 0; q < kept.size(); q++) {
         const IcRef& ref = *kept[q];
         // per-sample slices of this reference (ref.ID() indexes the index's reference array, indexcov.go:656)
@@ -1155,6 +1173,13 @@ static int cmd_indexcov(int argc, char** argv) {
             if (longest > 0) { std::vector<double> cn(S); for (size_t k = 0; k < S; k++) cn[k] = get_cn(dptr[k], (size_t)lens[k]); sexes[ref.name] = cn; }
         } else {
             for (size_t k = 0; k < S * 4; k++) bins[k] += b4[k];
+            if (pca_rank >= 3)
+                glhost::ThreadPool::global().run((int64_t)S, [&](int64_t k, int) {
+                    uint8_t* row = &pca_x[(size_t)k * (size_t)pca_ld + (size_t)pca_col[q]];
+                    const int32_t n = lens[(size_t)k];
+                    for (int32_t i = 0; i < n; i++) row[i] = glpca::pca8_byte(dptr[(size_t)k][i]);
+                    memset(row + n, 0, longest + 1 - (size_t)n);
+                });
         }
         if (longest > 0) {                                                  // writeROCs (indexcov.go:1018-1036)
             std::string h = "#chrom\tcov"; for (auto& n : names) h += "\t" + n; h += "\n";
@@ -1192,8 +1217,22 @@ static int cmd_indexcov(int argc, char** argv) {
         if (sexes.empty() && sex != "X,Y") fatal(1, "(FATAL) indexcov: expected %zu sex chromosomes, found: %zu.", sexes_wanted.size(), sexes.size());
         fprintf(stderr, "(WARNING) indexcov: expected %zu sex chromosomes, found: %zu.\nyou can set the expected with --sex '%s'\n", sexes_wanted.size(), sexes.size(), keys.c_str());
     }
-    // .ped (indexcov.go:815-894), without the PCA columns
+    // pca (indexcov.go:773-807): the first five components on GPU 0, once every reference's bytes are in; fewer than five
+    // components are logged, and fewer than three give no PC columns.  Without any kept autosome (D = 0) the reference's
+    // gonum panics on the empty matrix; here that is 0 components (DESIGN §1.11).
     if (sexes.empty()) fprintf(stderr, "sex chromosomes not found.\n");
+    int32_t n_pc = 0;
+    std::vector<double> pcs;
+    if (pca_rank < 5) fprintf(stderr, "got: %lld principal components\n", (long long)pca_rank);
+    if (pca_rank < 3) {
+        fprintf(stderr, "indexcov: %lld principal components, not plotting\n", (long long)pca_rank);
+    } else {
+        pcs.resize(S * 5);
+        double sv[5];
+        glck(ctx, gl_indexcov_pca(ctx, pca_x.data(), pca_ld, (int32_t)S, pca_D, 5, pcs.data(), sv, &n_pc, nullptr), "gl_indexcov_pca");
+    }
+    ic_mark("pca");
+    // .ped (indexcov.go:815-894)
     FILE* ped = fopen((base + ".ped").c_str(), "w");
     if (!ped) fatal(1, "cannot create %s.ped", base.c_str());
     bool anygt = false;
@@ -1201,6 +1240,7 @@ static int cmd_indexcov(int argc, char** argv) {
     fprintf(ped, "#family_id\tsample_id\tpaternal_id\tmaternal_id\tsex\tphenotype");
     for (auto& kv : sexes) fprintf(ped, "\tCN%s", kv.first.c_str());
     fprintf(ped, "\tbins.out\tbins.lo\tbins.hi\tbins.in\tslope\tp.out");
+    for (int j = 0; j < n_pc; j++) fprintf(ped, "\tPC%d", j + 1);
     if (anygt) fprintf(ped, "\tmapped\tunmapped");
     fputc('\n', ped);
     for (size_t k = 0; k < S; k++) {
@@ -1210,16 +1250,12 @@ static int cmd_indexcov(int argc, char** argv) {
         fprintf(ped, "\t%lld\t%lld\t%lld\t%lld\t%s\t%s", (long long)bins[k * 4 + 0], (long long)bins[k * 4 + 1], (long long)bins[k * 4 + 2],
                 (long long)bins[k * 4 + 3], go_float("%.3f", (double)slopes[k]).c_str(),
                 go_float("%.2f", (double)bins[k * 4 + 0] / (double)bins[k * 4 + 3]).c_str());
+        for (int j = 0; j < n_pc; j++) fprintf(ped, "\t%s", go_float("%.2f", pcs[k * 5 + (size_t)j]).c_str());
         if (anygt) fprintf(ped, "\t%llu\t%llu", (unsigned long long)mapped[k], (unsigned long long)unmapped[k]);
         fputc('\n', ped);
     }
     fclose(ped);
-    // The reference's PCA (indexcov.go:772-810) and its HTML/PNG plots are out of scope (SURVEY.md section 2); the log lines its
-    // functional tests look for (functional-tests.sh:49,82) are kept, and index.html is a plain list of the outputs.
-    if (S < 3) {
-        fprintf(stderr, "got: %zu principal components\n", S);
-        fprintf(stderr, "indexcov: %zu principal components, not plotting\n", S);
-    }
+    // The reference's HTML/PNG plots are out of scope (SURVEY.md section 2): index.html is a plain list of the outputs.
     {
         const std::string index_path = dir + "/index.html";
         FILE* ih = fopen(index_path.c_str(), "w");

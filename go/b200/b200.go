@@ -321,6 +321,30 @@ func (c *Ctx) Emdepth(depths []float32, samples int) (cells []uint8, lambda []fl
 	return cells[:n*samples], lambda[:n*9], c.err(rc)
 }
 
+// IndexcovPCA replaces indexcov's pca (indexcov/indexcov.go:773-807) on the samples x d byte matrix x (row-major, one row
+// of PCA bytes per sample): the projections X V[:, :k] (samples x k, row-major) for k = min(5, samples, d), with the sign
+// and rank rules of DESIGN §1.11, and the singular values.  The Gram runs on the tensor cores.
+func (c *Ctx) IndexcovPCA(x []uint8, samples int) (proj []float64, sv []float64, k int, err error) {
+	if samples < 1 || len(x) < samples || len(x)%samples != 0 {
+		return nil, nil, 0, fmt.Errorf("IndexcovPCA: %d bytes are not %d rows", len(x), samples)
+	}
+	d := len(x) / samples
+	proj = make([]float64, samples*5)
+	sv = make([]float64, 5)
+	var ko C.int32_t
+	rc := C.gl_indexcov_pca(c.h, (*C.uint8_t)(&x[0]), C.int64_t(d), C.int32_t(samples), C.int64_t(d), 5,
+		(*C.double)(&proj[0]), (*C.double)(&sv[0]), &ko, nil)
+	if err = c.err(rc); err != nil {
+		return nil, nil, 0, err
+	}
+	k = int(ko)
+	out := make([]float64, samples*k)
+	for i := 0; i < samples; i++ {
+		copy(out[i*k:(i+1)*k], proj[i*5:i*5+k])
+	}
+	return out, sv[:k], k, nil
+}
+
 // EmdepthStats reports, for the last Emdepth call, the rows done, the cells decided inside the error band of the
 // reference's CPU-dependent Exp / Log, and the bin means summed in sample order.
 func (c *Ctx) EmdepthStats() (rows, uncertified, sequential int64) {

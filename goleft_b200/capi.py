@@ -194,6 +194,11 @@ _proto("gl_emdepth_factors", C.c_int, _vp)
 _proto("gl_emdepth_cnvs", C.c_int, _vp, C.c_int64, C.c_int32, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_int64, _i64p,
        _vp, C.c_int64, _i64p)
 _proto("gl_emdepth_sum_host", C.c_int, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_uint8))
+_proto("gl_indexcov_pca8", C.c_int, _vp, C.c_int64, _vp)
+_proto("gl_indexcov_pca", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _vp, _vp, _i32p, _vp)
+_proto("gl_indexcov_pca_device", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _vp, _vp, _i32p, _vp)
+_proto("gl_indexcov_pca_phases", C.c_int, _vp, C.POINTER(C.c_double))
+_proto("gl_pca_tridiag_top", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp)
 
 
 def version() -> str:
@@ -374,6 +379,26 @@ def emdepth_sum_host(v):
     if rc != GL_OK:
         raise GlError(rc, "gl_emdepth_sum_host: bad arguments")
     return s.value, bool(ok.value)
+
+
+# ---- indexcov PCA (indexcov.go:686-705,773-807), host-only parts
+def indexcov_pca8(d) -> np.ndarray:
+    """the PCA byte of each float32 depth (clip at 8, uint8(8191.875 d + 0.5) the way Go converts it)"""
+    d = _as(d, np.float32).ravel()
+    out = np.empty(d.size, np.uint8)
+    if lib.gl_indexcov_pca8(_ptr(d), d.size, _ptr(out)) != GL_OK:
+        raise GlError(GL_EINVAL, "gl_indexcov_pca8: bad arguments")
+    return out
+
+
+def pca_tridiag_top(d, e, k: int, vectors: bool = True):
+    """(w[k] descending, z (k x n) or None): the k largest eigenpairs of the symmetric tridiagonal (d, e)"""
+    d, e = _as(d, np.float64), _as(e, np.float64)
+    w = np.empty(k, np.float64)
+    z = np.empty((k, d.size), np.float64) if vectors else None
+    if lib.gl_pca_tridiag_top(_ptr(d), _ptr(e), d.size, k, _ptr(w), _ptr(z)) != GL_OK:
+        raise GlError(GL_EINVAL, "gl_pca_tridiag_top: bad arguments")
+    return w, z
 
 
 def chunk_rows(rs: int, re: int, W: int, run_start: np.ndarray, run_class: np.ndarray):
@@ -1208,6 +1233,29 @@ class Ctx:
         v = [C.c_int64(0) for _ in range(3)]
         self._ck(lib.gl_emdepth_stats(self.h, *[C.byref(x) for x in v]))
         return dict(zip(("rows", "uncertified", "sequential"), (x.value for x in v)))
+
+    # ---- indexcov PCA
+    def indexcov_pca(self, x: np.ndarray, k: int = 5, D: Optional[int] = None, want_gram: bool = False):
+        """(proj S x k, sv[k], k_out, gram S x S or None) of the uint8 rows of x (columns [0, D) of each row)"""
+        x = np.ascontiguousarray(x, np.uint8)
+        S, ld = x.shape
+        D = ld if D is None else D
+        proj, sv, ko = np.empty((S, k), np.float64), np.empty(k, np.float64), C.c_int32(0)
+        gram = np.empty((S, S), np.int64) if want_gram else None
+        self._ck(lib.gl_indexcov_pca(self.h, _ptr(x), ld, S, D, k, _ptr(proj), _ptr(sv), C.byref(ko), _ptr(gram)))
+        return proj, sv, ko.value, gram
+
+    def indexcov_pca_device(self, d_x: DevBuf, ld: int, S: int, D: int, k: int = 5, want_gram: bool = False):
+        proj, sv, ko = np.empty((S, k), np.float64), np.empty(k, np.float64), C.c_int32(0)
+        gram = np.empty((S, S), np.int64) if want_gram else None
+        self._ck(lib.gl_indexcov_pca_device(self.h, d_x.ptr, ld, S, D, k, _ptr(proj), _ptr(sv), C.byref(ko), _ptr(gram)))
+        return proj, sv, ko.value, gram
+
+    def indexcov_pca_phases(self):
+        """seconds of the last indexcov_pca call: {upload, gram, eigen}"""
+        t = (C.c_double * 3)()
+        self._ck(lib.gl_indexcov_pca_phases(self.h, t))
+        return dict(zip(("upload", "gram", "eigen"), list(t)))
 
     # ---- multi-GPU
     def comm_init(self, id128: bytes, rank: int, world: int):

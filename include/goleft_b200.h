@@ -409,6 +409,27 @@ int  gl_format_g3_device(gl_ctx* ctx, const float* d_vals, int64_t n, uint8_t* d
 /* I7: in-place cross-sample normalisation of one chromosome; depths is S rows of stride T,
  * lens[i] valid entries in row i.  No-op for S < 5 (indexcov.go:551). */
 int  gl_indexcov_xnorm(gl_ctx* ctx, float* depths, const int32_t* lens, int32_t S, int32_t T);
+/* PCA (the .ped's PC1..PC5, indexcov.go:686-705,773-807; DESIGN §1.11).
+ *   gl_indexcov_pca8       : host-only: the byte of each depth: clip at 8, uint8(8191.875f * d + 0.5f) as Go converts it
+ *                            (truncation to int32, low byte).
+ *   gl_indexcov_pca        : x is S rows of D bytes (row stride ld >= D).  k_out = min(k, S, D); proj (S x k, row-major) gets
+ *                            X V[:, :k_out] (gonum stat.PC: V from the SVD of the column-centred X; X uncentred), each
+ *                            column's sign chosen so the left singular vector's largest-magnitude entry is positive (lowest
+ *                            sample on a tie); sv[0..k) the singular values.  A column whose squared singular value is at most
+ *                            1e-12 times the first one (or all of them when the first is 0) is 0 with sv 0.  Columns from
+ *                            k_out on are 0.  gram (nullable, S x S) receives the exact X X^T.  1 <= S <= 65535.
+ *                            GL_ENOMEM when X and the S x S buffers do not fit in free device memory.
+ *   gl_indexcov_pca_device : the same on a device-resident X; d_x and ld must be multiples of 16 bytes.  The outputs are host.
+ *   gl_indexcov_pca_phases : seconds of the last call: upload, Gram + centring, eigenvectors + projections.
+ *   gl_pca_tridiag_top     : host-only: the k largest eigenvalues w (descending) of the symmetric tridiagonal (d[n], e[n-1])
+ *                            and, when z is not NULL, unit eigenvectors (column j at z[j*n]), as gl_indexcov_pca finds them. */
+int  gl_indexcov_pca8(const float* d, int64_t n, uint8_t* out);
+int  gl_indexcov_pca(gl_ctx* ctx, const uint8_t* x, int64_t ld, int32_t S, int64_t D, int32_t k, double* proj, double* sv,
+                     int32_t* k_out, int64_t* gram);
+int  gl_indexcov_pca_device(gl_ctx* ctx, const uint8_t* d_x, int64_t ld, int32_t S, int64_t D, int32_t k, double* proj, double* sv,
+                            int32_t* k_out, int64_t* gram);
+int  gl_indexcov_pca_phases(gl_ctx* ctx, double* t3);
+int  gl_pca_tridiag_top(const double* d, const double* e, int32_t n, int32_t k, double* w, double* z);
 
 /* indexsplit (indexsplit/indexsplit.go:92-115): amount of cohort data per 16 KB tile = sum over the S samples, in path
  * order, of float64(size)/1e9 — bit-identical to the reference's sequential adds.  sizes: every sample's tile sizes

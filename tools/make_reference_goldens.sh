@@ -15,6 +15,7 @@
 #                                                        (9 samples with planted CN1 / CN3 runs; ref_depthwed.tsv has 2 samples,
 #                                                        where the reference's median32 panics)
 #   tests/golden/ref_emdepth_gotest.txt                  `go test ./emdepth` (its TestBig fails: it expects CN 8, the code gives 9)
+#   tests/golden/ref_indexcov_pca{8,4}.ped               goleft indexcov --fai on the .bai cohorts of tests/golden/make_pca_cohort.py
 #
 # This image has neither toolchain (`go version`, `samtools --version`: command not found), so the files cannot be made
 # here; until they exist every report says "bit-exact vs the restated oracle, parity unpinned".  tests/test_reference_goldens.py
@@ -205,5 +206,12 @@ awk 'BEGIN{OFS="\t"; srand(11); printf "#chrom\tstart\tend"; for(i=0;i<9;i++) pr
        print ""}}' > "$OUT/emdepth_cohort.tsv"
 "$TMP/emdrv_bin" "$OUT/emdepth_cohort.tsv" "$TMP/em" && cp "$TMP/em.cn.bed" "$OUT/ref_emdepth.cn.bed" && cp "$TMP/em.cnv.bed" "$OUT/ref_emdepth.cnv.bed" || true
 ( cd "$REF" && go test ./emdepth 2>&1 || true ) > "$OUT/ref_emdepth_gotest.txt"
+# indexcov's PC1..PC5 .ped columns (indexcov.go:773-807): the full .ped of two generated .bai cohorts with planted groups,
+# 8 samples and 4 samples (rank 3 after centring: the reference's 4th column is a constant).  tests/golden/make_pca_cohort.py
+# writes the same bytes wherever it runs; tests/test_reference_goldens_indexcov_pca.py regenerates them for our side.
+python3 "$(dirname "$0")/../tests/golden/make_pca_cohort.py" "$TMP/pcac"
+for c in pca8 pca4; do
+  "$G" indexcov -d "$TMP/$c" --fai "$TMP/pcac/g.fa.fai" "$TMP/pcac/$c"/s*.bai && cp "$TMP/$c/$c-indexcov.ped" "$OUT/ref_indexcov_$c.ped" || true
+done
 samtools --version | head -1 > "$OUT/ref_PROVENANCE.txt"; go version >> "$OUT/ref_PROVENANCE.txt"; (cd "$REF" && git rev-parse HEAD 2>/dev/null || true) >> "$OUT/ref_PROVENANCE.txt"
 echo "wrote $(ls "$OUT"/ref_* | wc -l) files to $OUT"

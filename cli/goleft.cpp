@@ -805,6 +805,117 @@ struct DevBufs {
     }
 };
 
+// Where kept reference q's tiles of sample k lie in the cohort depths: off/len at [q * S + k] (ref.ID() indexes the index's
+// reference array, indexcov.go:656).  len is 0 when the sample lacks the reference or its median is 0 (indexcov.go:140-142);
+// such an empty slice starts at the sample's first tile.  longest[q] is over every sample, so the table needs every median.
+struct IcSlices {
+    std::vector<int64_t> off, len, longest;
+};
+
+static IcSlices ic_slices(const std::vector<const IcRef*>& kept, const std::vector<std::vector<int64_t>>& size_ptr,
+                          const std::vector<int64_t>& sample_ptr, const std::vector<double>& med) {
+    const size_t S = med.size();
+    IcSlices sl;
+    sl.off.resize(kept.size() * S); sl.len.assign(kept.size() * S, 0); sl.longest.assign(kept.size(), 0);
+    for (size_t q = 0; q < kept.size(); q++) {
+        const int id = kept[q]->id;
+        for (size_t k = 0; k < S; k++) {
+            const size_t j = q * S + k;
+            sl.off[j] = sample_ptr[k];
+            if (id + 1 >= (int)size_ptr[k].size() || med[k] == 0) continue;
+            sl.off[j] += size_ptr[k][id];
+            sl.len[j] = size_ptr[k][id + 1] - size_ptr[k][id];
+            sl.longest[q] = std::max(sl.longest[q], sl.len[j]);
+        }
+    }
+    return sl;
+}
+
+// -n (I7, indexcov.go:670-672): the values of each kept non-sex reference are normalised across the samples as one
+// S x longest matrix and written back into their slices of dep.  Each reference id is normalised once, so a reference that
+// -c lists twice shows the same values both times, as the reference's fresh NormalizedDepth slices do (indexcov.go:129-151).
+static void ic_extranorm(gl_ctx* ctx, const std::vector<const IcRef*>& kept, const std::vector<std::string>& sexes_wanted,
+                         const IcSlices& sl, size_t S, float* dep) {
+    std::vector<float> mat;
+    std::vector<int32_t> lens(S);
+    for (size_t q = 0; q < kept.size(); q++) {
+        const size_t longest = (size_t)sl.longest[q];
+        const int id = kept[q]->id;
+        if (longest == 0 || same_chrom(sexes_wanted, kept[q]->name) ||
+            std::any_of(kept.begin(), kept.begin() + (long)q, [&](const IcRef* r) { return r->id == id; }))
+            continue;
+        const int64_t* off = &sl.off[q * S];
+        mat.assign(S * longest, 0.f);
+        for (size_t k = 0; k < S; k++) {
+            lens[k] = (int32_t)sl.len[q * S + k];
+            memcpy(&mat[k * longest], dep + off[k], (size_t)lens[k] * 4);
+        }
+        glck(ctx, gl_indexcov_xnorm(ctx, mat.data(), lens.data(), (int32_t)S, (int32_t)longest), "gl_indexcov_xnorm");
+        for (size_t k = 0; k < S; k++) memcpy(dep + off[k], &mat[k * longest], (size_t)lens[k] * 4);
+    }
+}
+
+// Phase B on one GPU, over the resident depths d_dep of samples [a, b), which begin at cohort tile t0: the "%.3g" token of
+// every value (I6) into tok_all, and the slot histograms + counters (I4+I5) of every (sample, kept reference) pair into
+// counts_all / b4_all at [k * nq + q].  That order keeps one GPU's samples together, so each array comes home in one copy.
+static void ic_tokens_counts(gl_ctx* c, const float* d_dep, size_t a, size_t b, const std::vector<int64_t>& sample_ptr,
+                             const IcSlices& sl, uint8_t* tok_all, int32_t* counts_all, int64_t* b4_all) {
+    const size_t S = sample_ptr.size() - 1, nq = sl.longest.size(), nseg = nq * (b - a);
+    const int64_t t0 = sample_ptr[a], tiles = sample_ptr[b] - t0;
+    DevBufs tmp(c);
+    if (tiles) {
+        uint8_t* d_tok = tmp.alloc<uint8_t>((size_t)tiles * 10);
+        glck(c, gl_format_g3_device(c, d_dep, tiles, d_tok), "gl_format_g3_device");
+        glck(c, gl_memcpy_d2h(c, tok_all + (size_t)t0 * 10, d_tok, tiles * 10), "gl_memcpy_d2h");
+    }
+    if (nseg == 0) return;
+    std::vector<int64_t> seg_start(nseg), seg_len(nseg), seg_longest(nseg);
+    for (size_t k = a; k < b; k++)
+        for (size_t q = 0; q < nq; q++) {
+            const size_t j = (k - a) * nq + q;
+            seg_start[j] = sl.off[q * S + k] - t0;
+            seg_len[j] = sl.len[q * S + k];
+            seg_longest[j] = sl.longest[q];
+        }
+    const int64_t* d_ss = tmp.upload(seg_start.data(), nseg);
+    const int64_t* d_sl = tmp.upload(seg_len.data(), nseg);
+    const int64_t* d_lg = tmp.upload(seg_longest.data(), nseg);
+    int32_t* d_c = tmp.alloc<int32_t>(nseg * GL_INDEXCOV_SLOTS);
+    int64_t* d_b = tmp.alloc<int64_t>(nseg * 4);
+    glck(c, gl_indexcov_counts_segs_device(c, d_dep, d_ss, d_sl, d_lg, (int32_t)nseg, d_c, d_b), "gl_indexcov_counts_segs_device");
+    glck(c, gl_memcpy_d2h(c, counts_all + a * nq * GL_INDEXCOV_SLOTS, d_c, (int64_t)nseg * GL_INDEXCOV_SLOTS * 4), "gl_memcpy_d2h");
+    glck(c, gl_memcpy_d2h(c, b4_all + a * nq * 4, d_b, (int64_t)nseg * 32), "gl_memcpy_d2h");
+}
+
+// .ped (indexcov.go:815-894)
+static void ic_write_ped(const std::string& base, const std::vector<std::string>& names, const std::map<std::string, std::vector<double>>& sexes,
+                         const std::vector<int64_t>& bins, const std::vector<float>& slopes, const std::vector<double>& pcs, int32_t n_pc,
+                         const std::vector<uint64_t>& mapped, const std::vector<uint64_t>& unmapped) {
+    const size_t S = names.size();
+    FILE* ped = fopen((base + ".ped").c_str(), "w");
+    if (!ped) fatal(1, "cannot create %s.ped", base.c_str());
+    bool anygt = false;
+    for (size_t k = 0; k < S; k++) if (mapped[k] > 0 || unmapped[k] > 0) anygt = true;
+    fprintf(ped, "#family_id\tsample_id\tpaternal_id\tmaternal_id\tsex\tphenotype");
+    for (auto& kv : sexes) fprintf(ped, "\tCN%s", kv.first.c_str());
+    fprintf(ped, "\tbins.out\tbins.lo\tbins.hi\tbins.in\tslope\tp.out");
+    for (int j = 0; j < n_pc; j++) fprintf(ped, "\tPC%d", j + 1);
+    if (anygt) fprintf(ped, "\tmapped\tunmapped");
+    fputc('\n', ped);
+    for (size_t k = 0; k < S; k++) {
+        const int inferred = sexes.empty() ? -9 : (int)(0.5 + sexes.begin()->second[k]);
+        fprintf(ped, "unknown\t%s\t-9\t-9\t%d\t-9", names[k].c_str(), inferred);
+        for (auto& kv : sexes) fprintf(ped, "\t%s", go_float("%.2f", kv.second[k]).c_str());
+        fprintf(ped, "\t%lld\t%lld\t%lld\t%lld\t%s\t%s", (long long)bins[k * 4 + 0], (long long)bins[k * 4 + 1], (long long)bins[k * 4 + 2],
+                (long long)bins[k * 4 + 3], go_float("%.3f", (double)slopes[k]).c_str(),
+                go_float("%.2f", (double)bins[k * 4 + 0] / (double)bins[k * 4 + 3]).c_str());
+        for (int j = 0; j < n_pc; j++) fprintf(ped, "\t%s", go_float("%.2f", pcs[k * 5 + (size_t)j]).c_str());
+        if (anygt) fprintf(ped, "\t%llu\t%llu", (unsigned long long)mapped[k], (unsigned long long)unmapped[k]);
+        fputc('\n', ped);
+    }
+    fclose(ped);
+}
+
 static int cmd_indexcov(int argc, char** argv) {
     std::string dir, exclude = "^chrEBV$|^NC|_random$|Un_|^HLA\\-|_alt$|hap\\d$", sex = "X,Y", chrom, fai, gpus = "0";
     bool includegl = false, extranorm = false;
@@ -941,15 +1052,15 @@ static int cmd_indexcov(int argc, char** argv) {
     // cohort-sized arrays that the GPUs overwrite completely: not zero-filled (a std::vector's constructor page-faulted through
     // 0.8 GB on one thread: 0.6 s of the 313-sample run)
     std::vector<double> med(S);
+    const size_t nq = kept.size();
     RawBuf<float> dep; dep.resize((size_t)total);
-    RawBuf<uint8_t> tok_all;
-    RawBuf<int32_t> counts_all;
-    RawBuf<int64_t> b4_all;
-    if (!extranorm) { tok_all.resize((size_t)total * 10 + 16); counts_all.resize(kept.size() * S * GL_INDEXCOV_SLOTS); b4_all.resize(kept.size() * S * 4); }
+    RawBuf<uint8_t> tok_all; tok_all.resize((size_t)total * 10 + 16);
+    RawBuf<int32_t> counts_all; counts_all.resize(S * nq * GL_INDEXCOV_SLOTS);
+    RawBuf<int64_t> b4_all; b4_all.resize(S * nq * 4);
 
     std::vector<gl_ctx*> ctxs((size_t)G, nullptr);
     // phase A (per GPU, its samples): I1 + I2 + I3 on the device, medians + depths home; the depths stay resident for phase B
-    struct Shard { DevBufs resident; float* d_dep = nullptr; int64_t tiles = 0; };
+    struct Shard { DevBufs resident; float* d_dep = nullptr; };
     std::vector<Shard> shard((size_t)G);
     // a single GPU's work runs on this thread: on a worker thread the row assembly below, which reads what the D2H copies
     // wrote, took about 0.3 s longer for 313 samples
@@ -969,7 +1080,6 @@ static int cmd_indexcov(int argc, char** argv) {
         const int64_t t0 = sample_ptr[a], tiles = sample_ptr[b] - t0;
         Shard& sd = shard[(size_t)g];
         sd.resident.ctx = c;
-        sd.tiles = tiles;
         if (b == a) return;
         DevBufs tmp(c);
         int64_t* d_sizes = tmp.alloc<int64_t>((size_t)tiles);
@@ -1017,66 +1127,24 @@ static int cmd_indexcov(int argc, char** argv) {
     if (!bgz.ok() || !roc) fatal(1, "cannot create outputs in %s", dir.c_str());
     { std::string h = "#chrom\tstart\tend"; for (auto& n : names) h += "\t" + n; h += "\n"; bgz.write(h.data(), h.size()); }
 
-    // ---- phase B.  Without -n the values never change after I3: the "%.3g" token of EVERY value (I6) and the slot histograms
-    //      + counters of EVERY (reference, sample) pair (I4+I5) come from two launches per GPU over its resident depths.
-    //      `longest` of a reference is over all samples (and needs every median), hence the barrier between the phases.
-    if (!extranorm) {
-        const size_t nq = kept.size();
-        std::vector<int64_t> longest_q(nq, 0);
-        for (size_t q = 0; q < nq; q++)
-            for (size_t k = 0; k < S; k++)
-                if (kept[q]->id + 1 < (int)size_ptr[k].size() && med[k] != 0)
-                    longest_q[q] = std::max(longest_q[q], size_ptr[k][kept[q]->id + 1] - size_ptr[k][kept[q]->id]);
+    // `longest` of a reference is over all samples (and needs every median), hence the barrier between the phases
+    const IcSlices sl = ic_slices(kept, size_ptr, sample_ptr, med);
+    gl_ctx* ctx = ctxs[0];                                                  // -n and the PCA run on GPU 0
+    if (extranorm) {                                                        // -n rewrites the values; each GPU takes its range back
+        ic_extranorm(ctx, kept, sexes_wanted, sl, S, dep.data());
         run_on_gpus([&](int g) {
-            gl_ctx* c = ctxs[(size_t)g];
-            const size_t a = cut[(size_t)g], b = cut[(size_t)g + 1], Sg = b - a;
-            Shard& sd = shard[(size_t)g];
-            if (Sg == 0) return;
-            const int64_t t0 = sample_ptr[a], tiles = sd.tiles;
-            {
-                DevBufs tmp(c);
-                uint8_t* d_tok = tmp.alloc<uint8_t>((size_t)tiles * 10);
-                if (tiles) glck(c, gl_format_g3_device(c, sd.d_dep, tiles, d_tok), "gl_format_g3_device");
-                if (tiles) glck(c, gl_memcpy_d2h(c, tok_all.data() + (size_t)t0 * 10, d_tok, tiles * 10), "gl_memcpy_d2h");
-            }
-            const size_t nseg = nq * Sg;
-            if (nseg) {
-                std::vector<int64_t> seg_start(nseg, 0), seg_len(nseg, 0), seg_longest(nseg, 0);
-                for (size_t q = 0; q < nq; q++)
-                    for (size_t k = a; k < b; k++) {
-                        const size_t j = q * Sg + (k - a);
-                        if (kept[q]->id + 1 < (int)size_ptr[k].size() && med[k] != 0) {
-                            seg_start[j] = sample_ptr[k] - t0 + size_ptr[k][kept[q]->id];
-                            seg_len[j] = size_ptr[k][kept[q]->id + 1] - size_ptr[k][kept[q]->id];
-                        }
-                        seg_longest[j] = longest_q[q];
-                    }
-                DevBufs tmp(c);
-                const int64_t* d_ss = tmp.upload(seg_start.data(), nseg);
-                const int64_t* d_sl = tmp.upload(seg_len.data(), nseg);
-                const int64_t* d_lg = tmp.upload(seg_longest.data(), nseg);
-                int32_t* d_c = tmp.alloc<int32_t>(nseg * GL_INDEXCOV_SLOTS);
-                int64_t* d_b = tmp.alloc<int64_t>(nseg * 4);
-                glck(c, gl_indexcov_counts_segs_device(c, sd.d_dep, d_ss, d_sl, d_lg, (int32_t)nseg, d_c, d_b), "gl_indexcov_counts_segs_device");
-                if (G == 1) {
-                    glck(c, gl_memcpy_d2h(c, counts_all.data(), d_c, (int64_t)nseg * GL_INDEXCOV_SLOTS * 4), "gl_memcpy_d2h");
-                    glck(c, gl_memcpy_d2h(c, b4_all.data(), d_b, (int64_t)nseg * 32), "gl_memcpy_d2h");
-                } else {                                                         // this GPU's columns of every reference's block
-                    std::vector<int32_t> cc(nseg * GL_INDEXCOV_SLOTS);
-                    std::vector<int64_t> bb(nseg * 4);
-                    glck(c, gl_memcpy_d2h(c, cc.data(), d_c, (int64_t)nseg * GL_INDEXCOV_SLOTS * 4), "gl_memcpy_d2h");
-                    glck(c, gl_memcpy_d2h(c, bb.data(), d_b, (int64_t)nseg * 32), "gl_memcpy_d2h");
-                    for (size_t q = 0; q < nq; q++) {
-                        memcpy(&counts_all[(q * S + a) * GL_INDEXCOV_SLOTS], &cc[q * Sg * GL_INDEXCOV_SLOTS], Sg * GL_INDEXCOV_SLOTS * 4);
-                        memcpy(&b4_all[(q * S + a) * 4], &bb[q * Sg * 4], Sg * 32);
-                    }
-                }
-            }
+            const int64_t t0 = sample_ptr[cut[(size_t)g]], tiles = sample_ptr[cut[(size_t)g + 1]] - t0;
+            if (tiles) glck(ctxs[(size_t)g], gl_memcpy_h2d(ctxs[(size_t)g], shard[(size_t)g].d_dep, dep.data() + t0, tiles * 4), "gl_memcpy_h2d");
         });
+        ic_mark("-n (GPU 0, + H2D)");
     }
+    // ---- phase B: the values no longer change, so every token and count comes from two launches per GPU
+    run_on_gpus([&](int g) {
+        const size_t a = cut[(size_t)g], b = cut[(size_t)g + 1];
+        if (b > a) ic_tokens_counts(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, tok_all.data(), counts_all.data(), b4_all.data());
+    });
     shard.clear();                                                          // frees the resident depths
     for (int g = 1; g < G; g++) gl_ctx_destroy(ctxs[(size_t)g]);
-    gl_ctx* ctx = ctxs[0];                                                  // -n (I7) runs per reference on GPU 0
     ic_mark("tokens + counts (GPU, + D2H)");
 
     std::map<std::string, std::vector<double>> sexes;
@@ -1085,65 +1153,20 @@ static int cmd_indexcov(int argc, char** argv) {
     int n_slopes = 0;
     // the PCA's byte matrix (indexcov.go:686-705): every kept reference that is not a sex chromosome gives each sample
     // longest + 1 columns, its clipped values' bytes and then zeros (the range loop leaves i at the last index, or -1)
-    std::vector<int64_t> pca_col(kept.size(), -1);
+    std::vector<int64_t> pca_col(nq, -1);
     int64_t pca_D = 0;
-    for (size_t q = 0; q < kept.size(); q++) {
-        if (same_chrom(sexes_wanted, kept[q]->name)) continue;
-        int64_t lg = 0;
-        for (size_t k = 0; k < S; k++)
-            if (kept[q]->id + 1 < (int)size_ptr[k].size() && med[k] != 0)
-                lg = std::max(lg, size_ptr[k][kept[q]->id + 1] - size_ptr[k][kept[q]->id]);
-        pca_col[q] = pca_D;
-        pca_D += lg + 1;
-    }
+    for (size_t q = 0; q < nq; q++)
+        if (!same_chrom(sexes_wanted, kept[q]->name)) { pca_col[q] = pca_D; pca_D += sl.longest[q] + 1; }
     const int64_t pca_rank = std::min<int64_t>((int64_t)S, pca_D);          // gonum's min(S, D) components
     const int64_t pca_ld = (pca_D + 63) / 64 * 64;
     RawBuf<uint8_t> pca_x;
     if (pca_rank >= 3) pca_x.resize(S * (size_t)pca_ld);
-    for (size_t q = 0; q < kept.size(); q++) {
+    for (size_t q = 0; q < nq; q++) {
         const IcRef& ref = *kept[q];
-        // per-sample slices of this reference (ref.ID() indexes the index's reference array, indexcov.go:656)
-        std::vector<const float*> dptr(S, nullptr);
-        std::vector<int64_t> doff(S, 0);
-        std::vector<int32_t> lens(S, 0);
-        size_t longest = 0;
-        for (size_t k = 0; k < S; k++) {
-            if (ref.id + 1 < (int)size_ptr[k].size() && med[k] != 0) {
-                const int64_t a = size_ptr[k][ref.id], b = size_ptr[k][ref.id + 1];
-                doff[k] = sample_ptr[k] + a;
-                dptr[k] = dep.data() + doff[k];
-                lens[k] = (int32_t)(b - a);
-            }
-            longest = std::max(longest, (size_t)lens[k]);
-        }
+        const size_t longest = (size_t)sl.longest[q];
+        const int64_t* off = &sl.off[q * S];
+        const int64_t* lens = &sl.len[q * S];
         const bool is_sex = same_chrom(sexes_wanted, ref.name);
-        std::vector<float> mat;                                             // S x longest, used when values are rewritten
-        std::vector<int32_t> counts_ref;
-        std::vector<int64_t> b4_ref;
-        std::vector<uint8_t> tok_ref;
-        std::vector<int64_t> seg_ptr(1, 0);
-        const int32_t* counts = nullptr;
-        const int64_t* b4 = nullptr;
-        if (extranorm) {
-            if (!is_sex && longest > 0) {
-                mat.assign(S * longest, 0.f);
-                for (size_t k = 0; k < S; k++) if (lens[k]) memcpy(&mat[k * longest], dptr[k], (size_t)lens[k] * 4);
-                glck(ctx, gl_indexcov_xnorm(ctx, mat.data(), lens.data(), (int32_t)S, (int32_t)longest), "gl_indexcov_xnorm");
-                for (size_t k = 0; k < S; k++) dptr[k] = &mat[k * longest];
-            }
-            // -n rewrites the values per reference: slot histograms, counters and tokens from this reference's values
-            std::vector<float> flat;
-            std::vector<int64_t> lg(S, (int64_t)longest);
-            for (size_t k = 0; k < S; k++) { flat.insert(flat.end(), dptr[k], dptr[k] + lens[k]); seg_ptr.push_back((int64_t)flat.size()); }
-            counts_ref.resize(S * GL_INDEXCOV_SLOTS); b4_ref.resize(S * 4);
-            glck(ctx, gl_indexcov_counts_batch(ctx, flat.data(), seg_ptr.data(), lg.data(), (int32_t)S, counts_ref.data(), b4_ref.data()), "gl_indexcov_counts_batch");
-            tok_ref.resize(flat.size() * 10 + 10);
-            glck(ctx, gl_format_g3(ctx, flat.data(), (int64_t)flat.size(), tok_ref.data()), "gl_format_g3");
-            counts = counts_ref.data(); b4 = b4_ref.data();
-        } else {
-            counts = &counts_all[q * S * GL_INDEXCOV_SLOTS];
-            b4 = &b4_all[q * S * 4];
-        }
         // bed.gz rows (indexcov.go:678-680,1038-1048): every "%.3g" comes from the GPU formatter as a 10-byte token; the rows
         // are put together by all host threads, 256 rows per task, and handed to the BGZF writer in order
         {
@@ -1160,9 +1183,10 @@ static int cmd_indexcov(int argc, char** argv) {
                     for (size_t k = 0; k < S; k++) {
                         out.push_back('\t');
                         if (i >= (size_t)lens[k]) { out.push_back('0'); continue; }
-                        const uint8_t* tk = extranorm ? &tok_ref[((size_t)seg_ptr[k] + i) * 10] : &tok_all[((size_t)doff[k] + i) * 10];
+                        const size_t t = (size_t)off[k] + i;
+                        const uint8_t* tk = &tok_all[t * 10];
                         if (tk[9]) out.append(reinterpret_cast<const char*>(tk), tk[9]);
-                        else out += go_float("%.3g", (double)dptr[k][i]);                           // magnitude outside the kernel's range
+                        else out += go_float("%.3g", (double)dep[t]);                               // magnitude outside the kernel's range
                     }
                     out.push_back('\n');
                 }
@@ -1170,15 +1194,16 @@ static int cmd_indexcov(int argc, char** argv) {
             for (const std::string& part : parts) bgz.write(part.data(), part.size());
         }
         if (is_sex) {
-            if (longest > 0) { std::vector<double> cn(S); for (size_t k = 0; k < S; k++) cn[k] = get_cn(dptr[k], (size_t)lens[k]); sexes[ref.name] = cn; }
+            if (longest > 0) { std::vector<double> cn(S); for (size_t k = 0; k < S; k++) cn[k] = get_cn(&dep[(size_t)off[k]], (size_t)lens[k]); sexes[ref.name] = cn; }
         } else {
-            for (size_t k = 0; k < S * 4; k++) bins[k] += b4[k];
+            for (size_t k = 0; k < S; k++)
+                for (size_t j = 0; j < 4; j++) bins[k * 4 + j] += b4_all[(k * nq + q) * 4 + j];
             if (pca_rank >= 3)
                 glhost::ThreadPool::global().run((int64_t)S, [&](int64_t k, int) {
                     uint8_t* row = &pca_x[(size_t)k * (size_t)pca_ld + (size_t)pca_col[q]];
-                    const int32_t n = lens[(size_t)k];
-                    for (int32_t i = 0; i < n; i++) row[i] = glpca::pca8_byte(dptr[(size_t)k][i]);
-                    memset(row + n, 0, longest + 1 - (size_t)n);
+                    const size_t n = (size_t)lens[k];
+                    for (size_t i = 0; i < n; i++) row[i] = glpca::pca8_byte(dep[(size_t)off[k] + i]);
+                    memset(row + n, 0, longest + 1 - n);
                 });
         }
         if (longest > 0) {                                                  // writeROCs (indexcov.go:1018-1036)
@@ -1187,7 +1212,7 @@ static int cmd_indexcov(int argc, char** argv) {
             std::vector<float> rocs(S * GL_INDEXCOV_SLOTS);
             for (size_t k = 0; k < S; k++) {
                 int tot[GL_INDEXCOV_SLOTS];
-                const int32_t* c = &counts[k * GL_INDEXCOV_SLOTS];
+                const int32_t* c = &counts_all[(k * nq + q) * GL_INDEXCOV_SLOTS];
                 tot[GL_INDEXCOV_SLOTS - 1] = c[GL_INDEXCOV_SLOTS - 1];
                 for (int i = GL_INDEXCOV_SLOTS - 2; i >= 0; i--) tot[i] = tot[i + 1] + c[i];
                 const float mx = (float)tot[0];
@@ -1232,29 +1257,7 @@ static int cmd_indexcov(int argc, char** argv) {
         glck(ctx, gl_indexcov_pca(ctx, pca_x.data(), pca_ld, (int32_t)S, pca_D, 5, pcs.data(), sv, &n_pc, nullptr), "gl_indexcov_pca");
     }
     ic_mark("pca");
-    // .ped (indexcov.go:815-894)
-    FILE* ped = fopen((base + ".ped").c_str(), "w");
-    if (!ped) fatal(1, "cannot create %s.ped", base.c_str());
-    bool anygt = false;
-    for (size_t k = 0; k < S; k++) if (mapped[k] > 0 || unmapped[k] > 0) anygt = true;
-    fprintf(ped, "#family_id\tsample_id\tpaternal_id\tmaternal_id\tsex\tphenotype");
-    for (auto& kv : sexes) fprintf(ped, "\tCN%s", kv.first.c_str());
-    fprintf(ped, "\tbins.out\tbins.lo\tbins.hi\tbins.in\tslope\tp.out");
-    for (int j = 0; j < n_pc; j++) fprintf(ped, "\tPC%d", j + 1);
-    if (anygt) fprintf(ped, "\tmapped\tunmapped");
-    fputc('\n', ped);
-    for (size_t k = 0; k < S; k++) {
-        const int inferred = sexes.empty() ? -9 : (int)(0.5 + sexes.begin()->second[k]);
-        fprintf(ped, "unknown\t%s\t-9\t-9\t%d\t-9", names[k].c_str(), inferred);
-        for (auto& kv : sexes) fprintf(ped, "\t%s", go_float("%.2f", kv.second[k]).c_str());
-        fprintf(ped, "\t%lld\t%lld\t%lld\t%lld\t%s\t%s", (long long)bins[k * 4 + 0], (long long)bins[k * 4 + 1], (long long)bins[k * 4 + 2],
-                (long long)bins[k * 4 + 3], go_float("%.3f", (double)slopes[k]).c_str(),
-                go_float("%.2f", (double)bins[k * 4 + 0] / (double)bins[k * 4 + 3]).c_str());
-        for (int j = 0; j < n_pc; j++) fprintf(ped, "\t%s", go_float("%.2f", pcs[k * 5 + (size_t)j]).c_str());
-        if (anygt) fprintf(ped, "\t%llu\t%llu", (unsigned long long)mapped[k], (unsigned long long)unmapped[k]);
-        fputc('\n', ped);
-    }
-    fclose(ped);
+    ic_write_ped(base, names, sexes, bins, slopes, pcs, n_pc, mapped, unmapped);
     // The reference's HTML/PNG plots are out of scope (SURVEY.md section 2): index.html is a plain list of the outputs.
     {
         const std::string index_path = dir + "/index.html";

@@ -417,12 +417,30 @@ def test_indexsplit(tmp_path, N):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("extranorm", [False, True])
-def test_indexcov_cohort(tmp_path, extranorm):
+@pytest.mark.parametrize("extranorm,form", [(False, "bai"), (True, "bai"), (False, "bam"), (True, "bam")],
+                         ids=["False", "True", "bam-False", "bam-True"])
+def test_indexcov_cohort(tmp_path, extranorm, form):
+    """form "bam": header-only BAMs next to the same indexes, with `-c 2`.  RefsFromBam appends the named reference to the
+    header's (indexcov.go:333-335), so "2" is reported twice: its rows and ROC block twice, its bins counted twice, and with
+    -n both copies normalised from the original values (NormalizedDepth returns a fresh slice, indexcov.go:129-151)."""
     refs, fai, paths, lin = _cohort_bais(tmp_path)
     out = tmp_path / "tt"
-    args = ["indexcov", "-d", str(out), "--fai", fai] + (["-n"] if extranorm else []) + paths
-    p = run(*args)
+    order = list(range(len(refs)))
+    names = ["smp%d-rest" % k for k in range(len(paths))]          # GetShortName for .bai (indexcov.go:238-245)
+    args = ["indexcov", "-d", str(out)] + (["-n"] if extranorm else [])
+    if form == "bam":
+        bams = []
+        for k, bai in enumerate(paths):
+            b = tmp_path / ("smp%d.bam" % k)
+            b.write_bytes(make_bam(refs, [], sample="smp%d" % k))
+            (tmp_path / ("smp%d.bam.bai" % k)).write_bytes(open(bai, "rb").read())
+            bams.append(str(b))
+        paths, names = bams, ["smp%d" % k for k in range(len(bams))]              # names from SM
+        args += ["-c", "2"]
+        order.append(1)
+    else:
+        args += ["--fai", fai]
+    p = run(*args, *paths)
     assert "indexcov finished" in p.stderr
     S = len(paths)
     # oracle
@@ -435,11 +453,11 @@ def test_indexcov_cohort(tmp_path, extranorm):
         med.append(m)
         d = orc.ic_normalize(sizes, float(m))
         depths.append([d[sptr[r]:sptr[r + 1]] for r in range(len(refs))])
-    names = ["smp%d-rest" % k for k in range(S)]                  # GetShortName for .bai (indexcov.go:238-245)
     exp_rows = ["#chrom\tstart\tend\t" + "\t".join(names)]
     bins = np.zeros((S, 4), np.int64)
     roc_txt = ""
-    for r, (name, L) in enumerate(refs):
+    for r in order:
+        name, L = refs[r]
         if name.startswith("NC"):
             continue                                                # default --excludepatt
         ds = [depths[k][r] for k in range(S)]
@@ -476,16 +494,16 @@ def test_indexcov_cohort(tmp_path, extranorm):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("gpus", [2, 3, 7])
-def test_indexcov_cohort_sample_sharded(tmp_path, gpus):
+@pytest.mark.parametrize("gpus,extranorm", [(2, False), (3, False), (7, False), (3, True)], ids=["2", "3", "7", "n-3"])
+def test_indexcov_cohort_sample_sharded(tmp_path, gpus, extranorm):
     """SURVEY 8(e): samples shard across the GPUs through I5, the rows gather on the host.  `--gpus N` must give the bytes of
-    `--gpus 1` (GL_OVERSUBSCRIBE lets a one-GPU box run N shards: shard g -> device g % n_dev)."""
+    `--gpus 1` (GL_OVERSUBSCRIBE lets a one-GPU box run N shards: shard g -> device g % n_dev), with -n too."""
     refs, fai, paths, lin = _cohort_bais(tmp_path)
     outs = []
     for g in (1, gpus):
         out = tmp_path / ("g%d" % g) / "tt"
         os.makedirs(str(out.parent))
-        run("indexcov", "-d", str(out), "--gpus", str(g), "--fai", fai, *paths, env={"GL_OVERSUBSCRIBE": "1"})
+        run("indexcov", "-d", str(out), "--gpus", str(g), "--fai", fai, *(["-n"] if extranorm else []), *paths, env={"GL_OVERSUBSCRIBE": "1"})
         outs.append([open(str(out / ("tt-indexcov." + ext)), "rb").read() for ext in ("bed.gz", "roc", "ped")])
     assert gzip.decompress(outs[0][0]) == gzip.decompress(outs[1][0]) and outs[0][1] == outs[1][1] and outs[0][2] == outs[1][2]
     assert len(gzip.decompress(outs[1][0]).splitlines()) > 400

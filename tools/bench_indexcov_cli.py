@@ -4,6 +4,7 @@ hs37d5-shaped reference (86 sequences, ~189k 16 KB tiles), written here with num
 read S indexes -> I1..I5 on the GPU -> %.3g tokens on the GPU -> rows on all host threads -> BGZF.  Prints one JSON object.
 
     python tools/bench_indexcov_cli.py --samples 313          # one GPU's share of the 2504-sample cohort
+    python tools/bench_indexcov_cli.py --samples 313 --extranorm   # the same with -n (I7)
 """
 import argparse
 import json
@@ -42,6 +43,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--samples", type=int, default=313)
     ap.add_argument("--keep", action="store_true")
+    ap.add_argument("--extranorm", action="store_true", help="run indexcov with -n")
     args = ap.parse_args()
     exe = os.path.join(ROOT, "bin", "goleft")
     tmp = tempfile.mkdtemp(prefix="glcohort_")
@@ -59,13 +61,13 @@ def main():
         out = os.path.join(tmp, "out")
         t0 = time.perf_counter()
         os.environ["GL_TIMING"] = "1"
-        p = subprocess.run([exe, "indexcov", "-d", out, "--fai", os.path.join(tmp, "ref.fai"), "--includegl", "--excludepatt", "^$"] + paths, capture_output=True, text=True)
+        p = subprocess.run([exe, "indexcov", "-d", out, "--fai", os.path.join(tmp, "ref.fai"), "--includegl", "--excludepatt", "^$"] + (["-n"] if args.extranorm else []) + paths, capture_output=True, text=True)
         wall = time.perf_counter() - t0
         if p.returncode != 0:
             print(json.dumps({"error": p.stderr[-500:]})); return
         tiles = sum(L // 16384 for L in HS37D5)
         bed = os.path.join(out, "out-indexcov.bed.gz")
-        res = {"samples": args.samples, "tiles_per_sample": tiles, "tile_samples": args.samples * tiles, "index_bytes": sum(os.path.getsize(x) for x in paths),
+        res = {"samples": args.samples, "extranorm": args.extranorm, "tiles_per_sample": tiles, "tile_samples": args.samples * tiles, "index_bytes": sum(os.path.getsize(x) for x in paths),
                "write_indexes_s": t_write, "cli_wall_s": wall, "tile_samples_per_s": args.samples * tiles / wall,
                "bed_gz_bytes": os.path.getsize(bed), "host_threads": os.cpu_count(),
                "phases": [ln.replace("[indexcov timing]", "").strip() for ln in p.stderr.splitlines() if ln.startswith("[indexcov timing]")],

@@ -25,19 +25,9 @@ extern "C" int gl_bgzf_inflate_device(gl_ctx* ctx, const uint8_t* d_comp, const 
 
 namespace {
 
-__device__ __forceinline__ unsigned ld32(const unsigned char* p) {          // unaligned little-endian load
-    return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
-}
-
-// glbam::record_cigar out of line, called only for a record whose first op is S of length l_seq: records without the
-// placeholder walk their CIGAR exactly as before
-__device__ __noinline__ void cg_cigar(const unsigned char* r, unsigned bs, const unsigned char** cg, unsigned* n_op) {
-    glbam::record_cigar(r, bs, cg, n_op);
-}
-
 // one thread per unit: records in [unit_pos[u], unit_pos[u+1]) of the inflated stream.  kEmit = false: count the M/=/X blocks of
-// the passing records; kEmit = true: write them at seg_off[u].  Same walk as host/bam_feed.cpp Emitter::record (blocks
-// separated only by I/S/H/P merge; D and N advance without counting), on the CIGAR glbam::record_cigar picks (CG tag).
+// the passing records; kEmit = true: write them at seg_off[u].  Filter and walk are glbam::depth_counts / depth_blocks, as
+// on the host.
 template <bool kEmit>
 __global__ void __launch_bounds__(128) bam_parse_kernel(const unsigned char* __restrict__ data, const long long* __restrict__ unit_pos, int n_units,
                                                        int tid_want, int min_mapq, long long* __restrict__ seg_cnt, const long long* __restrict__ seg_off,
@@ -51,42 +41,20 @@ __global__ void __launch_bounds__(128) bam_parse_kernel(const unsigned char* __r
     int maxlen = 0;
     bool bad = false;
     while (p + 36 <= pe) {
-        const unsigned char* r = data + p;
-        const unsigned bs = ld32(r);
+        const unsigned char* r = data + p + 4;
+        const unsigned bs = glbam::ld_u32(data + p);
         if (bs < 32 || p + 4 + (long long)bs > pe) { bad = true; break; }       // corrupt size, or a record crossing a unit edge (the index lied)
-        const int rtid = (int)ld32(r + 4), rpos = (int)ld32(r + 8);
-        const unsigned l_name = r[12], mapq = r[13];
-        const unsigned n_cig = r[16] | (r[17] << 8), flag = r[18] | (r[19] << 8);
+        const int rtid = (int)glbam::ld_u32(r);
         p += 4 + (long long)bs;
         if (rtid != tid_want) { if (rtid > tid_want || rtid < 0) break; continue; }
         n_rec++;
-        if ((flag & 0x704u) != 0 || (int)mapq < min_mapq) continue;             // samtools depth defaults + -Q (depth.go:45)
-        if (32u + l_name + 4u * n_cig > bs) continue;
+        if (!glbam::depth_counts(r, bs, min_mapq)) continue;
         n_pass++;
-        const unsigned char* cg = r + 36 + l_name;
-        unsigned n_op = n_cig;
-        int ref = rpos, b0 = 0, b1 = 0;
-        bool open = false, checked = false;
-        for (unsigned k = 0; k < n_op; k++) {
-            const unsigned v = ld32(cg + 4 * k);
-            const unsigned op = v & 15u;
-            const int len = (int)(v >> 4);
-            if (op == 0 || op == 7 || op == 8) {
-                if (len == 0) continue;
-                if (open && b1 == ref) b1 = ref + len;
-                else {
-                    if (open && b1 > b0) { if (kEmit) { start[out] = b0; end[out] = b1; out++; } n_seg++; maxlen = max(maxlen, b1 - b0); }
-                    b0 = ref; b1 = ref + len; open = true;
-                }
-                ref += len;
-            } else if (op == 2 || op == 3) ref += len;
-            else if (op == 4 && k == 0 && !checked && v == ((ld32(r + 20) << 4) | 4u)) {   // S of length l_seq first: maybe the CG placeholder
-                checked = true;
-                cg_cigar(r + 4, bs, &cg, &n_op);
-                k = ~0u;                                                        // walk the CIGAR it chose from its first op
-            }
-        }
-        if (open && b1 > b0) { if (kEmit) { start[out] = b0; end[out] = b1; out++; } n_seg++; maxlen = max(maxlen, b1 - b0); }
+        glbam::depth_blocks(r, bs, [&](int b0, int b1) {
+            if (kEmit) { start[out] = b0; end[out] = b1; out++; }
+            n_seg++;
+            maxlen = max(maxlen, b1 - b0);
+        });
     }
     if (!kEmit) {
         seg_cnt[u] = n_seg;

@@ -1,4 +1,4 @@
-// bam_feed.cpp — see bam_feed.h.  BAM / BAI layouts: SAM spec sections 4.2, 5.2 (SURVEY.md Appendix D).
+// bam_feed.cpp — see bam_feed.h.  BGZF / BAM / BAI layouts: SAM spec sections 4.1, 4.2, 5.2 (SURVEY.md Appendix D).
 #include "bam_feed.h"
 #include <fcntl.h>
 #include <string.h>
@@ -25,6 +25,7 @@ inline int32_t rdi32(const uint8_t* p) { return (int32_t)rd32(p); }
 
 constexpr int64_t kUnitBytes = 1 << 20;          // compressed bytes per work unit (about 64 tiles of a 30x BAM)
 constexpr int64_t kWindow = (1 << 20) + (1 << 16);
+constexpr int64_t kStreamChunk = int64_t(32) << 20;   // compressed bytes per BamFile::stream read
 
 // size of the BGZF block at p (0: not a block header / not enough bytes to tell)
 size_t block_size(const uint8_t* p, size_t avail) {
@@ -40,7 +41,7 @@ size_t block_size(const uint8_t* p, size_t avail) {
     return 0;
 }
 
-struct Inflater {                                 // one z_stream per worker, reset per block
+struct Inflater {                                 // one z_stream per thread (inflater()), reset per block
     z_stream zs;
     bool ok = false;
     Inflater() { memset(&zs, 0, sizeof zs); ok = inflateInit2(&zs, -15) == Z_OK; }
@@ -59,6 +60,11 @@ struct Inflater {                                 // one z_stream per worker, re
         return rc == Z_STREAM_END && zs.total_out == isize;
     }
 };
+
+Inflater& inflater() {
+    thread_local Inflater inf;
+    return inf;
+}
 
 struct Unit { uint64_t v0 = 0, v1 = 0; };
 
@@ -95,28 +101,12 @@ struct Emitter {
         while (j > 0 && pend[j - 1].first > s) { pend[j] = pend[j - 1]; j--; }
         pend[j] = Piece(s, len);
     }
-    inline void record(int32_t pos, const uint8_t* cg, uint32_t n_cig) {
+    inline void record(const uint8_t* r, uint32_t bs) {
+        const int32_t pos = rdi32(r + 4);
         if (pos < last_pos) sorted = false;         // not coordinate-sorted: fixed up at the end
         last_pos = pos;
         if (!pend.empty()) flush_upto(pos);
-        int32_t ref = pos, bs = 0, be = 0;
-        bool open = false;
-        for (uint32_t k = 0; k < n_cig; k++) {
-            const uint32_t v = rd32(cg + 4 * k);
-            const uint32_t op = v & 15, len = v >> 4;
-            if (op == 0 || op == 7 || op == 8) {                               // M = X count
-                if (len == 0) continue;
-                if (open && be == ref) be = ref + (int32_t)len;               // blocks separated only by I/S/H/P merge
-                else {
-                    if (open && be > bs) add(bs, be - bs);
-                    bs = ref; be = ref + (int32_t)len; open = true;
-                }
-                ref += (int32_t)len;
-            } else if (op == 2 || op == 3) {                                   // D N advance without counting
-                ref += (int32_t)len;
-            }                                                                  // I S H P: no reference movement
-        }
-        if (open && be > bs) add(bs, be - bs);
+        glbam::depth_blocks(r, bs, [&](int32_t b, int32_t e) { add(b, e - b); });
     }
     void finish() {
         for (const Piece& p : pend) out.push_back(p);
@@ -129,7 +119,7 @@ struct Emitter {
 
 BamFile::~BamFile() { if (fd_ >= 0) close(fd_); }
 
-std::string BamFile::open(const std::string& p) {
+std::string BamFile::open(const std::string& p, bool with_index) {
     path = p;
     fd_ = ::open(p.c_str(), O_RDONLY);
     if (fd_ < 0) return "cannot open " + p;
@@ -138,7 +128,7 @@ std::string BamFile::open(const std::string& p) {
     size_ = (int64_t)st.st_size;
     // header: inflate block by block until it parses (a header is a few blocks; the old reader inflated 32 MB)
     std::vector<uint8_t> cin, text;
-    Inflater inf;
+    Inflater& inf = inflater();
     int64_t c = 0;
     bool done = false;
     while (!done && c < size_) {
@@ -181,6 +171,8 @@ std::string BamFile::open(const std::string& p) {
                         header.text.assign(reinterpret_cast<const char*>(text.data() + 8), l_text);
                         while (!header.text.empty() && header.text.back() == 0) header.text.pop_back();
                         header.refs = refs;
+                        rec_member_ = c + (int64_t)(q - bs);            // the header ends in this member
+                        rec_skip_ = (uint32_t)(o - at);
                         done = true;
                         break;
                     }
@@ -191,7 +183,7 @@ std::string BamFile::open(const std::string& p) {
         c += (int64_t)q;
     }
     if (!done) return "truncated BAM header: " + p;
-    // index
+    if (!with_index) return "";
     std::string cand[2] = {p + ".bai", p};
     if (p.size() > 4 && p.compare(p.size() - 4, 4, ".bam") == 0) cand[1] = p.substr(0, p.size() - 4) + ".bai"; else cand[1].clear();
     for (const std::string& ip : cand) {
@@ -242,12 +234,11 @@ std::string BamFile::decode(int tid, int64_t beg, int64_t end, int min_mapq, int
     std::vector<UnitOut> res(units.size());
     glhost::ThreadPool& pool = glhost::ThreadPool::global();
     const int T = threads > 0 ? std::min(threads, pool.size()) : pool.size();
-    std::atomic<bool> stop_all(false);
     pool.run((int64_t)units.size(), [&](int64_t ui, int) {
         UnitOut& R = res[(size_t)ui];
         const Unit& U = units[(size_t)ui];
         thread_local std::vector<uint8_t> cin, buf;
-        thread_local Inflater inf;
+        Inflater& inf = inflater();
         cin.resize((size_t)kWindow);
         buf.clear();
         size_t pos = 0;
@@ -316,15 +307,9 @@ std::string BamFile::decode(int tid, int64_t beg, int64_t end, int min_mapq, int
                 if (rtid != tid) { if (rtid > tid || rtid < 0) { finished = true; break; } continue; }
                 if (rpos >= end_pos) { finished = true; break; }
                 R.n_records++;
-                const uint8_t l_name = r[8], mapq = r[9];
-                const uint16_t n_cig = rd16(r + 12), flag = rd16(r + 14);
-                if ((flag & 0x704) != 0 || (int)mapq < min_mapq) continue;      // samtools depth defaults + -Q (depth.go:45)
-                if (32u + l_name + 4u * n_cig > bs) continue;
+                if (!glbam::depth_counts(r, bs, min_mapq)) continue;
                 R.n_pass++;
-                const uint8_t* cg;
-                uint32_t n_op;
-                glbam::record_cigar(r, bs, &cg, &n_op);                         // the stored CIGAR, or the real one from CG
-                em.record(rpos, cg, n_op);
+                em.record(r, bs);
             }
             R.parse_s += now_s() - tp;
             if (done_reading) break;
@@ -335,7 +320,6 @@ std::string BamFile::decode(int tid, int64_t beg, int64_t end, int min_mapq, int
         R.max_len = em.max_len;
         if (buf.capacity() > (size_t(64) << 20)) { std::vector<uint8_t>().swap(buf); }
     }, T);
-    (void)stop_all;
     DecodeStats S;
     S.units = (int)units.size();
     int64_t sum_len = 0;
@@ -375,6 +359,137 @@ std::string BamFile::decode(int tid, int64_t beg, int64_t end, int min_mapq, int
     S.wall_s = now_s() - t_wall;
     if (st) *st = S;
     return "";
+}
+
+std::string BamFile::stream(int threads, const std::function<bool(const uint8_t*, uint32_t)>& fn) {
+    if (fd_ < 0) return "BAM not open";
+    glhost::ThreadPool& pool = glhost::ThreadPool::global();
+    const int T = threads > 0 ? std::min(threads, pool.size()) : pool.size();
+    struct Member { size_t at, size, out; uint32_t isize; };
+    std::vector<Member> mem;
+    std::vector<uint8_t> cin, buf;                    // buf: the record cut by the last chunk's end, then this chunk inflated
+    size_t carry = 0, pos = rec_skip_;
+    int64_t c = rec_member_;
+    while (c < size_) {
+        const size_t want = (size_t)std::min<int64_t>(kStreamChunk, size_ - c);
+        cin.resize(want);
+        for (size_t got = 0; got < want;) {
+            const ssize_t k = pread(fd_, cin.data() + got, want - got, c + (int64_t)got);
+            if (k <= 0) return "read failed in " + path;
+            got += (size_t)k;
+        }
+        const bool eof = c + (int64_t)want == size_;
+        // the chunk's whole members; the one its end cuts is read again with the next chunk
+        mem.clear();
+        size_t q = 0, out = carry;
+        while (q < want) {
+            const size_t bs = block_size(cin.data() + q, want - q);
+            if (bs == 0) {
+                if (!eof && want - q < 18) break;
+                return "not a BGZF block in " + path;
+            }
+            if (q + bs > want) {
+                if (eof) return "truncated BGZF block in " + path;
+                break;
+            }
+            const uint32_t isize = rd32(cin.data() + q + bs - 4);
+            if (isize > 65536) return "bad BGZF ISIZE in " + path;
+            mem.push_back(Member{q, bs, out, isize});
+            out += isize;
+            q += bs;
+        }
+        c += (int64_t)q;
+        buf.resize(out);
+        std::atomic<bool> bad(false);
+        pool.run((int64_t)mem.size(), [&](int64_t i, int) {
+            const Member& m = mem[(size_t)i];
+            if (!inflater().block(cin.data() + m.at, m.size, buf.data() + m.out, m.isize)) bad = true;
+        }, T);
+        if (bad) return "inflate failed in " + path;
+        for (;;) {
+            const size_t av = buf.size() - pos;
+            if (av < 4) break;
+            const uint32_t bs = rd32(buf.data() + pos);
+            if (bs < 32) return "corrupt BAM record: " + path;
+            if (av < 4 + (size_t)bs) break;
+            if (!fn(buf.data() + pos + 4, bs)) return "";
+            pos += 4 + (size_t)bs;
+        }
+        carry = buf.size() - pos;
+        memmove(buf.data(), buf.data() + pos, carry);
+        pos = 0;
+    }
+    return "";
+}
+
+std::string bam_read_header(const std::string& path, BamHeader& out) {
+    BamFile f;
+    const std::string err = f.open(path, false);
+    if (!err.empty()) return err;
+    out = f.header;
+    return "";
+}
+
+std::string bam_decode_segments(const std::string& path, int min_mapq, int threads, int only_tid, SegmentSet& out) {
+    BamFile f;
+    const std::string err = f.open(path, false);
+    if (!err.empty()) return err;
+    out.header = f.header;
+    const int32_t n_ref = (int32_t)out.header.refs.size();
+    out.start.assign((size_t)n_ref, {});
+    out.end.assign((size_t)n_ref, {});
+    out.n_records = out.n_pass = 0;
+    return f.stream(std::max(threads, 1), [&](const uint8_t* r, uint32_t bs) {
+        out.n_records++;
+        const int32_t tid = rdi32(r);
+        if (tid < 0 || tid >= n_ref || (only_tid >= 0 && tid != only_tid)) return true;
+        if (!glbam::depth_counts(r, bs, min_mapq)) return true;
+        out.n_pass++;
+        std::vector<int32_t>& S = out.start[(size_t)tid];
+        std::vector<int32_t>& E = out.end[(size_t)tid];
+        glbam::depth_blocks(r, bs, [&](int32_t b, int32_t e) { S.push_back(b); E.push_back(e); });
+        return true;
+    });
+}
+
+// covstats reads the stored CIGAR: the reference reads BAM through biogo/hts, whose handling of CG is not established
+std::string bam_covstats_sample(const std::string& path, int n, int skip, BamHeader& hdr, CovstatsSample& o) {
+    BamFile f;
+    const std::string err = f.open(path, false);
+    if (!err.empty()) return err;
+    hdr = f.header;
+    int64_t seen = 0;
+    return f.stream(0, [&](const uint8_t* r, uint32_t size) {
+        if (seen++ < skip) return true;                                        // covstats.go:128-134
+        if ((int64_t)o.insert.size() >= n) return false;                       // :138
+        const int32_t pos = rdi32(r + 4);
+        const uint8_t l_name = r[8];
+        const uint16_t n_cig = rd16(r + 12), flag = rd16(r + 14);
+        const int32_t mate_pos = rdi32(r + 24), tlen = rdi32(r + 28);
+        if (flag & 0x4) { o.n_unmapped++; return true; }                       // :144-147
+        o.k++;
+        if (flag & (0x400 | 0x200)) {                                          // :149-155
+            if (flag & 0x400) o.n_dup++;
+            o.n_bad++;
+            return true;
+        }
+        if (flag & 0x2) o.n_proper++;                                          // :156-158
+        if (32u + l_name + 4u * n_cig > size) return true;
+        const uint8_t* cg = r + 32 + l_name;
+        int32_t ref_len = 0, read_len = 0;
+        for (uint16_t k = 0; k < n_cig; k++) {
+            const uint32_t v = rd32(cg + 4 * k), op = v & 15, len = v >> 4;
+            if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ref_len += (int32_t)len;
+            if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) read_len += (int32_t)len;
+        }
+        if ((int64_t)o.read_len.size() < 2 * (int64_t)n) o.read_len.push_back(read_len);      // :159-161
+        else if (o.insert.empty()) return false;                                               // :163-166
+        if (pos < mate_pos && (flag & 0x2) && n_cig == 1 && (rd32(cg) & 15) == 0) {            // :169-172
+            o.insert.push_back(mate_pos - (pos + ref_len));
+            o.tmpl.push_back(tlen);
+        }
+        return true;
+    });
 }
 
 }  // namespace glhts

@@ -1,5 +1,8 @@
-// bam_feed.h — the index-guided, parallel BAM feeder of `goleft depth`.
-// Replaces what the reference gets from its `samtools depth -Q q -r chr:b-e` children (depth/depth.go:45,116,152):
+// bam_feed.h — the BAM reader: header, index, and the two ways through the records.
+//   BamFile::stream  every record from the first to EOF, in file order (no index needed): bam_decode_segments (an unindexed
+//                    `goleft depth` / multidepth input) and bam_covstats_sample.
+//   BamFile::decode  the index-guided, parallel feeder of `goleft depth`.
+// decode replaces what the reference gets from its `samtools depth -Q q -r chr:b-e` children (depth/depth.go:45,116,152):
 // only the BGZF blocks of the requested reference range are read (BAI linear index -> record-aligned virtual offsets),
 // the range is cut into units at those offsets, and every pool thread inflates AND parses its own units — no serial
 // record walk.  Each unit yields its M/=/X blocks already in start order (the parser knows the read position, so the
@@ -7,6 +10,7 @@
 // assembled into the engine's packed8 words (short reads) or sorted int32 arrays (long reads) by seg_pack.h.
 #pragma once
 #include <stdint.h>
+#include <functional>
 #include <string>
 #include <vector>
 #include "hts_io.h"
@@ -33,21 +37,45 @@ public:
     BamFile() {}
     ~BamFile();
     BamFile(const BamFile&) = delete;
-    // opens path and path + ".bai" (or path with .bam replaced by .bai); has_index tells whether one was found
-    std::string open(const std::string& path);
+    // opens path and parses its header; with_index: also loads path + ".bai" (or path with .bam replaced by .bai), and
+    // has_index tells whether one was found
+    std::string open(const std::string& path, bool with_index = true);
     bool has_index = false;
     BamHeader header;
     BaiIndex bai;
     std::string path;
-    // M/=/X blocks of the records of reference `tid` that pass (flag & 0x704) == 0 && MAPQ >= min_mapq and can overlap
-    // [beg, end).  want: 0 = choose (packed8 unless the blocks are long), 8, 32.  Needs the index.
+    // M/=/X blocks of the records of reference `tid` that pass the samtools-depth filter (glbam::depth_counts) and can
+    // overlap [beg, end).  want: 0 = choose (packed8 unless the blocks are long), 8, 32.  Needs the index.
     std::string decode(int tid, int64_t beg, int64_t end, int min_mapq, int threads, int want, ContigSegs& out, DecodeStats* st);
+    // fn(r, bs) for every record from the first to EOF, in file order, on the calling thread (r: the record after its
+    // block_size field, bs: block_size); fn returns false to stop.  The file is read in 32 MB compressed chunks whose
+    // BGZF members are inflated on `threads` threads of the library's pool (0 = all of it), so it must not be called from
+    // a pool task.
+    std::string stream(int threads, const std::function<bool(const uint8_t*, uint32_t)>& fn);
     int fd() const { return fd_; }
     int64_t file_size() const { return size_; }
 private:
     int fd_ = -1;
     int64_t size_ = 0;
+    int64_t rec_member_ = 0;                    // the first record: the file offset of its BGZF member and its offset
+    uint32_t rec_skip_ = 0;                     // in that member's inflated bytes (may be the member's whole size)
 };
+
+// What `samtools depth -Q q` counts (SURVEY.md §8a D0, glbam::depth_counts / depth_blocks) from every record of the file.
+struct SegmentSet {
+    BamHeader header;
+    std::vector<std::vector<int32_t>> start, end;        // per reference id, in record order
+    int64_t n_records = 0, n_pass = 0;
+};
+std::string bam_decode_segments(const std::string& path, int min_mapq, int threads, int only_tid, SegmentSet& out);
+std::string bam_read_header(const std::string& path, BamHeader& out);
+
+// covstats (covstats/covstats.go:122-173): the sampled per-record values
+struct CovstatsSample {
+    std::vector<int32_t> read_len, insert, tmpl;
+    int64_t n_unmapped = 0, k = 0, n_bad = 0, n_dup = 0, n_proper = 0;
+};
+std::string bam_covstats_sample(const std::string& path, int n, int skip, BamHeader& hdr, CovstatsSample& out);
 
 }  // namespace glhts
 

@@ -1,7 +1,5 @@
-// hts_io.cpp — BGZF / BAM / BAI / FAI readers and a BGZF writer (see hts_io.h).
+// hts_io.cpp — BAI / CRAI / FAI readers, the BAM header's sample names and a BGZF writer (see hts_io.h).
 #include "hts_io.h"
-#include "bam_cigar.h"
-#include "bam_feed.h"
 #include <stdio.h>
 #include <string.h>
 #include <zlib.h>
@@ -13,114 +11,11 @@ namespace glhts {
 
 namespace {
 
-inline uint16_t rd16(const uint8_t* p) { return (uint16_t)(p[0] | (p[1] << 8)); }
 inline uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24); }
 inline int32_t rdi32(const uint8_t* p) { return (int32_t)rd32(p); }
 inline uint64_t rd64(const uint8_t* p) { return (uint64_t)rd32(p) | ((uint64_t)rd32(p + 4) << 32); }
 
-struct Block { size_t off, csize; uint32_t isize; size_t out_off; };
-
-// size of the BGZF block starting at p (needs >= 18 bytes), 0 if not a BGZF header
-size_t bgzf_block_size(const uint8_t* p, size_t avail) {
-    if (avail < 18) return 0;
-    if (p[0] != 0x1f || p[1] != 0x8b || p[2] != 8 || !(p[3] & 4)) return 0;
-    const uint16_t xlen = rd16(p + 10);
-    size_t q = 12;
-    while (q + 4 <= 12u + xlen && q + 4 <= avail) {
-        const uint16_t slen = rd16(p + q + 2);
-        if (p[q] == 'B' && p[q + 1] == 'C' && slen == 2 && q + 6 <= avail) return (size_t)rd16(p + q + 4) + 1;
-        q += 4u + slen;
-    }
-    return 0;
-}
-
-bool inflate_block(const uint8_t* src, size_t csize, uint8_t* dst, uint32_t isize) {
-    const uint16_t xlen = rd16(src + 10);
-    const size_t hdr = 12u + xlen;
-    if (csize < hdr + 8) return false;
-    if (isize == 0) return true;
-    z_stream zs;
-    memset(&zs, 0, sizeof zs);
-    if (inflateInit2(&zs, -15) != Z_OK) return false;
-    zs.next_in = const_cast<Bytef*>(src + hdr);
-    zs.avail_in = (uInt)(csize - hdr - 8);
-    zs.next_out = dst;
-    zs.avail_out = isize;
-    const int rc = inflate(&zs, Z_FINISH);
-    inflateEnd(&zs);
-    return rc == Z_STREAM_END && zs.total_out == isize;
-}
-
 }  // namespace
-
-std::string bgzf_inflate_stream(const std::string& path, int threads, bgzf_sink_fn sink, void* user) {
-    FILE* f = fopen(path.c_str(), "rb");
-    if (!f) return "cannot open " + path;
-    if (threads < 1) threads = 1;
-    const size_t kChunk = size_t(32) << 20;
-    std::vector<uint8_t> in;
-    std::vector<uint8_t> out;
-    size_t have = 0;
-    bool eof = false, stop = false;
-    std::string err;
-    while (!stop && (!eof || have > 0)) {
-        in.resize(have + kChunk);
-        if (!eof) {
-            const size_t got = fread(in.data() + have, 1, kChunk, f);
-            if (got < kChunk) eof = true;
-            have += got;
-        }
-        // split into complete blocks
-        std::vector<Block> blocks;
-        size_t p = 0, out_total = 0;
-        while (p < have) {
-            const size_t bs = bgzf_block_size(in.data() + p, have - p);
-            if (bs == 0) {
-                if (have - p < 18 && !eof) break;
-                if (have - p == 0) break;
-                err = "not a BGZF block in " + path;
-                break;
-            }
-            if (p + bs > have) {
-                if (eof) err = "truncated BGZF block in " + path;
-                break;
-            }
-            const uint32_t isize = rd32(in.data() + p + bs - 4);
-            if (isize > 65536) { err = "bad BGZF ISIZE in " + path; break; }
-            blocks.push_back({p, bs, isize, out_total});
-            out_total += isize;
-            p += bs;
-        }
-        if (!err.empty()) break;
-        if (blocks.empty()) {
-            if (eof) { if (have) err = "trailing garbage in " + path; break; }
-            continue;
-        }
-        out.resize(out_total);
-        std::atomic<size_t> next(0);
-        std::atomic<bool> bad(false);
-        auto work = [&]() {
-            for (;;) {
-                const size_t i = next.fetch_add(1);
-                if (i >= blocks.size()) break;
-                const Block& b = blocks[i];
-                if (!inflate_block(in.data() + b.off, b.csize, out.data() + b.out_off, b.isize)) bad = true;
-            }
-        };
-        const int nt = (int)std::min<size_t>((size_t)threads, blocks.size());
-        std::vector<std::thread> pool;
-        for (int t = 1; t < nt; t++) pool.emplace_back(work);
-        work();
-        for (auto& t : pool) t.join();
-        if (bad) { err = "inflate failed in " + path; break; }
-        if (out_total && !sink(user, out.data(), out_total)) stop = true;
-        // keep the unconsumed tail
-        memmove(in.data(), in.data() + p, have - p);
-        have -= p;
-    }
-    fclose(f);
-    return err;
-}
 
 // ---------------------------------------------------------------------------------------------- writer
 namespace {
@@ -222,194 +117,6 @@ std::vector<std::string> BamHeader::sample_names() const {
         p = e + 1;
     }
     return names;
-}
-
-namespace {
-
-// incremental BAM parser fed by the BGZF sink
-struct BamParser {
-    std::vector<uint8_t> pend;
-    size_t pos = 0;
-    bool header_done = false;
-    BamHeader* hdr = nullptr;
-    std::string err;
-    // record callback: return false to stop
-    bool (*on_record)(void* user, const uint8_t* rec, uint32_t size) = nullptr;
-    void* user = nullptr;
-    bool header_only = false;
-
-    bool parse_header() {
-        const uint8_t* p = pend.data() + pos;
-        const size_t av = pend.size() - pos;
-        if (av < 12) return false;
-        if (memcmp(p, "BAM\1", 4) != 0) { err = "not a BAM file"; return false; }
-        const uint32_t l_text = rd32(p + 4);
-        if (av < 8 + (size_t)l_text + 4) return false;
-        const uint32_t n_ref = rd32(p + 8 + l_text);
-        size_t q = 8 + (size_t)l_text + 4;
-        std::vector<RefInfo> refs;
-        for (uint32_t r = 0; r < n_ref; r++) {
-            if (av < q + 4) return false;
-            const uint32_t l_name = rd32(p + q);
-            if (av < q + 4 + l_name + 4) return false;
-            RefInfo ri;
-            ri.name.assign(reinterpret_cast<const char*>(p + q + 4), l_name ? l_name - 1 : 0);
-            ri.length = rdi32(p + q + 4 + l_name);
-            refs.push_back(ri);
-            q += 4 + l_name + 4;
-        }
-        hdr->text.assign(reinterpret_cast<const char*>(p + 8), l_text);
-        while (!hdr->text.empty() && hdr->text.back() == 0) hdr->text.pop_back();
-        hdr->refs = refs;
-        pos += q;
-        header_done = true;
-        return true;
-    }
-
-    bool feed(const uint8_t* data, size_t n) {
-        if (pos > 0 && pos == pend.size()) { pend.clear(); pos = 0; }
-        if (pos > (size_t(64) << 20)) { pend.erase(pend.begin(), pend.begin() + (long)pos); pos = 0; }
-        pend.insert(pend.end(), data, data + n);
-        if (!header_done) {
-            if (!parse_header()) return err.empty();
-            if (header_only) return false;
-        }
-        for (;;) {
-            const size_t av = pend.size() - pos;
-            if (av < 4) break;
-            const uint32_t bs = rd32(pend.data() + pos);
-            if (bs < 32) { err = "corrupt BAM record"; return false; }
-            if (av < 4 + (size_t)bs) break;
-            if (!on_record(user, pend.data() + pos + 4, bs)) { pos += 4 + bs; return false; }
-            pos += 4 + bs;
-        }
-        return true;
-    }
-};
-
-bool parser_sink(void* user, const uint8_t* data, size_t n) { return static_cast<BamParser*>(user)->feed(data, n); }
-
-struct SegCtx { SegmentSet* out; int min_mapq, only_tid; };
-
-bool seg_record(void* user, const uint8_t* r, uint32_t size) {
-    SegCtx* c = static_cast<SegCtx*>(user);
-    SegmentSet& o = *c->out;
-    o.n_records++;
-    const int32_t tid = rdi32(r), pos = rdi32(r + 4);
-    const uint8_t l_name = r[8], mapq = r[9];
-    const uint16_t n_cig = rd16(r + 12), flag = rd16(r + 14);
-    if (tid < 0 || tid >= (int32_t)o.start.size()) return true;
-    if (c->only_tid >= 0 && tid != c->only_tid) return true;
-    if ((flag & 0x704) != 0 || (int)mapq < c->min_mapq) return true;       // samtools depth defaults + -Q (depth.go:45)
-    if (32u + l_name + 4u * n_cig > size) return true;
-    o.n_pass++;
-    const uint8_t* cg;
-    uint32_t n_op;
-    glbam::record_cigar(r, size, &cg, &n_op);                              // the stored CIGAR, or the real one from CG
-    int32_t ref = pos, bs = 0, be = 0;
-    bool open = false;
-    std::vector<int32_t>& S = o.start[tid];
-    std::vector<int32_t>& E = o.end[tid];
-    for (uint32_t k = 0; k < n_op; k++) {
-        const uint32_t v = rd32(cg + 4 * k);
-        const uint32_t op = v & 15, len = v >> 4;
-        if (op == 0 || op == 7 || op == 8) {                               // M = X count
-            if (len == 0) continue;
-            if (open && be == ref) be = ref + (int32_t)len;
-            else {
-                if (open && be > bs) { S.push_back(bs); E.push_back(be); }
-                bs = ref; be = ref + (int32_t)len; open = true;
-            }
-            ref += (int32_t)len;
-        } else if (op == 2 || op == 3) {                                   // D N advance without counting
-            ref += (int32_t)len;
-        }                                                                  // I S H P: no reference movement
-    }
-    if (open && be > bs) { S.push_back(bs); E.push_back(be); }
-    return true;
-}
-
-struct HdrReady { BamParser* p; SegmentSet* out; bool sized = false; };
-
-}  // namespace
-
-std::string bam_read_header(const std::string& path, BamHeader& out) {
-    // block by block until the header parses (BamFile::open): indexcov reads one header per input BAM for the sample name,
-    // and inflating a 32 MB chunk for each cost ~0.5 s per sample
-    BamFile f;
-    const std::string err = f.open(path);
-    if (!err.empty()) return err;
-    out = f.header;
-    return "";
-}
-
-std::string bam_decode_segments(const std::string& path, int min_mapq, int threads, int only_tid, SegmentSet& out) {
-    // the per-reference vectors must exist before the first record: read the header first
-    std::string err = bam_read_header(path, out.header);
-    if (!err.empty()) return err;
-    out.start.assign(out.header.refs.size(), {});
-    out.end.assign(out.header.refs.size(), {});
-    out.n_records = out.n_pass = 0;
-    BamHeader scratch;
-    BamParser bp;
-    bp.hdr = &scratch;
-    SegCtx ctx{&out, min_mapq, only_tid};
-    bp.on_record = seg_record;
-    bp.user = &ctx;
-    err = bgzf_inflate_stream(path, threads, parser_sink, &bp);
-    if (!err.empty()) return err;
-    if (!bp.err.empty()) return bp.err + ": " + path;
-    return "";
-}
-
-namespace {
-struct CsCtx { CovstatsSample* o; int n, skip; int64_t seen = 0; };
-
-bool cs_record(void* user, const uint8_t* r, uint32_t size) {
-    CsCtx* c = static_cast<CsCtx*>(user);
-    CovstatsSample& o = *c->o;
-    if (c->seen++ < c->skip) return true;                                  // covstats.go:128-134
-    if ((int64_t)o.insert.size() >= c->n) return false;                    // :138
-    const int32_t pos = rdi32(r + 4);
-    const uint8_t l_name = r[8];
-    const uint16_t n_cig = rd16(r + 12), flag = rd16(r + 14);
-    const int32_t mate_pos = rdi32(r + 24), tlen = rdi32(r + 28);
-    if (flag & 0x4) { o.n_unmapped++; return true; }                       // :144-147
-    o.k++;
-    if (flag & (0x400 | 0x200)) {                                          // :149-155
-        if (flag & 0x400) o.n_dup++;
-        o.n_bad++;
-        return true;
-    }
-    if (flag & 0x2) o.n_proper++;                                          // :156-158
-    if (32u + l_name + 4u * n_cig > size) return true;
-    const uint8_t* cg = r + 32 + l_name;
-    int32_t ref_len = 0, read_len = 0;
-    for (uint16_t k = 0; k < n_cig; k++) {
-        const uint32_t v = rd32(cg + 4 * k), op = v & 15, len = v >> 4;
-        if (op == 0 || op == 2 || op == 3 || op == 7 || op == 8) ref_len += (int32_t)len;
-        if (op == 0 || op == 1 || op == 4 || op == 7 || op == 8) read_len += (int32_t)len;
-    }
-    if ((int64_t)o.read_len.size() < 2 * (int64_t)c->n) o.read_len.push_back(read_len);   // :159-161
-    else if (o.insert.empty()) return false;                                             // :163-166
-    if (pos < mate_pos && (flag & 0x2) && n_cig == 1 && (rd32(cg) & 15) == 0) {          // :169-172
-        o.insert.push_back(mate_pos - (pos + ref_len));
-        o.tmpl.push_back(tlen);
-    }
-    return true;
-}
-}  // namespace
-
-std::string bam_covstats_sample(const std::string& path, int n, int skip, BamHeader& hdr, CovstatsSample& out) {
-    BamParser bp;
-    bp.hdr = &hdr;
-    CsCtx ctx{&out, n, skip};
-    bp.on_record = cs_record;
-    bp.user = &ctx;
-    std::string err = bgzf_inflate_stream(path, 2, parser_sink, &bp);
-    if (!err.empty()) return err;
-    if (!bp.err.empty()) return bp.err + ": " + path;
-    return "";
 }
 
 // ---------------------------------------------------------------------------------------------- BAI

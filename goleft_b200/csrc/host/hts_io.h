@@ -1,7 +1,6 @@
-// hts_io.h — host-side readers the feeder needs: BGZF (multi-threaded inflate), BAM records -> filtered
-// M/=/X segments, BAI linear index + stats bin, .fai, BGZF writer.  Written from the SAM/BAM spec
-// (SURVEY.md Appendix D); replaces what the reference gets from the `samtools depth` child
-// (depth/depth.go:45) and from github.com/biogo/hts (indexcov/indexcov.go:514, covstats/covstats.go:122-173).
+// hts_io.h — host-side readers: BAI linear index + stats bin, .crai, .fai, and a BGZF writer; the BAM header type (the
+// BAM reader itself is bam_feed.h).  Written from the SAM/BAM spec (SURVEY.md Appendix D); replaces what the reference
+// gets from github.com/biogo/hts (indexcov/indexcov.go:514).
 #pragma once
 #include <stdint.h>
 #include <string>
@@ -19,11 +18,6 @@ struct RefInfo {
 inline int64_t fasta_position(const RefInfo& r, int64_t p) { return r.line_bases > 0 ? p / r.line_bases * r.line_width + p % r.line_bases : p; }
 
 // ---------------------------------------------------------------------------------------------- BGZF
-// Inflates a whole BGZF stream with `threads` workers, in batches of blocks, handing every batch's
-// concatenated payload to `sink(data, n)` in file order.  Returns "" or an error message.
-typedef bool (*bgzf_sink_fn)(void* user, const uint8_t* data, size_t n);
-std::string bgzf_inflate_stream(const std::string& path, int threads, bgzf_sink_fn sink, void* user);
-
 // BGZF writer (indexcov's *.bed.gz, indexcov.go:248-257): 64 KB blocks, ModTime 0, OS 0xff, EOF block.
 class BgzfWriter {
 public:
@@ -44,23 +38,6 @@ struct BamHeader {
     std::vector<RefInfo> refs;
     std::vector<std::string> sample_names() const;      // distinct @RG SM values, in order of appearance
 };
-
-// What `samtools depth -Q q` counts (SURVEY.md §8a D0): records with (flag & 0x704) == 0 and MAPQ >= q;
-// their M/=/X blocks (adjacent blocks separated only by I/S/H/P are merged); D and N advance without counting.
-struct SegmentSet {
-    BamHeader header;
-    std::vector<std::vector<int32_t>> start, end;        // per reference id, in record order
-    int64_t n_records = 0, n_pass = 0;
-};
-std::string bam_decode_segments(const std::string& path, int min_mapq, int threads, int only_tid, SegmentSet& out);
-std::string bam_read_header(const std::string& path, BamHeader& out);
-
-// covstats (covstats/covstats.go:122-173): the sampled per-record values
-struct CovstatsSample {
-    std::vector<int32_t> read_len, insert, tmpl;
-    int64_t n_unmapped = 0, k = 0, n_bad = 0, n_dup = 0, n_proper = 0;
-};
-std::string bam_covstats_sample(const std::string& path, int n, int skip, BamHeader& hdr, CovstatsSample& out);
 
 // ---------------------------------------------------------------------------------------------- BAI
 struct BaiIndex {

@@ -134,7 +134,7 @@ def _cg_bam(tmp_path):
 
 
 def test_stream_decoder_cg_reads(tmp_path):
-    """seg_record (the whole-file decoder) on ultra-long reads whose CIGAR is in the CG tag, the CG edge cases and filtered
+    """bam_decode_segments (the whole-file decoder) on ultra-long reads whose CIGAR is in the CG tag, the CG edge cases and filtered
     placeholders, against bamref: the real CIGAR's blocks where htslib swaps it in, nothing where the placeholder stays"""
     p, refs, recs = _cg_bam(tmp_path)
     for q in (1, 30):
@@ -257,3 +257,25 @@ def test_indexed_feeder_equals_stream_decoder(tmp_path):
         assert np.array_equal(got, orc.pileup_diff(s, e, rs, re))
         assert d["n_records"] < 400_000 * (re - rs + 40_000) / 3_000_000 + 20_000     # only the region's blocks were parsed
     b.close()
+
+
+def test_stream_decoder_across_read_chunks(tmp_path):
+    """the whole-file decoder on an unindexed BAM larger than one 32 MiB read: members cut by a chunk's end are read again
+    and records cut by it are carried over, so every reference's blocks equal the generator's, in record order"""
+    sys.path.insert(0, os.path.join(ROOT, "tools", "synth"))
+    import glsynth
+    contigs = [("chrA", 4_000_000, 1), ("chrB", 700_000, 2), ("chrM", 16_569, 24)]
+    bam = str(tmp_path / "t.bam")
+    glsynth.write_bam(bam, contigs, coverage=20.0)
+    os.remove(bam + ".bai")
+    assert os.path.getsize(bam) > 36 << 20
+    exp = [glsynth.segments(L, idx, coverage=20.0) for _, L, idx in contigs]
+    for threads in (1, 4):
+        r = capi.bam_segments(bam, 1, threads)
+        assert [n for n, _ in r["refs"]] == [c[0] for c in contigs]
+        for tid, (s, e) in enumerate(exp):
+            gs, ge = r["segments"][tid]
+            assert np.array_equal(gs, s) and np.array_equal(ge, e), (threads, tid)
+    only = capi.bam_segments(bam, 1, 4, only_tid=1)
+    assert list(only["segments"]) == [1] and only["n_records"] == r["n_records"] and only["n_pass"] < r["n_pass"]
+    assert np.array_equal(only["segments"][1][0], exp[1][0]) and np.array_equal(only["segments"][1][1], exp[1][1])

@@ -1799,17 +1799,22 @@ struct Matrix {
     std::vector<std::pair<const char*, size_t>> chrom;       // into text
 };
 
+// the whole of a plain, gzip/BGZF or "-" (stdin) file, as xopen.Ropen reads it; a failure is the reference's panic (exit 2)
+std::string read_whole(const std::string& path) {
+    std::string text;
+    gzFile f = path == "-" ? gzdopen(dup(0), "rb") : gzopen(path.c_str(), "rb");
+    if (!f) fatal(2, "panic: open %s: %s", path.c_str(), strerror(errno));
+    gzbuffer(f, 1 << 20);
+    std::vector<char> buf((size_t)1 << 22);
+    int n;
+    while ((n = gzread(f, buf.data(), (unsigned)buf.size())) > 0) text.append(buf.data(), (size_t)n);
+    if (n < 0) fatal(2, "panic: read %s", path.c_str());
+    gzclose(f);
+    return text;
+}
+
 void matrix_read(const std::string& path, Matrix& m) {
-    {
-        gzFile f = path == "-" ? gzdopen(dup(0), "rb") : gzopen(path.c_str(), "rb");
-        if (!f) fatal(2, "panic: open %s: %s", path.c_str(), strerror(errno));
-        gzbuffer(f, 1 << 20);
-        std::vector<char> buf((size_t)1 << 22);
-        int n;
-        while ((n = gzread(f, buf.data(), (unsigned)buf.size())) > 0) m.text.append(buf.data(), (size_t)n);
-        if (n < 0) fatal(2, "panic: read %s", path.c_str());
-        gzclose(f);
-    }
+    m.text = read_whole(path);
     const std::string& text = m.text;
     bool have_header = false;
     for (size_t a = 0; a < text.size();) {
@@ -2109,6 +2114,158 @@ static int cmd_emdepth(int argc, char** argv) {
     return 0;
 }
 
+// ------------------------------------------------------------------------------------------------ cnveval
+// cnveval/cmd/cnveval/cnveval.go (a separate binary of the reference; DESIGN §1.12): `goleft cnveval [-m|--minoverlap 0.4]
+// [-s|--limitsamples] truth.bed test.bed` scores the test set's CNV calls against the truth set and prints precision and
+// recall per size class.  Both files are chrom, start, end, CN and comma-separated samples (a test line uses its first
+// sample), read whole (plain, gzip or "-"); ReadString('\n') drops a final line without "\n"; lines starting with '#' are
+// skipped.  The counts come from gl_cnveval on the GPU.  Argument errors exit 255 (go-arg), the reference's panics exit 2.
+// Unlike the reference, no x.cpu.pprof profile is written into the working directory.
+namespace {
+
+struct CnvLine { std::string chrom; int64_t start, end, cn; std::vector<std::string> samples; };
+
+// strconv.Atoi: optional sign, decimal digits, int64 range
+bool go_atoi(const std::string& t, int64_t& v) {
+    size_t k = 0;
+    const bool neg = !t.empty() && t[0] == '-';
+    if (!t.empty() && (t[0] == '+' || t[0] == '-')) k = 1;
+    if (k == t.size()) return false;
+    unsigned long long u = 0;
+    for (; k < t.size(); k++) {
+        if (t[k] < '0' || t[k] > '9') return false;
+        const unsigned d = (unsigned)(t[k] - '0');
+        if (u > (~0ull - d) / 10) return false;
+        u = u * 10 + d;
+    }
+    if (neg ? u > (1ull << 63) : u > (1ull << 63) - 1) return false;
+    v = neg ? (int64_t)(0 - u) : (int64_t)u;
+    return true;
+}
+
+std::vector<std::string> split(const std::string& s, char sep) {
+    std::vector<std::string> out;
+    for (size_t a = 0;;) {
+        const size_t b = s.find(sep, a);
+        if (b == std::string::npos) { out.push_back(s.substr(a)); return out; }
+        out.push_back(s.substr(a, b - a));
+        a = b + 1;
+    }
+}
+
+// parseTruth (cnveval.go:65-107); samples (non-null): keep a line only when one of its samples is in the set
+std::vector<CnvLine> cnv_parse(const std::string& path, const std::map<std::string, int>* samples) {
+    const std::string text = read_whole(path);
+    std::vector<CnvLine> out;
+    for (size_t a = 0; a < text.size();) {
+        const size_t nl = text.find('\n', a);
+        if (nl == std::string::npos) break;
+        std::string line = text.substr(a, nl - a);
+        a = nl + 1;
+        if (line.empty() || line[0] != '#') {
+            while (!line.empty() && (line.back() == '\r' || line.back() == '\n')) line.pop_back();   // TrimRight(l, "\r\n")
+            std::vector<std::string> f = split(line, '\t');
+            if (f.size() < 5) fatal(2, "panic: expected five fields for CNVs");
+            CnvLine c;
+            c.chrom = f[0];
+            for (int k = 1; k <= 3; k++)
+                if (!go_atoi(f[(size_t)k], k == 1 ? c.start : (k == 2 ? c.end : c.cn)))
+                    fatal(2, "panic: strconv.Atoi: parsing \"%s\": invalid syntax or value out of range", f[(size_t)k].c_str());
+            c.samples = split(f[4], ',');
+            if (samples) {
+                bool found = false;
+                for (const std::string& s : c.samples) found = found || samples->count(s);
+                if (!found) continue;
+            }
+            out.push_back(std::move(c));
+        }
+    }
+    return out;
+}
+
+}  // namespace
+
+static int cmd_cnveval(int argc, char** argv) {
+    std::string m = "0.4";
+    bool limit = false;
+    ArgParser ap;
+    ap.prog = "cnveval";
+    ap.add("minoverlap", 'm', &m);
+    ap.addb("limitsamples", 's', &limit);
+    ap.parse(argc, argv);
+    if (ap.positional.size() < 2) ap.fail(ap.positional.empty() ? "truth is required" : "test is required");
+    if (ap.positional.size() > 2) ap.fail("too many positional arguments at '" + ap.positional[2] + "'");
+    char* endp = nullptr;
+    const double po = strtod(m.c_str(), &endp);
+    if (m.empty() || *endp) ap.fail("error processing minoverlap: strconv.ParseFloat: parsing \"" + m + "\": invalid syntax");
+    if (po > 1 || po <= 0) ap.fail("minoverlap must be between 0 and 1");              // NaN passes, as in the reference
+    const bool timing = getenv("GL_TIMING") != nullptr;        // phase wall clocks on stderr
+    double tp = now_s();
+    auto mark = [&](const char* what) { if (timing) { const double t = now_s(); fprintf(stderr, "[cnveval timing] %-22s %.3f s\n", what, t - tp); tp = t; } };
+
+    const std::vector<CnvLine> tests = cnv_parse(ap.positional[1], nullptr);
+    char msg[128];
+    snprintf(msg, sizeof msg, "cnvs in test-set (%zu)", tests.size());
+    go_log(msg);
+    std::map<std::string, int> first;                            // -s: the first sample of every test line
+    for (const CnvLine& c : tests) first.emplace(c.samples[0], 0);
+    const std::vector<CnvLine> truths = cnv_parse(ap.positional[0], limit ? &first : nullptr);
+    size_t n_mem = 0;
+    for (const CnvLine& t : truths) n_mem += t.samples.size();
+    snprintf(msg, sizeof msg, "%zu total cnvs in truth-set (%zu)", n_mem, truths.size());
+    go_log(msg);
+    mark("read + parse");
+
+    // chrom ranks in bytewise name order; samples numbered as met
+    std::map<std::string, int32_t> chrom;
+    for (const CnvLine& c : tests) chrom.emplace(c.chrom, 0);
+    for (const CnvLine& t : truths) chrom.emplace(t.chrom, 0);
+    int32_t r = 0;
+    for (auto& kv : chrom) kv.second = r++;
+    std::map<std::string, int32_t> sample;
+    auto sid = [&](const std::string& s) { return sample.emplace(s, (int32_t)sample.size()).first->second; };
+    std::vector<int32_t> c_sample, c_chrom, t_chrom, t_mem_sample;
+    std::vector<int64_t> c_start, c_end, c_cn, t_start, t_end, t_cn, t_mem_ptr{0};
+    for (const CnvLine& c : tests) {
+        c_sample.push_back(sid(c.samples[0])); c_chrom.push_back(chrom[c.chrom]);
+        c_start.push_back(c.start); c_end.push_back(c.end); c_cn.push_back(c.cn);
+    }
+    for (const CnvLine& t : truths) {
+        t_chrom.push_back(chrom[t.chrom]); t_start.push_back(t.start); t_end.push_back(t.end); t_cn.push_back(t.cn);
+        for (const std::string& s : t.samples) t_mem_sample.push_back(sid(s));
+        t_mem_ptr.push_back((int64_t)t_mem_sample.size());
+    }
+    const int32_t S = (int32_t)sample.size();
+    mark("intern");
+
+    gl_ctx* ctx = open_ctx(0, "goleft cnveval");
+    std::vector<uint64_t> st((size_t)S * 12);
+    const int rc = gl_cnveval(ctx, S, c_sample.data(), c_chrom.data(), c_start.data(), c_end.data(), c_cn.data(), (int64_t)tests.size(),
+                              t_chrom.data(), t_start.data(), t_end.data(), t_cn.data(), (int64_t)truths.size(), t_mem_ptr.data(),
+                              t_mem_sample.data(), po, st.data());
+    if (rc == GL_EINVAL) fatal(2, "panic: %s (calls count test-set lines, truths truth-set lines, from 0, without '#' lines)", gl_last_error(ctx));
+    glck(ctx, rc, "gl_cnveval");
+    mark("evaluate");
+
+    uint64_t tab[4][4] = {};                                      // Tabulate (cnveval.go:118-133)
+    for (int32_t s = 0; s < S; s++)
+        for (int c = 0; c < 3; c++)
+            for (int k = 0; k < 4; k++) tab[c][k] += st[(size_t)s * 12 + (size_t)c * 4 + (size_t)k];
+    for (int c = 0; c < 3; c++)
+        for (int k = 0; k < 4; k++) tab[3][k] += tab[c][k];
+    static const char* kClass[4] = {"0-20000", "20000-100000", ">=100000", "all"};
+    for (int c = 0; c < 4; c++) {
+        const long long TP = (long long)tab[c][0], FP = (long long)tab[c][1], FN = (long long)tab[c][2];
+        const std::string p = go_float("%.4f", (double)TP / (double)(TP + FP)), q = go_float("%.4f", (double)TP / (double)(TP + FN));
+        // Stat.String's "%-04d": with '-', Go and C both ignore '0' and pad with spaces on the right
+        printf("size-class: %-12s | precision: %s (%-4lld / (%-4lld + %-4lld)) recall: %s (%-4lld / (%-4lld + %-4lld))\n",
+               kClass[c], p.c_str(), TP, TP, FP, q.c_str(), TP, TP, FN);
+    }
+    mark("tabulate + print");
+    gl_ctx_destroy(ctx);
+    return 0;
+}
+
 static void print_progs() {                                                          // cmd/goleft/goleft.go:33-53
     fprintf(stderr, "goleft Version: %s (GPU engine: %s)\n\n", kVersion, gl_version());
     fprintf(stderr, "covstats    : coverage and insert-size statistics on bams by sampling\n");
@@ -2120,6 +2277,7 @@ static void print_progs() {                                                     
     fprintf(stderr, "multidepth  : (extension; a separate binary in goleft) blocks of sufficient coverage across many bams\n");
     fprintf(stderr, "dcnv        : (extension; a separate binary in goleft) GC-debias and median-normalise a depthwed matrix\n");
     fprintf(stderr, "emdepth     : (extension; a library in goleft) per-sample copy numbers and CNVs from a depth matrix\n");
+    fprintf(stderr, "cnveval     : (extension; a separate binary in goleft) precision and recall of CNV calls against a truth set\n");
 }
 
 int main(int argc, char** argv) {
@@ -2134,6 +2292,7 @@ int main(int argc, char** argv) {
     if (prog == "multidepth") return cmd_multidepth(argc - 1, argv + 1);
     if (prog == "dcnv") return cmd_dcnv(argc - 1, argv + 1);
     if (prog == "emdepth") return cmd_emdepth(argc - 1, argv + 1);
+    if (prog == "cnveval") return cmd_cnveval(argc - 1, argv + 1);
     print_progs();
     return 1;
 }

@@ -321,6 +321,47 @@ func (c *Ctx) Emdepth(depths []float32, samples int) (cells []uint8, lambda []fl
 	return cells[:n*samples], lambda[:n*9], c.err(rc)
 }
 
+// CNVCall is one test-set call: the sample's index, the chromosome's rank in bytewise name order, start, end and CN.
+type CNVCall struct {
+	Sample, Chrom  int32
+	Start, End, CN int64
+}
+
+// CNVTruth is one truth-set site: the chromosome's rank, start, end, CN and the samples that carry it (a sample listed
+// twice counts twice).
+type CNVTruth struct {
+	Chrom          int32
+	Start, End, CN int64
+	Samples        []int32
+}
+
+// CNVEval replaces cnveval.Evaluate (cnveval/cnveval.go:163-341) for calls in file order: stats[s*12 + class*4 + k] is
+// the count k (TP, FP, FN, TN) of sample s in size class 0 (< 20000), 1 (< 100000) or 2, the reference's CohortStats.
+// Each sample's calls are put in Go's sort.Slice order on the host; the comparison runs on the GPU (DESIGN §1.12).
+func (c *Ctx) CNVEval(samples int, calls []CNVCall, truths []CNVTruth, minOverlap float64) ([]uint64, error) {
+	nc, nt := len(calls), len(truths)
+	cs, cc := make([]int32, nc+1), make([]int32, nc+1)
+	cb, ce, ccn := make([]int64, nc+1), make([]int64, nc+1), make([]int64, nc+1)
+	for i, x := range calls {
+		cs[i], cc[i], cb[i], ce[i], ccn[i] = x.Sample, x.Chrom, x.Start, x.End, x.CN
+	}
+	tc, mp := make([]int32, nt+1), make([]int64, nt+1)
+	tb, te, tcn := make([]int64, nt+1), make([]int64, nt+1), make([]int64, nt+1)
+	ms := make([]int32, 0, nt+1)
+	for i, t := range truths {
+		tc[i], tb[i], te[i], tcn[i] = t.Chrom, t.Start, t.End, t.CN
+		ms = append(ms, t.Samples...)
+		mp[i+1] = int64(len(ms))
+	}
+	ms = append(ms, 0)
+	stats := make([]uint64, samples*12+1)
+	rc := C.gl_cnveval(c.h, C.int32_t(samples), (*C.int32_t)(&cs[0]), (*C.int32_t)(&cc[0]), (*C.int64_t)(&cb[0]),
+		(*C.int64_t)(&ce[0]), (*C.int64_t)(&ccn[0]), C.int64_t(nc), (*C.int32_t)(&tc[0]), (*C.int64_t)(&tb[0]),
+		(*C.int64_t)(&te[0]), (*C.int64_t)(&tcn[0]), C.int64_t(nt), (*C.int64_t)(&mp[0]), (*C.int32_t)(&ms[0]),
+		C.double(minOverlap), (*C.uint64_t)(&stats[0]))
+	return stats[:samples*12], c.err(rc)
+}
+
 // IndexcovPCA replaces indexcov's pca (indexcov/indexcov.go:773-807) on the samples x d byte matrix x (row-major, one row
 // of PCA bytes per sample): the projections X V[:, :k] (samples x k, row-major) for k = min(5, samples, d), with the sign
 // and rank rules of DESIGN §1.11, and the singular values.  The Gram runs on the tensor cores.

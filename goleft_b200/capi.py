@@ -194,6 +194,10 @@ _proto("gl_emdepth_factors", C.c_int, _vp)
 _proto("gl_emdepth_cnvs", C.c_int, _vp, C.c_int64, C.c_int32, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_int64, _i64p,
        _vp, C.c_int64, _i64p)
 _proto("gl_emdepth_sum_host", C.c_int, _vp, C.c_int64, C.POINTER(C.c_double), C.POINTER(C.c_uint8))
+_proto("gl_cnveval_order", C.c_int, _vp, _vp, C.c_int64, _vp)
+_proto("gl_cnveval", C.c_int, _vp, C.c_int32, _vp, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, C.c_double, _vp)
+_proto("gl_cnveval_device", C.c_int, _vp, C.c_int32, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, _vp,
+       C.c_int64, _vp, C.c_double, _vp)
 _proto("gl_indexcov_pca8", C.c_int, _vp, C.c_int64, _vp)
 _proto("gl_indexcov_pca", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _vp, _vp, _i32p, _vp)
 _proto("gl_indexcov_pca_device", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _vp, _vp, _i32p, _vp)
@@ -379,6 +383,19 @@ def emdepth_sum_host(v):
     if rc != GL_OK:
         raise GlError(rc, "gl_emdepth_sum_host: bad arguments")
     return s.value, bool(ok.value)
+
+
+# ---- cnveval (cnveval/cnveval.go), host-only part
+def cnveval_order(chrom, start) -> np.ndarray:
+    """Host-only: the permutation Go 1.21's sort.Slice leaves when it sorts calls given in file order by (chrom, start)"""
+    chrom, start = _as(chrom, np.int32), _as(start, np.int64)
+    if chrom.size != start.size:
+        raise ValueError("cnveval_order: chrom and start differ in length")
+    perm = np.empty(chrom.size, np.int64)
+    rc = lib.gl_cnveval_order(_ptr(chrom), _ptr(start), chrom.size, _ptr(perm))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_cnveval_order: bad arguments")
+    return perm
 
 
 # ---- indexcov PCA (indexcov.go:686-705,773-807), host-only parts
@@ -1233,6 +1250,29 @@ class Ctx:
         v = [C.c_int64(0) for _ in range(3)]
         self._ck(lib.gl_emdepth_stats(self.h, *[C.byref(x) for x in v]))
         return dict(zip(("rows", "uncertified", "sequential"), (x.value for x in v)))
+
+    # ---- cnveval
+    def cnveval(self, S: int, c_sample, c_chrom, c_start, c_end, c_cn, t_chrom, t_start, t_end, t_cn, t_mem_ptr, t_mem_sample,
+                po: float = 0.4) -> np.ndarray:
+        """(S, 3, 4) uint64 TP, FP, FN, TN per sample and size class.  Calls in file order; truth t carries the samples
+        t_mem_sample[t_mem_ptr[t]:t_mem_ptr[t + 1]]; chrom ranks follow the names' bytewise order."""
+        c = [_as(c_sample, np.int32), _as(c_chrom, np.int32), _as(c_start, np.int64), _as(c_end, np.int64), _as(c_cn, np.int64)]
+        t = [_as(t_chrom, np.int32), _as(t_start, np.int64), _as(t_end, np.int64), _as(t_cn, np.int64)]
+        mp, ms = _as(t_mem_ptr, np.int64), _as(t_mem_sample, np.int32)
+        if any(a.size != c[0].size for a in c) or any(a.size != t[0].size for a in t) or mp.size != t[0].size + 1 or ms.size != mp[-1]:
+            raise ValueError("cnveval: array lengths disagree")
+        out = np.empty((S, 3, 4), np.uint64)
+        self._ck(lib.gl_cnveval(self.h, S, *[_ptr(a) for a in c], c[0].size, *[_ptr(a) for a in t], t[0].size, _ptr(mp), _ptr(ms),
+                                float(po), _ptr(out)))
+        return out
+
+    def cnveval_device(self, S: int, d_c_ptr: DevBuf, n_calls: int, d_c_chrom: DevBuf, d_c_start: DevBuf, d_c_end: DevBuf,
+                       d_c_cn: DevBuf, n_truths: int, d_t_chrom: DevBuf, d_t_start: DevBuf, d_t_end: DevBuf, d_t_cn: DevBuf,
+                       d_m_ptr: DevBuf, n_mem: int, d_m_truth: DevBuf, po: float, d_stats: DevBuf):
+        """the resident layout of include/goleft_b200.h (gl_cnveval_device); d_stats: S x 12 uint64"""
+        self._ck(lib.gl_cnveval_device(self.h, S, d_c_ptr.ptr, n_calls, d_c_chrom.ptr, d_c_start.ptr, d_c_end.ptr, d_c_cn.ptr, n_truths,
+                                       d_t_chrom.ptr, d_t_start.ptr, d_t_end.ptr, d_t_cn.ptr, d_m_ptr.ptr, n_mem, d_m_truth.ptr,
+                                       float(po), d_stats.ptr))
 
     # ---- indexcov PCA
     def indexcov_pca(self, x: np.ndarray, k: int = 5, D: Optional[int] = None, want_gram: bool = False):

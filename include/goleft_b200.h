@@ -544,6 +544,34 @@ int  gl_emdepth_cnvs(const uint8_t* cells, int64_t n, int32_t S, const int64_t* 
                      int64_t* rows, int64_t rows_cap, int64_t* n_rows);
 int  gl_emdepth_sum_host(const float* v, int64_t n, double* sum, uint8_t* certified);
 
+/* ---------------------------------------------------------------- cnveval
+ * Restates cnveval/cnveval.go Evaluate (a separate binary of the reference): TP, FP, FN and TN of CNV calls against a truth
+ * set, per sample and size class (DESIGN §1.12).  stats is uint64 [S][3][4]: class 0 (end - start < 20000), 1 (< 100000),
+ * 2 (the rest); counts TP, FP, FN, TN.  A sample without calls counts nothing (the reference's updatePositive and updateFP
+ * return early for it, so its missed truths are not FNs).  Chromosomes are ranks (int32 >= 0) that must follow the bytewise
+ * order of their names: the reference compares names, the library compares ranks.  Coordinates are int64; a call or truth
+ * with end < start or a coordinate outside [0, 2^62) is GL_EINVAL naming it (a policy: the reference takes them, but its
+ * walk then has no order-free form, and lengths must fit int64).  po is the minimum overlap, in (0, 1] or NaN (NaN: nothing
+ * qualifies, as in the reference), else GL_EINVAL.
+ *   gl_cnveval_order  : host-only: perm = the permutation Go 1.21's sort.Slice leaves when it sorts n calls given in file order
+ *                       by (chrom, start) (pdqsort, unstable: the order inside a tie is Go's own and changes the counts).
+ *   gl_cnveval        : from host arrays.  Calls (sample, chrom, start, end, CN) in file order; truths (chrom, start, end, CN)
+ *                       and their samples as a CSR: truth t carries t_mem_sample[t_mem_ptr[t], t_mem_ptr[t+1]) (a sample listed
+ *                       twice counts twice).  Orders on the host, uploads, runs the device pass, downloads stats.
+ *   gl_cnveval_device : the same on resident arrays laid out as gl_cnveval lays them out: calls grouped by sample (sample s has
+ *                       calls [c_ptr[s], c_ptr[s+1]), n_calls in all) in gl_cnveval_order's order; truths sorted by (chrom,
+ *                       start); memberships sample-major (sample s carries truths m_truth[m_ptr[s], m_ptr[s+1]), ascending,
+ *                       n_mem in all).  The layout is checked on the device (GL_EINVAL naming the first bad position). */
+int  gl_cnveval_order(const int32_t* chrom, const int64_t* start, int64_t n, int64_t* perm);
+int  gl_cnveval(gl_ctx* ctx, int32_t S, const int32_t* c_sample, const int32_t* c_chrom, const int64_t* c_start, const int64_t* c_end,
+                const int64_t* c_cn, int64_t n_calls, const int32_t* t_chrom, const int64_t* t_start, const int64_t* t_end,
+                const int64_t* t_cn, int64_t n_truths, const int64_t* t_mem_ptr, const int32_t* t_mem_sample, double po,
+                uint64_t* stats);
+int  gl_cnveval_device(gl_ctx* ctx, int32_t S, const int64_t* d_c_ptr, int64_t n_calls, const int32_t* d_c_chrom, const int64_t* d_c_start,
+                       const int64_t* d_c_end, const int64_t* d_c_cn, int64_t n_truths, const int32_t* d_t_chrom, const int64_t* d_t_start,
+                       const int64_t* d_t_end, const int64_t* d_t_cn, const int64_t* d_m_ptr, int64_t n_mem, const int64_t* d_m_truth,
+                       double po, uint64_t* d_stats);
+
 /* ---------------------------------------------------------------- covstats
  * V2: histogram of int32 values in [lo,hi) -> hist[v-lo].  `goleft covstats` builds it over the sampled insert sizes,
  * template lengths and read lengths and reads every order statistic of covstats/covstats.go:57-76,175-199 off its running

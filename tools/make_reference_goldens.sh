@@ -16,6 +16,7 @@
 #                                                        where the reference's median32 panics)
 #   tests/golden/ref_emdepth_gotest.txt                  `go test ./emdepth` (its TestBig fails: it expects CN 8, the code gives 9)
 #   tests/golden/ref_indexcov_pca{8,4}.ped               goleft indexcov --fai on the .bai cohorts of tests/golden/make_pca_cohort.py
+#   tests/golden/ref_cnveval_<case>_<mode>.txt           cnveval stdout on the sets of tests/golden/make_cnveval_sets.py
 #
 # This image has neither toolchain (`go version`, `samtools --version`: command not found), so the files cannot be made
 # here; until they exist every report says "bit-exact vs the restated oracle, parity unpinned".  tests/test_reference_goldens.py
@@ -212,6 +213,16 @@ awk 'BEGIN{OFS="\t"; srand(11); printf "#chrom\tstart\tend"; for(i=0;i<9;i++) pr
 python3 "$(dirname "$0")/../tests/golden/make_pca_cohort.py" "$TMP/pcac"
 for c in pca8 pca4; do
   "$G" indexcov -d "$TMP/$c" --fai "$TMP/pcac/g.fa.fai" "$TMP/pcac/$c"/s*.bai && cp "$TMP/$c/$c-indexcov.ped" "$OUT/ref_indexcov_$c.ped" || true
+done
+# cnveval (cnveval/cmd/cnveval): stdout on the sets tests/golden/make_cnveval_sets.py writes, for each argument list of
+# its MODES.  Run inside $TMP: the reference writes its CPU profile x.cpu.pprof into the working directory.
+( cd "$REF" && CGO_ENABLED=0 go build -o "$TMP/cnveval" ./cnveval/cmd/cnveval )
+python3 "$(dirname "$0")/../tests/golden/make_cnveval_sets.py" "$TMP/cnv"
+for c in cohort quirks; do
+  for m in default:"" limit:"-s" m05:"-m 0.5"; do
+    # shellcheck disable=SC2086
+    ( cd "$TMP" && "$TMP/cnveval" ${m#*:} "$TMP/cnv/$c.truth.bed" "$TMP/cnv/$c.test.bed" > "$OUT/ref_cnveval_${c}_${m%%:*}.txt" ) || rm -f "$OUT/ref_cnveval_${c}_${m%%:*}.txt"
+  done
 done
 samtools --version | head -1 > "$OUT/ref_PROVENANCE.txt"; go version >> "$OUT/ref_PROVENANCE.txt"; (cd "$REF" && git rev-parse HEAD 2>/dev/null || true) >> "$OUT/ref_PROVENANCE.txt"
 echo "wrote $(ls "$OUT"/ref_* | wc -l) files to $OUT"

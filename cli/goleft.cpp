@@ -1729,6 +1729,9 @@ static int cmd_samplename(int argc, char** argv) {
 // GC as Go does (gl_go_argsort_f64), debias and median-normalise every sample on the GPU (gl_dcnv_normalize, column blocks
 // sized to device memory), and write depth.bed with "%.2f" tokens made on the GPU (gl_format_f2).  The reference's panics
 // are an error message and exit 2.  Parsing and row assembly run on the host pool.
+// `dcnv --svd PCT` (also --svd=PCT, before the positionals; DESIGN §1.13) then removes the cohort's leading components from
+// the normalised matrix (gl_dcnv_svd, row blocks sized to device memory) and logs "variance:" with the removed ones' shares.
+// PCT must be finite and >= 0, else exit 255 as go-arg's flag errors.
 namespace {
 
 struct DcnvRow { const char* p; size_t n; };                 // one line, without its "\n"
@@ -1889,6 +1892,21 @@ void matrix_parse(Matrix& m) {
 }  // namespace
 
 static int cmd_dcnv(int argc, char** argv) {
+    double svd_pct = -1;                                         // --svd PCT; < 0: off
+    if (argc >= 2 && strncmp(argv[1], "--svd", 5) == 0 && (argv[1][5] == 0 || argv[1][5] == '=')) {
+        ArgParser ap;
+        ap.prog = "goleft dcnv";
+        const int used = argv[1][5] == '=' ? 1 : 2;
+        if (used == 2 && argc < 3) ap.fail("missing value for --svd");
+        const std::string v = used == 1 ? argv[1] + 6 : argv[2];
+        char* endp = nullptr;
+        const double pct = strtod(v.c_str(), &endp);
+        if (v.empty() || *endp) ap.fail("error processing svd: strconv.ParseFloat: parsing \"" + v + "\": invalid syntax");
+        if (!std::isfinite(pct) || pct < 0) ap.fail("svd must be a finite percentage >= 0");
+        svd_pct = pct;
+        argc -= used;
+        argv += used;
+    }
     if (argc < 3) fatal(2, "panic: runtime error: index out of range (usage: goleft dcnv <depthwed matrix> <ref.fa>)");
     const std::string path = argv[1], fasta = argv[2];
     const bool timing = getenv("GL_TIMING") != nullptr;        // phase wall clocks on stderr
@@ -1964,6 +1982,17 @@ static int cmd_dcnv(int argc, char** argv) {
     if (rc == GL_ERANGE) fatal(2, "panic: runtime error: index out of range: %s", gl_last_error(ctx));
     glck(ctx, rc, "gl_dcnv_normalize");
     mark("normalize");
+    if (svd_pct >= 0) {
+        std::vector<double> sv(S);
+        int32_t n_removed = 0;
+        glck(ctx, gl_dcnv_svd(ctx, X.data(), (int64_t)R, (int64_t)S, (int32_t)S, svd_pct, 0, sv.data(), nullptr, &n_removed, nullptr), "gl_dcnv_svd");
+        double sum = 0;
+        for (double v : sv) if (v > 0) sum += v;
+        std::string msg = "variance:";
+        for (int32_t i = 0; i < n_removed; i++) msg += " " + go_float("%.2f", 100 * sv[(size_t)i] / sum);
+        go_log(msg.c_str());
+        mark("svd");
+    }
 
     // ---- depth.bed: "%.2f" tokens from the GPU, rows assembled on the host pool
     FILE* fo = fopen("depth.bed", "w");

@@ -301,6 +301,20 @@ func (c *Ctx) Dcnv(depths []float64, gcs []float64, samples int) ([]float64, err
 	return medians, c.err(rc)
 }
 
+// DcnvSVD replaces scalers.ZScore.Scale + debiaser.SVD{MinVariancePct}.Debias + ZScore.UnScale (dcnv/scalers/scalers.go:25-56,
+// dcnv/debiaser/debiaser.go:173-200) on the normalised n x S row-major matrix `depths`, in place: rows whose values are all
+// equal are left as they are, the leading components whose share of the singular values is above minPct (at most 15) are
+// removed from the z-scores of the others.  Returns the S singular values and how many components were removed; the
+// reference logs "variance:" with 100 s[i] / sum(s) of each removed one.
+func (c *Ctx) DcnvSVD(depths []float64, samples int, minPct float64) (sv []float64, removed int, err error) {
+	n := len(depths) / samples
+	sv = make([]float64, samples)
+	var nr C.int32_t
+	rc := C.gl_dcnv_svd(c.h, (*C.double)(&depths[0]), C.int64_t(n), C.int64_t(samples), C.int32_t(samples), C.double(minPct), 0,
+		(*C.double)(&sv[0]), nil, &nr, nil)
+	return sv, int(nr), c.err(rc)
+}
+
 // FormatF2 is fmt.Sprintf("%.2f", v) of every value, made on the GPU: 16 bytes per value, the text NUL-padded; an empty
 // token means the text is longer and the caller formats that value itself.
 func (c *Ctx) FormatF2(vals []float64) ([]byte, error) {

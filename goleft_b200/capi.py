@@ -203,6 +203,10 @@ _proto("gl_indexcov_pca", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.
 _proto("gl_indexcov_pca_device", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _vp, _vp, _i32p, _vp)
 _proto("gl_indexcov_pca_phases", C.c_int, _vp, C.POINTER(C.c_double))
 _proto("gl_pca_tridiag_top", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp)
+_proto("gl_dcnv_svd", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_double, C.c_int64, _vp, _vp, _i32p, _i64p)
+_proto("gl_dcnv_svd_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_double, _vp, _vp, _i32p, _i64p)
+_proto("gl_dcnv_svd_phases", C.c_int, _vp, C.POINTER(C.c_double))
+_proto("gl_pca_tridiag_above", C.c_int, _vp, _vp, C.c_int32, C.c_double, _vp, _i32p)
 
 
 def version() -> str:
@@ -416,6 +420,15 @@ def pca_tridiag_top(d, e, k: int, vectors: bool = True):
     if lib.gl_pca_tridiag_top(_ptr(d), _ptr(e), d.size, k, _ptr(w), _ptr(z)) != GL_OK:
         raise GlError(GL_EINVAL, "gl_pca_tridiag_top: bad arguments")
     return w, z
+
+
+def pca_tridiag_above(d, e, rel: float = 1e-12) -> np.ndarray:
+    """every eigenvalue above rel times the largest of the symmetric tridiagonal (d, e), descending, bisected on the host pool"""
+    d, e = _as(d, np.float64), _as(e, np.float64)
+    w, k = np.empty(d.size, np.float64), C.c_int32(0)
+    if lib.gl_pca_tridiag_above(_ptr(d), _ptr(e), d.size, rel, _ptr(w), C.byref(k)) != GL_OK:
+        raise GlError(GL_EINVAL, "gl_pca_tridiag_above: bad arguments")
+    return w[:k.value].copy()
 
 
 def chunk_rows(rs: int, re: int, W: int, run_start: np.ndarray, run_class: np.ndarray):
@@ -1230,6 +1243,30 @@ class Ctx:
 
     def format_f2_device(self, d_vals: DevBuf, n: int, d_tokens: DevBuf):
         self._ck(lib.gl_format_f2_device(self.h, d_vals.ptr, n, d_tokens.ptr))
+
+    def dcnv_svd(self, x: np.ndarray, min_pct: float, block_rows: int = 0, want_gram: bool = False):
+        """dcnv --svd on a copy of the n x S float64 matrix x -> (result, singular values[S], n_removed, n_kept,
+        Z^T Z (S x S) or None)"""
+        out = np.array(x, np.float64, order="C", copy=True)
+        n, S = out.shape
+        sv, nr, nk = np.empty(S, np.float64), C.c_int32(0), C.c_int64(0)
+        gram = np.empty((S, S), np.float64) if want_gram else None
+        self._ck(lib.gl_dcnv_svd(self.h, _ptr(out), n, S, S, float(min_pct), block_rows, _ptr(sv), _ptr(gram), C.byref(nr),
+                                 C.byref(nk)))
+        return out, sv, nr.value, nk.value, gram
+
+    def dcnv_svd_device(self, d_x: DevBuf, n: int, ld: int, S: int, min_pct: float, want_gram: bool = False):
+        """dcnv --svd in place on the device matrix d_x -> (singular values[S], n_removed, n_kept, Z^T Z or None)"""
+        sv, nr, nk = np.empty(S, np.float64), C.c_int32(0), C.c_int64(0)
+        gram = np.empty((S, S), np.float64) if want_gram else None
+        self._ck(lib.gl_dcnv_svd_device(self.h, d_x.ptr, n, ld, S, float(min_pct), _ptr(sv), _ptr(gram), C.byref(nr), C.byref(nk)))
+        return sv, nr.value, nk.value, gram
+
+    def dcnv_svd_phases(self):
+        """seconds of the last dcnv_svd call: {gram, eigen, project, copies}"""
+        t = (C.c_double * 4)()
+        self._ck(lib.gl_dcnv_svd_phases(self.h, t))
+        return dict(zip(("gram", "eigen", "project", "copies"), list(t)))
 
     # ---- emdepth
     def emdepth(self, x: np.ndarray, block_rows: int = 0, ld: Optional[int] = None, S: Optional[int] = None, want_lambda: bool = True):

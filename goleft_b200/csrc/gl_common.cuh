@@ -139,6 +139,7 @@ struct gl_ctx {
     unsigned cohort_fallbacks = 0;   // ic_cohort2_kernel: samples that took the exact fallback select in the last call
     int64_t em_rows = 0, em_uncertified = 0, em_sequential = 0;   // emdepth.cu: the last gl_emdepth* call (gl_emdepth_stats)
     double pca_phase[3] = {0, 0, 0};   // pca.cu: upload, Gram + centring, eigen of the last gl_indexcov_pca* call (seconds)
+    double svd_phase[4] = {0, 0, 0, 0};   // dcnv_svd.cu: stats + Gram, eigen, projection, copies of the last gl_dcnv_svd* call
     cudaStream_t comm_stream = nullptr; cudaEvent_t ev_comm = nullptr;   // gl_allgather_device_async
     void* nccl = nullptr; // ncclComm_t when gl_comm_init was called
     int rank = 0, world = 1;

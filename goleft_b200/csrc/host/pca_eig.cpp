@@ -1,4 +1,5 @@
-// pca_eig.cpp — see pca_eig.h.  Host-only, single-threaded, deterministic: the same input gives the same bits.
+// pca_eig.cpp — see pca_eig.h.  Host-only and deterministic: the same input gives the same bits.  Only
+// tridiag_values_above runs on the host pool, one independent bisection per index.
 #include "pca_eig.h"
 
 #include <float.h>
@@ -9,6 +10,7 @@
 #include <vector>
 
 #include "../../../include/goleft_b200.h"
+#include "thread_pool.h"
 
 namespace glpca {
 namespace {
@@ -32,33 +34,58 @@ double inf_norm(const double* d, const double* e, int n) {
     return nrm;
 }
 
+// what every bisection of one T shares: the squared off-diagonal, the pivot floor and the padded Gershgorin interval
+struct Sturm {
+    const double* d;
+    int n;
+    std::vector<double> e2;
+    double pivmin, glo, ghi;
+    Sturm(const double* d_, const double* e, int n_) : d(d_), n(n_), e2(n_ > 1 ? n_ - 1 : 1, 0.0) {
+        double emax2 = 0;
+        for (int i = 0; i + 1 < n; i++) { e2[i] = e[i] * e[i]; emax2 = std::max(emax2, e2[i]); }
+        pivmin = DBL_MIN * std::max(1.0, emax2);
+        glo = d[0], ghi = d[0];                                      // Gershgorin interval
+        for (int i = 0; i < n; i++) {
+            const double r = (i ? fabs(e[i - 1]) : 0.0) + (i + 1 < n ? fabs(e[i]) : 0.0);
+            glo = std::min(glo, d[i] - r);
+            ghi = std::max(ghi, d[i] + r);
+        }
+        const double pad = 4 * DBL_EPSILON * n * std::max(fabs(glo), fabs(ghi)) + 2 * pivmin;
+        glo -= pad;
+        ghi += pad;
+    }
+    int below(double x) const { return count_below(d, e2.data(), n, x, pivmin); }
+    // the eigenvalue with ascending index t, bisected until no double lies strictly inside (lo, hi)
+    double value(int t) const {
+        double lo = glo, hi = ghi;
+        for (;;) {
+            const double mid = lo + 0.5 * (hi - lo);
+            if (!(mid > lo && mid < hi)) break;
+            if (below(mid) <= t) lo = mid;
+            else hi = mid;
+        }
+        return lo + 0.5 * (hi - lo);
+    }
+};
+
 }  // namespace
 
 void tridiag_top_values(const double* d, const double* e, int n, int k, double* w) {
-    std::vector<double> e2(n > 1 ? n - 1 : 1, 0.0);
-    double emax2 = 0;
-    for (int i = 0; i + 1 < n; i++) { e2[i] = e[i] * e[i]; emax2 = std::max(emax2, e2[i]); }
-    const double pivmin = DBL_MIN * std::max(1.0, emax2);
-    double glo = d[0], ghi = d[0];                                   // Gershgorin interval
-    for (int i = 0; i < n; i++) {
-        const double r = (i ? fabs(e[i - 1]) : 0.0) + (i + 1 < n ? fabs(e[i]) : 0.0);
-        glo = std::min(glo, d[i] - r);
-        ghi = std::max(ghi, d[i] + r);
-    }
-    const double pad = 4 * DBL_EPSILON * n * std::max(fabs(glo), fabs(ghi)) + 2 * pivmin;
-    glo -= pad;
-    ghi += pad;
-    for (int j = 0; j < k; j++) {
-        const int t = n - 1 - j;                                     // ascending index of the j-th largest
-        double lo = glo, hi = ghi;
-        for (;;) {                                                   // ends when no double lies strictly inside (lo, hi)
-            const double mid = lo + 0.5 * (hi - lo);
-            if (!(mid > lo && mid < hi)) break;
-            if (count_below(d, e2.data(), n, mid, pivmin) <= t) lo = mid;
-            else hi = mid;
-        }
-        w[j] = lo + 0.5 * (hi - lo);
-    }
+    const Sturm st(d, e, n);
+    for (int j = 0; j < k; j++) w[j] = st.value(n - 1 - j);           // ascending index of the j-th largest
+}
+
+int tridiag_values_above(const double* d, const double* e, int n, double rel, double* w) {
+    const Sturm st(d, e, n);
+    const double top = st.value(n - 1);
+    if (!(top > 0)) return 0;
+    const double thr = rel * top;
+    const int m = std::max(1, n - st.below(thr));                    // eigenvalues >= thr; the bisection settles the rest
+    w[0] = top;
+    if (m > 1) glhost::ThreadPool::global().run(m - 1, [&](int64_t j, int) { w[j + 1] = st.value(n - 2 - (int)j); });
+    int k = 1;
+    while (k < m && w[k] > thr) k++;
+    return k;
 }
 
 void tridiag_vectors(const double* d, const double* e, int n, const double* w, int k, double* z) {
@@ -165,5 +192,11 @@ extern "C" int gl_pca_tridiag_top(const double* d, const double* e, int32_t n, i
     if (!d || (n > 1 && !e) || !w || n < 1 || k < 1 || k > n) return GL_EINVAL;
     glpca::tridiag_top_values(d, e, n, k, w);
     if (z) glpca::tridiag_vectors(d, e, n, w, k, z);
+    return GL_OK;
+}
+
+extern "C" int gl_pca_tridiag_above(const double* d, const double* e, int32_t n, double rel, double* w, int32_t* count) {
+    if (!d || (n > 1 && !e) || !w || !count || n < 1 || !(rel >= 0) || !(rel < 1)) return GL_EINVAL;
+    *count = glpca::tridiag_values_above(d, e, n, rel, w);
     return GL_OK;
 }

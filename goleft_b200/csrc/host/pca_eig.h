@@ -10,6 +10,10 @@ namespace glpca {
 
 // w[0..k) = the k largest eigenvalues of T = tridiag(e, d, e) (d[0..n), e[0..n-1)), in descending order; k <= n
 void tridiag_top_values(const double* d, const double* e, int n, int k, double* w);
+// w[0..k) = every eigenvalue of T above rel * (the largest), descending, as tridiag_top_values finds each (bit for bit);
+// returns k (0 when the largest is not positive).  One Sturm count finds how many lie at or above the threshold, so only those
+// are bisected, each on its own task of the host pool.  w has room for n values.
+int tridiag_values_above(const double* d, const double* e, int n, double rel, double* w);
 // z[j*n .. j*n+n) = a unit eigenvector of T for w[j], j < k (w descending, as tridiag_top_values made them)
 void tridiag_vectors(const double* d, const double* e, int n, const double* w, int k, double* z);
 // The reference's projections from the eigenpairs (lambda descending, u column j at u[j*S..]) of the centred Gram Gc and

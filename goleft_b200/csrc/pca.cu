@@ -9,7 +9,7 @@
 //                   at most 32768 columns (32768 * 255^2 < 2^31, so s32 cannot overflow) and adds its tile into the int64
 //                   Gram with integer atomics, which are exact, so the result does not depend on order or on the SM count.
 //   centre_kernel   mirrors the upper triangle, forms Gc in place over the Gram (int64 -> double).
-//   house/symv/rank2_kernel  Householder tridiagonalisation of Gc (Golub & Van Loan 8.3.1), one reflector per step; every
+//   house/symv/rank2_kernel  Householder tridiagonalisation of Gc (Golub & Van Loan 8.3.1; sym_tridiag, shared with dcnv_svd.cu), one reflector per step; every
 //                   reduction has a fixed order (lane-strided partial sums, then a fixed shuffle tree).
 // The top k eigenvalues (Sturm bisection), their vectors (inverse iteration) and the back-transformation through the
 // reflectors run on the host (host/pca_eig.cpp), on O(S k) and O(S^2 k) data.
@@ -18,6 +18,7 @@
 #include "gl_common.cuh"
 #include "host/pca8.h"
 #include "host/pca_eig.h"
+#include "sym_eig.cuh"
 
 namespace {
 
@@ -274,6 +275,58 @@ int check_shape(gl_ctx* ctx, const char* fn, int64_t ld, int32_t S, int64_t D, i
     return GL_OK;
 }
 
+}  // namespace
+
+int sym_tridiag(gl_ctx* ctx, double* A, int S, SymTridiag& t) {
+    gl_scratch tmp(ctx);
+    double *d_d, *d_e, *d_tau, *d_p;
+    GL_CHECK(tmp.alloc(d_d, (size_t)S));
+    GL_CHECK(tmp.alloc(d_e, (size_t)S));
+    GL_CHECK(tmp.alloc(d_tau, (size_t)S));
+    GL_CHECK(tmp.alloc(d_p, (size_t)S));
+    for (int j = 0; j + 2 < S; j++) {                              // Householder tridiagonalisation
+        const int m = S - j - 1;
+        house_kernel<<<1, 256, 0, ctx->stream>>>(A, S, j, d_d, d_e, d_tau);
+        symv_kernel<<<(m + 7) / 8, 256, 0, ctx->stream>>>(A, S, j, d_tau, d_p);
+        rank2_kernel<<<(m + kRank2Rows - 1) / kRank2Rows, 256, 0, ctx->stream>>>(A, S, j, d_tau, d_p);
+        GL_LAUNCHED(ctx, 3);
+    }
+    const size_t n2 = (size_t)S * S;
+    t.n = S;
+    t.hA.assign(n2, 0.0);
+    t.d.assign((size_t)S, 0.0);
+    t.e.assign((size_t)S, 0.0);
+    t.tau.assign((size_t)S, 0.0);
+    GL_CUDA(ctx, cudaMemcpyAsync(t.hA.data(), A, n2 * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (S > 2) {
+        GL_CUDA(ctx, cudaMemcpyAsync(t.d.data(), d_d, (size_t)(S - 2) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        GL_CUDA(ctx, cudaMemcpyAsync(t.e.data(), d_e, (size_t)(S - 2) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+        GL_CUDA(ctx, cudaMemcpyAsync(t.tau.data(), d_tau, (size_t)(S - 2) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int i = std::max(0, S - 2); i < S; i++) t.d[(size_t)i] = t.hA[(size_t)i * S + i];
+    if (S >= 2) t.e[(size_t)S - 2] = t.hA[(size_t)(S - 1) * S + (S - 2)];
+    return GL_OK;
+}
+
+void SymTridiag::back_transform(double* u, int k) const {
+    const int S = n;
+    for (int jv = 0; jv < k; jv++) {                               // u = H_0 H_1 ... H_{S-3} z
+        double* y = &u[(size_t)jv * S];
+        for (int j = S - 3; j >= 0; j--) {
+            const double t = tau[(size_t)j];
+            if (t == 0) continue;
+            const double* v = &hA[(size_t)j * S + j + 1];
+            double s = 0;
+            for (int i = 0; i < S - j - 1; i++) s += v[i] * y[j + 1 + i];
+            s *= t;
+            for (int i = 0; i < S - j - 1; i++) y[j + 1 + i] -= s * v[i];
+        }
+    }
+}
+
+namespace {
+
 // the whole computation on the byte matrix d_x (row stride ld, 16-byte aligned) already on the device
 int pca_run(gl_ctx* ctx, const uint8_t* d_x, int64_t ld, int32_t S, int64_t D, int32_t k, double* proj, double* sv,
             int32_t* k_out, int64_t* gram, double t_upload) {
@@ -288,13 +341,8 @@ int pca_run(gl_ctx* ctx, const uint8_t* d_x, int64_t ld, int32_t S, int64_t D, i
     gl_scratch tmp(ctx);
     unsigned long long* d_G;
     long long* d_r;
-    double *d_d, *d_e, *d_tau, *d_p;
     GL_CHECK(tmp.alloc(d_G, n2));
     GL_CHECK(tmp.alloc(d_r, (size_t)S));
-    GL_CHECK(tmp.alloc(d_d, (size_t)S));
-    GL_CHECK(tmp.alloc(d_e, (size_t)S));
-    GL_CHECK(tmp.alloc(d_tau, (size_t)S));
-    GL_CHECK(tmp.alloc(d_p, (size_t)S));
     GL_CUDA(ctx, cudaMemsetAsync(d_G, 0, n2 * 8, ctx->stream));
     const int T = (S + kBM - 1) / kBM, tiles = T * (T + 1) / 2;
     const int64_t want = std::max<int64_t>(1, (2 * (int64_t)ctx->sm_count + tiles - 1) / tiles);
@@ -331,39 +379,12 @@ int pca_run(gl_ctx* ctx, const uint8_t* d_x, int64_t ld, int32_t S, int64_t D, i
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     const double t_gram = now() - t0;
     t0 = now();
-    double* A = reinterpret_cast<double*>(d_G);
-    for (int j = 0; j + 2 < S; j++) {                              // Householder tridiagonalisation
-        const int m = S - j - 1;
-        house_kernel<<<1, 256, 0, ctx->stream>>>(A, S, j, d_d, d_e, d_tau);
-        symv_kernel<<<(m + 7) / 8, 256, 0, ctx->stream>>>(A, S, j, d_tau, d_p);
-        rank2_kernel<<<(m + kRank2Rows - 1) / kRank2Rows, 256, 0, ctx->stream>>>(A, S, j, d_tau, d_p);
-        GL_LAUNCHED(ctx, 3);
-    }
-    std::vector<double> hA(n2), d((size_t)S), e((size_t)S, 0.0), tau((size_t)S, 0.0);
-    GL_CUDA(ctx, cudaMemcpyAsync(hA.data(), A, n2 * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    if (S > 2) {
-        GL_CUDA(ctx, cudaMemcpyAsync(d.data(), d_d, (size_t)(S - 2) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        GL_CUDA(ctx, cudaMemcpyAsync(e.data(), d_e, (size_t)(S - 2) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        GL_CUDA(ctx, cudaMemcpyAsync(tau.data(), d_tau, (size_t)(S - 2) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (int i = std::max(0, S - 2); i < S; i++) d[(size_t)i] = hA[(size_t)i * S + i];
-    if (S >= 2) e[(size_t)S - 2] = hA[(size_t)(S - 1) * S + (S - 2)];
+    SymTridiag tri;
+    GL_CHECK(sym_tridiag(ctx, reinterpret_cast<double*>(d_G), S, tri));
     std::vector<double> lam((size_t)kk), u((size_t)kk * S);
-    glpca::tridiag_top_values(d.data(), e.data(), S, kk, lam.data());
-    glpca::tridiag_vectors(d.data(), e.data(), S, lam.data(), kk, u.data());
-    for (int jv = 0; jv < kk; jv++) {                              // u = H_0 H_1 ... H_{S-3} z
-        double* y = &u[(size_t)jv * S];
-        for (int j = S - 3; j >= 0; j--) {
-            const double t = tau[(size_t)j];
-            if (t == 0) continue;
-            const double* v = &hA[(size_t)j * S + j + 1];
-            double s = 0;
-            for (int i = 0; i < S - j - 1; i++) s += v[i] * y[j + 1 + i];
-            s *= t;
-            for (int i = 0; i < S - j - 1; i++) y[j + 1 + i] -= s * v[i];
-        }
-    }
+    glpca::tridiag_top_values(tri.d.data(), tri.e.data(), S, kk, lam.data());
+    glpca::tridiag_vectors(tri.d.data(), tri.e.data(), S, lam.data(), kk, u.data());
+    tri.back_transform(u.data(), kk);
     std::vector<double> pj((size_t)S * kk);
     glpca::project(lam.data(), u.data(), c.data(), S, kk, pj.data(), sv);
     for (int i = 0; i < S; i++)

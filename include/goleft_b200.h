@@ -511,6 +511,28 @@ int  gl_dcnv_normalize(gl_ctx* ctx, const double* x, int64_t n, int64_t ld, cons
 int  gl_format_f2(gl_ctx* ctx, const double* vals, int64_t n, uint8_t* tokens);
 int  gl_format_f2_device(gl_ctx* ctx, const double* d_vals, int64_t n, uint8_t* d_tokens);
 int  gl_format_f2_host(const double* vals, int64_t n, uint8_t* tokens);
+/* dcnv --svd (DESIGN §1.13): remove a cohort's leading components from the n x S row-major float64 matrix (row stride ld >= S),
+ * in place: the reference's ZScore.Scale, SVD.Debias{MinVariancePct} and ZScore.UnScale.  Each row is z-scored (m = mean,
+ * sd with S - 1, z = (x - m) * (1 / sd)); a row whose values are all equal, and every row when S < 2, is excluded and never
+ * written.  s = the singular values of Z (the kept rows), from the eigenvalues of the S x S Gram Z^T Z, descending; an
+ * eigenvalue <= 1e-12 times the largest counts as 0.  n_removed = the first index n with n >= min(15, rank) or
+ * 100 s[n] / sum(s) <= min_pct; each kept row becomes max(0, (z - V_n V_n^T z) sd + m).  n_removed = 0 leaves x untouched.
+ *   gl_dcnv_svd        : host x, streamed through the device in row blocks of block_rows (0: as many as fit; rounded down to a
+ *                        multiple of 4), twice when the matrix does not fit.  The result does not depend on block_rows.
+ *   gl_dcnv_svd_device : the same on a device-resident d_x (8-byte aligned).
+ *   sv (nullable) receives S values (0 past the rank); gram (nullable) the S x S Z^T Z; n_kept (nullable) the rows that took part.  min_pct must be finite and
+ *   >= 0; a non-finite value in a row that is not excluded is GL_EINVAL naming the row; GL_ENOMEM when the S x S Gram and its
+ *   workspace do not fit.  1 <= S <= 65535.
+ *   gl_dcnv_svd_phases : seconds of the last call: stats + Gram, eigen, projection, host <-> device copies.
+ *   gl_pca_tridiag_above : host-only: every eigenvalue above rel times the largest of the symmetric tridiagonal (d[n], e[n-1]),
+ *                        descending, into w (room for n), *count of them; each bisected on the host pool, bit for bit as
+ *                        gl_pca_tridiag_top finds it.  0 <= rel < 1. */
+int  gl_dcnv_svd(gl_ctx* ctx, double* x, int64_t n, int64_t ld, int32_t S, double min_pct, int64_t block_rows, double* sv,
+                 double* gram, int32_t* n_removed, int64_t* n_kept);
+int  gl_dcnv_svd_device(gl_ctx* ctx, double* d_x, int64_t n, int64_t ld, int32_t S, double min_pct, double* sv, double* gram,
+                        int32_t* n_removed, int64_t* n_kept);
+int  gl_dcnv_svd_phases(gl_ctx* ctx, double* t4);
+int  gl_pca_tridiag_above(const double* d, const double* e, int32_t n, double rel, double* w, int32_t* count);
 
 /* ---------------------------------------------------------------- emdepth
  * Restates emdepth/emdepth.go (a library of the reference with no command): a cn.mops-style EM per row of an n x S depth

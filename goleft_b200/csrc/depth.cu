@@ -15,7 +15,7 @@
 // region on the next path down.
 //
 // Tile core (every path, DESIGN §1.3): 16 or 32 consecutive bases per thread (swizzled smem transpose), one thread-local
-// + one warp scan, REDUX-based window sums from registers, class runs detected on warp min/max with a
+// + one warp scan, REDUX-based window sums (one LDS per lane and window edge), class runs detected on warp min/max with a
 // per-base slow path, runs claimed per tile with one atomic and put in position order by K_gather.
 // All arithmetic is integer; results are bit-exact against oracle/oracle_depth.c.
 #include "gl_common.cuh"
@@ -357,6 +357,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     constexpr int kWElems = BPT * 32;                         // bases per warp
     __shared__ int s_warp_tot[WARPS];
     __shared__ int s_has_break;
+    __shared__ int s_tbase[WARPS * 32];                       // depth before each thread's first base (slow paths)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int tile_base = tile * kTile;                       // relative position of the tile
@@ -364,12 +365,14 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     const int idx0 = tile_base + tid * BPT;                   // relative position of this thread's first base
 
     // ---- BPT consecutive differences per thread; thread-local inclusive scan; one warp scan
+    // a thread's chunks: swz_chunk_t<BPT>(t * (BPT / 4) + j) == c0 ^ j for j < BPT / 4 (the XOR only reads bits of t)
+    const int c0 = swz_chunk_t<BPT>(tid * (BPT / 4));
     int x[BPT];
 #pragma unroll
     for (int j = 0; j < BPT / 4; j++) {
-        const int4 q = reinterpret_cast<const int4*>(s_tile)[swz_chunk_t<BPT>(tid * (BPT / 4) + j)];
+        const int4 q = reinterpret_cast<const int4*>(s_tile)[c0 ^ j];
         x[4 * j] = q.x; x[4 * j + 1] = q.y; x[4 * j + 2] = q.z; x[4 * j + 3] = q.w;
-        if (kZeroAfterRead) reinterpret_cast<int4*>(s_tile)[swz_chunk_t<BPT>(tid * (BPT / 4) + j)] = make_int4(0, 0, 0, 0);
+        if (kZeroAfterRead) reinterpret_cast<int4*>(s_tile)[c0 ^ j] = make_int4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int k = 1; k < BPT; k++) x[k] += x[k - 1];
@@ -486,13 +489,19 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     const bool fast_win = p.do_windows && full_warp && p.W >= BPT && p.win_min == nullptr && wmax < (1 << 22);
     const bool slow_win = p.do_windows && !fast_win;
 
-    // The slow paths index depth by position: this warp's private slice of s_depth (linear layout).
+    // Depth by position: this warp's private slice of s_depth holds x[k] (depth relative to the thread's tbase), swizzled
+    // like s_tile (base e of the slice at sw[swz_elem_t<BPT>(e)]) so that both a lane storing its BPT/4 chunks and 32 lanes
+    // reading 32 consecutive bases of one thread are conflict-free; the threads' tbase go to s_tbase.  Storing x instead of
+    // depth saves BPT adds per thread; a reader adds the owner's tbase.  s_tile cannot hold the slice: a warp that leaves the
+    // core early starts the next tile's atomics there.
     int* sw = s_depth + warp * kWElems;
-    if (slow_runs || slow_win) {
+    int* stb = s_tbase + warp * 32;
+    if (slow_runs || p.do_windows) {
         __syncwarp();
 #pragma unroll
         for (int j = 0; j < BPT / 4; j++)
-            reinterpret_cast<int4*>(sw + lane * BPT)[j] = make_int4(GL_D(4 * j), GL_D(4 * j + 1), GL_D(4 * j + 2), GL_D(4 * j + 3));
+            reinterpret_cast<int4*>(s_depth)[c0 ^ j] = make_int4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
+        stb[lane] = tbase;
         __syncwarp();
     }
 
@@ -539,11 +548,11 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
 
     // ---- window partial sums of this warp's 512 bases
     if (fast_win) {
-        // From registers.  For every window edge inside the warp each lane contributes the part of its 16 bases left
-        // of the edge that was not counted yet: all 16 (s16) for lanes left of the edge's lane, the first `cu` for the
-        // edge's lane, nothing right of it; one REDUX adds the lanes (< 2^31), lane 0 issues one 64-bit red per window.
-        // cu = edge % 16 is the same for the whole warp, so the partial sum is a jump into a fall-through chain
-        // (cu adds, no divergence) instead of a 16-way register select per lane.
+        // The sum of the warp's depths left of an edge at offset el * BPT + cu is, summed over the lanes j: all BPT depths
+        // of lane j (s16) for j < el, plus base j of lane el for j < cu — one LDS from the slice plus lane el's tbase by
+        // SHFL, no per-lane select.
+        // Each lane keeps what it has contributed so far (counted), so one REDUX of the differences gives the window's part
+        // in this warp (< 2^32 since depth < 2^22), and lane 0 issues one 64-bit red per window.
         const int s16 = BPT * tbase + xsum;
         const unsigned a0 = (unsigned)p.rs + (unsigned)warp_base;     // absolute, < 2^32
         const unsigned uW = (unsigned)p.W;
@@ -555,29 +564,18 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
         unsigned edge = uW - rem;                                     // offset of the next window edge in the warp, in (0, W]
         int counted = 0;
 #pragma unroll 1
-        while (true) {
-            const int el = (int)(edge / BPT);                         // lane holding the edge (>= 32: beyond the warp)
-            const unsigned cu = edge % BPT;                           // bases of that lane left of the edge (warp-uniform)
-            // sum of the first cu depths of a thread = cu * tbase + x[0] + .. + x[cu-1]: a jump into a fall-through chain
-            int part = 0;
-            switch (cu) {
-#define GL_CASE(k) case k: part += x[(k - 1) < BPT ? (k - 1) : 0]; [[fallthrough]];
-                GL_CASE(31) GL_CASE(30) GL_CASE(29) GL_CASE(28) GL_CASE(27) GL_CASE(26) GL_CASE(25) GL_CASE(24)
-                GL_CASE(23) GL_CASE(22) GL_CASE(21) GL_CASE(20) GL_CASE(19) GL_CASE(18) GL_CASE(17) GL_CASE(16)
-                GL_CASE(15) GL_CASE(14) GL_CASE(13) GL_CASE(12) GL_CASE(11) GL_CASE(10) GL_CASE(9) GL_CASE(8)
-                GL_CASE(7) GL_CASE(6) GL_CASE(5) GL_CASE(4) GL_CASE(3) GL_CASE(2) GL_CASE(1)
-#undef GL_CASE
-                default: break;
-            }
-            part += (int)cu * tbase;
-            const int cur = lane < el ? s16 : (lane == el ? part : 0);
+        for (; edge < (unsigned)kWElems; edge += uW, iw++) {         // edges inside the warp
+            const int el = (int)(edge / BPT);                         // lane holding the edge (warp-uniform)
+            const int cu = (int)(edge % BPT);                         // bases of that lane left of the edge (warp-uniform)
+            const int d = sw[swz_elem_t<BPT>(el * BPT + (lane & (BPT - 1)))] + __shfl_sync(kFull, tbase, el);
+            const int cur = (lane < el ? s16 : 0) + (lane < cu ? d : 0);
             const unsigned tot = (unsigned)__reduce_add_sync(kFull, cur - counted);
             counted = cur;
             if (lane == 0) atomicAdd(p.win_sum + ((long long)iw - p.w0), (unsigned long long)tot);
-            if (edge >= (unsigned)kWElems) break;
-            iw++;
-            edge += uW;
         }
+        // the window that runs past the warp's end (or ends exactly at it) gets the rest of the warp
+        const unsigned tot = (unsigned)__reduce_add_sync(kFull, s16 - counted);
+        if (lane == 0) atomicAdd(p.win_sum + ((long long)iw - p.w0), (unsigned long long)tot);
     } else if (slow_win) {
         // General path from this warp's smem slice: any W, min, ragged end, depth up to 2^31.
         const unsigned a0 = (unsigned)p.rs + (unsigned)warp_base;
@@ -592,7 +590,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
                     unsigned long long sum = 0;
                     int m = 0x7fffffff;
                     for (int xx = s + lane; xx < e; xx += 32) {
-                        const int dd = sw[xx];
+                        const int dd = sw[swz_elem_t<BPT>(xx)] + stb[xx / BPT];
                         sum += (unsigned long long)(unsigned)dd;
                         m = min(m, dd);
                     }
@@ -611,7 +609,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
                     unsigned long long sum = 0;
                     int m = 0x7fffffff;
                     for (int xx = s; xx < e; xx++) {
-                        const int dd = sw[xx];
+                        const int dd = sw[swz_elem_t<BPT>(xx)] + stb[xx / BPT];
                         sum += (unsigned long long)(unsigned)dd;
                         m = min(m, dd);
                     }
@@ -642,7 +640,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
                 m &= m - 1;
                 if (rank < p.run_cap) {
                     p.tmp_start[rank] = p.rs + idx0 + k;
-                    p.tmp_class[rank] = (unsigned char)cov_class(sw[lane * BPT + k], p.mincov, p.maxmean);
+                    p.tmp_class[rank] = (unsigned char)cov_class(tbase + sw[swz_elem_t<BPT>(lane * BPT + k)], p.mincov, p.maxmean);
                 }
                 rank++;
             }

@@ -161,6 +161,8 @@ _proto("gl_depth_text_bound", C.c_int64, C.c_char_p, C.c_int64)
 _proto("gl_depth_format_rows", C.c_int, _vp, C.c_char_p, _vp, _vp, _vp, C.c_int64, _vp, C.c_int64, _i64p)
 _proto("gl_depth_bed_contig", C.c_int, _vp, C.c_char_p, C.c_int64, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int64,
        C.c_int32, _vp, C.c_int64, _i64p, _vp, C.c_int64, _i64p)
+_proto("gl_depth_bed_region", C.c_int, _vp, C.c_char_p, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+       C.c_int64, C.c_int32, _vp, C.c_int64, _i64p, _vp, C.c_int64, _i64p)
 _proto("gl_depth_bed_contig_packed8", C.c_int, _vp, C.c_char_p, C.c_int64, _vp, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
        C.c_int64, _vp, C.c_int64, _i64p, _vp, C.c_int64, _i64p)
 _proto("gl_indexsplit_accumulate", C.c_int, _vp, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp)
@@ -950,42 +952,38 @@ class Ctx:
                                           out.size, C.byref(ln)))
         return out[: ln.value].tobytes()
 
-    def depth_bed_contig(self, chrom: str, length: int, start, end, W: int, mincov: int = 4, maxmean: int = 0,
-                         step: int = 10_000_000, threads: int = 0, out=None, raw: bool = False):
-        """One call: host int32 segments in -> (depth.bed, callable.bed) bytes out.  raw=True returns the two lengths only
-        (the bytes are in `out`)."""
-        n_win = (length - 1) // W + 1
+    def _bed_text(self, fn, args, chrom: str, n_win: int, out, raw: bool):
+        """fn(*args, depth_bed, cap, &len, callable_bed, cap, &len): BED text into `out` or buffers of the size it asks for"""
         keep = out is not None
         hd, ca = self._text_bufs(chrom, n_win, out)
         hl, cl = C.c_int64(0), C.c_int64(0)
-        cb = chrom.encode()
-        rc = lib.gl_depth_bed_contig(self.h, cb, length, _ptr(start), _ptr(end), start.size, W, mincov, maxmean, step, threads,
-                                     _ptr(hd), hd.size, C.byref(hl), _ptr(ca), ca.size, C.byref(cl))
+        rc = fn(*args, _ptr(hd), hd.size, C.byref(hl), _ptr(ca), ca.size, C.byref(cl))
         if rc == GL_ERANGE and not keep:
             hd, ca = np.empty(hl.value + 16, np.uint8), np.empty(cl.value + 16, np.uint8)
-            rc = lib.gl_depth_bed_contig(self.h, cb, length, _ptr(start), _ptr(end), start.size, W, mincov, maxmean, step, threads,
-                                         _ptr(hd), hd.size, C.byref(hl), _ptr(ca), ca.size, C.byref(cl))
+            rc = fn(*args, _ptr(hd), hd.size, C.byref(hl), _ptr(ca), ca.size, C.byref(cl))
         self._ck(rc)
         if raw:
             return hl.value, cl.value
         return hd[: hl.value].tobytes(), ca[: cl.value].tobytes()
 
+    def depth_bed_contig(self, chrom: str, length: int, start, end, W: int, mincov: int = 4, maxmean: int = 0,
+                         step: int = 10_000_000, threads: int = 0, out=None, raw: bool = False):
+        """One call: host int32 segments in -> (depth.bed, callable.bed) bytes out.  raw=True returns the two lengths only
+        (the bytes are in `out`)."""
+        args = (self.h, chrom.encode(), length, _ptr(start), _ptr(end), start.size, W, mincov, maxmean, step, threads)
+        return self._bed_text(lib.gl_depth_bed_contig, args, chrom, (length - 1) // W + 1, out, raw)
+
+    def depth_bed_region(self, chrom: str, rs: int, re: int, start, end, W: int, mincov: int = 4, maxmean: int = 0,
+                         step: int = 10_000_000, threads: int = 0, out=None, raw: bool = False):
+        """depth_bed_contig for the whole chunks [rs, re) of a contig (rs a multiple of step): what `goleft depth` writes for
+        one pass over a contig longer than a pass"""
+        args = (self.h, chrom.encode(), rs, re, _ptr(start), _ptr(end), start.size, W, mincov, maxmean, step, threads)
+        return self._bed_text(lib.gl_depth_bed_region, args, chrom, (re - 1) // W - rs // W + 1, out, raw)
+
     def depth_bed_contig_packed8(self, chrom: str, length: int, anchors, dstart, ln, W: int, mincov: int = 4, maxmean: int = 0,
                                  step: int = 10_000_000, out=None, raw: bool = False):
-        n_win = (length - 1) // W + 1
-        keep = out is not None
-        hd, ca = self._text_bufs(chrom, n_win, out)
-        hl, cl = C.c_int64(0), C.c_int64(0)
-        cb = chrom.encode()
-        args = (self.h, cb, length, _ptr(anchors), _ptr(dstart), _ptr(ln), anchors.size, W, mincov, maxmean, step)
-        rc = lib.gl_depth_bed_contig_packed8(*args, _ptr(hd), hd.size, C.byref(hl), _ptr(ca), ca.size, C.byref(cl))
-        if rc == GL_ERANGE and not keep:
-            hd, ca = np.empty(hl.value + 16, np.uint8), np.empty(cl.value + 16, np.uint8)
-            rc = lib.gl_depth_bed_contig_packed8(*args, _ptr(hd), hd.size, C.byref(hl), _ptr(ca), ca.size, C.byref(cl))
-        self._ck(rc)
-        if raw:
-            return hl.value, cl.value
-        return hd[: hl.value].tobytes(), ca[: cl.value].tobytes()
+        args = (self.h, chrom.encode(), length, _ptr(anchors), _ptr(dstart), _ptr(ln), anchors.size, W, mincov, maxmean, step)
+        return self._bed_text(lib.gl_depth_bed_contig_packed8, args, chrom, (length - 1) // W + 1, out, raw)
 
     def bgzf_inflate(self, data: bytes):
         """GPU inflate of a whole BGZF byte string -> (inflated bytes, per-block status int32[]); test / tool helper"""

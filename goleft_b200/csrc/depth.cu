@@ -894,8 +894,9 @@ struct SegRange { unsigned lo, hi, cnt; };
 
 __device__ __forceinline__ void fused_cells_of(const ScanParams& p, int tile, int maxlen, int& lo_cell, int& hi_cell) {
     // cells whose segments can cover base t0-1 or touch the tile: starts in [t0 - maxlen, t1)
+    // (t1 = t0 + min(kTile, re - t0): t0 + kTile itself overflows int when the last tile starts at 2^31 - kTile or later)
     const int t0 = p.rs + tile * kTile;
-    const int t1 = min(t0 + kTile, p.re);
+    const int t1 = t0 + min(kTile, p.re - t0);
     lo_cell = (max(t0 - maxlen, p.origin) - p.origin) >> kCellShift;
     hi_cell = min(((t1 - 1 - p.origin) >> kCellShift) + 1, p.ncells);   // exclusive; at most 82 cells
 }
@@ -991,7 +992,7 @@ __global__ void __launch_bounds__(kScanThreads, 4) depth_fused_kernel(const Scan
     int acc_max = 0;
     for (int it = 0; tile < p.num_tiles; tile += G, it ^= 1) {
         int* s_carry = s_carry2[it];
-        const int t0 = p.rs + tile * kTile, t1 = min(t0 + kTile, p.re);
+        const int t0 = p.rs + tile * kTile, t1 = t0 + min(kTile, p.re - t0);   // no overflow at the top of int32 (fused_cells_of)
         const bool first_tile = tile == 0;
         // (the previous core's barrier guarantees every warp has read + cleared its slice of the tile)
         if (fused_out_of_order(cur)) {                                  // uniform: every thread holds the same range

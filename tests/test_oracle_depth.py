@@ -97,6 +97,49 @@ def test_pileup_diff_equals_bruteforce():
         assert np.array_equal(a, c)
 
 
+@pytest.mark.parametrize("W", [1, 3, 16, 500, 4096, 10 ** 7, 2 ** 30])
+def test_oracle_at_top_of_int32(W):
+    """the GPU tests at the top of the int32 range (test_depth_int32_top_gpu.py) rest on the oracle there: its per-base
+    counts, window sums / minima and class runs against a numpy int64 restatement, for regions ending at INT32_MAX whose
+    genome-aligned last window ends past it, reads that end on INT32_MAX and forced run breaks inside the region"""
+    top = 2 ** 31 - 1
+    rng = np.random.default_rng(W)
+    for rs, re in [(top - 3 * 4096 - 4095, top), (top - 13_000, top - 1), (2 ** 31 - 4096 - 3 * 4096, 2 ** 31 - 4095)]:
+        s = rng.integers(rs - 300, re, 2500)
+        e = np.minimum(s + rng.integers(-5, 300, s.size), top)
+        s[:4] = [top - 1, top - 255, top - 4096, rs - 10]
+        e[:4] = top
+        s32, e32 = s.astype(np.int32), e.astype(np.int32)
+        x = np.arange(rs, re, dtype=np.int64)
+        lo, hi = np.clip(s, rs, re), np.clip(e, rs, re)
+        live = lo < hi
+        diff = np.zeros(re - rs + 1, np.int64)
+        np.add.at(diff, lo[live] - rs, 1)
+        np.add.at(diff, hi[live] - rs, -1)
+        depth = np.cumsum(diff)[:-1]
+        assert np.array_equal(orc.pileup_diff(s32, e32, rs, re), depth)
+        assert np.array_equal(orc.pileup_brute(s32, e32, rs, re), depth)
+        # windows k = rs//W .. (re-1)//W over [max(rs, kW), min(re, (k+1)W)); with re = INT32_MAX the last one's genome end
+        # is past it for every W here except 1
+        k = np.arange(rs // W, (re - 1) // W + 1, dtype=np.int64)
+        assert re != top or W == 1 or (k[-1] + 1) * W > top
+        edge = np.maximum(k * W, rs) - rs
+        ws, wm = orc.window_sums(depth, rs, re, W)
+        assert np.array_equal(ws, np.add.reduceat(depth, edge))
+        assert np.array_equal(wm, np.minimum.reduceat(depth, edge))
+        for mincov, maxmean, brk in [(4, 0, 0), (1, 6, 4096), (3, 8, 999), (2, 0, W)]:
+            cls = np.where(depth == 0, 0, np.where(depth < mincov, 1, np.where((maxmean > 0) & (depth >= maxmean), 3, 2)))
+            new = np.ones(x.size, bool)
+            new[1:] = cls[1:] != cls[:-1]
+            if brk:
+                new |= x % brk == 0
+            ra, rc = orc.class_runs(depth, rs, re, mincov, maxmean, brk)
+            assert np.array_equal(ra, x[new]) and np.array_equal(rc, cls[new])
+        # the walker's rows end on the region end
+        hd, ca = orc.walk_chunk("big", rs, re, W, 4, 0, depth)
+        assert parse_bed(hd)[-1][2] == re and parse_bed(ca)[-1][2] == re
+
+
 def test_synth_segments_shape():
     r = synth.reads(2_000_000)
     s, e = synth.segments(r)

@@ -1087,6 +1087,15 @@ class Ctx:
         self._ck(lib.gl_indexcov_cohort_device(self.h, d_sizes.ptr, d_sample_ptr.ptr, S, d_medians.ptr,
                                                d_depth.ptr if d_depth is not None else None))
 
+    def indexcov_counts_segs_device(self, d_depth: DevBuf, d_seg_start: DevBuf, d_seg_len: DevBuf, d_longest: Optional[DevBuf],
+                                    n_seg: int, d_counts70: DevBuf, d_bins4: DevBuf):
+        self._ck(lib.gl_indexcov_counts_segs_device(self.h, d_depth.ptr, d_seg_start.ptr, d_seg_len.ptr,
+                                                    d_longest.ptr if d_longest is not None else None, n_seg, d_counts70.ptr,
+                                                    d_bins4.ptr))
+
+    def format_g3_device(self, d_vals: DevBuf, n: int, d_tokens: DevBuf):
+        self._ck(lib.gl_format_g3_device(self.h, d_vals.ptr, n, d_tokens.ptr))
+
     def depthwed_aggregate_device(self, d_means: DevBuf, S: int, R: int, d_grp: Optional[DevBuf], n_out: int, d_out: DevBuf):
         self._ck(lib.gl_depthwed_aggregate_device(self.h, d_means.ptr, S, R, d_grp.ptr if d_grp is not None else None, n_out,
                                                   d_out.ptr))

@@ -14,6 +14,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import bamref  # noqa: E402
 from bamutil import cg_mix_records, cigar_lens, make_bai, make_bam, make_bam_indexed  # noqa: E402
 from goleft_b200 import capi  # noqa: E402
+from indexcov_cli_oracle import check_ped_columns, cohort_bais, expected_outputs, oracle_depths, read_ped  # noqa: E402
 from oracle import loader as orc  # noqa: E402
 
 GOLEFT = os.path.join(ROOT, "bin", "goleft")
@@ -363,38 +364,12 @@ def test_depth_empty_bam(tmp_path):
     assert len(hd) == 1658 + 2001 and all(r[3] == "0" for r in hd)
 
 
-def _cohort_bais(tmp_path, S=7, seed=3):
-    rng = np.random.default_rng(seed)
-    refs = [("1", 3_000_000), ("2", 2_000_000), ("GL000207.1", 4262), ("X", 1_500_000), ("Y", 600_000), ("NC_007605", 171823)]
-    fai = tmp_path / "g.fa.fai"
-    fai.write_text("".join("%s\t%d\t6\t60\t61\n" % r for r in refs))
-    paths, lin = [], []
-    for k in range(S):
-        male = k % 2 == 0
-        per_ref = []
-        v = 100000
-        for name, L in refs:
-            nt = L // 16384 + 1
-            if k == 3 and name == "2":
-                nt -= 5                                            # a shorter sample: "0" columns
-            scale = {"X": 0.5 if male else 1.0, "Y": 0.5 if male else 0.01}.get(name, 1.0)
-            sizes = np.maximum(0, rng.normal(1.6e9 * scale, 1.5e8, nt)).astype(np.int64)
-            iv = [v]
-            for sz in sizes:
-                v += int(sz); iv.append(v)
-            per_ref.append(iv if nt > 0 else [])
-        p = tmp_path / ("smp%d.rest.bai" % k)
-        p.write_bytes(make_bai(per_ref, [(1000 * (k + 1), 10 + k) for _ in refs]))
-        paths.append(str(p)); lin.append(per_ref)
-    return refs, str(fai), paths, lin
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("N", [10, 200])
 def test_indexsplit(tmp_path, N):
     """goleft indexsplit (indexsplit/indexsplit.go): regions of about equal cohort data.  Text equals the oracle's
     restatement of Split; the regions tile every chromosome exactly once (indexsplit/functional-tests.sh:33-36)."""
-    refs, fai, paths, lin = _cohort_bais(tmp_path, S=9, seed=N)
+    refs, fai, paths, lin = cohort_bais(tmp_path, S=9, seed=N)
     bed = tmp_path / "prob.bed"
     bed.write_text("1\t1000000\t1100000\nX\t5\t10\n2\t7\t3\n")
     p = run("indexsplit", "-n", str(N), "--fai", fai, "-p", str(bed), *paths)
@@ -423,7 +398,7 @@ def test_indexcov_cohort(tmp_path, extranorm, form):
     """form "bam": header-only BAMs next to the same indexes, with `-c 2`.  RefsFromBam appends the named reference to the
     header's (indexcov.go:333-335), so "2" is reported twice: its rows and ROC block twice, its bins counted twice, and with
     -n both copies normalised from the original values (NormalizedDepth returns a fresh slice, indexcov.go:129-151)."""
-    refs, fai, paths, lin = _cohort_bais(tmp_path)
+    refs, fai, paths, lin = cohort_bais(tmp_path)
     out = tmp_path / "tt"
     order = list(range(len(refs)))
     names = ["smp%d-rest" % k for k in range(len(paths))]          # GetShortName for .bai (indexcov.go:238-245)
@@ -442,55 +417,11 @@ def test_indexcov_cohort(tmp_path, extranorm, form):
         args += ["--fai", fai]
     p = run(*args, *paths)
     assert "indexcov finished" in p.stderr
-    S = len(paths)
-    # oracle
-    med, depths = [], []
-    for k in range(S):
-        voff = np.array([v for r in lin[k] for v in r], np.uint64)
-        ptr = np.concatenate([[0], np.cumsum([len(r) for r in lin[k]])]).astype(np.int64)
-        sizes, sptr = orc.ic_sizes(voff, ptr)
-        m = orc.ic_median(sizes)
-        med.append(m)
-        d = orc.ic_normalize(sizes, float(m))
-        depths.append([d[sptr[r]:sptr[r + 1]] for r in range(len(refs))])
-    exp_rows = ["#chrom\tstart\tend\t" + "\t".join(names)]
-    bins = np.zeros((S, 4), np.int64)
-    roc_txt = ""
-    for r in order:
-        name, L = refs[r]
-        if name.startswith("NC"):
-            continue                                                # default --excludepatt
-        ds = [depths[k][r] for k in range(S)]
-        longest = max(len(d) for d in ds)
-        is_sex = name in ("X", "Y")
-        if extranorm and not is_sex:
-            mat = np.zeros((S, longest), np.float32)
-            for k in range(S):
-                mat[k, :len(ds[k])] = ds[k]
-            mat = orc.ic_xnorm(mat, np.array([len(d) for d in ds], np.int32))
-            ds = [mat[k, :len(ds[k])] for k in range(S)]
-        for i in range(longest):
-            exp_rows.append("%s\t%d\t%d\t" % (name, i * 16384, (i + 1) * 16384) +
-                            "\t".join("0" if i >= len(ds[k]) else "%.3g" % ds[k][i] for k in range(S)))
-        if not is_sex:
-            for k in range(S):
-                bins[k] += orc.ic_bins(ds[k], longest)
-        rocs = [orc.ic_roc(orc.ic_counts(ds[k])) for k in range(S)]
-        roc_txt += "#chrom\tcov\t" + "\t".join(names) + "\n"
-        for i in range(70):
-            roc_txt += "%s\t%.2f\t" % (name, i / (70 * (2.0 / 3.0))) + "\t".join("%.2f" % rocs[k][i] for k in range(S)) + "\n"
-    got = gzip.open(str(out / "tt-indexcov.bed.gz"), "rt").read().splitlines()
-    assert got == exp_rows
+    depths = oracle_depths(lin)
+    rows, roc_txt, bins = expected_outputs(refs, depths, names, order, extranorm)
+    assert gzip.open(str(out / "tt-indexcov.bed.gz"), "rt").read().splitlines() == rows
     assert open(str(out / "tt-indexcov.roc")).read() == roc_txt
-    ped = [ln.split("\t") for ln in open(str(out / "tt-indexcov.ped")).read().splitlines()]
-    assert ped[0][:8] == ["#family_id", "sample_id", "paternal_id", "maternal_id", "sex", "phenotype", "CNX", "CNY"]
-    assert len({len(r) for r in ped}) == 1                        # num_colcounts == 1 (functional-tests.sh:26-30,50)
-    col = ped[0].index("bins.out")
-    for k in range(S):
-        assert [int(x) for x in ped[k + 1][col:col + 4]] == bins[k].tolist()
-        assert ped[k + 1][ped[0].index("CNX")] == "%.2f" % orc.ic_getcn(depths[k][3])
-        assert ped[k + 1][4] == str(int(0.5 + orc.ic_getcn(depths[k][3])))
-        assert ped[k + 1][-2:] == [str(1000 * (k + 1) * len(refs)), str((10 + k) * len(refs))]
+    check_ped_columns(read_ped(out), refs, depths, bins)
 
 
 @pytest.mark.gpu
@@ -498,7 +429,7 @@ def test_indexcov_cohort(tmp_path, extranorm, form):
 def test_indexcov_cohort_sample_sharded(tmp_path, gpus, extranorm):
     """SURVEY 8(e): samples shard across the GPUs through I5, the rows gather on the host.  `--gpus N` must give the bytes of
     `--gpus 1` (GL_OVERSUBSCRIBE lets a one-GPU box run N shards: shard g -> device g % n_dev), with -n too."""
-    refs, fai, paths, lin = _cohort_bais(tmp_path)
+    refs, fai, paths, lin = cohort_bais(tmp_path)
     outs = []
     for g in (1, gpus):
         out = tmp_path / ("g%d" % g) / "tt"

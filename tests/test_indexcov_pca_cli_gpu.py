@@ -11,6 +11,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from bamutil import make_bai  # noqa: E402
+from indexcov_cli_oracle import compare_pcs, expected_pcs, oracle_depths, read_ped  # noqa: E402
 from oracle import indexcov_pca as op  # noqa: E402
 from oracle import loader as orc  # noqa: E402
 
@@ -55,64 +56,15 @@ def _cohort(tmp_path, S, seed=1):
     return str(fai), paths, lin
 
 
-def _oracle_depths(lin):
-    out = []
-    for per_ref in lin:
-        voff = np.array([v for r in per_ref for v in r], np.uint64)
-        ptr = np.concatenate([[0], np.cumsum([len(r) for r in per_ref])]).astype(np.int64)
-        sizes, sptr = orc.ic_sizes(voff, ptr)
-        m = orc.ic_median(sizes)
-        d = orc.ic_normalize(sizes, float(m))
-        out.append([d[sptr[r]:sptr[r + 1]] for r in range(len(per_ref))])
-    return out
-
-
-def _expected_pcs(depths, names, extranorm, autosomes):
-    S = len(depths)
-    refs = []
-    for r, name in enumerate(names):
-        if name not in autosomes:
-            continue
-        ds = [depths[k][r] for k in range(S)]
-        if extranorm:
-            longest = max(len(d) for d in ds)
-            mat = np.zeros((S, longest), np.float32)
-            for k in range(S):
-                mat[k, :len(ds[k])] = ds[k]
-            mat = orc.ic_xnorm(mat, np.array([len(d) for d in ds], np.int32))
-            ds = [mat[k, :len(ds[k])] for k in range(S)]
-        refs.append(ds)
-    return op.pca(op.pca8_matrix(refs))
-
-
-def _ped(out):
-    stem = os.path.basename(str(out))
-    return [ln.split("\t") for ln in open(os.path.join(str(out), stem + "-indexcov.ped")).read().splitlines()]
-
-
-def _compare(ped, proj, kk):
-    hdr = ped[0]
-    c0 = hdr.index("p.out") + 1
-    assert hdr[c0:c0 + kk] == ["PC%d" % (j + 1) for j in range(kk)]
-    assert hdr[c0 + kk:] == ["mapped", "unmapped"]
-    for j in range(kk):
-        tol = 1e-7 * max(np.abs(proj[:, j]).max(), 1e-300)
-        nr = op.half_cent_near(proj[:, j], tol)
-        for k in range(len(ped) - 1):
-            if not nr[k]:
-                assert ped[k + 1][c0 + j] == "%.2f" % proj[k, j], (k, j, ped[k + 1][c0 + j], proj[k, j])
-        assert nr.sum() <= 2 * len(nr) * min(1.0, 200 * tol) + 1
-
-
 @pytest.mark.parametrize("extranorm", [False, True])
 def test_ped_pcs_against_oracle(tmp_path, extranorm):
     fai, paths, lin = _cohort(tmp_path, 9)
     out = tmp_path / "pp"
     p = run("indexcov", "-d", str(out), "--fai", fai, *(["-n"] if extranorm else []), *paths)
     assert "principal components" not in p.stderr
-    proj, sv, kk = _expected_pcs(_oracle_depths(lin), [n for n, _ in REFS], extranorm, {"1", "2", "GL000207.1"})
+    proj, sv, kk = expected_pcs(oracle_depths(lin), [n for n, _ in REFS], extranorm, {"1", "2", "GL000207.1"})
     assert kk == 5 and sv[4] > 0
-    _compare(_ped(out), proj, kk)
+    compare_pcs(read_ped(out), proj, kk)
 
 
 @pytest.mark.parametrize("S", [1, 2, 3, 4])
@@ -121,15 +73,15 @@ def test_few_samples(tmp_path, S):
     out = tmp_path / "fs"
     p = run("indexcov", "-d", str(out), "--fai", fai, *paths)
     assert "got: %d principal components" % S in p.stderr
-    ped = _ped(out)
+    ped = read_ped(out)
     if S < 3:
         assert "indexcov: %d principal components, not plotting" % S in p.stderr
         assert not any(h.startswith("PC") for h in ped[0])
         return
     assert "not plotting" not in p.stderr
-    proj, sv, kk = _expected_pcs(_oracle_depths(lin), [n for n, _ in REFS], False, {"1", "2", "GL000207.1"})
+    proj, sv, kk = expected_pcs(oracle_depths(lin), [n for n, _ in REFS], False, {"1", "2", "GL000207.1"})
     assert kk == S and sv[S - 1] == 0                                  # rank S - 1 after centring: the last column is 0.00
-    _compare(ped, proj, kk)
+    compare_pcs(ped, proj, kk)
     c0 = ped[0].index("p.out") + 1
     assert all(r[c0 + S - 1] == "0.00" for r in ped[1:])
 
@@ -140,7 +92,7 @@ def test_no_autosome_kept(tmp_path):
     out = tmp_path / "na"
     p = run("indexcov", "-d", str(out), "--fai", fai, "--excludepatt", "^(1|2|GL.*|NC.*)$", *paths)
     assert "got: 0 principal components" in p.stderr and "indexcov: 0 principal components, not plotting" in p.stderr
-    assert not any(h.startswith("PC") for h in _ped(out)[0])
+    assert not any(h.startswith("PC") for h in read_ped(out)[0])
 
 
 def test_crai_cohort(tmp_path):
@@ -168,8 +120,8 @@ def test_crai_cohort(tmp_path):
         sz = [orc.crai_sizes(*slices[k][r]) for r in range(2)]
         m = orc.ic_median(np.concatenate(sz))
         depths.append([orc.ic_normalize(x, float(m)) for x in sz])
-    proj, sv, kk = _expected_pcs(depths, ["1", "2"], False, {"1", "2"})
-    ped = _ped(out)
+    proj, sv, kk = expected_pcs(depths, ["1", "2"], False, {"1", "2"})
+    ped = read_ped(out)
     hdr = ped[0]
     c0 = hdr.index("p.out") + 1
     assert hdr[c0:] == ["PC%d" % (j + 1) for j in range(kk)]          # CRAM indexes carry no mapped / unmapped counts

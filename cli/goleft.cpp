@@ -23,6 +23,7 @@
 #include <map>
 #include <mutex>
 #include <regex>
+#include <set>
 #include <string>
 #include <thread>
 #include <vector>
@@ -33,6 +34,7 @@
 #include "../goleft_b200/csrc/host/thread_pool.h"
 #include "../goleft_b200/csrc/host/pca8.h"
 #include "goleft_b200.h"
+#include "plot_html.h"
 
 static const char* kVersion = "0.2.6";          // goleft.go:3 (the surface this build mirrors)
 
@@ -887,6 +889,354 @@ static void ic_tokens_counts(gl_ctx* c, const float* d_dep, size_t a, size_t b, 
     glck(c, gl_memcpy_d2h(c, b4_all + a * nq * 4, d_b, (int64_t)nseg * 32), "gl_memcpy_d2h");
 }
 
+// ---- the depth and ROC charts (plot.cu, DESIGN §1.14).  Chart c shows kept reference q_of[c]; dataset (c, k) is sample
+// k's line, drawn with index k + 1, so the last sample lies on top as in the reference (plot.go:142-144 + asPng:480-481).
+struct IcPlots {
+    std::vector<size_t> q_of;
+    std::vector<int64_t> sel;          // gl_plot_select's {first, m, stride} of dataset (c, k) at [(c * S + k) * 3]
+    std::vector<float> yext;           // ... and its y extent at [(c * S + k) * 2]
+    std::vector<double> xf;            // per chart: gl_plot_transform of the extent over every sample
+    std::vector<double> ext;           // per chart: that extent, {xmin, xmax, ymin, ymax}
+};
+
+// The extent of chart c over every drawn dataset (gonum's DataRange over the plotted vertices); mult scales the index.
+static void ic_plot_extent(IcPlots& pl, size_t c, size_t S, double mult) {
+    double e[4] = {INFINITY, -INFINITY, INFINITY, -INFINITY};
+    for (size_t k = 0; k < S; k++) {
+        const int64_t* s3 = &pl.sel[(c * S + k) * 3];
+        if (s3[1] == 0) continue;
+        e[0] = std::min(e[0], (double)s3[0] * mult);
+        e[1] = std::max(e[1], (double)(s3[0] + (s3[1] - 1) * s3[2]) * mult);
+        e[2] = std::min(e[2], (double)pl.yext[(c * S + k) * 2]);
+        e[3] = std::max(e[3], (double)pl.yext[(c * S + k) * 2 + 1]);
+    }
+    if (e[0] > e[1]) e[0] = e[1] = e[2] = e[3] = 0;                       // nothing drawn
+    pl.ext.insert(pl.ext.end(), e, e + 4);
+    double xf[4];
+    if (gl_plot_transform(e, GL_PLOT_W, GL_PLOT_H, xf) != GL_OK) fatal(1, "gl_plot_transform failed");
+    pl.xf.insert(pl.xf.end(), xf, xf + 4);
+}
+
+// The datasets of samples [a, b) on the GPU holding them from cohort tile t0: off / len inside d_dep, in (c, k) order.
+static void ic_plot_slices(const IcPlots& pl, const IcSlices& sl, size_t S, size_t a, size_t b, int64_t t0, std::vector<int64_t>& off,
+                           std::vector<int64_t>& len) {
+    off.clear(); len.clear();
+    for (size_t c = 0; c < pl.q_of.size(); c++)
+        for (size_t k = a; k < b; k++) {
+            off.push_back(sl.off[pl.q_of[c] * S + k] - t0);
+            len.push_back(sl.len[pl.q_of[c] * S + k]);
+        }
+}
+
+// round 1 on one GPU: the selection of its samples' datasets, into pl.sel / pl.yext
+static void ic_plot_select(gl_ctx* c, const float* d_dep, size_t a, size_t b, const std::vector<int64_t>& sample_ptr, const IcSlices& sl,
+                           IcPlots& pl) {
+    const size_t S = sample_ptr.size() - 1, nk = b - a, n = pl.q_of.size() * nk;
+    if (n == 0) return;
+    std::vector<int64_t> off, len, sel(n * 3);
+    std::vector<float> yext(n * 2);
+    ic_plot_slices(pl, sl, S, a, b, sample_ptr[a], off, len);
+    DevBufs tmp(c);
+    int64_t* d_sel = tmp.alloc<int64_t>(n * 3);
+    float* d_y = tmp.alloc<float>(n * 2);
+    glck(c, gl_plot_select_device(c, d_dep, tmp.upload(off.data(), n), tmp.upload(len.data(), n), (int32_t)n, d_sel, d_y), "gl_plot_select_device");
+    glck(c, gl_memcpy_d2h(c, sel.data(), d_sel, (int64_t)n * 24), "gl_memcpy_d2h");
+    glck(c, gl_memcpy_d2h(c, yext.data(), d_y, (int64_t)n * 8), "gl_memcpy_d2h");
+    for (size_t j = 0; j < n; j++) {
+        const size_t g = (j / nk) * S + a + j % nk;
+        std::copy(&sel[j * 3], &sel[j * 3 + 3], &pl.sel[g * 3]);
+        std::copy(&yext[j * 2], &yext[j * 2 + 2], &pl.yext[g * 2]);
+    }
+}
+
+// round 2 on one GPU: the index images of its samples' lines, with the cohort's extents (img: every chart)
+static void ic_plot_raster(gl_ctx* c, const float* d_dep, size_t a, size_t b, const std::vector<int64_t>& sample_ptr, const IcSlices& sl,
+                           const IcPlots& pl, double r, uint32_t* img) {
+    const size_t S = sample_ptr.size() - 1, nk = b - a, nc = pl.q_of.size(), n = nc * nk;
+    std::vector<int64_t> off, len, sel(n * 3);
+    std::vector<int32_t> chart(n);
+    std::vector<uint32_t> draw(n);
+    ic_plot_slices(pl, sl, S, a, b, sample_ptr[a], off, len);
+    for (size_t j = 0; j < n; j++) {
+        const size_t k = a + j % nk, ch = j / nk;
+        std::copy(&pl.sel[(ch * S + k) * 3], &pl.sel[(ch * S + k) * 3 + 3], &sel[j * 3]);
+        chart[j] = (int32_t)ch; draw[j] = (uint32_t)(k + 1);
+    }
+    DevBufs tmp(c);
+    uint32_t* d_img = tmp.alloc<uint32_t>(nc * GL_PLOT_W * GL_PLOT_H);
+    glck(c, gl_plot_raster_series_device(c, d_dep, tmp.upload(off.data(), n), tmp.upload(sel.data(), n * 3), (double)GL_TILE_WIDTH,
+                                         tmp.upload(chart.data(), n), tmp.upload(draw.data(), n), (int32_t)n, tmp.upload(pl.xf.data(), nc * 4),
+                                         (int32_t)nc, GL_PLOT_W, GL_PLOT_H, r, d_img), "gl_plot_raster_series_device");
+    glck(c, gl_memcpy_d2h(c, img, d_img, (int64_t)(nc * GL_PLOT_W * GL_PLOT_H * 4)), "gl_memcpy_d2h");
+}
+
+static void ic_write_png(const std::string& path, const uint32_t* img, const std::vector<uint8_t>& palette, int kind, const double* ext,
+                         const std::string& xtitle, const std::string& ytitle) {
+    std::vector<uint8_t> rgb((size_t)GL_PLOT_CW * GL_PLOT_CH * 3);
+    if (gl_plot_compose(img, palette.data(), (int32_t)(palette.size() / 3), kind, ext, xtitle.c_str(), ytitle.c_str(), rgb.data()) != GL_OK)
+        fatal(1, "gl_plot_compose: %s", gl_last_error(nullptr));
+    int64_t n = 0;
+    gl_plot_png(rgb.data(), GL_PLOT_CW, GL_PLOT_CH, nullptr, 0, &n);
+    std::vector<uint8_t> png((size_t)n);
+    if (gl_plot_png(rgb.data(), GL_PLOT_CW, GL_PLOT_CH, png.data(), n, &n) != GL_OK) fatal(1, "gl_plot_png: %s", gl_last_error(nullptr));
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f || fwrite(png.data(), 1, (size_t)n, f) != (size_t)n || fclose(f) != 0) fatal(1, "cannot write %s", path.c_str());
+}
+
+// The ROC charts (their lines rasterised on GPU 0 from host vertex arrays), every chart's PNG on the host pool, and
+// index.html.  INDEXCOV_N_BACKGROUNDS=n greys the first n samples in every chart (plot.go:87-101).
+// what the pages show besides the depth and ROC lines
+struct IcReport {
+    const std::vector<std::string>& names;
+    const float* dep;                                        // the cohort depths (after -n) at the slices of sl
+    const IcSlices& sl;
+    const std::map<std::string, std::vector<double>>& sexes;
+    const std::vector<uint64_t>& mapped, & unmapped;
+    const std::vector<int64_t>& bins;                        // per sample: out, lo, hi, in
+    const std::vector<double>& pcs;                          // S x 5
+    int32_t n_pc;
+    const double* vars;                                      // n_pc variance-explained fractions
+};
+
+// tooltip titles: names[dataset][point]
+static std::string ic_tooltip(const std::vector<std::vector<std::string>>& names) {
+    std::string js = "  var names = [";
+    for (size_t d = 0; d < names.size(); d++) {
+        js += d ? ",[" : "[";
+        for (size_t i = 0; i < names[d].size(); i++) js += (i ? "," : "") + glhtml::quote(names[d][i]);
+        js += "]";
+    }
+    return js + "];\n  chart.options.tooltips.callbacks.title = function(tts, data) {\n    var out = [];\n"
+                "    tts.forEach(function(ti) { out.push(names[ti.datasetIndex][ti.index]); });\n    return out.join(\",\");\n  };";
+}
+
+// asValues (plot.go:66-83) of n values at v, every vertex: x = i * mult, y = min(v, 2.5)
+static void ic_as_values(const float* v, size_t n, double mult, glhtml::Dataset& ds) {
+    size_t i = 0;
+    while (i < n && v[i] == 0.f) i++;
+    for (; i < n; i++) { ds.x.push_back((double)i * mult); ds.y.push_back((double)(v[i] > 2.5f ? 2.5f : v[i])); }
+}
+
+static void ic_write_text(const std::string& path, const std::string& text) {
+    FILE* f = fopen(path.c_str(), "w");
+    if (!f || fwrite(text.data(), 1, text.size(), f) != text.size() || fclose(f) != 0) fatal(1, "cannot write %s", path.c_str());
+}
+
+static void ic_plots_write(gl_ctx* ctx, const std::string& base, const std::string& dir, const std::vector<const IcRef*>& kept,
+                           const IcPlots& pl, const std::vector<std::vector<float>>& roc_vals, const std::vector<uint32_t>& depth_img,
+                           double r, size_t S, const IcReport& rep) {
+    const size_t kMaxSamples = 100;                                         // indexcov.go:528 maxSamples
+    if (S > kMaxSamples)
+        fprintf(stderr, "indexcov: creating only static (no interactive) plots for depth because # of samples %zu is > %zu\n", S, kMaxSamples);
+    int32_t n_bg = 0;
+    if (const char* v = getenv("INDEXCOV_N_BACKGROUNDS")) {
+        char* end = nullptr;
+        const long n = strtol(v, &end, 10);
+        if (*v && end && !*end) {
+            n_bg = (int32_t)std::max(-1L, std::min(n, (long)INT32_MAX));
+            fprintf(stderr, "[indexcov] setting first %d samples as background\n", n_bg);
+        }
+    }
+    std::vector<uint8_t> palette(3 * (S + 1), 255);                         // palette[v] for draw index v; 0 stays white
+    for (size_t k = 0; k < S; k++) gl_plot_color((int32_t)k, n_bg, &palette[3 * (k + 1)]);
+    const size_t nc = pl.q_of.size(), img_n = (size_t)GL_PLOT_W * GL_PLOT_H;
+    const double roc_mult = (1.0 / (double)GL_INDEXCOV_SLOTS) / (2.0 / 3.0);   // plot.go:336, x = i * (1/70) / (2/3)
+    IcPlots rp;
+    rp.q_of = pl.q_of;
+    rp.sel.resize(nc * S * 3); rp.yext.resize(nc * S * 2);
+    std::vector<double> x, y;
+    std::vector<int64_t> ptr(1, 0);
+    std::vector<int32_t> chart;
+    std::vector<uint32_t> draw;
+    std::vector<int64_t> off(S), len(S, GL_INDEXCOV_SLOTS);
+    for (size_t k = 0; k < S; k++) off[k] = (int64_t)k * GL_INDEXCOV_SLOTS;
+    for (size_t c = 0; c < nc; c++) {
+        const float* v = roc_vals[c].data();
+        if (roc_vals[c].size() != S * GL_INDEXCOV_SLOTS) fatal(1, "indexcov: no ROC values for chart %zu", c);
+        gl_plot_select_host(v, off.data(), len.data(), (int32_t)S, &rp.sel[c * S * 3], &rp.yext[c * S * 2]);
+        ic_plot_extent(rp, c, S, roc_mult);
+        for (size_t k = 0; k < S; k++) {
+            const int64_t* s3 = &rp.sel[(c * S + k) * 3];
+            if (s3[1] < 2) continue;
+            for (int64_t j = 0; j < s3[1]; j++) {
+                const int64_t i = s3[0] + j * s3[2];
+                const float f = v[k * GL_INDEXCOV_SLOTS + (size_t)i];
+                x.push_back((double)i * roc_mult);
+                y.push_back((double)(f > 2.5f ? 2.5f : f));
+            }
+            ptr.push_back((int64_t)x.size()); chart.push_back((int32_t)c); draw.push_back((uint32_t)(k + 1));
+        }
+    }
+    std::vector<uint32_t> roc_img(nc * img_n);
+    if (nc) glck(ctx, gl_plot_raster_xy(ctx, x.data(), y.data(), ptr.data(), chart.data(), draw.data(), (int32_t)chart.size(), rp.xf.data(),
+                                        (int32_t)nc, GL_PLOT_W, GL_PLOT_H, r, roc_img.data()), "gl_plot_raster_xy");
+    const std::string stem = base.substr(base.find_last_of('/') + 1);
+    const std::string back = "<p><a href=\"index.html\">back to index</a></p>\n";
+    glhost::ThreadPool::global().run((int64_t)(4 * nc), [&](int64_t t, int) {
+        const size_t c = (size_t)t / 4;
+        const std::string& chrom = kept[pl.q_of[c]]->name;
+        if (t % 4 == 2) {                                                   // plotDepths' page (plot.go:110-164), S <= 100 only
+            if (S > kMaxSamples) return;
+            glhtml::Chart ch;
+            ch.name = "depth"; ch.xlabel = "position on " + chrom; ch.ylabel = "scaled coverage";
+            const double w = S > 50 ? 0.2 : (S > 30 ? 0.3 : 0.4);
+            for (size_t kk = S; kk-- > 0;) {                                // the reference adds the datasets last sample first
+                glhtml::Dataset ds;
+                ds.label = rep.names[kk]; ds.xfmt = "%.0f"; ds.width = w;
+                gl_plot_color((int32_t)kk, n_bg, ds.rgb);
+                const size_t j = pl.q_of[c] * S + kk;
+                ic_as_values(rep.dep + rep.sl.off[j], (size_t)rep.sl.len[j], (double)GL_TILE_WIDTH, ds);
+                ch.data.push_back(std::move(ds));
+            }
+            ic_write_text(base + "-depth-" + chrom + ".html", glhtml::page("indexcov depth " + chrom, back + glhtml::chart_html(ch, 850, 550)));
+            return;
+        }
+        if (t % 4 == 3) {                                                   // plotROCs' page (plot.go:318-353)
+            glhtml::Chart ch;
+            ch.name = "roc"; ch.xlabel = "scaled coverage for " + chrom; ch.ylabel = "proportion of regions covered";
+            for (size_t kk = S; kk-- > 0;) {
+                glhtml::Dataset ds;
+                ds.label = (int64_t)kk < n_bg ? "background" : rep.names[kk]; ds.width = 2;
+                gl_plot_color((int32_t)kk, n_bg, ds.rgb);
+                ic_as_values(&roc_vals[c][kk * GL_INDEXCOV_SLOTS], GL_INDEXCOV_SLOTS, roc_mult, ds);
+                ch.data.push_back(std::move(ds));
+            }
+            ic_write_text(base + "-roc-" + chrom + ".html", glhtml::page("indexcov roc " + chrom, back + glhtml::chart_html(ch, 850, 550)));
+            return;
+        }
+        if (t % 4 == 0)
+            ic_write_png(base + "-depth-" + chrom + ".png", &depth_img[c * img_n], palette, GL_PLOT_DEPTH, &pl.ext[c * 4], "position on " + chrom,
+                         "scaled coverage");
+        else
+            ic_write_png(base + "-roc-" + chrom + ".png", &roc_img[c * img_n], palette, GL_PLOT_PLAIN, &rp.ext[c * 4],
+                         "scaled coverage for " + chrom, "proportion of regions covered");
+    });
+    // ---- index.html (indexcov.go:896-953): the cohort charts, then every chromosome's images
+    std::string body = "<h3>indexcov: " + std::to_string(S) + " samples</h3>\n<p><a href=\"" + stem + ".ped\">" + stem + ".ped</a> | <a href=\"" +
+                       stem + ".bed.gz\">" + stem + ".bed.gz</a> | <a href=\"" + stem + ".roc\">" + stem + ".roc</a></p>\n";
+    const uint8_t green[3] = {110, 250, 59}, grey[3] = {180, 180, 180};
+    auto scatter = [&](glhtml::Dataset& ds, const uint8_t* rgb, const char* label) {
+        ds.line = false; ds.width = 4; ds.label = label; std::copy(rgb, rgb + 3, ds.rgb);
+    };
+    if (rep.sexes.size() >= 2) {                                            // plotSex (plot.go:412-474) + its PNG (indexcov.go:918-921)
+        auto it = rep.sexes.begin();
+        const std::string k0 = it->first, k1 = std::next(it)->first;
+        const std::vector<double>& cn0 = it->second;
+        const std::vector<double>& cn1 = std::next(it)->second;
+        std::vector<int> inferred(S);
+        std::set<int> cns;
+        for (size_t k = 0; k < S; k++) { inferred[k] = (int)(0.5 + cn0[k]); cns.insert(inferred[k]); }
+        glhtml::Chart ch;
+        ch.name = "sex"; ch.xlabel = k0 + " Copy Number"; ch.ylabel = k1 + " Copy Number"; ch.legend = true;
+        std::vector<std::vector<std::string>> tips;
+        std::vector<double> sx, sy;
+        std::vector<int64_t> sptr(1, 0);
+        std::vector<int32_t> schart;
+        std::vector<uint32_t> sdraw;
+        std::vector<uint8_t> spal(3, 255);
+        double e[4] = {INFINITY, -INFINITY, INFINITY, -INFINITY};
+        for (int cn : cns) {                                                 // ascending inferred CN
+            glhtml::Dataset ds;
+            scatter(ds, green, "");
+            ds.label = "Inferred CN for " + k0 + ": " + std::to_string(cn); ds.width = 6;
+            gl_plot_color(cn, 0, ds.rgb);
+            tips.emplace_back();
+            for (size_t k = (size_t)std::max<int32_t>(n_bg, 0); k < S; k++) {
+                if (inferred[k] != cn) continue;
+                ds.x.push_back(cn0[k]); ds.y.push_back(cn1[k]); tips.back().push_back(rep.names[k]);
+                e[0] = std::min(e[0], cn0[k]); e[1] = std::max(e[1], cn0[k]); e[2] = std::min(e[2], cn1[k]); e[3] = std::max(e[3], cn1[k]);
+            }
+            sx.insert(sx.end(), ds.x.begin(), ds.x.end()); sy.insert(sy.end(), ds.y.begin(), ds.y.end());
+            sptr.push_back((int64_t)sx.size()); schart.push_back(0); sdraw.push_back((uint32_t)(sdraw.size() + 1));
+            spal.insert(spal.end(), ds.rgb, ds.rgb + 3);
+            ch.data.push_back(std::move(ds));
+        }
+        ch.tooltip_js = "  chart.options.hover.mode = 'index';\n" + ic_tooltip(tips);
+        body += "<h4>sex</h4>\n" + glhtml::chart_html(ch, 550, 550);
+        if (!(e[0] <= e[1])) e[0] = e[1] = e[2] = e[3] = 0;
+        // asPng draws the scatter as lines joining each dataset's points in sample order
+        double xf[4];
+        std::vector<uint32_t> simg((size_t)GL_PLOT_SQ_W * GL_PLOT_SQ_H);
+        if (gl_plot_transform(e, GL_PLOT_SQ_W, GL_PLOT_SQ_H, xf) != GL_OK) fatal(1, "gl_plot_transform failed");
+        glck(ctx, gl_plot_raster_xy(ctx, sx.data(), sy.data(), sptr.data(), schart.data(), sdraw.data(), (int32_t)schart.size(), xf, 1,
+                                    GL_PLOT_SQ_W, GL_PLOT_SQ_H, gl_plot_line_radius((int32_t)schart.size()), simg.data()), "gl_plot_raster_xy");
+        std::vector<uint8_t> rgb((size_t)GL_PLOT_SQ_CW * GL_PLOT_SQ_CH * 3);
+        if (gl_plot_compose(simg.data(), spal.data(), (int32_t)(spal.size() / 3), GL_PLOT_SQUARE, e, (k0 + " Copy Number").c_str(),
+                            (k1 + " Copy Number").c_str(), rgb.data()) != GL_OK)
+            fatal(1, "gl_plot_compose: %s", gl_last_error(nullptr));
+        int64_t n = 0;
+        gl_plot_png(rgb.data(), GL_PLOT_SQ_CW, GL_PLOT_SQ_CH, nullptr, 0, &n);
+        std::vector<uint8_t> png((size_t)n);
+        if (gl_plot_png(rgb.data(), GL_PLOT_SQ_CW, GL_PLOT_SQ_CH, png.data(), n, &n) != GL_OK) fatal(1, "gl_plot_png failed");
+        ic_write_text(base + "-sex.png", std::string(png.begin(), png.begin() + n));
+        body += "<p><img src=\"" + stem + "-sex.png\" alt=\"sex\"></p>\n";
+    }
+    std::vector<std::string> fg_names;
+    for (size_t k = (size_t)std::max<int32_t>(n_bg, 0); k < S; k++) fg_names.push_back(rep.names[k]);
+    bool anygt = false;
+    for (size_t k = 0; k < S; k++) if (rep.mapped[k] || rep.unmapped[k]) anygt = true;
+    if (anygt) {                                                            // plotMapped (plot.go:355-410)
+        glhtml::Chart ch;
+        ch.name = "mapped"; ch.xlabel = "log(mapped reads)"; ch.ylabel = "log(unmapped reads)";
+        glhtml::Dataset ds;
+        scatter(ds, green, "samples");
+        for (size_t k = (size_t)std::max<int32_t>(n_bg, 0); k < S; k++) {
+            ds.x.push_back(log1p((double)rep.mapped[k])); ds.y.push_back(log1p((double)rep.unmapped[k]));
+        }
+        ch.data.push_back(std::move(ds));
+        ch.tooltip_js = "  chart.options.hover.mode = 'index';\n" + ic_tooltip({fg_names});
+        body += "<h4>mapped and unmapped reads</h4>\n" + glhtml::chart_html(ch, 550, 550);
+    }
+    std::vector<std::string> bg_names((size_t)std::min<int64_t>(std::max<int32_t>(n_bg, 0), (int64_t)S), "background");
+    auto two_sets = [&](glhtml::Chart& ch, const std::function<void(size_t, double&, double&)>& xy, const char* xf, const char* yf) {
+        glhtml::Dataset bg, fg;
+        scatter(bg, grey, "samples"); scatter(fg, green, "samples");
+        bg.xfmt = fg.xfmt = xf; bg.yfmt = fg.yfmt = yf;
+        for (size_t k = 0; k < S; k++) {
+            double x, y;
+            xy(k, x, y);
+            glhtml::Dataset& d = (int64_t)k < n_bg ? bg : fg;
+            d.x.push_back(x); d.y.push_back(y);
+        }
+        std::vector<std::vector<std::string>> tips;
+        if (n_bg > 0) { ch.data.push_back(std::move(bg)); tips.push_back(bg_names); }
+        ch.data.push_back(std::move(fg)); tips.push_back(fg_names);
+        ch.tooltip_js = ic_tooltip(tips);
+    };
+    {                                                                       // plotBins (plot.go:166-249)
+        glhtml::Chart ch;
+        ch.name = "bins"; ch.xlabel = "proportion of bins with depth < 0.15"; ch.ylabel = "proportion of bins with depth outside of (0.85, 1.15)";
+        two_sets(ch, [&](size_t k, double& x, double& y) {
+            const double tot = (double)(rep.bins[k * 4 + 3] + rep.bins[k * 4 + 0]);
+            x = (double)rep.bins[k * 4 + 1] / std::max(tot, 1.0);
+            y = (double)rep.bins[k * 4 + 0] / tot;
+        }, "%.5f", "%.3f");
+        body += "<h4>bins</h4>\n" + glhtml::chart_html(ch, 550, 550);
+    }
+    if (rep.n_pc >= 3)                                                      // plotPCA (plot.go:251-316)
+        for (int pc : {2, 3}) {
+            glhtml::Chart ch;
+            ch.name = "pca" + std::to_string(pc);
+            char lx[96], ly[96];
+            snprintf(lx, sizeof lx, "PC1 (variance explained: %.2f%%)", 100 * rep.vars[0]);
+            snprintf(ly, sizeof ly, "PC%d (variance explained: %.2f%%)", pc, 100 * rep.vars[pc - 1]);
+            ch.xlabel = lx; ch.ylabel = ly;
+            two_sets(ch, [&](size_t k, double& x, double& y) { x = rep.pcs[k * 5]; y = rep.pcs[k * 5 + (size_t)pc - 1]; }, "%.2f", "%.2f");
+            ch.tooltip_js = "  chart.options.hover.mode = 'index';\n" + ch.tooltip_js;
+            body += "<h4>PCA: PC1 vs PC" + std::to_string(pc) + "</h4>\n" + glhtml::chart_html(ch, 550, 550);
+        }
+    for (size_t c = 0; c < nc; c++) {
+        const std::string& chrom = kept[pl.q_of[c]]->name;
+        const std::string dimg = "<img src=\"" + stem + "-depth-" + chrom + ".png\" alt=\"depth " + chrom + "\">";
+        body += "<div><h4>" + chrom + "</h4><a href=\"" + stem + "-roc-" + chrom + ".html\"><img src=\"" + stem + "-roc-" + chrom +
+                ".png\" alt=\"roc " + chrom + "\"></a> " +
+                (S <= kMaxSamples ? "<a href=\"" + stem + "-depth-" + chrom + ".html\">" + dimg + "</a>" : dimg) + "</div>\n";
+    }
+    const std::string index_path = dir + "/index.html";
+    ic_write_text(index_path, glhtml::page("indexcov", body));
+    fprintf(stderr, "indexcov finished: see %s for overview of output\n", index_path.c_str());   // indexcov.go:454
+}
+
 // .ped (indexcov.go:815-894)
 static void ic_write_ped(const std::string& base, const std::vector<std::string>& names, const std::map<std::string, std::vector<double>>& sexes,
                          const std::vector<int64_t>& bins, const std::vector<float>& slopes, const std::vector<double>& pcs, int32_t n_pc,
@@ -924,6 +1274,8 @@ static int cmd_indexcov(int argc, char** argv) {
     ap.add("directory", 'd', &dir, true); ap.addb("includegl", 'e', &includegl); ap.add("excludepatt", 0, &exclude);
     ap.add("sex", 'X', &sex); ap.add("chrom", 'c', &chrom); ap.add("fai", 'f', &fai); ap.addb("extranormalize", 'n', &extranorm);
     ap.add("gpus", 0, &gpus);                       // extension: GPUs to use (0 = every visible one); samples are sharded over them
+    bool noplots = false;
+    ap.addb("noplots", 0, &noplots);                // extension: no charts; index.html only lists the outputs
     ap.parse(argc, argv);
     std::vector<std::string> bams = ap.positional;
     if (bams.empty()) ap.fail("bam is required");
@@ -1139,10 +1491,36 @@ static int cmd_indexcov(int argc, char** argv) {
         ic_mark("-n (GPU 0, + H2D)");
     }
     // ---- phase B: the values no longer change, so every token and count comes from two launches per GPU
+    // the charts (indexcov.go:707-726): every kept reference with more than 2 tiles, GL* ones only with -e
+    IcPlots pl;
+    if (!noplots)
+        for (size_t q = 0; q < nq; q++)
+            if ((includegl || kept[q]->name.compare(0, 2, "GL") != 0) && sl.longest[q] > 2) pl.q_of.push_back(q);
+    const size_t n_charts = pl.q_of.size();
+    pl.sel.assign(n_charts * S * 3, 0); pl.yext.assign(n_charts * S * 2, 0);
     run_on_gpus([&](int g) {
         const size_t a = cut[(size_t)g], b = cut[(size_t)g + 1];
-        if (b > a) ic_tokens_counts(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, tok_all.data(), counts_all.data(), b4_all.data());
+        if (b == a) return;
+        ic_tokens_counts(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, tok_all.data(), counts_all.data(), b4_all.data());
+        ic_plot_select(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, pl);
     });
+    // depth charts: the extents over every sample, then each GPU draws its samples' lines and the images combine by max
+    const size_t img_n = (size_t)GL_PLOT_W * GL_PLOT_H;
+    const double plot_r = gl_plot_line_radius((int32_t)S);
+    std::vector<uint32_t> depth_img;
+    if (n_charts) {
+        for (size_t c = 0; c < n_charts; c++) ic_plot_extent(pl, c, S, (double)GL_TILE_WIDTH);
+        std::vector<std::vector<uint32_t>> part((size_t)G);
+        run_on_gpus([&](int g) {
+            const size_t a = cut[(size_t)g], b = cut[(size_t)g + 1];
+            if (b == a) return;
+            part[(size_t)g].resize(n_charts * img_n);
+            ic_plot_raster(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, pl, plot_r, part[(size_t)g].data());
+        });
+        depth_img.assign(n_charts * img_n, 0);
+        for (auto& p : part)
+            for (size_t i = 0; i < p.size(); i++) depth_img[i] = std::max(depth_img[i], p[i]);
+    }
     shard.clear();                                                          // frees the resident depths
     for (int g = 1; g < G; g++) gl_ctx_destroy(ctxs[(size_t)g]);
     ic_mark("tokens + counts (GPU, + D2H)");
@@ -1153,6 +1531,7 @@ static int cmd_indexcov(int argc, char** argv) {
     int n_slopes = 0;
     // the PCA's byte matrix (indexcov.go:686-705): every kept reference that is not a sex chromosome gives each sample
     // longest + 1 columns, its clipped values' bytes and then zeros (the range loop leaves i at the last index, or -1)
+    std::vector<std::vector<float>> roc_vals(n_charts);                     // the ROC values (S x 70) of each chart's reference
     std::vector<int64_t> pca_col(nq, -1);
     int64_t pca_D = 0;
     for (size_t q = 0; q < nq; q++)
@@ -1218,6 +1597,7 @@ static int cmd_indexcov(int argc, char** argv) {
                 const float mx = (float)tot[0];
                 for (int i = 0; i < GL_INDEXCOV_SLOTS; i++) rocs[k * GL_INDEXCOV_SLOTS + i] = (float)tot[i] / mx;
             }
+            for (size_t c = 0; c < n_charts; c++) if (pl.q_of[c] == q) roc_vals[c] = rocs;
             for (int i = 0; i < GL_INDEXCOV_SLOTS; i++) {
                 fprintf(roc, "%s\t%.2f", ref.name.c_str(), (double)i / (70.0 * (2.0 / 3.0)));
                 for (size_t k = 0; k < S; k++) fprintf(roc, "\t%s", go_float("%.2f", (double)rocs[k * GL_INDEXCOV_SLOTS + i]).c_str());
@@ -1248,18 +1628,24 @@ static int cmd_indexcov(int argc, char** argv) {
     if (sexes.empty()) fprintf(stderr, "sex chromosomes not found.\n");
     int32_t n_pc = 0;
     std::vector<double> pcs;
+    double sv[5] = {0, 0, 0, 0, 0}, vars[5] = {0, 0, 0, 0, 0};
     if (pca_rank < 5) fprintf(stderr, "got: %lld principal components\n", (long long)pca_rank);
     if (pca_rank < 3) {
         fprintf(stderr, "indexcov: %lld principal components, not plotting\n", (long long)pca_rank);
     } else {
         pcs.resize(S * 5);
-        double sv[5];
         glck(ctx, gl_indexcov_pca(ctx, pca_x.data(), pca_ld, (int32_t)S, pca_D, 5, pcs.data(), sv, &n_pc, nullptr), "gl_indexcov_pca");
+        double total = 0;                                                   // the PCA labels' vars: s_k^2 / ||X_c||_F^2
+        if (!noplots && gl_indexcov_pca_total(pca_x.data(), pca_ld, (int32_t)S, pca_D, &total) != GL_OK) fatal(1, "gl_indexcov_pca_total failed");
+        for (int j = 0; j < n_pc; j++) vars[j] = total > 0 ? sv[j] * sv[j] / total : 0;
     }
     ic_mark("pca");
     ic_write_ped(base, names, sexes, bins, slopes, pcs, n_pc, mapped, unmapped);
-    // The reference's HTML/PNG plots are out of scope (SURVEY.md section 2): index.html is a plain list of the outputs.
-    {
+    if (!noplots) {
+        ic_plots_write(ctx, base, dir, kept, pl, roc_vals, depth_img, plot_r, S,
+                       IcReport{names, dep.data(), sl, sexes, mapped, unmapped, bins, pcs, n_pc, vars});
+        ic_mark("charts");
+    } else {                                                                // --noplots: a plain list of the outputs
         const std::string index_path = dir + "/index.html";
         FILE* ih = fopen(index_path.c_str(), "w");
         if (ih) {

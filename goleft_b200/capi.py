@@ -107,6 +107,23 @@ _proto("gl_indexcov_counts_batch", C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, 
 _proto("gl_indexcov_counts_batch_device", C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, _vp)
 _proto("gl_indexcov_counts_segs_device", C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, _vp)
 _proto("gl_indexcov_xnorm", C.c_int, _vp, _vp, _vp, C.c_int32, C.c_int32)
+_proto("gl_indexcov_pca_total", C.c_int, _vp, C.c_int64, C.c_int32, C.c_int64, _f64p)
+_proto("gl_plot_select_device", C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, _vp)
+_proto("gl_plot_select_host", C.c_int, _vp, _vp, _vp, C.c_int32, _vp, _vp)
+_proto("gl_plot_transform", C.c_int, _vp, C.c_int32, C.c_int32, _vp)
+_proto("gl_plot_line_radius", C.c_double, C.c_int32)
+_proto("gl_plot_raster_series_device", C.c_int, _vp, _vp, _vp, _vp, C.c_double, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32,
+       C.c_int32, C.c_double, _vp)
+_proto("gl_plot_raster_series_host", C.c_int, _vp, _vp, _vp, C.c_double, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32,
+       C.c_double, _vp)
+_proto("gl_plot_raster_xy", C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, _vp)
+_proto("gl_plot_raster_xy_host", C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, _vp)
+_proto("gl_plot_color", None, C.c_int32, C.c_int32, _vp)
+_proto("gl_plot_ticks", C.c_int, C.c_double, C.c_double, _vp, C.c_int32, _i32p)
+_proto("gl_plot_millions", C.c_int, C.c_double, C.c_char_p, C.c_int32)
+_proto("gl_plot_text", C.c_int, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_char_p, C.c_int32)
+_proto("gl_plot_compose", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, C.c_char_p, C.c_char_p, _vp)
+_proto("gl_plot_png", C.c_int, _vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p)
 _proto("gl_format_g3", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_g3_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_bincount_i32", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp)
@@ -431,6 +448,96 @@ def pca_tridiag_above(d, e, rel: float = 1e-12) -> np.ndarray:
     if lib.gl_pca_tridiag_above(_ptr(d), _ptr(e), d.size, rel, _ptr(w), C.byref(k)) != GL_OK:
         raise GlError(GL_EINVAL, "gl_pca_tridiag_above: bad arguments")
     return w[:k.value].copy()
+
+
+# ---- indexcov charts (plot.cu)
+PLOT_CW, PLOT_CH, PLOT_AX, PLOT_AY, PLOT_W, PLOT_H = 384, 288, 56, 8, 316, 244
+PLOT_DEPTH, PLOT_PLAIN = 0, 1
+
+
+def _ck0(rc: int):
+    if rc != GL_OK:
+        raise GlError(rc, lib.gl_last_error(None).decode())
+
+
+def plot_select_host(vals, off, lens):
+    """(sel (n,3) int64 {first, m, stride}, yext (n,2) float32) of every dataset vals[off[d]:off[d]+lens[d]]"""
+    vals, off, lens = _as(vals, np.float32), _as(off, np.int64), _as(lens, np.int64)
+    n = off.size
+    sel, yext = np.empty((n, 3), np.int64), np.empty((n, 2), np.float32)
+    _ck0(lib.gl_plot_select_host(_ptr(vals), _ptr(off), _ptr(lens), n, _ptr(sel), _ptr(yext)))
+    return sel, yext
+
+
+def plot_transform(ext4, W: int, H: int) -> np.ndarray:
+    e, xf = _as(ext4, np.float64), np.empty(4, np.float64)
+    _ck0(lib.gl_plot_transform(_ptr(e), W, H, _ptr(xf)))
+    return xf
+
+
+def plot_line_radius(n_datasets: int) -> float:
+    return lib.gl_plot_line_radius(n_datasets)
+
+
+def plot_raster_series_host(vals, off, sel, mult: float, chart, draw, xf, n_charts: int, W: int, H: int, r: float) -> np.ndarray:
+    vals, off, sel = _as(vals, np.float32), _as(off, np.int64), _as(sel, np.int64)
+    chart, draw, xf = _as(chart, np.int32), _as(draw, np.uint32), _as(xf, np.float64)
+    img = np.empty((n_charts, H, W), np.uint32)
+    _ck0(lib.gl_plot_raster_series_host(_ptr(vals), _ptr(off), _ptr(sel), mult, _ptr(chart), _ptr(draw), chart.size, _ptr(xf), n_charts,
+                                        W, H, r, _ptr(img)))
+    return img
+
+
+def plot_raster_xy_host(x, y, ptr, chart, draw, xf, n_charts: int, W: int, H: int, r: float) -> np.ndarray:
+    x, y, ptr = _as(x, np.float64), _as(y, np.float64), _as(ptr, np.int64)
+    chart, draw, xf = _as(chart, np.int32), _as(draw, np.uint32), _as(xf, np.float64)
+    img = np.empty((n_charts, H, W), np.uint32)
+    _ck0(lib.gl_plot_raster_xy_host(_ptr(x), _ptr(y), _ptr(ptr), _ptr(chart), _ptr(draw), chart.size, _ptr(xf), n_charts, W, H, r,
+                                    _ptr(img)))
+    return img
+
+
+def plot_color(k: int, n_background: int = 0):
+    c = (C.c_uint8 * 3)()
+    lib.gl_plot_color(k, n_background, c)
+    return tuple(c)
+
+
+def plot_ticks(lo: float, hi: float) -> np.ndarray:
+    out, n = np.empty(64, np.float64), C.c_int32()
+    _ck0(lib.gl_plot_ticks(lo, hi, _ptr(out), 64, C.byref(n)))
+    return out[:n.value].copy()
+
+
+def plot_millions(v: float) -> str:
+    b = C.create_string_buffer(64)
+    _ck0(lib.gl_plot_millions(v, b, 64))
+    return b.value.decode()
+
+
+def plot_text(rgb: np.ndarray, x: int, y: int, s: str, vertical: bool = False) -> np.ndarray:
+    """draws s into rgb (H, W, 3) uint8 in place"""
+    assert rgb.dtype == np.uint8 and rgb.flags.c_contiguous and rgb.ndim == 3
+    _ck0(lib.gl_plot_text(_ptr(rgb), rgb.shape[1], rgb.shape[0], x, y, s.encode(), int(vertical)))
+    return rgb
+
+
+def plot_compose(img, palette, kind: int, ext4, xtitle: str, ytitle: str) -> np.ndarray:
+    img, pal, e = _as(img, np.uint32), _as(palette, np.uint8), _as(ext4, np.float64)
+    assert img.size == PLOT_W * PLOT_H
+    rgb = np.empty((PLOT_CH, PLOT_CW, 3), np.uint8)
+    _ck0(lib.gl_plot_compose(_ptr(img), _ptr(pal), pal.size // 3, kind, _ptr(e), xtitle.encode(), ytitle.encode(), _ptr(rgb)))
+    return rgb
+
+
+def plot_png(rgb) -> bytes:
+    rgb = _as(rgb, np.uint8)
+    H, W = rgb.shape[:2]
+    n = C.c_int64()
+    _ck0(lib.gl_plot_png(_ptr(rgb), W, H, None, 0, C.byref(n)))
+    out = np.empty(n.value, np.uint8)
+    _ck0(lib.gl_plot_png(_ptr(rgb), W, H, _ptr(out), out.size, C.byref(n)))
+    return out[:n.value].tobytes()
 
 
 def chunk_rows(rs: int, re: int, W: int, run_start: np.ndarray, run_class: np.ndarray):
@@ -1092,6 +1199,47 @@ class Ctx:
         self._ck(lib.gl_indexcov_counts_segs_device(self.h, d_depth.ptr, d_seg_start.ptr, d_seg_len.ptr,
                                                     d_longest.ptr if d_longest is not None else None, n_seg, d_counts70.ptr,
                                                     d_bins4.ptr))
+
+    def plot_select_device(self, d_vals: DevBuf, d_off: DevBuf, d_len: DevBuf, n: int, d_sel3: DevBuf, d_yext2: DevBuf):
+        self._ck(lib.gl_plot_select_device(self.h, d_vals.ptr, d_off.ptr, d_len.ptr, n, d_sel3.ptr, d_yext2.ptr))
+
+    def plot_raster_series_device(self, d_vals: DevBuf, d_off: DevBuf, d_sel3: DevBuf, mult: float, d_chart: DevBuf, d_draw: DevBuf,
+                                  n: int, d_xf: DevBuf, n_charts: int, W: int, H: int, r: float, d_img: DevBuf):
+        self._ck(lib.gl_plot_raster_series_device(self.h, d_vals.ptr, d_off.ptr, d_sel3.ptr, mult, d_chart.ptr, d_draw.ptr, n, d_xf.ptr,
+                                                  n_charts, W, H, r, d_img.ptr))
+
+    def plot_select(self, vals, off, lens):
+        """gl_plot_select_device on host arrays: (sel (n,3), yext (n,2))"""
+        vals, off, lens = _as(vals, np.float32), _as(off, np.int64), _as(lens, np.int64)
+        n = off.size
+        bufs = [DevBuf(self, max(16, a.nbytes)).upload(a) for a in (vals, off, lens)] + [DevBuf(self, max(16, n * 24)), DevBuf(self, max(16, n * 8))]
+        try:
+            self.plot_select_device(*bufs[:3], n, *bufs[3:])
+            return bufs[3].download(np.int64, n * 3).reshape(n, 3), bufs[4].download(np.float32, n * 2).reshape(n, 2)
+        finally:
+            for b in bufs:
+                b.free()
+
+    def plot_raster_series(self, vals, off, sel, mult: float, chart, draw, xf, n_charts: int, W: int, H: int, r: float) -> np.ndarray:
+        """gl_plot_raster_series_device on host arrays: the (n_charts, H, W) index image"""
+        arrs = [_as(vals, np.float32), _as(off, np.int64), _as(sel, np.int64), _as(chart, np.int32), _as(draw, np.uint32),
+                _as(xf, np.float64)]
+        bufs = [DevBuf(self, max(16, a.nbytes)).upload(a) for a in arrs] + [DevBuf(self, max(16, n_charts * W * H * 4))]
+        try:
+            v, o, sl, ch, dr, x, img = bufs
+            self.plot_raster_series_device(v, o, sl, mult, ch, dr, arrs[3].size, x, n_charts, W, H, r, img)
+            return img.download(np.uint32, n_charts * W * H).reshape(n_charts, H, W)
+        finally:
+            for b in bufs:
+                b.free()
+
+    def plot_raster_xy(self, x, y, ptr, chart, draw, xf, n_charts: int, W: int, H: int, r: float) -> np.ndarray:
+        x, y, ptr = _as(x, np.float64), _as(y, np.float64), _as(ptr, np.int64)
+        chart, draw, xf = _as(chart, np.int32), _as(draw, np.uint32), _as(xf, np.float64)
+        img = np.empty((n_charts, H, W), np.uint32)
+        self._ck(lib.gl_plot_raster_xy(self.h, _ptr(x), _ptr(y), _ptr(ptr), _ptr(chart), _ptr(draw), chart.size, _ptr(xf), n_charts,
+                                       W, H, r, _ptr(img)))
+        return img
 
     def format_g3_device(self, d_vals: DevBuf, n: int, d_tokens: DevBuf):
         self._ck(lib.gl_format_g3_device(self.h, d_vals.ptr, n, d_tokens.ptr))

@@ -200,3 +200,16 @@ extern "C" int gl_pca_tridiag_above(const double* d, const double* e, int32_t n,
     *count = glpca::tridiag_values_above(d, e, n, rel, w);
     return GL_OK;
 }
+
+extern "C" int gl_indexcov_pca_total(const uint8_t* x, int64_t ld, int32_t S, int64_t D, double* total) {
+    if (!total || S < 1 || D < 0 || ld < D || (D > 0 && !x)) return GL_EINVAL;
+    std::vector<int64_t> sum((size_t)D, 0), sq((size_t)D, 0);
+    for (int32_t i = 0; i < S; i++) {
+        const uint8_t* row = x + (size_t)i * (size_t)ld;
+        for (int64_t j = 0; j < D; j++) { sum[(size_t)j] += row[j]; sq[(size_t)j] += (int64_t)row[j] * row[j]; }
+    }
+    __int128 acc = 0;
+    for (int64_t j = 0; j < D; j++) acc += (__int128)S * sq[(size_t)j] - (__int128)sum[(size_t)j] * sum[(size_t)j];
+    *total = (double)acc / (double)S;
+    return GL_OK;
+}

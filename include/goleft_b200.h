@@ -429,7 +429,75 @@ int  gl_indexcov_pca(gl_ctx* ctx, const uint8_t* x, int64_t ld, int32_t S, int64
 int  gl_indexcov_pca_device(gl_ctx* ctx, const uint8_t* d_x, int64_t ld, int32_t S, int64_t D, int32_t k, double* proj, double* sv,
                             int32_t* k_out, int64_t* gram);
 int  gl_indexcov_pca_phases(gl_ctx* ctx, double* t3);
+/* host-only: ||X_c||_F^2, the squared Frobenius norm of the column-centred byte matrix (S rows of D bytes, stride ld), exactly:
+ * sum over columns of (S * sum x^2 - (sum x)^2), in 128-bit integers, divided by S once.  sv[k]^2 / total is gonum's
+ * normalised `vars` (indexcov.go:787-789), the "variance explained" of component k. */
+int  gl_indexcov_pca_total(const uint8_t* x, int64_t ld, int32_t S, int64_t D, double* total);
 int  gl_pca_tridiag_top(const double* d, const double* e, int32_t n, int32_t k, double* w, double* z);
+
+/* ---------------------------------------------------------------- indexcov charts (plot.cu; DESIGN §1.14)
+ * A chart's lines are drawn into an INDEX IMAGE: W x H uint32 over its data area (row 0 at the top), 0 where no line passes,
+ * else the largest draw index whose line covers the pixel (opaque lines: the last one drawn shows).  Images of several
+ * charts are stacked: chart c at img + c*W*H.  A dataset d is one line: chart[d] is its chart, draw[d] (>= 1) its index.
+ * The depth and ROC charts are GL_PLOT_CW x GL_PLOT_CH pixels (4 x 3 in at 96 px/in) with a GL_PLOT_W x GL_PLOT_H data area
+ * whose top-left pixel is (GL_PLOT_AX, GL_PLOT_AY).
+ *   gl_plot_select_device / _host : per dataset (values at off[d], len[d] of them): sel3 = {first, m, stride}: the first
+ *       value != 0 (NaN counts), the number of plotted vertices (0 when none or when one of them is NaN: not drawn) and the
+ *       thinning stride (10 above 2000 values after the skip, 5 above 1000, else 1); yext2 = min, max of min(v, 2.5) over
+ *       them (0, 0 when not drawn).  Vertex j is x = (first + j*stride) * mult, y = min(v[first + j*stride], 2.5).
+ *   gl_plot_transform : ext4 = {xmin, xmax, ymin, ymax} of the plotted vertices (an empty extent widened to +-1) ->
+ *       xf4 = {xmin, W / (xmax - xmin), ymin, H / (ymax - ymin)}: X = (x - xmin) * sx, Y = H - (y - ymin) * sy.
+ *   gl_plot_line_radius : r = max(0.5, w * 96 / 72 / 2) for w = 0.8 pt, or 0.65 pt above 30 datasets.
+ *   gl_plot_raster_series_device / _host : the image of selected value series (xf4: 4 doubles per chart).  A segment AB
+ *       covers pixel (i, j) when the squared float64 distance from (i + 0.5, j + 0.5) to AB is <= r*r (see plot.cu for the
+ *       exact order of operations).  The image is cleared first.
+ *   gl_plot_raster_xy / _host : the same for explicit float64 vertices: dataset d is x[ptr[d] .. ptr[d+1]), y likewise;
+ *       host arrays in, host image out (the device entry rasterises on the GPU).
+ *   gl_plot_color   : host-only: the colour of sample k: grey (180,180,180) below n_background, else a hash of k.
+ *   gl_plot_ticks   : host-only: multiples of the smallest step 1, 2 or 5 x 10^k that gives at most 8 ticks in [lo, hi].
+ *   gl_plot_millions: host-only: an x label of a depth chart (indexcov/plot.go makeMillions).
+ *   gl_plot_text    : host-only: s in the built-in 5x7 font, black, top-left at (x, y); vertical: bottom to top from (x, y).
+ *   gl_plot_compose : host-only: the GL_PLOT_CW x GL_PLOT_CH RGB8 chart: palette[3*v] for pixel value v (palette[0..2] for
+ *       v >= n_pal), white where 0, axes, ticks, tick labels and titles.  kind GL_PLOT_DEPTH: y ticks 0.0..2.0, x labels
+ *       in KB/MB; GL_PLOT_PLAIN: nice ticks on both axes; GL_PLOT_SQUARE: the same on the square canvas (rgb and img then
+ *       have its sizes).  ext4 as gl_plot_transform takes it.
+ *   gl_plot_png     : host-only: the PNG of W x H RGB8 pixels: filter 0 on every row, one IDAT.  out == NULL: *len = the
+ *       room needed. */
+#define GL_PLOT_CW 384
+#define GL_PLOT_CH 288
+#define GL_PLOT_AX 56
+#define GL_PLOT_AY 8
+#define GL_PLOT_W  316
+#define GL_PLOT_H  244
+#define GL_PLOT_DEPTH 0
+#define GL_PLOT_PLAIN 1
+#define GL_PLOT_SQUARE 2   /* the sex chart: GL_PLOT_SQ_CW x GL_PLOT_SQ_CH (6 x 6 in), data area GL_PLOT_SQ_W x GL_PLOT_SQ_H, plain ticks */
+#define GL_PLOT_SQ_CW 576
+#define GL_PLOT_SQ_CH 576
+#define GL_PLOT_SQ_W  508
+#define GL_PLOT_SQ_H  532
+int  gl_plot_select_device(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_len, int32_t n, int64_t* d_sel3,
+                           float* d_yext2);
+int  gl_plot_select_host(const float* vals, const int64_t* off, const int64_t* len, int32_t n, int64_t* sel3, float* yext2);
+int  gl_plot_transform(const double* ext4, int32_t W, int32_t H, double* xf4);
+double gl_plot_line_radius(int32_t n_datasets);
+int  gl_plot_raster_series_device(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_sel3, double mult,
+                                  const int32_t* d_chart, const uint32_t* d_draw, int32_t n, const double* d_xf4, int32_t n_charts,
+                                  int32_t W, int32_t H, double r, uint32_t* d_img);
+int  gl_plot_raster_series_host(const float* vals, const int64_t* off, const int64_t* sel3, double mult, const int32_t* chart,
+                                const uint32_t* draw, int32_t n, const double* xf4, int32_t n_charts, int32_t W, int32_t H, double r,
+                                uint32_t* img);
+int  gl_plot_raster_xy(gl_ctx* ctx, const double* x, const double* y, const int64_t* ptr, const int32_t* chart, const uint32_t* draw,
+                       int32_t n, const double* xf4, int32_t n_charts, int32_t W, int32_t H, double r, uint32_t* img);
+int  gl_plot_raster_xy_host(const double* x, const double* y, const int64_t* ptr, const int32_t* chart, const uint32_t* draw, int32_t n,
+                            const double* xf4, int32_t n_charts, int32_t W, int32_t H, double r, uint32_t* img);
+void gl_plot_color(int32_t k, int32_t n_background, uint8_t* rgb3);
+int  gl_plot_ticks(double lo, double hi, double* out, int32_t cap, int32_t* n);
+int  gl_plot_millions(double v, char* buf, int32_t cap);
+int  gl_plot_text(uint8_t* rgb, int32_t CW, int32_t CH, int32_t x, int32_t y, const char* s, int32_t vertical);
+int  gl_plot_compose(const uint32_t* img, const uint8_t* palette, int32_t n_pal, int32_t kind, const double* ext4, const char* xtitle,
+                     const char* ytitle, uint8_t* rgb);
+int  gl_plot_png(const uint8_t* rgb, int32_t W, int32_t H, uint8_t* out, int64_t cap, int64_t* len);
 
 /* indexsplit (indexsplit/indexsplit.go:92-115): amount of cohort data per 16 KB tile = sum over the S samples, in path
  * order, of float64(size)/1e9 — bit-identical to the reference's sequential adds.  sizes: every sample's tile sizes

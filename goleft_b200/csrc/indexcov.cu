@@ -557,7 +557,7 @@ constexpr int kBinSmem = 8192;
 __global__ void __launch_bounds__(256) bincount_kernel(const int* __restrict__ v, long long n, int lo, int hi,
                                                       unsigned long long* __restrict__ hist) {
     __shared__ unsigned s_h[kBinSmem];
-    const int nb = hi - lo;
+    const long long nb = (long long)hi - lo;                       // up to 2^32 - 1: the width and x - lo need 64 bits
     const bool priv = nb <= kBinSmem;
     if (priv) {
         for (int i = threadIdx.x; i < nb; i += blockDim.x) s_h[i] = 0;
@@ -566,8 +566,9 @@ __global__ void __launch_bounds__(256) bincount_kernel(const int* __restrict__ v
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const int x = v[i];
         if (x >= lo && x < hi) {
-            if (priv) atomicAdd(&s_h[x - lo], 1u);
-            else atomicAdd(&hist[x - lo], 1ull);
+            const long long b = (long long)x - lo;
+            if (priv) atomicAdd(&s_h[b], 1u);
+            else atomicAdd(&hist[b], 1ull);
         }
     }
     if (priv) {
@@ -578,22 +579,32 @@ __global__ void __launch_bounds__(256) bincount_kernel(const int* __restrict__ v
 }
 
 // ------------------------------------------------------------------------------------------------ W1
+// Go's int(0.5 + dep) (depthwed.go:103) as amd64 compiles it (CVTTSD2SQ): truncation toward zero, and NaN, +-Inf and
+// anything outside [-2^63, 2^63) become INT64_MIN.  __double2ll_rz leaves those inputs undefined (the H100 clamps +Inf and
+// 0.5 + dep >= 2^63 to INT64_MAX), so they are sorted out first.  Returned as the two's-complement bits, for wrapping sums.
+__device__ __forceinline__ unsigned long long go_int_half_up(double mean) {
+    const double x = __dadd_rn(0.5, mean);
+    if (!(x >= -9223372036854775808.0 && x < 9223372036854775808.0)) return 0x8000000000000000ull;
+    return (unsigned long long)__double2ll_rz(x);
+}
+
 // means: S x R sample-major.  Group g sums rows [grp[g], grp[g+1]) of int(0.5+mean); out is n_out x S
-// row-major.  A 32x32 tile goes through shared memory so both the reads and the writes are coalesced.
+// row-major.  A 32x32 tile goes through shared memory so both the reads and the writes are coalesced.  The sums wrap
+// modulo 2^64 as Go's int additions do (taken unsigned: signed overflow is undefined in C++).
 __global__ void __launch_bounds__(256) depthwed_kernel(const double* __restrict__ means, int S, long long R,
                                                       const long long* __restrict__ grp, long long n_out, int simple,
                                                       long long* __restrict__ out) {
-    __shared__ long long s_t[32][33];
+    __shared__ unsigned long long s_t[32][33];
     const long long g0 = (long long)blockIdx.x * 32;
     const int s0 = blockIdx.y * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;       // 32 x 8
     for (int k = ty; k < 32; k += 8) {                             // k: sample inside the tile, tx: group
         const int s = s0 + k;
         const long long g = g0 + tx;
-        long long acc = 0;
+        unsigned long long acc = 0;
         if (s < S && g < n_out) {
             const long long a = simple ? g : grp[g], b = simple ? g + 1 : grp[g + 1];
-            for (long long r = a; r < b; r++) acc += (long long)__double2ll_rz(__dadd_rn(0.5, means[(size_t)s * R + r]));
+            for (long long r = a; r < b; r++) acc += go_int_half_up(means[(size_t)s * R + r]);
         }
         s_t[k][tx] = acc;
     }
@@ -601,7 +612,7 @@ __global__ void __launch_bounds__(256) depthwed_kernel(const double* __restrict_
     for (int k = ty; k < 32; k += 8) {                             // k: group inside the tile, tx: sample
         const long long g = g0 + k;
         const int s = s0 + tx;
-        if (s < S && g < n_out) out[(size_t)g * S + s] = s_t[tx][k];
+        if (s < S && g < n_out) out[(size_t)g * S + s] = (long long)s_t[tx][k];
     }
 }
 
@@ -646,11 +657,12 @@ struct WedPeers { int* dst[16]; };
 // A CTA takes 32 rows (groups) x 128 samples.  Phase 1 reads the sample-major input coalesced along the rows (one warp
 // instruction = 32 consecutive rows of one sample) and parks the group sums in shared memory; phase 2 stores them
 // row-major with 16-BYTE stores: a lane owns 4 consecutive samples of one row, a warp instruction covers 512 B of it —
-// NVLink likes wide stores (4-byte stores reached a quarter of the link rate).  Needs row_stride and col_off to be
-// multiples of 4 (callers pad the per-rank width to a multiple of 4); otherwise scalar stores.
+// NVLink likes wide stores (4-byte stores reached a quarter of the link rate).  `vec` (decided on the host) says every
+// destination is 16-byte aligned and row_stride and col_off are multiples of 4 (callers pad the per-rank width to a
+// multiple of 4); otherwise scalar stores.
 __global__ void __launch_bounds__(256) depthwed_i32_p2p_kernel(const int* __restrict__ depth, int S, long long R, const long long* __restrict__ grp,
                                                               long long g_begin, long long g_end, int simple, WedPeers peers, int world,
-                                                              long long row_stride, int col_off, int* __restrict__ overflow) {
+                                                              long long row_stride, int col_off, int vec, int* __restrict__ overflow) {
     __shared__ __align__(16) int s_t[32][132];                     // [row][sample], padded: 132 keeps int4 alignment and spreads banks
     const long long g0 = g_begin + (long long)blockIdx.x * 32;
     const int s0 = blockIdx.y * 128;
@@ -667,7 +679,6 @@ __global__ void __launch_bounds__(256) depthwed_i32_p2p_kernel(const int* __rest
         s_t[tx][k] = (int)acc;
     }
     __syncthreads();
-    const bool vec = ((row_stride | (long long)col_off) & 3) == 0;
     const int rot = (int)((blockIdx.x + blockIdx.y) % (unsigned)world);
     for (int k = ty; k < 32; k += 8) {                             // k: row inside the tile, tx: 4 consecutive samples
         const long long g = g0 + k;
@@ -1209,17 +1220,21 @@ int gl_depthwed_aggregate_i32_device(gl_ctx* ctx, const int32_t* d_depth, int32_
 int gl_depthwed_aggregate_i32_p2p(gl_ctx* ctx, const int32_t* d_depth, int32_t S, int64_t R, const int64_t* d_grp, int64_t g_begin, int64_t g_end,
                                   int32_t* const* d_dst, int32_t world, int64_t row_stride, int32_t col_off, int32_t* d_overflow) {
     GL_CHECK(gl_use(ctx));
-    if (S <= 0 || R < 0 || g_begin < 0 || g_end < g_begin || !d_depth || !d_dst || world < 1 || world > 16 || row_stride < col_off + S || col_off < 0 || !d_overflow)
+    if (S <= 0 || R < 0 || g_begin < 0 || g_end < g_begin || !d_depth || !d_dst || world < 1 || world > 16 || row_stride < (int64_t)col_off + S || col_off < 0 || !d_overflow)
         return gl_fail(ctx, GL_EINVAL, "gl_depthwed_aggregate_i32_p2p: bad argument");
     if (g_end == g_begin) return GL_OK;
     WedPeers peers;
     for (int d = 0; d < 16; d++) peers.dst[d] = d < world ? d_dst[d] : nullptr;
     for (int d = 0; d < world; d++) if (!peers.dst[d]) return gl_fail(ctx, GL_EINVAL, "gl_depthwed_aggregate_i32_p2p: null destination %d", d);
+    // 16-byte stores only where every one of them is aligned: a 4-sample group starts at a multiple of 4 ints from
+    // each destination's base
+    bool vec = ((row_stride | (int64_t)col_off) & 3) == 0;
+    for (int d = 0; d < world; d++) vec = vec && (reinterpret_cast<uintptr_t>(peers.dst[d]) & 15) == 0;
     dim3 grid((unsigned)((g_end - g_begin + 31) / 32), (unsigned)((S + 127) / 128));
     {
         gl_prof_scope prof(ctx, "depthwed_i32_p2p_kernel");
         depthwed_i32_p2p_kernel<<<grid, 256, 0, ctx->stream>>>(d_depth, S, R, reinterpret_cast<const long long*>(d_grp), g_begin, g_end, d_grp ? 0 : 1,
-                                                               peers, world, row_stride, col_off, d_overflow);
+                                                               peers, world, row_stride, col_off, vec ? 1 : 0, d_overflow);
     }
     GL_LAUNCHED(ctx, 1);
     return GL_OK;

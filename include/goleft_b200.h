@@ -666,14 +666,15 @@ int  gl_cnveval_device(gl_ctx* ctx, int32_t S, const int64_t* d_c_ptr, int64_t n
  * V2: histogram of int32 values in [lo,hi) -> hist[v-lo].  `goleft covstats` builds it over the sampled insert sizes,
  * template lengths and read lengths and reads every order statistic of covstats/covstats.go:57-76,175-199 off its running
  * count (k-th smallest = a search, madFilter's cut = a count) and feeds meanStd (:78-89) the values in ascending order
- * with multiplicity — no host sort (cli/goleft.cpp SortedCounts). */
+ * with multiplicity — no host sort (cli/goleft.cpp SortedCounts).  Any lo < hi: up to 2^32 - 1 bins. */
 int  gl_bincount_i32(gl_ctx* ctx, const int32_t* v, int64_t n, int32_t lo, int32_t hi, uint64_t* hist);
 
 /* ---------------------------------------------------------------- depthwed
  * W1: depthwed/depthwed.go:93-157.  means: S samples x R rows (sample-major) of the float64 4th BED
  * column; starts/ends/chrom_id[R] of the rows.  Computes int(0.5+mean) and sums consecutive rows of
  * one chrom until end-start >= size.  out: n_out rows x S (row-major by OUTPUT ROW, like the
- * reference's TSV lines). */
+ * reference's TSV lines).  The conversion is Go's on amd64: NaN, +-Inf and 0.5+mean outside
+ * [-2^63, 2^63) give INT64_MIN, and the sums wrap modulo 2^64. */
 int  gl_depthwed_aggregate(gl_ctx* ctx, const double* means, int32_t S, int64_t R,
                            const int32_t* starts, const int32_t* ends, const int32_t* chrom_id, int64_t size,
                            int32_t* out_start, int32_t* out_end, int32_t* out_chrom, int64_t* out, int64_t out_cap,
@@ -698,7 +699,8 @@ int  gl_depthwed_aggregate_i32_device(gl_ctx* ctx, const int32_t* d_depth, int32
  * n-samples matrix of EVERY GPU of the box (its own + NVLink peer mappings of the others): d_dst[d] = base of rank d's matrix
  * as a pointer valid on this ctx's device (gl_ipc_open between processes; plain peer pointers inside one process), row stride
  * `row_stride` ints, this rank's samples at columns [col_off, col_off + S).  No separate all-gather, no re-assembly.
- * ASYNCHRONOUS on the ctx stream; after gl_sync on every rank and a host barrier the matrix is complete everywhere. */
+ * 16-byte stores when row_stride and col_off are multiples of 4 and every d_dst[d] is 16-byte aligned; 4-byte stores
+ * otherwise (any 4-byte aligned destination is accepted).  ASYNCHRONOUS on the ctx stream; after gl_sync on every rank and a host barrier the matrix is complete everywhere. */
 int  gl_depthwed_aggregate_i32_p2p(gl_ctx* ctx, const int32_t* d_depth, int32_t S, int64_t R, const int64_t* d_grp, int64_t g_begin,
                                    int64_t g_end, int32_t* const* d_dst, int32_t world, int64_t row_stride, int32_t col_off,
                                    int32_t* d_overflow);

@@ -2275,23 +2275,120 @@ void matrix_parse(Matrix& m) {
     for (const std::string& e : errs) if (!e.empty()) fatal(2, "%s", e.c_str());
 }
 
+// The depth chart (dcnv.go:265-321 plotDepths; DESIGN §1.9) of the n x S values depth.bed holds: the reference's Chart.js
+// page dd-depth-<label>.html, one stepped dataset per sample in sample order with every vertex of asValues (x = i * 16384,
+// y = min(v, 2.5) as "%.2f" tokens from the GPU, written in row-block pieces made on the host pool), and dd-depth-<label>.png,
+// the same lines drawn on the GPU (gl_dcnv_chart).  A file that cannot be written is reported on stderr and skipped, as
+// the reference ignores plotDepths' error.
+void dcnv_charts(gl_ctx* ctx, const double* X, size_t R, size_t S, const std::vector<std::string>& samples, const std::string& label) {
+    const std::string png_path = "dd-depth-" + label + ".png", html_path = "dd-depth-" + label + ".html";
+    const std::string xtitle = "position on " + label;
+    std::vector<int64_t> first(S);
+    std::vector<double> yext(2 * S), ext(4);
+    std::vector<uint32_t> img((size_t)GL_PLOT_W * GL_PLOT_H);
+    const char* br = getenv("GL_DCNV_CHART_BLOCK_ROWS");
+    glck(ctx, gl_dcnv_chart(ctx, X, (int64_t)R, (int64_t)S, br ? atoll(br) : 0, GL_PLOT_W, GL_PLOT_H, gl_plot_line_radius((int32_t)S), first.data(),
+                            yext.data(), ext.data(), img.data()), "gl_dcnv_chart");
+    std::vector<uint8_t> palette(3 * (S + 1), 255);                 // draw index S - k is sample k
+    for (size_t k = 0; k < S; k++) gl_plot_color((int32_t)k, 0, &palette[3 * (S - k)]);
+    {
+        std::vector<uint8_t> rgb((size_t)GL_PLOT_CW * GL_PLOT_CH * 3);
+        if (gl_plot_compose(img.data(), palette.data(), (int32_t)(S + 1), GL_PLOT_DEPTH, ext.data(), xtitle.c_str(), "scaled coverage", rgb.data()) != GL_OK)
+            fatal(1, "gl_plot_compose: %s", gl_last_error(nullptr));
+        int64_t n = 0;
+        gl_plot_png(rgb.data(), GL_PLOT_CW, GL_PLOT_CH, nullptr, 0, &n);
+        std::vector<uint8_t> png((size_t)n);
+        if (gl_plot_png(rgb.data(), GL_PLOT_CW, GL_PLOT_CH, png.data(), n, &n) != GL_OK) fatal(1, "gl_plot_png: %s", gl_last_error(nullptr));
+        FILE* f = fopen(png_path.c_str(), "wb");
+        bool ok = f && fwrite(png.data(), 1, (size_t)n, f) == (size_t)n;
+        if (f && fclose(f) != 0) ok = false;
+        if (!ok) fprintf(stderr, "dcnv: cannot write %s: %s\n", png_path.c_str(), strerror(errno));
+    }
+    // ---- the page
+    FILE* fo = fopen(html_path.c_str(), "w");
+    if (!fo) { fprintf(stderr, "dcnv: cannot write %s: %s\n", html_path.c_str(), strerror(errno)); return; }
+    glhtml::Chart ch;
+    ch.name = "depth"; ch.xlabel = xtitle; ch.ylabel = "scaled coverage"; ch.ymin = 0; ch.ymax = 2.5;
+    std::string s = glhtml::page_open("dcnv depth " + label) + "<p><a href=\"index.html\">back to index</a></p>\n" + glhtml::chart_open(ch, 850, 550);
+    fwrite(s.data(), 1, s.size(), fo);
+    const size_t cols = std::max<size_t>(1, ((size_t)1 << 24) / std::max<size_t>(R, 1)), per_text = 1 << 16;
+    std::vector<double> y;
+    std::vector<uint8_t> tok;
+    std::vector<std::string> parts;
+    for (size_t k0 = 0; k0 < S; k0 += cols) {
+        const size_t k1 = std::min(S, k0 + cols);
+        std::vector<size_t> off(k1 - k0 + 1, 0);                     // the plotted rows of samples k0..k1, one after another
+        for (size_t k = k0; k < k1; k++) off[k - k0 + 1] = off[k - k0] + (R - (size_t)first[k]);
+        y.resize(off.back());
+        tok.resize(off.back() * 16);
+        glhost::ThreadPool::global().run((int64_t)(k1 - k0), [&](int64_t t, int) {
+            const size_t k = k0 + (size_t)t;
+            for (size_t i = (size_t)first[k]; i < R; i++) {
+                const double v = X[i * S + k];
+                y[off[t] + i - (size_t)first[k]] = v > 2.5 ? 2.5 : v;
+            }
+        });
+        if (!y.empty()) glck(ctx, gl_format_f2(ctx, y.data(), (int64_t)y.size(), tok.data()), "gl_format_f2");
+        for (size_t k = k0; k < k1; k++) {
+            glhtml::Dataset ds;
+            ds.label = samples[k]; ds.stepped = true; ds.width = S > 50 ? 0.2 : (S > 30 ? 0.3 : 0.4);
+            gl_plot_color((int32_t)k, 0, ds.rgb);
+            s = (k ? "," : "") + glhtml::dataset_head(ds);
+            fwrite(s.data(), 1, s.size(), fo);
+            const size_t f0 = (size_t)first[k], m = R - f0, groups = (m + per_text - 1) / per_text;
+            parts.assign(groups, std::string());
+            glhost::ThreadPool::global().run((int64_t)groups, [&](int64_t g, int) {
+                std::string& o = parts[(size_t)g];
+                o.reserve(per_text * 26);
+                char num[32];
+                for (size_t j = (size_t)g * per_text; j < std::min(m, ((size_t)g + 1) * per_text); j++) {
+                    const size_t q = off[k - k0] + j;
+                    const char* t = reinterpret_cast<const char*>(tok.data() + q * 16);
+                    o += j ? ",{\"x\":" : "{\"x\":";
+                    o.append(num, (size_t)snprintf(num, sizeof num, "%lld", (long long)(f0 + j) * 16384));
+                    o += ",\"y\":";
+                    if (!std::isfinite(y[q])) o += glhtml::num("%.2f", y[q]);                  // NaN / -Infinity, as the pages spell them
+                    else if (t[0]) o.append(t, strnlen(t, 16));
+                    else o += go_float("%.2f", y[q]);                                           // text longer than a token
+                    o += '}';
+                }
+            });
+            for (const std::string& p : parts) fwrite(p.data(), 1, p.size(), fo);
+            fwrite("]}", 1, 2, fo);
+        }
+    }
+    s = glhtml::chart_close(ch) + glhtml::page_close();
+    fwrite(s.data(), 1, s.size(), fo);
+    const bool bad = ferror(fo) != 0;
+    if (fclose(fo) != 0 || bad) fprintf(stderr, "dcnv: cannot write %s: %s\n", html_path.c_str(), strerror(errno));
+}
+
 }  // namespace
 
 static int cmd_dcnv(int argc, char** argv) {
     double svd_pct = -1;                                         // --svd PCT; < 0: off
-    if (argc >= 2 && strncmp(argv[1], "--svd", 5) == 0 && (argv[1][5] == 0 || argv[1][5] == '=')) {
-        ArgParser ap;
-        ap.prog = "goleft dcnv";
-        const int used = argv[1][5] == '=' ? 1 : 2;
-        if (used == 2 && argc < 3) ap.fail("missing value for --svd");
-        const std::string v = used == 1 ? argv[1] + 6 : argv[2];
-        char* endp = nullptr;
-        const double pct = strtod(v.c_str(), &endp);
-        if (v.empty() || *endp) ap.fail("error processing svd: strconv.ParseFloat: parsing \"" + v + "\": invalid syntax");
-        if (!std::isfinite(pct) || pct < 0) ap.fail("svd must be a finite percentage >= 0");
-        svd_pct = pct;
-        argc -= used;
-        argv += used;
+    bool noplots = false;                                        // --noplots (extension, as in indexcov): no chart files
+    for (bool more = true; more && argc >= 2;) {                 // the flags, in either order, before the positionals
+        more = false;
+        if (strcmp(argv[1], "--noplots") == 0) {
+            noplots = more = true;
+            argc -= 1;
+            argv += 1;
+        } else if (strncmp(argv[1], "--svd", 5) == 0 && (argv[1][5] == 0 || argv[1][5] == '=')) {
+            ArgParser ap;
+            ap.prog = "goleft dcnv";
+            const int used = argv[1][5] == '=' ? 1 : 2;
+            if (used == 2 && argc < 3) ap.fail("missing value for --svd");
+            const std::string v = used == 1 ? argv[1] + 6 : argv[2];
+            char* endp = nullptr;
+            const double pct = strtod(v.c_str(), &endp);
+            if (v.empty() || *endp) ap.fail("error processing svd: strconv.ParseFloat: parsing \"" + v + "\": invalid syntax");
+            if (!std::isfinite(pct) || pct < 0) ap.fail("svd must be a finite percentage >= 0");
+            svd_pct = pct;
+            more = true;
+            argc -= used;
+            argv += used;
+        }
     }
     if (argc < 3) fatal(2, "panic: runtime error: index out of range (usage: goleft dcnv <depthwed matrix> <ref.fa>)");
     const std::string path = argv[1], fasta = argv[2];
@@ -2378,6 +2475,10 @@ static int cmd_dcnv(int argc, char** argv) {
         for (int32_t i = 0; i < n_removed; i++) msg += " " + go_float("%.2f", 100 * sv[(size_t)i] / sum);
         go_log(msg.c_str());
         mark("svd");
+    }
+    if (!noplots) {                                              // plotDepths comes before depth.bed in the reference's main
+        dcnv_charts(ctx, X.data(), R, S, mx.samples, label);
+        mark("chart");
     }
 
     // ---- depth.bed: "%.2f" tokens from the GPU, rows assembled on the host pool

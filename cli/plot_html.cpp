@@ -25,22 +25,43 @@ std::string quote(const std::string& s) {
     return o + "\"";
 }
 
-static std::string axis(const std::string& label) {
-    return "[{\"type\":\"linear\",\"scaleLabel\":{\"display\":true,\"fontSize\":16,\"labelString\":" + quote(label) + "}}]";
+static std::string axis(const std::string& label, double lo = NAN, double hi = NAN) {
+    const std::string ticks = isnan(lo) ? "" : ",\"ticks\":{\"min\":" + num("%g", lo) + ",\"max\":" + num("%g", hi) + "}";
+    return "[{\"type\":\"linear\",\"scaleLabel\":{\"display\":true,\"fontSize\":16,\"labelString\":" + quote(label) + "}" + ticks + "}]";
+}
+
+std::string dataset_head(const Dataset& ds) {
+    char col[48];
+    snprintf(col, sizeof col, "\"rgba(%d,%d,%d,0.94)\"", ds.rgb[0], ds.rgb[1], ds.rgb[2]);
+    std::string o = "{\"label\":" + quote(ds.label) + ",\"borderColor\":" + col + ",\"backgroundColor\":" + col + ",\"pointBackgroundColor\":" + col +
+                    ",\"fill\":false";
+    o += ds.line ? ",\"showLine\":true,\"pointRadius\":0,\"borderWidth\":" + num("%g", ds.width)
+                 : ",\"showLine\":false,\"borderWidth\":0,\"pointRadius\":" + num("%g", ds.width);
+    if (ds.stepped) o += ",\"steppedLine\":true";
+    return o + ",\"pointHitRadius\":6,\"data\":[";
+}
+
+std::string chart_open(const Chart& c, int width, int height) {
+    const std::string& n = c.name;
+    char dims[64];
+    snprintf(dims, sizeof dims, " width=\"%d\" height=\"%d\"", width, height);
+    return "<canvas id=\"" + n + "\"" + dims + "></canvas>\n<script>\n/*chart " + n + " begin*/var cfg_" + n + " = {\"type\":\"line\",\"data\":{\"datasets\":[";
+}
+
+std::string chart_close(const Chart& c) {
+    const std::string& n = c.name;
+    return "]},\"options\":{\"responsive\":false,\"animation\":{\"duration\":0},\"legend\":{\"display\":" + std::string(c.legend ? "true" : "false") +
+           "},\"tooltips\":{\"mode\":\"nearest\"},\"hover\":{\"mode\":\"nearest\"},\"scales\":{\"xAxes\":" + axis(c.xlabel) +
+           ",\"yAxes\":" + axis(c.ylabel, c.ymin, c.ymax) + "}}};/*chart " + n + " end*/\n(function() {\n  var chart = new Chart(document.getElementById(\"" +
+           n + "\"), cfg_" + n + ");\n" + c.tooltip_js + "\n  chart.update();\n})();\n</script>\n";
 }
 
 std::string chart_html(const Chart& c, int width, int height) {
-    std::string cfg = "{\"type\":\"line\",\"data\":{\"datasets\":[";
+    std::string cfg = chart_open(c, width, height);
     for (size_t d = 0; d < c.data.size(); d++) {
         const Dataset& ds = c.data[d];
-        char col[48];
-        snprintf(col, sizeof col, "\"rgba(%d,%d,%d,0.94)\"", ds.rgb[0], ds.rgb[1], ds.rgb[2]);
         if (d) cfg += ",";
-        cfg += "{\"label\":" + quote(ds.label) + ",\"borderColor\":" + col + ",\"backgroundColor\":" + col + ",\"pointBackgroundColor\":" + col +
-               ",\"fill\":false";
-        cfg += ds.line ? ",\"showLine\":true,\"pointRadius\":0,\"borderWidth\":" + num("%g", ds.width)
-                       : ",\"showLine\":false,\"borderWidth\":0,\"pointRadius\":" + num("%g", ds.width);
-        cfg += ",\"pointHitRadius\":6,\"data\":[";
+        cfg += dataset_head(ds);
         std::string pts;
         pts.reserve(ds.x.size() * 24);
         for (size_t i = 0; i < ds.x.size(); i++) {
@@ -49,22 +70,17 @@ std::string chart_html(const Chart& c, int width, int height) {
         }
         cfg += pts + "]}";
     }
-    cfg += "]},\"options\":{\"responsive\":false,\"animation\":{\"duration\":0},\"legend\":{\"display\":" + std::string(c.legend ? "true" : "false") +
-           "},\"tooltips\":{\"mode\":\"nearest\"},\"hover\":{\"mode\":\"nearest\"},\"scales\":{\"xAxes\":" + axis(c.xlabel) +
-           ",\"yAxes\":" + axis(c.ylabel) + "}}}";
-    const std::string& n = c.name;
-    char dims[64];
-    snprintf(dims, sizeof dims, " width=\"%d\" height=\"%d\"", width, height);
-    return "<canvas id=\"" + n + "\"" + dims + "></canvas>\n<script>\n/*chart " + n + " begin*/var cfg_" + n + " = " + cfg + ";/*chart " + n +
-           " end*/\n(function() {\n  var chart = new Chart(document.getElementById(\"" + n + "\"), cfg_" + n + ");\n" + c.tooltip_js +
-           "\n  chart.update();\n})();\n</script>\n";
+    return cfg + chart_close(c);
 }
 
-std::string page(const std::string& title, const std::string& body) {
+std::string page_open(const std::string& title) {
     return "<!DOCTYPE html>\n<html><head><meta charset=\"utf-8\"><title>" + title +
            "</title>\n<script src=\"https://code.jquery.com/jquery-2.2.4.min.js\"></script>\n"
-           "<script src=\"https://cdnjs.cloudflare.com/ajax/libs/Chart.js/2.3.0/Chart.bundle.js\"></script>\n</head><body>\n" +
-           body + "</body></html>\n";
+           "<script src=\"https://cdnjs.cloudflare.com/ajax/libs/Chart.js/2.3.0/Chart.bundle.js\"></script>\n</head><body>\n";
 }
+
+const char* page_close() { return "</body></html>\n"; }
+
+std::string page(const std::string& title, const std::string& body) { return page_open(title) + body + page_close(); }
 
 }  // namespace glhtml

@@ -206,6 +206,10 @@ _proto("gl_dcnv_normalize", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_in
 _proto("gl_format_f2", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_f2_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_f2_host", C.c_int, _vp, C.c_int64, _vp)
+_proto("gl_dcnv_chart_select_host", C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp)
+_proto("gl_dcnv_chart_extent", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp)
+_proto("gl_dcnv_chart_raster_host", C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int32, C.c_int32, C.c_double, _vp)
+_proto("gl_dcnv_chart", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_double, _vp, _vp, _vp, _vp)
 _proto("gl_emdepth_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, _vp, _vp)
 _proto("gl_emdepth", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_int64, _vp, _vp)
 _proto("gl_emdepth_stats", C.c_int, _vp, _i64p, _i64p, _i64p)
@@ -494,6 +498,32 @@ def plot_raster_xy_host(x, y, ptr, chart, draw, xf, n_charts: int, W: int, H: in
     img = np.empty((n_charts, H, W), np.uint32)
     _ck0(lib.gl_plot_raster_xy_host(_ptr(x), _ptr(y), _ptr(ptr), _ptr(chart), _ptr(draw), chart.size, _ptr(xf), n_charts, W, H, r,
                                     _ptr(img)))
+    return img
+
+
+def dcnv_chart_select_host(x):
+    """dcnv's chart selection of the n x S float64 matrix x: (first[S] int64, yext (S,2) float64)"""
+    x = np.ascontiguousarray(x, np.float64)
+    n, S = x.shape
+    first, yext = np.empty(S, np.int64), np.empty((S, 2), np.float64)
+    _ck0(lib.gl_dcnv_chart_select_host(_ptr(x), n, S, _ptr(first), _ptr(yext)))
+    return first, yext
+
+
+def dcnv_chart_extent(first, yext, n: int) -> np.ndarray:
+    first, yext = _as(first, np.int64), _as(yext, np.float64)
+    ext = np.empty(4, np.float64)
+    _ck0(lib.gl_dcnv_chart_extent(_ptr(first), _ptr(yext), n, first.size, _ptr(ext)))
+    return ext
+
+
+def dcnv_chart_raster_host(x, first, xf, W: int = PLOT_W, H: int = PLOT_H, r: Optional[float] = None) -> np.ndarray:
+    """the (H, W) index image of dcnv's stepped lines of x (sample k drawn with index S - k)"""
+    x = np.ascontiguousarray(x, np.float64)
+    n, S = x.shape
+    first, xf = _as(first, np.int64), _as(xf, np.float64)
+    img = np.empty((H, W), np.uint32)
+    _ck0(lib.gl_dcnv_chart_raster_host(_ptr(x), n, S, _ptr(first), _ptr(xf), W, H, plot_line_radius(S) if r is None else r, _ptr(img)))
     return img
 
 
@@ -1422,6 +1452,16 @@ class Ctx:
         t = (C.c_double * 4)()
         self._ck(lib.gl_dcnv_svd_phases(self.h, t))
         return dict(zip(("gram", "eigen", "project", "copies"), list(t)))
+
+    def dcnv_chart(self, x: np.ndarray, block_rows: int = 0, W: int = PLOT_W, H: int = PLOT_H, r: Optional[float] = None):
+        """dcnv's chart of the n x S float64 matrix x on the GPU: (first[S], yext (S,2), ext4, the (H, W) index image)"""
+        x = np.ascontiguousarray(x, np.float64)
+        n, S = x.shape
+        first, yext, ext = np.empty(S, np.int64), np.empty((S, 2), np.float64), np.empty(4, np.float64)
+        img = np.empty((H, W), np.uint32)
+        self._ck(lib.gl_dcnv_chart(self.h, _ptr(x), n, S, block_rows, W, H, plot_line_radius(S) if r is None else r, _ptr(first),
+                                   _ptr(yext), _ptr(ext), _ptr(img)))
+        return first, yext, ext, img
 
     # ---- emdepth
     def emdepth(self, x: np.ndarray, block_rows: int = 0, ld: Optional[int] = None, S: Optional[int] = None, want_lambda: bool = True):

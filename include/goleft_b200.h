@@ -602,6 +602,28 @@ int  gl_dcnv_svd_device(gl_ctx* ctx, double* d_x, int64_t n, int64_t ld, int32_t
 int  gl_dcnv_svd_phases(gl_ctx* ctx, double* t4);
 int  gl_pca_tridiag_above(const double* d, const double* e, int32_t n, double rel, double* w, int32_t* count);
 
+/* ---------------------------------------------------------------- dcnv's depth chart (dcnv_chart.cu; DESIGN §1.9)
+ * x is the n x S row-major float64 matrix depth.bed holds (after the normalisation, and --svd when given).  Sample k's line
+ * (dcnv.go asValues, no thinning): rows i >= first[k], the first row whose value is not == 0 (NaN is not; n when none), are
+ * vertices x = i * 16384, y = min(v, 2.5).  The line is stepped: step i runs (x_i, y_i) -> (x_{i+1}, y_i) -> (x_{i+1}, y_{i+1})
+ * and is not drawn when either y is NaN or -Inf.  The image is an index image as the gl_plot_* entries describe it, sample k
+ * drawn with index S - k (sample 0 on top, as Chart.js 2 stacks the page's datasets), under the same float64 pixel rule.
+ *   gl_dcnv_chart_select_host : first[S] and yext2[2S] = min, max of the drawn y of each sample (-0.0 as 0.0; +Inf, -Inf when
+ *       it has none).
+ *   gl_dcnv_chart_extent : host-only: ext4 = {xmin, xmax, ymin, ymax} over every sample's vertices (x) and drawn y, 0 where
+ *       there are none; gl_plot_transform's input.
+ *   gl_dcnv_chart_raster_host : the W x H image of every sample's steps under transform xf4 and line radius r; cleared first.
+ *       W * H <= 393216.
+ *   gl_dcnv_chart : the select, the extent and the image on the GPU, the matrix streamed through the device in row blocks of
+ *       block_rows (0: as many as fit in free device memory), once when it fits and twice when it does not.  xf4 is
+ *       gl_plot_transform(ext4, W, H).  Nothing depends on block_rows. */
+int  gl_dcnv_chart_select_host(const double* x, int64_t n, int64_t S, int64_t* first, double* yext2);
+int  gl_dcnv_chart_extent(const int64_t* first, const double* yext2, int64_t n, int64_t S, double* ext4);
+int  gl_dcnv_chart_raster_host(const double* x, int64_t n, int64_t S, const int64_t* first, const double* xf4, int32_t W, int32_t H,
+                               double r, uint32_t* img);
+int  gl_dcnv_chart(gl_ctx* ctx, const double* x, int64_t n, int64_t S, int64_t block_rows, int32_t W, int32_t H, double r, int64_t* first,
+                   double* yext2, double* ext4, uint32_t* img);
+
 /* ---------------------------------------------------------------- emdepth
  * Restates emdepth/emdepth.go (a library of the reference with no command): a cn.mops-style EM per row of an n x S depth
  * matrix, the copy number (CN) of every cell, and the Cache that merges non-CN2 rows into per-sample CNVs (DESIGN §1.10).

@@ -224,6 +224,14 @@ __global__ void __launch_bounds__(128) md_walk_kernel(const int* __restrict__ bl
     val[(long long)b * S + sample] = __dmul_rn(__ddiv_rn(acc, (double)(e - s)), 1000.0);
 }
 
+// minSamples = int(0.5 + MinSamples * S) (multidepth.go:64) as Go compiles it on amd64 (CVTTSD2SQ): truncation toward
+// zero, and NaN, +-Inf and anything outside [-2^63, 2^63) become INT64_MIN.  A C++ cast leaves those inputs undefined.
+int64_t md_min_samples(double frac, int32_t S) {
+    const double x = 0.5 + frac * (double)S;
+    if (!(x >= -9223372036854775808.0 && x < 9223372036854775808.0)) return INT64_MIN;
+    return (int64_t)x;
+}
+
 int md_need(gl_ctx* ctx, const char* who) {
     GL_CHECK(gl_use(ctx));
     if (!ctx->md) return gl_fail(ctx, GL_ESTATE, "%s: call gl_multidepth_begin first", who);
@@ -271,7 +279,7 @@ int gl_multidepth_begin(gl_ctx* ctx, int64_t contig_len, int32_t n_samples, int3
     m->n_runs = m->nb = m->n_pairs = m->walked = m->certified = 0;
     m->L = contig_len; m->words = bases / 32; m->tiles = tiles;
     m->S = n_samples; m->mincov = mincov;
-    m->min_samples = (int64_t)(0.5 + min_samples * (double)n_samples);     // multidepth.go:64
+    m->min_samples = md_min_samples(min_samples, n_samples);
     GL_CHECK(gl_buf_reserve(ctx, m->ge, (size_t)bases / 8));
     GL_CHECK(gl_buf_reserve(ctx, m->pos, (size_t)bases / 8));
     GL_CHECK(gl_buf_reserve(ctx, m->site, (size_t)bases / 8));
@@ -317,10 +325,12 @@ int gl_multidepth_sites(gl_ctx* ctx, int32_t* run_start, uint8_t* run_class, int
         const unsigned ctas = (unsigned)((words + kRunThreads - 1) / kRunThreads);
         GL_CHECK(gl_buf_reserve(ctx, m->cta_cnt, (size_t)ctas * 4));
         {
+            // counts lie in [0, 65535]: every threshold below -1 acts as -1, every one above 65535 as 65535
+            const int thr = (int)std::max<int64_t>(-1, std::min<int64_t>(m->min_samples, 65535));
             gl_prof_scope prof(ctx, "md_classify_kernel");
             md_classify_kernel<<<(unsigned)((words + 255) / 256), 256, 0, ctx->stream>>>(
                 static_cast<const unsigned short*>(m->cnt.p), static_cast<const unsigned*>(m->site.p), static_cast<unsigned*>(m->suf.p),
-                words, (int)std::min<int64_t>(m->min_samples, INT32_MAX));
+                words, thr);
         }
         {
             gl_prof_scope prof(ctx, "md_runs_count_kernel");

@@ -519,7 +519,8 @@ int  gl_indexsplit_chunks(const double* tile_sum, const int64_t* out_ptr, int32_
  * Replaces multidepth/multidepth.go: the `samtools depth -Q q -r chrom:k*C+1` child over all BAMs of one chunk (:208-221),
  * sufficientDepth (:158-166), the chunk state machine of aggregate (:222-266), splitBlocks (:183-200) and means (:268-283).
  * One contig [0, L), S samples, L < 2^30, 1 <= S <= 65535.  Device memory is O(L) plus the blocks x S outputs.
- *   gl_multidepth_begin   : minSamples = int(0.5 + min_samples * S) (:64); zeroes the per-base counters.
+ *   gl_multidepth_begin   : minSamples = int(0.5 + min_samples * S) (:64) as Go converts on amd64 (NaN, +-Inf and values
+ *                           outside [-2^63, 2^63) give INT64_MIN); zeroes the per-base counters.
  *   pass 1, per sample    : gl_depth_begin(ctx, 0, L), gl_depth_add_segments* (any form), gl_multidepth_count.  The depth tile
  *                           core (any path, same eligibility checks and fallbacks as gl_depth_reduce) counts, per base, the
  *                           samples with d >= mincov and whether any sample has d > 0 (a `samtools depth` line).

@@ -44,7 +44,13 @@ static void split_blocks(md_out* o, const int64_t* cache, int64_t n, int64_t win
 }
 
 int64_t orc_md_chunk_size(int64_t S) { return S > 50 ? 5000000 / 5 : 5000000; }
-int64_t orc_md_min_samples(double frac, int64_t S) { return (int64_t)(0.5 + frac * (double)S); }
+/* int(0.5 + MinSamples * S) as Go compiles it on amd64 (CVTTSD2SQ): truncation toward zero; NaN, +-Inf and anything
+ * outside [-2^63, 2^63) give INT64_MIN (a C cast leaves those undefined) */
+int64_t orc_md_min_samples(double frac, int64_t S) {
+    const double x = 0.5 + frac * (double)S;
+    if (!(x >= -9223372036854775808.0 && x < 9223372036854775808.0)) return INT64_MIN;
+    return (int64_t)x;
+}
 
 /* cls[x]: 0 = not a site, 1 = insufficient site, 2 = sufficient site */
 static void aggregate_all(const uint8_t* cls, int64_t L, int64_t C, int64_t max_skip, int64_t min_size, int64_t window, md_out* o) {

@@ -348,9 +348,20 @@ __device__ __forceinline__ void flush_max(const ScanParams& p, int acc_max) {
         atomicMax(reinterpret_cast<unsigned long long*>(p.header + 2), (unsigned long long)acc_max);
 }
 
+// Clears one warp's kElems-element region of a tile with 32 consecutive chunks per store.  The warp owns the region, so
+// the order does not matter, and the addresses are one base plus constants (no per-chunk swizzle kept in registers).
+template <int kElems>
+__device__ __forceinline__ void clear_warp_region(int* region, int lane) {
+#pragma unroll
+    for (int j = 0; j < kElems / 128; j++) reinterpret_cast<int4*>(region)[lane + 32 * j] = make_int4(0, 0, 0, 0);
+}
+
 // BPT bases per thread (16 or 32), WARPS warps per CTA, BPT * 32 * WARPS == kTile.  32 bases per thread halves the work
 // that is paid per thread and tile (warp scan, class check, window loop, run claim, barrier) — K_fused8 uses <32, 4>.
-template <int BPT, int WARPS, bool kZeroAfterRead, bool kMD = false>
+// kSliceInTile (K_fused8): the depth slice goes over the warp's own region of s_tile instead of s_depth (unused, may be
+// null), and the region is cleared when the core is done with it.  The caller must then hold every warp at a barrier
+// between the core and the next tile's atomics.
+template <int BPT, int WARPS, bool kZeroAfterRead, bool kMD = false, bool kSliceInTile = false>
 __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__ s_tile, int* __restrict__ s_depth,
                                           const int* s_carry, int tile, int& acc_max) {
     static_assert(BPT * 32 * WARPS == kTile, "tile shape");
@@ -372,7 +383,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     for (int j = 0; j < BPT / 4; j++) {
         const int4 q = reinterpret_cast<const int4*>(s_tile)[c0 ^ j];
         x[4 * j] = q.x; x[4 * j + 1] = q.y; x[4 * j + 2] = q.z; x[4 * j + 3] = q.w;
-        if (kZeroAfterRead) reinterpret_cast<int4*>(s_tile)[c0 ^ j] = make_int4(0, 0, 0, 0);
+        if (kZeroAfterRead && !kSliceInTile) reinterpret_cast<int4*>(s_tile)[c0 ^ j] = make_int4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int k = 1; k < BPT; k++) x[k] += x[k - 1];
@@ -492,17 +503,23 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     // Depth by position: this warp's private slice of s_depth holds x[k] (depth relative to the thread's tbase), swizzled
     // like s_tile (base e of the slice at sw[swz_elem_t<BPT>(e)]) so that both a lane storing its BPT/4 chunks and 32 lanes
     // reading 32 consecutive bases of one thread are conflict-free; the threads' tbase go to s_tbase.  Storing x instead of
-    // depth saves BPT adds per thread; a reader adds the owner's tbase.  s_tile cannot hold the slice: a warp that leaves the
-    // core early starts the next tile's atomics there.
-    int* sw = s_depth + warp * kWElems;
+    // depth saves BPT adds per thread; a reader adds the owner's tbase.  The slice uses the same chunks as the warp's region
+    // of s_tile, so a warp only ever touches its own kWElems elements of either buffer.  With kSliceInTile it overwrites
+    // that region, which is safe because no warp starts the next tile's atomics before the caller's barrier; otherwise a
+    // warp that leaves the core early may already be adding into s_tile, and the slice goes to s_depth.
+    int* const s_slice = kSliceInTile ? s_tile : s_depth;
+    int* sw = s_slice + warp * kWElems;
     int* stb = s_tbase + warp * 32;
-    if (slow_runs || p.do_windows) {
+    const bool need_slice = slow_runs || p.do_windows;       // warp-uniform
+    if (need_slice) {
         __syncwarp();
 #pragma unroll
         for (int j = 0; j < BPT / 4; j++)
-            reinterpret_cast<int4*>(s_depth)[c0 ^ j] = make_int4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
+            reinterpret_cast<int4*>(s_slice)[c0 ^ j] = make_int4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
         stb[lane] = tbase;
         __syncwarp();
+    } else if (kSliceInTile) {
+        clear_warp_region<kWElems>(sw, lane);                 // every lane has read its differences (block barrier above)
     }
 
     // ---- run starts (slow path): one mask bit per base, rank inside the warp in position order
@@ -645,6 +662,10 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
                 rank++;
             }
         }
+    }
+    if (kSliceInTile && need_slice) {                         // the run claim was the slice's last reader: clear for the next tile
+        __syncwarp();
+        clear_warp_region<kWElems>(sw, lane);
     }
 }
 
@@ -1143,12 +1164,13 @@ __device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t
 }
 
 // K_fused8: persistent, software-pipelined like K_fused: while tile n runs its core, the packed words of tile n+1 (two
-// passes = 16 blocks, what a 30x tile needs) and the block range of tile n+2 are in flight.
+// passes = 16 blocks, what a 30x tile needs) and the block range of tile n+2 are in flight.  The core keeps its depth
+// slice in s_tile (16 KB less shared memory than a separate slice buffer), so a barrier at the top of each tile holds
+// every warp until all have cleared their regions.
 template <bool kMD>
 __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanParams p) {
     __shared__ __align__(16) int s_tile[kTile];
-    __shared__ __align__(16) int s_depth[kTile];
-    __shared__ int s_carry2[2][kF8Warps];
+    __shared__ int s_carry[kF8Warps];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = gridDim.x;
     if (p.header[3] != 0) return;                           // K_tileidx8 found unsorted anchors: the host falls back
@@ -1160,11 +1182,10 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
     if (tile < p.tile_end) { lo = max(0, p.tile_lo[tile] - 1); hi = min(nb, p.tile_hi[tile + 1]); }
     if (tile + G < p.tile_end) { lo2 = max(0, p.tile_lo[tile + G] - 1); hi2 = min(nb, p.tile_hi[tile + G + 1]); }
     P8Regs regs0 = fused8_load(p, lo, hi, 0), regs1 = fused8_load(p, lo, hi, 1);
-    __syncthreads();
 
     int acc_max = 0;
-    for (int it = 0; tile < p.tile_end; tile += G, it ^= 1) {
-        int* s_carry = s_carry2[it];
+    for (; tile < p.tile_end; tile += G) {
+        __syncthreads();                                    // every warp has cleared its region of s_tile
         const int t0 = p.rs + tile * kTile;
         int carry = 0;
         fused8_apply(regs0, s_tile, t0, carry);
@@ -1179,7 +1200,7 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
         regs1 = fused8_load(p, lo, hi, 1);
         lo2 = hi2 = 0;
         if (tile + 2 * G < p.tile_end) { lo2 = max(0, p.tile_lo[tile + 2 * G] - 1); hi2 = min(nb, p.tile_hi[tile + 2 * G + 1]); }
-        tile_core<kF8BPT, kF8Warps, true, kMD>(p, s_tile, s_depth, s_carry, tile, acc_max);
+        tile_core<kF8BPT, kF8Warps, true, kMD, true>(p, s_tile, nullptr, s_carry, tile, acc_max);
     }
     flush_max(p, acc_max);
 }

@@ -1663,86 +1663,39 @@ static int cmd_indexcov(int argc, char** argv) {
 }
 
 // ------------------------------------------------------------------------------------------------ covstats
-// V2 (covstats.go:57-89,175-218).  The reference sorts the sampled insert sizes / template lengths / read lengths and reads
-// order statistics off the sorted slices.  Here the multiset is a histogram made on the GPU (gl_bincount_i32): the k-th
-// smallest value is a search in its running count, madFilter's cut is a count, and meanStd's float64 accumulation visits
-// the values in ascending order with their multiplicities — the same sequence of additions as over the sorted slice, so
-// the results are bit-identical without a sort.
-struct SortedCounts {
-    int32_t lo = 0;
-    std::vector<uint64_t> cum;                               // cum[i] = how many values are <= lo + i
-    std::vector<int32_t> sorted;                             // fallback when the value range is too wide for a histogram
-    size_t n = 0;
-    void build(gl_ctx* ctx, const std::vector<int32_t>& v) {
-        n = v.size();
-        cum.clear(); sorted.clear();
-        if (n == 0) return;
-        int32_t mn = v[0], mx = v[0];
-        for (int32_t x : v) { mn = std::min(mn, x); mx = std::max(mx, x); }
-        const long long range = (long long)mx - mn + 1;
-        if (range > (1LL << 22)) { sorted = v; std::sort(sorted.begin(), sorted.end()); return; }
-        lo = mn;
-        cum.assign((size_t)range, 0);
-        glck(ctx, gl_bincount_i32(ctx, v.data(), (int64_t)n, mn, (int32_t)((long long)mx + 1 > INT32_MAX ? INT32_MAX : mx + 1), cum.data()), "gl_bincount_i32");
-        if ((long long)mx + 1 > INT32_MAX) { sorted = v; std::sort(sorted.begin(), sorted.end()); cum.clear(); return; }
-        for (size_t i = 1; i < cum.size(); i++) cum[i] += cum[i - 1];
-    }
-    int32_t kth(size_t k) const {                            // k-th smallest, 0-based
-        if (!sorted.empty()) return sorted[k];
-        return lo + (int32_t)(std::upper_bound(cum.begin(), cum.end(), (uint64_t)k) - cum.begin());
-    }
-    size_t count_le(long long v) const {
-        if (!sorted.empty()) return (size_t)(std::upper_bound(sorted.begin(), sorted.end(), v, [](long long a, int32_t b) { return a < (long long)b; }) - sorted.begin());
-        if (v < lo) return 0;
-        const long long i = v - lo;
-        return (size_t)(i >= (long long)cum.size() ? cum.back() : cum[(size_t)i]);
-    }
-    template <class F> void for_first(size_t m, F f) const { // the m smallest values, ascending, with multiplicity
-        if (!sorted.empty()) { for (size_t i = 0; i < m; i++) f(sorted[i]); return; }
-        size_t done = 0;
-        for (size_t i = 0; i < cum.size() && done < m; i++) {
-            const size_t c = std::min<size_t>((size_t)(cum[i] - (i ? cum[i - 1] : 0)), m - done);
-            for (size_t k = 0; k < c; k++) f(lo + (int32_t)i);
-            done += c;
-        }
-    }
-};
-static void mean_std(const SortedCounts& a, size_t n, double& mean, double& sd) {     // covstats.go:78-89 over the n smallest
-    const double l = (double)n;
-    mean = 0; sd = 0;
-    a.for_first(n, [&](int32_t x) { mean += (double)x / l; });
-    const double mu = mean;
-    a.for_first(n, [&](int32_t x) { sd += pow((double)x - mu, 2) / l; });
-    sd = sqrt(sd);
-}
-static size_t mad_filter(const SortedCounts& a, int nmads) {                        // covstats.go:57-76: how many values are kept
-    const size_t n = a.n;
-    const int32_t med = a.kth(n / 2);
-    // upper_mads = arr[n/2+1:] - med is already sorted: its middle element is arr[n/2+1 + len/2] - med
-    const size_t len = n - (n / 2 + 1);
-    const long long umad = (long long)a.kth(n / 2 + 1 + len / 2) - med;
-    const long long upper = (long long)med + (long long)nmads * umad;
-    size_t i = a.count_le(upper);                                                   // first index with arr[i] > upper
-    if (i == n) i = n - 1;                                                          // Go's range loop leaves i at the last index
-    return i;
-}
-
+// V1 + V2 (covstats.go:122-220): gl_bam_covstats samples the records and computes the reference's Stats on the device;
+// a file it cannot take (GL_ESTATE), or GL_GPU_FEED=0, goes through gl_bam_covstats_host, with the same tail.
 static int cmd_covstats(int argc, char** argv) {
     // the header is printed before the arguments are parsed (covstats.go:224-226)
     printf("coverage\tinsert_mean\tinsert_sd\tinsert_5th\tinsert_95th\ttemplate_mean\ttemplate_sd\tpct_unmapped\tpct_bad_reads\tpct_duplicate\tpct_proper_pair\tread_length\tbam\tsample\n");
-    std::string nstr = "1000000", regions, fasta;
+    std::string nstr = "1000000", regions, fasta, hist;
     ArgParser ap;
     ap.prog = "goleft covstats";
-    ap.add("n", 'n', &nstr); ap.add("regions", 'r', &regions); ap.add("fasta", 'f', &fasta);
+    ap.add("n", 'n', &nstr); ap.add("regions", 'r', &regions); ap.add("fasta", 'f', &fasta); ap.add("hist", 0, &hist);
     ap.parse(argc, argv);
     if (ap.positional.empty()) ap.fail("bams is required");
     const int N = atoi(nstr.c_str());
     gl_ctx* ctx = open_ctx(0, "goleft covstats");
     for (const std::string& bam : ap.positional) {
-        glhts::BamHeader hdr;
-        glhts::CovstatsSample cs;
-        std::string e = glhts::bam_covstats_sample(bam, N, 100000, hdr, cs);
-        if (!e.empty()) fatal(1, "%s", e.c_str());
+        gl_bam* bh = nullptr;
+        char oerr[512] = {0};
+        if (gl_bam_open(bam.c_str(), &bh, oerr, sizeof oerr) != GL_OK) fatal(1, "%s", oerr);
+        const glhts::BamHeader& hdr = bh->f.header;
+        gl_covstats st;
+        std::vector<double> H;
+        auto sample = [&](bool device) {
+            int rc = device ? gl_bam_covstats(ctx, bh, N, 100000, &st, nullptr, 0) : gl_bam_covstats_host(ctx, bh, N, 100000, &st, nullptr, 0);
+            if (rc == GL_ERANGE && st.h_len > 0 && !hist.empty()) {              // H is wanted: the second call of the two
+                H.resize((size_t)st.h_len);
+                rc = device ? gl_bam_covstats(ctx, bh, N, 100000, &st, H.data(), st.h_len) : gl_bam_covstats_host(ctx, bh, N, 100000, &st, H.data(), st.h_len);
+            } else if (rc == GL_ERANGE && st.h_len > 0) rc = GL_OK;              // the row does not print H
+            return rc;
+        };
+        int rc = SegSource::gpu_feed() ? sample(true) : GL_ESTATE;
+        if (rc == GL_ESTATE) rc = sample(false);
+        if (rc == GL_EINVAL && st.n_insert > 0 && st.n_insert < 3) fatal(2, "panic: runtime error: index out of range (covstats madFilter needs at least 3 insert sizes)");
+        if (rc == GL_ERANGE) fatal(2, "panic: runtime error: makeslice: len out of range (%s)", gl_last_error(ctx));
+        if (rc != GL_OK) fatal(1, "%s", gl_last_error(ctx));
         std::string names;
         for (auto& s : hdr.sample_names()) names += (names.empty() ? "" : ",") + s;
         if (names.empty()) names = "<no-read-groups>";
@@ -1753,30 +1706,15 @@ static int cmd_covstats(int argc, char** argv) {
             if (!be.empty()) fatal(1, "%s", be.c_str());
             have_idx = true;
         }
-        double pBad = 0, pDup = 0, pProper = 0, pUnmapped = 0, rlMean = 0, insMean = 0, insSd = 0, tMean = 0, tSd = 0;
-        int pct5 = 0, pct95 = 0, maxRead = 0;
-        SortedCounts sc;
-        if (!cs.read_len.empty()) {                                                 // covstats.go:177-186
-            const double den = (double)(cs.k + cs.n_unmapped);
-            pBad = cs.n_bad / den; pDup = cs.n_dup / den; pProper = cs.n_proper / den; pUnmapped = cs.n_unmapped / den;
-            sc.build(ctx, cs.read_len);
-            double sd;
-            mean_std(sc, sc.n, rlMean, sd);
-            maxRead = sc.kth(sc.n - 1);
-        }
-        if (!cs.insert.empty()) {                                                   // covstats.go:188-199
-            sc.build(ctx, cs.insert);
-            const double l = (double)(cs.insert.size() - 1);
-            pct5 = sc.kth((size_t)(0.05 * l + 0.5));
-            pct95 = sc.kth((size_t)(0.95 * l + 0.5));
-            if (sc.n < 3) fatal(2, "panic: runtime error: index out of range (covstats madFilter needs at least 3 insert sizes)");
-            const size_t ki = mad_filter(sc, 10);
-            mean_std(sc, ki, insMean, insSd);
-            sc.build(ctx, cs.tmpl);
-            const size_t kt = mad_filter(sc, 10);
-            mean_std(sc, kt, tMean, tSd);
-            // (Stats.H, the template-length histogram of covstats.go:202-217, is consumed by smoove through the Go API and is
-            //  not part of the TSV row this command prints; it is not computed here)
+        const double pBad = st.proportion_bad, pDup = st.proportion_duplicate, pProper = st.proportion_properly_paired, pUnmapped = st.proportion_unmapped;
+        const double rlMean = st.read_length_mean, insMean = st.insert_mean, insSd = st.insert_sd, tMean = st.template_mean, tSd = st.template_sd;
+        const int pct5 = st.insert_pct5, pct95 = st.insert_pct95, maxRead = st.max_read_length;
+        if (!hist.empty()) {                                                        // Stats.H (covstats.go:202-217), one line per entry
+            const std::string hp = hist + "." + names + ".template_hist.tsv";
+            FILE* hf = fopen(hp.c_str(), "w");
+            if (!hf) fatal(1, "open %s: %s", hp.c_str(), strerror(errno));
+            for (size_t j = 0; j < H.size(); j++) fprintf(hf, "%lld\t%s\n", (long long)maxRead + (long long)j, go_float("%.6g", H[j]).c_str());
+            fclose(hf);
         }
         long long genome = 0;
         unsigned long long mapped = 0;
@@ -1804,6 +1742,7 @@ static int cmd_covstats(int argc, char** argv) {
         const double coverage = (1 - pBad) * (double)mapped * rlMean / (double)genome;     // covstats.go:277
         printf("%.2f\t%.2f\t%.2f\t%d\t%d\t%.2f\t%.2f\t%.2f\t%.1f\t%.1f\t%.1f\t%d\t%s\t%s\n", coverage, insMean, insSd, pct5, pct95, tMean, tSd,
                100 * pUnmapped, 100 * pBad, 100 * pDup, 100 * pProper, maxRead, bam.c_str(), names.c_str());
+        gl_bam_close(bh);
     }
     gl_ctx_destroy(ctx);
     return 0;

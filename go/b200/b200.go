@@ -446,3 +446,56 @@ func EmdepthCNVs(cells []uint8, samples int, starts, ends, breaks []int64) ([]Em
 	}
 	return out, nil
 }
+
+// Stats is covstats.Stats (covstats/covstats.go:92-112) as gl_bam_covstats computes it.
+type Stats struct {
+	InsertMean, InsertSD                 float64
+	InsertPct5, InsertPct95              int
+	TemplateMean, TemplateSD             float64
+	ReadLengthMean, ReadLengthMedian     float64
+	ProportionBad, ProportionUnmapped    float64
+	ProportionProperlyPaired             float64
+	ProportionDuplicate                  float64
+	MaxReadLength                        int
+	H                                    []float64
+	// OnDevice tells whether the records were sampled on the GPU (false: the file went through the host sampler)
+	OnDevice bool
+}
+
+// BamStats replaces covstats.BamStats(br, n, skipReads) (covstats/covstats.go:122-220): the records are sampled on the
+// GPU, or by the host sampler when the file cannot be taken there (GL_ESTATE: no index, a BGZF member the device rejects).
+// Where the reference panics (1 or 2 insert sizes, a negative histogram length) it returns the library's error.
+func (c *Ctx) BamStats(b *Bam, n, skipReads int) (Stats, error) {
+	var st C.gl_covstats
+	h := make([]float64, 1<<14)
+	call := func(device bool) C.int {
+		for {
+			var rc C.int
+			if device {
+				rc = C.gl_bam_covstats(c.h, b.h, C.int32_t(n), C.int32_t(skipReads), &st, (*C.double)(unsafe.Pointer(&h[0])), C.int64_t(len(h)))
+			} else {
+				rc = C.gl_bam_covstats_host(c.h, b.h, C.int32_t(n), C.int32_t(skipReads), &st, (*C.double)(unsafe.Pointer(&h[0])), C.int64_t(len(h)))
+			}
+			if rc == C.GL_ERANGE && int(st.h_len) > len(h) {
+				h = make([]float64, int(st.h_len))
+				continue
+			}
+			return rc
+		}
+	}
+	rc := call(true)
+	if rc == C.GL_ESTATE {
+		rc = call(false)
+	}
+	if e := c.err(rc); e != nil {
+		return Stats{}, e
+	}
+	return Stats{
+		InsertMean: float64(st.insert_mean), InsertSD: float64(st.insert_sd), InsertPct5: int(st.insert_pct5), InsertPct95: int(st.insert_pct95),
+		TemplateMean: float64(st.template_mean), TemplateSD: float64(st.template_sd),
+		ReadLengthMean: float64(st.read_length_mean), ReadLengthMedian: float64(st.read_length_median),
+		ProportionBad: float64(st.proportion_bad), ProportionUnmapped: float64(st.proportion_unmapped),
+		ProportionProperlyPaired: float64(st.proportion_properly_paired), ProportionDuplicate: float64(st.proportion_duplicate),
+		MaxReadLength: int(st.max_read_length), H: h[:int(st.h_len)], OnDevice: st.path == 1,
+	}, nil
+}

@@ -127,6 +127,11 @@ _proto("gl_plot_png", C.c_int, _vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p)
 _proto("gl_format_g3", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_g3_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_bincount_i32", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp)
+_proto("gl_bam_covstats", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
+_proto("gl_bam_covstats_host", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
+_proto("gl_bam_covstats_samples", C.c_int, _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp))
+_proto("gl_bam_covstats_host_samples", C.c_int, _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp))
+_proto("gl_covstats_tail", C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64)
 _proto("gl_depthwed_aggregate", C.c_int, _vp, _vp, C.c_int32, C.c_int64, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp,
        C.c_int64, _i64p)
 _proto("gl_depthwed_aggregate_device", C.c_int, _vp, _vp, C.c_int32, C.c_int64, _vp, C.c_int64, _vp)
@@ -780,6 +785,79 @@ def bam_decode_device(ctx: "Ctx", bam: Bam, tid: int, min_mapq: int = 1):
     else:
         out["start"], out["end"] = np.zeros(0, np.int32), np.zeros(0, np.int32)
     return out
+
+
+class CovStats(C.Structure):
+    """gl_covstats: the reference's Stats, the counters behind it, which route ran and its phase times"""
+    _fields_ = ([(k, C.c_double) for k in ("insert_mean", "insert_sd", "template_mean", "template_sd", "read_length_mean", "read_length_median",
+                                           "proportion_bad", "proportion_unmapped", "proportion_properly_paired", "proportion_duplicate")] +
+                [(k, C.c_int32) for k in ("insert_pct5", "insert_pct95", "max_read_length", "path")] +
+                [(k, C.c_int64) for k in ("n_unmapped", "k", "n_bad", "n_dup", "n_proper", "n_read_len", "n_insert", "n_records_read", "h_len",
+                                          "bytes_in", "bytes_out")] +
+                [(k, C.c_double) for k in ("read_s", "inflate_s", "index_s", "fields_s", "cut_s", "tail_s", "wall_s")] +
+                [("n_batches", C.c_int32), ("_pad", C.c_int32)])
+    STATS = ("insert_mean", "insert_sd", "insert_pct5", "insert_pct95", "template_mean", "template_sd", "read_length_mean", "read_length_median",
+             "proportion_bad", "proportion_unmapped", "proportion_properly_paired", "proportion_duplicate", "max_read_length")
+    COUNTERS = ("n_unmapped", "k", "n_bad", "n_dup", "n_proper", "n_read_len", "n_insert", "n_records_read")
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "_pad"}
+
+
+def _covstats_two_call(ctx, fn, st=None):
+    """the two-call convention: once for h_len, once more with room -> (CovStats, H)"""
+    st = st if st is not None else CovStats()
+    H = np.empty(1 << 14, np.float64)                      # room for most histograms, so one call is the usual case
+    rc = fn(C.byref(st), _ptr(H), H.size)
+    if rc == GL_ERANGE and st.h_len > H.size:
+        H = np.empty(st.h_len, np.float64)
+        rc = fn(C.byref(st), _ptr(H), H.size)
+    if rc != GL_OK:
+        e = GlError(rc, lib.gl_last_error(ctx.h if ctx is not None else None).decode())
+        e.stats = st
+        raise e
+    return st, H[: st.h_len].copy()
+
+
+def bam_covstats(ctx: "Ctx", bam: Bam, n: int, skip: int = 100000, samples: bool = False):
+    """covstats.BamStats sampled on the device -> (CovStats, H[, (read_len, insert, tmpl) in file order]); GlError(GL_ESTATE)
+    when the file cannot be sampled there."""
+    st, H = _covstats_two_call(ctx, lambda o, h, cap: lib.gl_bam_covstats(ctx.h, bam.h, n, skip, o, h, cap))
+    if not samples:
+        return st, H
+    ps = [_vp(), _vp(), _vp()]
+    ctx._ck(lib.gl_bam_covstats_samples(ctx.h, *[C.byref(p) for p in ps]))
+    out = []
+    for p, k in zip(ps, (st.n_read_len, st.n_insert, st.n_insert)):
+        a = np.empty(k, np.int32)
+        if k:
+            ctx._ck(lib.gl_memcpy_d2h(ctx.h, _ptr(a), p.value, k * 4))
+        out.append(a)
+    return st, H, tuple(out)
+
+
+def bam_covstats_host(ctx: Optional["Ctx"], bam: Bam, n: int, skip: int = 100000, samples: bool = False):
+    """the same from the host sampler; ctx may be None (no device is touched then)"""
+    h = ctx.h if ctx is not None else None
+    st, H = _covstats_two_call(ctx, lambda o, hh, cap: lib.gl_bam_covstats_host(h, bam.h, n, skip, o, hh, cap))
+    if not samples:
+        return st, H
+    ps = [_vp(), _vp(), _vp()]
+    lib.gl_bam_covstats_host_samples(bam.h, *[C.byref(p) for p in ps])
+    out = tuple(np.ctypeslib.as_array(C.cast(p, _i32p), (k,)).copy() if k else np.zeros(0, np.int32)
+                for p, k in zip(ps, (st.n_read_len, st.n_insert, st.n_insert)))
+    return st, H, out
+
+
+def covstats_tail(ctx: Optional["Ctx"], read_len, insert, tmpl, n_unmapped=0, k=0, n_bad=0, n_dup=0, n_proper=0):
+    """covstats.go:175-218 from host sample arrays and the five counters -> (CovStats, H); ctx may be None"""
+    read_len, insert, tmpl = _as(read_len, np.int32), _as(insert, np.int32), _as(tmpl, np.int32)
+    h = ctx.h if ctx is not None else None
+
+    st = CovStats()
+    st.n_unmapped, st.k, st.n_bad, st.n_dup, st.n_proper = n_unmapped, k, n_bad, n_dup, n_proper
+    return _covstats_two_call(ctx, lambda o, hh, cap: lib.gl_covstats_tail(h, _ptr(read_len), read_len.size, _ptr(insert), insert.size,
+                                                                         _ptr(tmpl), tmpl.size, o, hh, cap), st)
 
 
 def crai_make_sizes(start, span, nbytes) -> np.ndarray:

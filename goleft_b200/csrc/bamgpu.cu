@@ -13,6 +13,7 @@
 // Anything unexpected (a member the inflater rejects, a malformed record) makes the call return GL_ESTATE and the caller
 // uses the host feeder for that reference.
 #include "gl_common.cuh"
+#include "ll_scan.cuh"
 #include "host/bam_cigar.h"
 #include "host/bam_feed.h"
 #include "host/thread_pool.h"
@@ -63,24 +64,6 @@ __global__ void __launch_bounds__(128) bam_parse_kernel(const unsigned char* __r
         if (maxlen) atomicMax(stats + 2, (unsigned long long)maxlen);
         if (bad) atomicAdd(stats + 3, 1ull);
     }
-}
-
-// exclusive scan of n long longs, one CTA (n = units of one reference: thousands)
-__global__ void __launch_bounds__(1024) ll_scan_kernel(const long long* __restrict__ in, long long* __restrict__ out, int n) {
-    __shared__ long long s_w[32];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int per = (n + 1 + 1023) / 1024;
-    const int b = tid * per, e = min(n + 1, b + per);
-    long long loc = 0;
-    for (int i = b; i < e; i++) loc += i < n ? in[i] : 0;
-    long long inc = loc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const long long y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    if (lane == 31) s_w[warp] = inc;
-    __syncthreads();
-    long long run = inc - loc;
-    for (int k = 0; k < warp; k++) run += s_w[k];
-    for (int i = b; i < e; i++) { out[i] = run; run += i < n ? in[i] : 0; }
 }
 
 double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }

@@ -90,6 +90,7 @@ struct gl_ctx {
     int force_path = kPathNone;
     gl_md_ep md_ep;                         // the tile core's multidepth epilogue for the next reduce (mode 0: none)
     void* md = nullptr;                     // multidepth.cu state (gl_multidepth_begin)
+    void* cs = nullptr;                     // covstats.cu state (gl_bam_covstats): batch buffers and the last call's samples
     // a packed8 batch that is the region's only batch stays packed: K_fused8 reads it as it is (kPathPacked8); it is
     // unpacked into the store (its batch descriptor already points there) only when something needs int32 arrays
     struct { const int* anchors = nullptr; const void* ds = nullptr; const void* len = nullptr; int64_t n_blocks = 0, store_off = 0;
@@ -161,6 +162,10 @@ int depth_resolve(gl_ctx* ctx);
 int depth_reduce_epilogue(gl_ctx* ctx, int32_t* d_depth_out);
 // multidepth.cu: release ctx->md (gl_ctx_destroy)
 void md_free(gl_ctx* ctx);
+// covstats.cu: release ctx->cs (gl_ctx_destroy)
+void cs_free(gl_ctx* ctx);
+// indexcov.cu: bincount_kernel over device values into a device histogram of hi - lo bins (zeroed first), queued on ctx->stream
+__attribute__((visibility("hidden"))) int gl_bincount_device(gl_ctx* ctx, const int32_t* d_v, int64_t n, int32_t lo, int32_t hi, unsigned long long* d_hist);
 
 #define GL_CUDA(ctx, expr)                                                             \
     do {                                                                               \

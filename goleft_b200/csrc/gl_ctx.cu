@@ -192,6 +192,7 @@ int gl_ctx_destroy(gl_ctx* ctx) {
     cudaDeviceSynchronize();
     if (ctx->nccl) gl_comm_destroy(ctx);
     md_free(ctx);
+    cs_free(ctx);
     buf_free(ctx->diff); buf_free(ctx->win_min);
     buf_free(ctx->run_start); buf_free(ctx->run_class); buf_free(ctx->scratch);
     buf_free(ctx->run_tmp_start); buf_free(ctx->run_tmp_class);

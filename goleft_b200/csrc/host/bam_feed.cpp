@@ -453,15 +453,14 @@ std::string bam_decode_segments(const std::string& path, int min_mapq, int threa
 }
 
 // covstats reads the stored CIGAR: the reference reads BAM through biogo/hts, whose handling of CG is not established
-std::string bam_covstats_sample(const std::string& path, int n, int skip, BamHeader& hdr, CovstatsSample& o) {
-    BamFile f;
-    const std::string err = f.open(path, false);
-    if (!err.empty()) return err;
-    hdr = f.header;
+std::string bam_covstats_sample(BamFile& f, int n, int skip, CovstatsSample& o) {
+    o = CovstatsSample();
+    if (n <= 0) return "";                                                     // :138 is false at once: nothing is sampled
     int64_t seen = 0;
     return f.stream(0, [&](const uint8_t* r, uint32_t size) {
-        if (seen++ < skip) return true;                                        // covstats.go:128-134
+        if (seen++ < skip) { o.n_read = seen; return true; }                   // covstats.go:128-134
         if ((int64_t)o.insert.size() >= n) return false;                       // :138
+        o.n_read = seen;
         const int32_t pos = rdi32(r + 4);
         const uint8_t l_name = r[8];
         const uint16_t n_cig = rd16(r + 12), flag = rd16(r + 14);

@@ -54,6 +54,8 @@ public:
     std::string stream(int threads, const std::function<bool(const uint8_t*, uint32_t)>& fn);
     int fd() const { return fd_; }
     int64_t file_size() const { return size_; }
+    int64_t rec_member() const { return rec_member_; }
+    uint32_t rec_skip() const { return rec_skip_; }
 private:
     int fd_ = -1;
     int64_t size_ = 0;
@@ -74,10 +76,11 @@ std::string bam_read_header(const std::string& path, BamHeader& out);
 struct CovstatsSample {
     std::vector<int32_t> read_len, insert, tmpl;
     int64_t n_unmapped = 0, k = 0, n_bad = 0, n_dup = 0, n_proper = 0;
+    int64_t n_read = 0;                          // records up to and including the last one looked at, the skipped ones too
 };
-std::string bam_covstats_sample(const std::string& path, int n, int skip, BamHeader& hdr, CovstatsSample& out);
+std::string bam_covstats_sample(BamFile& f, int n, int skip, CovstatsSample& out);
 
 }  // namespace glhts
 
 // the C ABI's opaque BAM handle (feeder_api.cpp, bamgpu.cu)
-struct gl_bam { glhts::BamFile f; glhts::ContigSegs segs; };
+struct gl_bam { glhts::BamFile f; glhts::ContigSegs segs; glhts::CovstatsSample cs; };

@@ -847,6 +847,20 @@ __global__ void __launch_bounds__(256) indexsplit_sum_kernel(const long long* __
 
 }  // namespace
 
+// hist[x - lo] = how many of the n device values equal x, for x in [lo, hi); queued on ctx->stream
+int gl_bincount_device(gl_ctx* ctx, const int32_t* d_v, int64_t n, int32_t lo, int32_t hi, unsigned long long* d_hist) {
+    GL_CUDA(ctx, cudaMemsetAsync(d_hist, 0, (size_t)((int64_t)hi - lo) * 8, ctx->stream));
+    if (n) {
+        const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
+        {
+            gl_prof_scope prof(ctx, "bincount_kernel");
+            bincount_kernel<<<grid, 256, 0, ctx->stream>>>(d_v, n, lo, hi, d_hist);
+        }
+        GL_LAUNCHED(ctx, 1);
+    }
+    return GL_OK;
+}
+
 extern "C" {
 
 int gl_indexcov_sizes(gl_ctx* ctx, const uint64_t* voff, const int64_t* ref_ptr, int32_t n_refs, int64_t* sizes,
@@ -1150,15 +1164,7 @@ int gl_bincount_i32(gl_ctx* ctx, const int32_t* v, int64_t n, int32_t lo, int32_
     int32_t* d_v; unsigned long long* d_hist;
     GL_CHECK(tmp.upload(d_v, v, (size_t)n));
     GL_CHECK(tmp.alloc(d_hist, (size_t)nb));
-    GL_CUDA(ctx, cudaMemsetAsync(d_hist, 0, (size_t)nb * 8, ctx->stream));
-    if (n) {
-        const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)ctx->sm_count * 8);
-        {
-            gl_prof_scope prof(ctx, "bincount_kernel");
-            bincount_kernel<<<grid, 256, 0, ctx->stream>>>(d_v, n, lo, hi, d_hist);
-        }
-        GL_LAUNCHED(ctx, 1);
-    }
+    GL_CHECK(gl_bincount_device(ctx, d_v, n, lo, hi, d_hist));
     GL_CUDA(ctx, cudaMemcpyAsync(hist, d_hist, (size_t)nb * 8, cudaMemcpyDeviceToHost, ctx->stream));
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return GL_OK;

@@ -689,8 +689,49 @@ int  gl_cnveval_device(gl_ctx* ctx, int32_t S, const int64_t* d_c_ptr, int64_t n
  * V2: histogram of int32 values in [lo,hi) -> hist[v-lo].  `goleft covstats` builds it over the sampled insert sizes,
  * template lengths and read lengths and reads every order statistic of covstats/covstats.go:57-76,175-199 off its running
  * count (k-th smallest = a search, madFilter's cut = a count) and feeds meanStd (:78-89) the values in ascending order
- * with multiplicity — no host sort (cli/goleft.cpp SortedCounts).  Any lo < hi: up to 2^32 - 1 bins. */
+ * with multiplicity — no host sort (csrc/host/covstats.h SortedCounts).  Any lo < hi: up to 2^32 - 1 bins. */
 int  gl_bincount_i32(gl_ctx* ctx, const int32_t* v, int64_t n, int32_t lo, int32_t hi, uint64_t* hist);
+
+/* covstats.BamStats(br, n, skip) (covstats/covstats.go:122-220): every field of the reference's Stats, the counters behind
+ * the proportions, and H, the template-length histogram smoove hands to lumpy (H[j] is the share of the MAD-filtered
+ * template lengths equal to max_read_length + j).  The records are read in file order from the first; record i < skip is
+ * ignored, and the sample ends at the first of: the record that brings the inserts to n, the (2n+1)-th record that gave a
+ * read length while there is still no insert, end of file. */
+typedef struct {
+    double insert_mean, insert_sd, template_mean, template_sd, read_length_mean, read_length_median;
+    double proportion_bad, proportion_unmapped, proportion_properly_paired, proportion_duplicate;
+    int32_t insert_pct5, insert_pct95, max_read_length;
+    int32_t path;                 /* 1: sampled on the device, 0: on the host */
+    int64_t n_unmapped, k, n_bad, n_dup, n_proper;      /* covstats.go's nUnmapped, k, nBad and the two numerators */
+    int64_t n_read_len, n_insert; /* len(sizes), len(insertSizes) = len(templateLengths) */
+    int64_t n_records_read;       /* records up to and including the last one looked at, the skipped ones too */
+    int64_t h_len;                /* len(H) */
+    int64_t bytes_in, bytes_out;  /* device route: compressed bytes uploaded, bytes inflated */
+    /* seconds.  Device route: read = pread not hidden behind device work, inflate .. cut = device time of the phases (CUDA
+     * events).  Host route: read_s is read + inflate + the record walk together.  tail_s: histograms + the Stats arithmetic. */
+    double read_s, inflate_s, index_s, fields_s, cut_s, tail_s, wall_s;
+    int32_t n_batches, _pad;
+} gl_covstats;
+
+/* Sampled on the device: BGZF inflate, record index, per-record fields, cut + compaction and the three histograms are
+ * kernels; only compressed bytes go up and only histograms and counters come back.  H receives h_len doubles; when
+ * h_cap is smaller the call returns GL_ERANGE with out->h_len set (call again with room).  GL_ESTATE: this file cannot be
+ * sampled on the device (no index, a BGZF member the device rejects, index offsets that do not land on records, a large
+ * unplaced tail): call gl_bam_covstats_host.  GL_EINVAL with out->n_insert of 1 or 2, and GL_ERANGE with a message about
+ * H's length, are the two places the reference panics. */
+int  gl_bam_covstats(gl_ctx* ctx, gl_bam* b, int32_t n, int32_t skip, gl_covstats* out, double* H, int64_t h_cap);
+/* The last gl_bam_covstats on this ctx: its samples in file order, on the device (out->n_read_len, n_insert, n_insert
+ * values), valid until the next call. */
+int  gl_bam_covstats_samples(gl_ctx* ctx, const int32_t** d_read_len, const int32_t** d_insert, const int32_t** d_tmpl);
+/* The same from the host sampler (one thread walks the records, the library's pool inflates).  ctx may be NULL: then the
+ * order statistics come from sorted arrays instead of device histograms, with the same results. */
+int  gl_bam_covstats_host(gl_ctx* ctx, gl_bam* b, int32_t n, int32_t skip, gl_covstats* out, double* H, int64_t h_cap);
+/* ... and its samples in file order (host memory owned by the handle, valid until its next gl_bam_covstats_host). */
+int  gl_bam_covstats_host_samples(gl_bam* b, const int32_t** read_len, const int32_t** insert, const int32_t** tmpl);
+/* covstats.go:175-218 alone: host sample arrays and the five counters already in *io -> the rest of *io and H.  ctx may
+ * be NULL as above. */
+int  gl_covstats_tail(gl_ctx* ctx, const int32_t* read_len, int64_t n_read_len, const int32_t* insert, int64_t n_insert, const int32_t* tmpl,
+                      int64_t n_tmpl, gl_covstats* io, double* H, int64_t h_cap);
 
 /* ---------------------------------------------------------------- depthwed
  * W1: depthwed/depthwed.go:93-157.  means: S samples x R rows (sample-major) of the float64 4th BED

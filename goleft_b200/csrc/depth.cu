@@ -544,7 +544,8 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
             if (idx0 == 0) mask |= 1u;                        // the region's first base always starts a run
             if (tile_has_break) {
                 const unsigned a = (unsigned)p.rs + (unsigned)idx0;
-#pragma unroll
+                // rare (one tile in 2441 at 10 Mb): unrolled, its 32 divisions were the register peak of every kernel here
+#pragma unroll 1
                 for (int k = 0; k < BPT; k++)
                     if ((a + k) % p.run_break == 0) mask |= 1u << k;
             }
@@ -1112,25 +1113,30 @@ constexpr int kF8Warps = kF8Threads / 32;
 constexpr int kF8BPT = kTile / kF8Threads;          // 32
 constexpr int kF8BlocksPerPass = kF8Threads / 16;   // a block is 16 lanes x 4 slots
 
-// one segment [s, s+len) into the tile that starts at t0, in tile-relative coordinates a = s - t0, b = a + len:
-//   +1 at a when a is inside the tile, carried in when the segment starts before the tile and reaches it (a < 0 <= b:
-//   it covers base t0-1 or ends exactly at t0 — then its -1 lands on base 0 and cancels the carry);  -1 at b when inside.
+// K_fused8's tile buffer has a guard band of kF8Guard entries on either side of the tile: s_tile[-32, 0) is the lead
+// guard, s_tile[4096, 4128) the trailing one.  swz_elem_t<32> maps each guard onto itself (it XORs bits 2-4 with bits 5-7,
+// which are 7 for [-32, 0) and 0 for [4096, 4128)), so one address expression covers the whole buffer.
+constexpr int kF8Guard = 32;
+
+// One segment [s, s+len) into the tile that starts at t0, in tile-relative coordinates a = s - t0, b = a + len: +1 at
+// clamp(a) and -1 at clamp(b), where clamp() moves a position before the tile to this lane's slot of the lead guard
+// (lane - 32) and one at or past the tile's end to its slot of the trailing guard (4096 + lane):
+//   - a segment that ends before the tile puts both events in the lead guard, which adds 0 to the guard's sum;
+//   - a segment with a < 0 <= b puts +1 in the lead guard and -1 at b (on base 0 when it ends exactly at t0, as the
+//     carry then cancels there), so the lead guard sums to the depth carried into the tile;
+//   - starts and ends at or past the tile's end land in the trailing guard, which is never read;
+//   - a filler slot (len 0) and a thread past the tile's block range (all zero) add +1 and -1 at the same address.
 // A start before the region (first tile) is a carry like any other: the region's first base starts a run regardless, so
 // the depth "before" it is never looked at.  Starts / ends beyond the region end fall in the masked tail of the last tile.
 // `if (p) atomicAdd(smem, v)` compiles to a divergent region per atomic (BSSY / BRA / address math / ATOMS / BSYNC, ~15
-// instructions; ptxas does the same to a predicated `red.shared`).  Adding ZERO at an always-valid address instead keeps the
-// warp converged: the position is masked into the tile, the value is the predicate (+1 / -1 or 0), the atomic is
-// unconditional — 7 instructions per event, and the eight atomics of a thread interleave freely.  (The same
-// change made K_fused slower — a quarter of its 1024 register slots per tile are idle and would add zeros — so it keeps
-// the branches.)
-__device__ __forceinline__ void fused_apply32(int* s_tile, int a, int len, int& carry) {
-    const int b = a + len;
-    const bool live = len != 0;                             // 0 = filler / empty slot
-    const int va = (live & ((unsigned)a < (unsigned)kTile)) ? 1 : 0;
-    const int vb = (live & ((unsigned)b < (unsigned)kTile)) ? -1 : 0;
-    atomicAdd(s_tile + swz_elem_t<kF8BPT>(a & (kTile - 1)), va);
-    carry += (live & (a < 0) & (b >= 0)) ? 1 : 0;
-    atomicAdd(s_tile + swz_elem_t<kF8BPT>(b & (kTile - 1)), vb);
+// instructions; ptxas does the same to a predicated `red.shared`), so every event is one unconditional atomic at an
+// always-valid address: no predicate, no value select, no carry count, and the eight atomics of a thread interleave
+// freely.  Per-lane guard slots keep a warp's clamped events conflict-free.  (Adding zeros at masked positions instead of
+// branching made K_fused slower — a quarter of its 1024 register slots per tile are idle — so it keeps the branches.)
+__device__ __forceinline__ void fused_apply32(int* s_tile, int a, int len, int lane) {
+    const int lo = lane - kF8Guard, hi = kTile + lane;
+    atomicAdd(s_tile + swz_elem_t<kF8BPT>(min(max(a, lo), hi)), 1);
+    atomicAdd(s_tile + swz_elem_t<kF8BPT>(min(max(a + len, lo), hi)), -1);
 }
 
 // thread (tid) takes slots 4*(tid&15)..+3 of block lo + (tid>>4) + 8*pass
@@ -1145,8 +1151,8 @@ __device__ __forceinline__ P8Regs fused8_load(const ScanParams& p, int lo, int h
     return r;
 }
 
-__device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t0, int& carry) {
-    const int sub = threadIdx.x & 15;
+__device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t0) {
+    const int sub = threadIdx.x & 15, lane = threadIdx.x & 31;
     const int d0 = r.d & 0xff, d1 = d0 + ((r.d >> 8) & 0xff), d2 = d1 + ((r.d >> 16) & 0xff), d3 = d2 + (r.d >> 24);
     int inc = d3;
 #pragma unroll
@@ -1155,27 +1161,30 @@ __device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t
         if (sub >= o) inc += v;
     }
     if (__ballot_sync(kFull, r.l != 0) == 0) return;        // no live slot in the whole warp (warp-uniform: no divergence)
-    // tile-relative start of the slot before this thread's first; a thread without a live slot adds zeros at addresses of its own
-    const int base = r.l != 0 ? r.anchor + inc - d3 - t0 : (int)threadIdx.x;
-    fused_apply32(s_tile, base + d0, (int)(r.l & 0xff), carry);
-    fused_apply32(s_tile, base + d1, (int)((r.l >> 8) & 0xff), carry);
-    fused_apply32(s_tile, base + d2, (int)((r.l >> 16) & 0xff), carry);
-    fused_apply32(s_tile, base + d3, (int)(r.l >> 24), carry);
+    const int base = r.anchor + inc - d3 - t0;              // tile-relative start of the slot before this thread's first
+    fused_apply32(s_tile, base + d0, (int)(r.l & 0xff), lane);
+    fused_apply32(s_tile, base + d1, (int)((r.l >> 8) & 0xff), lane);
+    fused_apply32(s_tile, base + d2, (int)((r.l >> 16) & 0xff), lane);
+    fused_apply32(s_tile, base + d3, (int)(r.l >> 24), lane);
 }
 
 // K_fused8: persistent, software-pipelined like K_fused: while tile n runs its core, the packed words of tile n+1 (two
 // passes = 16 blocks, what a 30x tile needs) and the block range of tile n+2 are in flight.  The core keeps its depth
 // slice in s_tile (16 KB less shared memory than a separate slice buffer), so a barrier at the top of each tile holds
-// every warp until all have cleared their regions.
+// every warp until all have cleared their regions.  Segments are added into a guard-banded tile (fused_apply32); after the
+// second barrier warp 0 turns the lead guard into the carry (s_carry[0]; the other warps' entries stay 0) and clears it.
 template <bool kMD>
 __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanParams p) {
-    __shared__ __align__(16) int s_tile[kTile];
+    __shared__ __align__(16) int s_buf[kF8Guard + kTile + kF8Guard];
     __shared__ int s_carry[kF8Warps];
+    int* const s_tile = s_buf + kF8Guard;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = gridDim.x;
     if (p.header[3] != 0) return;                           // K_tileidx8 found unsorted anchors: the host falls back
 #pragma unroll
     for (int j = 0; j < kF8BPT / 4; j++) reinterpret_cast<int4*>(s_tile)[tid * (kF8BPT / 4) + j] = make_int4(0, 0, 0, 0);   // later tiles: cleared by the core
+    if (tid < 2 * kF8Guard) s_buf[tid < kF8Guard ? tid : kTile + tid] = 0;   // the lead guard is cleared again after each tile's read
+    if (tid < kF8Warps) s_carry[tid] = 0;
     int tile = p.tile_begin + blockIdx.x;
     const int nb = p.p8_nblocks;                            // (clamps: garbage ranges of a rejected input stay in bounds)
     int lo = 0, hi = 0, lo2 = 0, hi2 = 0;
@@ -1187,14 +1196,16 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
     for (; tile < p.tile_end; tile += G) {
         __syncthreads();                                    // every warp has cleared its region of s_tile
         const int t0 = p.rs + tile * kTile;
-        int carry = 0;
-        fused8_apply(regs0, s_tile, t0, carry);
-        fused8_apply(regs1, s_tile, t0, carry);
+        fused8_apply(regs0, s_tile, t0);
+        fused8_apply(regs1, s_tile, t0);
         for (int pass = 2; lo + kF8BlocksPerPass * pass < hi; pass++)     // deep tiles only (uniform trip count)
-            fused8_apply(fused8_load(p, lo, hi, pass), s_tile, t0, carry);
-        carry = __reduce_add_sync(kFull, carry);
-        if (lane == 0) s_carry[warp] = carry;
+            fused8_apply(fused8_load(p, lo, hi, pass), s_tile, t0);
         __syncthreads();
+        if (warp == 0) {                                    // the core reads s_carry after its own barrier
+            const int carry = __reduce_add_sync(kFull, s_tile[lane - kF8Guard]);
+            s_tile[lane - kF8Guard] = 0;                    // the next tile's atomics wait at the barrier at the loop's top
+            if (lane == 0) s_carry[0] = carry;
+        }
         lo = lo2; hi = hi2;
         regs0 = fused8_load(p, lo, hi, 0);                  // next tile's packed words: in flight during the core
         regs1 = fused8_load(p, lo, hi, 1);

@@ -1919,15 +1919,18 @@ static int cmd_indexsplit(int argc, char** argv) {
 // multidepth/multidepth.go: blocks of one chromosome where more than --minsamples of the BAMs reach --mincov, with every
 // sample's mean depth.  Two passes over each sample's segments on the GPU (counts, then block sums); the segments are
 // decoded once and kept in their compact form in between (packed8 words, or the GPU feeder's int32 copied to pinned memory).
-// The output is the reference's with -p 1 (chunks in order).
+// With --gpus, each worker (one gl_ctx per GPU) counts its own range of samples; worker 0 merges the others' per-base
+// counters (gl_multidepth_merge) and finds the sites, and every worker sums its samples against the same blocks.
+// The output is the reference's with -p 1 (chunks in order), whatever the number of workers.
 static int cmd_multidepth(int argc, char** argv) {
     std::string q = "10", chrom, mincov = "7", maxcov = "1000", maxskip = "10", minsize = "15", window = "10000000", procs = "0",
-                minsamples = "0.5";
+                minsamples = "0.5", gpus = "0";
     ArgParser ap;
     ap.prog = "goleft multidepth";
     ap.add("q", 'Q', &q); ap.add("chrom", 'c', &chrom, true); ap.add("mincov", 0, &mincov); ap.add("maxcov", 0, &maxcov);
     ap.add("maxskip", 'k', &maxskip); ap.add("minsize", 'm', &minsize); ap.add("window", 'w', &window); ap.add("processes", 'p', &procs);
     ap.add("minsamples", 0, &minsamples);
+    ap.add("gpus", 0, &gpus);                       // extension: GPUs to use (0 = every visible one); samples are sharded over them
     ap.parse(argc, argv);
     if (ap.positional.empty()) ap.fail("bams is required");
     const std::vector<std::string>& bams = ap.positional;
@@ -1946,56 +1949,89 @@ static int cmd_multidepth(int argc, char** argv) {
         for (size_t r = 0; r < refs.size(); r++) if (refs[r].name == chrom) { tid[(size_t)i] = (int)r; if (i == 0) L = refs[r].length; }
         if (tid[(size_t)i] < 0) fatal(2, "panic: multidepth: chromosome %s not found in %s", chrom.c_str(), bams[(size_t)i].c_str());
     }
-    gl_ctx* ctx = open_ctx(0, "goleft multidepth");
-    if (L <= 0) { printf("%s\n", hdr.c_str()); gl_ctx_destroy(ctx); return 0; }
-    glck(ctx, gl_multidepth_begin(ctx, L, S, atoi(mincov.c_str()), atof(minsamples.c_str())), "goleft multidepth");
+    // --gpus: the samples in contiguous ranges, one per worker, balanced by each sample's compressed bytes of the contig (the
+    // linear-index offsets of its first and last tile), or by file size without an index.  Any split prints the same bytes.
+    const GpuPlan gp = resolve_gpus(gpus, (size_t)S, "goleft multidepth");
+    if (L <= 0) { printf("%s\n", hdr.c_str()); return 0; }
+    std::vector<int> lo((size_t)gp.G + 1, S);
+    {
+        std::vector<double> pre((size_t)S + 1, 0.0);
+        for (int i = 0; i < S; i++) {
+            const glhts::BamFile& f = bam[(size_t)i].f;
+            double w = -1;
+            if (f.has_index && tid[(size_t)i] < (int)f.bai.ioffsets.size()) {
+                uint64_t a = 0, b = 0;
+                for (uint64_t v : f.bai.ioffsets[(size_t)tid[(size_t)i]]) if (v) { if (!a) a = v; b = v; }
+                if (a) w = (double)((b >> 16) - (a >> 16) + 1);
+            }
+            if (w < 0) { struct stat sb; w = stat(bams[(size_t)i].c_str(), &sb) == 0 ? (double)sb.st_size : 1.0; }
+            pre[(size_t)i + 1] = pre[(size_t)i] + std::max(w, 1.0);
+        }
+        lo[0] = 0;
+        for (int g = 1; g < gp.G; g++) {
+            const double target = pre[(size_t)S] * g / gp.G;
+            int i = lo[(size_t)g - 1] + 1;
+            while (i < S - (gp.G - g) && pre[(size_t)i] < target) i++;
+            lo[(size_t)g] = i;
+        }
+    }
+    const int mc = atoi(mincov.c_str());
+    const double ms = atof(minsamples.c_str());
     std::vector<SegSource> smp((size_t)S);
     std::vector<glhts::SegmentSet> whole((size_t)S);
-    std::vector<void*> pinned;
+    std::vector<gl_ctx*> ctx((size_t)gp.G, nullptr);
+    std::vector<std::vector<void*>> pinned((size_t)gp.G);
     // sample i's segments of the contig: without an index, a whole-file decode of that one reference; otherwise the GPU feeder
     // when it can, else the host feeder.  A sample that stays on the host is decoded on a helper thread beside the GPU work
     // of sample i-1.
     auto stays_on_host = [&](int i) { return !(SegSource::gpu_feed() && bam[(size_t)i].f.has_index); };
-    auto fetch = [&](int i) {
+    auto fetch = [&](gl_ctx* c, int i) {
         const size_t k = (size_t)i;
         if (!bam[k].f.has_index) {
             std::string e = glhts::bam_decode_segments(bams[k], Q, threads > 0 ? threads : 8, tid[k], whole[k]);
             if (!e.empty()) fatal(1, "%s", e.c_str());
             smp[k].whole = &whole[k];
         }
-        smp[k].fetch(ctx, bam[k], tid[k], 0, L, Q, threads, 0, true, nullptr, nullptr);
+        smp[k].fetch(c, bam[k], tid[k], 0, L, Q, threads, 0, true, nullptr, nullptr);
     };
-    // pass 1
-    std::thread next;
-    bool next_host = false;
-    for (int i = 0; i < S; i++) {
-        SegSource& m = smp[(size_t)i];
-        if (next.joinable()) next.join();
-        if (!next_host) fetch(i);
-        next_host = i + 1 < S && stays_on_host(i + 1);
-        if (next_host) next = std::thread(fetch, i + 1);
-        glck(ctx, gl_depth_begin(ctx, 0, L), "gl_depth_begin");
-        m.add(ctx);
-        glck(ctx, gl_multidepth_count(ctx), "gl_multidepth_count");
-        if (m.on_device) {                          // pass 2 needs the feeder's arrays after the next decode reuses them
-            void* p = nullptr;
-            glck(ctx, gl_host_alloc_pinned(ctx, std::max<int64_t>(m.n, 1) * 8, &p), "gl_host_alloc_pinned");
-            pinned.push_back(p);
-            int32_t* pin = static_cast<int32_t*>(p);
-            if (m.n > 0) {
-                glck(ctx, gl_memcpy_d2h(ctx, pin, m.s, m.n * 4), "gl_memcpy_d2h");
-                glck(ctx, gl_memcpy_d2h(ctx, pin + m.n, m.e, m.n * 4), "gl_memcpy_d2h");
-            }
-            m.view(pin, pin + m.n, m.n);
-        }
-    }
-    if (next.joinable()) next.join();
-    // blocks
+    // pass 1, per worker over its samples
+    for (std::thread& t : start_workers(gp, [&](int g) {
+             gl_ctx* c = ctx[(size_t)g] = open_ctx(g % gp.n_dev, "goleft multidepth");
+             glck(c, gl_multidepth_begin(c, L, S, mc, ms), "goleft multidepth");
+             const int i0 = lo[(size_t)g], i1 = lo[(size_t)g + 1];
+             std::thread next;
+             bool next_host = false;
+             for (int i = i0; i < i1; i++) {
+                 SegSource& m = smp[(size_t)i];
+                 if (next.joinable()) next.join();
+                 if (!next_host) fetch(c, i);
+                 next_host = i + 1 < i1 && stays_on_host(i + 1);
+                 if (next_host) next = std::thread(fetch, c, i + 1);
+                 glck(c, gl_depth_begin(c, 0, L), "gl_depth_begin");
+                 m.add(c);
+                 glck(c, gl_multidepth_count(c), "gl_multidepth_count");
+                 if (m.on_device) {                  // pass 2 needs the feeder's arrays after the next decode reuses them
+                     void* p = nullptr;
+                     glck(c, gl_host_alloc_pinned(c, std::max<int64_t>(m.n, 1) * 8, &p), "gl_host_alloc_pinned");
+                     pinned[(size_t)g].push_back(p);
+                     int32_t* pin = static_cast<int32_t*>(p);
+                     if (m.n > 0) {
+                         glck(c, gl_memcpy_d2h(c, pin, m.s, m.n * 4), "gl_memcpy_d2h");
+                         glck(c, gl_memcpy_d2h(c, pin + m.n, m.e, m.n * 4), "gl_memcpy_d2h");
+                     }
+                     m.view(pin, pin + m.n, m.n);
+                 }
+             }
+             if (next.joinable()) next.join();
+         }))
+        t.join();
+    // worker 0 adds up every worker's counts, then the blocks
+    if (gp.G > 1) glck(ctx[0], gl_multidepth_merge(ctx[0], ctx.data() + 1, gp.G - 1), "gl_multidepth_merge");
     int64_t nr = 0;
-    glck(ctx, gl_multidepth_sites(ctx, nullptr, nullptr, 0, &nr), "gl_multidepth_sites");
+    glck(ctx[0], gl_multidepth_sites(ctx[0], nullptr, nullptr, 0, &nr), "gl_multidepth_sites");
     std::vector<int32_t> rs((size_t)std::max<int64_t>(nr, 1));
     std::vector<uint8_t> rc((size_t)std::max<int64_t>(nr, 1));
-    glck(ctx, gl_multidepth_sites(ctx, rs.data(), rc.data(), nr, &nr), "gl_multidepth_sites");
+    glck(ctx[0], gl_multidepth_sites(ctx[0], rs.data(), rc.data(), nr, &nr), "gl_multidepth_sites");
     const int64_t max_skip = atoll(maxskip.c_str()), min_size = atoll(minsize.c_str()), win = atoll(window.c_str());
     int64_t nb = 0;
     if (gl_multidepth_blocks(rs.data(), rc.data(), nr, L, S, 0, max_skip, min_size, win, nullptr, nullptr, nullptr, 0, &nb) != GL_OK)
@@ -2003,18 +2039,33 @@ static int cmd_multidepth(int argc, char** argv) {
     std::vector<int64_t> bs((size_t)std::max<int64_t>(nb, 1)), be(bs.size()), bn(bs.size());
     if (gl_multidepth_blocks(rs.data(), rc.data(), nr, L, S, 0, max_skip, min_size, win, bs.data(), be.data(), bn.data(), nb, &nb) != GL_OK)
         fatal(1, "gl_multidepth_blocks failed");
-    glck(ctx, gl_multidepth_set_blocks(ctx, bs.data(), be.data(), bn.data(), nb), "gl_multidepth_set_blocks");
-    // pass 2
-    for (int i = 0; i < S; i++) {
-        glck(ctx, gl_depth_begin(ctx, 0, L), "gl_depth_begin");
-        smp[(size_t)i].add(ctx);
-        glck(ctx, gl_multidepth_sums(ctx, i), "gl_multidepth_sums");
-    }
+    // pass 2: every other worker takes worker 0's sites; the samples keep their cohort numbers
+    for (std::thread& t : start_workers(gp, [&](int g) {
+             gl_ctx* c = ctx[(size_t)g];
+             if (g > 0) glck(c, gl_multidepth_adopt_sites(c, ctx[0]), "gl_multidepth_adopt_sites");
+             glck(c, gl_multidepth_set_blocks(c, bs.data(), be.data(), bn.data(), nb), "gl_multidepth_set_blocks");
+             for (int i = lo[(size_t)g]; i < lo[(size_t)g + 1]; i++) {
+                 glck(c, gl_depth_begin(c, 0, L), "gl_depth_begin");
+                 smp[(size_t)i].add(c);
+                 glck(c, gl_multidepth_sums(c, i), "gl_multidepth_sums");
+             }
+         }))
+        t.join();
     const size_t cells = (size_t)nb * (size_t)S;
     std::vector<int64_t> qv(std::max<size_t>(cells, 1));
     std::vector<double> val(qv.size());
     std::vector<uint8_t> cert(qv.size());
-    glck(ctx, gl_multidepth_result(ctx, nullptr, qv.data(), val.data(), cert.data()), "gl_multidepth_result");
+    glck(ctx[0], gl_multidepth_result(ctx[0], nullptr, qv.data(), val.data(), cert.data()), "gl_multidepth_result");
+    if (gp.G > 1) {                                 // each sample's columns from the worker that summed it
+        std::vector<int64_t> tq(qv.size());
+        std::vector<double> tv(qv.size());
+        std::vector<uint8_t> tc(qv.size());
+        for (int g = 1; g < gp.G; g++) {
+            glck(ctx[(size_t)g], gl_multidepth_result(ctx[(size_t)g], nullptr, tq.data(), tv.data(), tc.data()), "gl_multidepth_result");
+            for (size_t r = 0; r < (size_t)nb; r++)
+                for (size_t k = r * S + lo[(size_t)g]; k < r * S + lo[(size_t)g + 1]; k++) { qv[k] = tq[k]; val[k] = tv[k]; cert[k] = tc[k]; }
+        }
+    }
     char* text = nullptr;
     int64_t tl = 0;
     if (gl_multidepth_text(chrom.c_str(), bs.data(), be.data(), nb, S, qv.data(), val.data(), cert.data(), threads, &text, &tl) != GL_OK)
@@ -2022,8 +2073,10 @@ static int cmd_multidepth(int argc, char** argv) {
     printf("%s\n", hdr.c_str());
     fwrite(text, 1, (size_t)tl, stdout);
     gl_free_text(text);
-    for (void* p : pinned) gl_host_free_pinned(ctx, p);
-    gl_ctx_destroy(ctx);
+    for (int g = 0; g < gp.G; g++) {
+        for (void* p : pinned[(size_t)g]) gl_host_free_pinned(ctx[(size_t)g], p);
+        gl_ctx_destroy(ctx[(size_t)g]);
+    }
     return 0;
 }
 

@@ -284,6 +284,26 @@ func (c *Ctx) Multidepth(chrom string, length, samples, minCov int, minSamples f
 	return C.GoBytes(unsafe.Pointer(text), C.int(tl)), nil
 }
 
+// MultidepthMerge adds the pass-1 counters, site bits and counted samples of every src context into c's, for a multidepth
+// run whose samples were counted on several contexts (any devices) begun with the same parameters.  Each src then refuses
+// counts, sites and merges until it adopts c's sites with MultidepthAdoptSites.
+func (c *Ctx) MultidepthMerge(src []*Ctx) error {
+	if len(src) == 0 {
+		return c.err(C.gl_multidepth_merge(c.h, nil, 0))
+	}
+	hs := make([]*C.gl_ctx, len(src))
+	for i, s := range src {
+		hs[i] = s.h
+	}
+	return c.err(C.gl_multidepth_merge(c.h, (**C.gl_ctx)(unsafe.Pointer(&hs[0])), C.int32_t(len(src))))
+}
+
+// MultidepthAdoptSites copies src's site and sufficient bits and class runs into c; src must have run its sites.  c then
+// takes the blocks and sums its own samples (with their cohort numbers) as if it had run its sites itself.
+func (c *Ctx) MultidepthAdoptSites(src *Ctx) error {
+	return c.err(C.gl_multidepth_adopt_sites(c.h, src.h))
+}
+
 // Dcnv replaces GeneralDebiaser.Sort / Debias / Unsort + NormalizeBySampleMedian of dcnv/dcnv.go:329-337 on the
 // n x S row-major depth matrix `depths` (rows in position order; normalised in place), with gcs the GC fraction of each row.
 // The argsort is Go's own sort.Sort order (gl_go_argsort_f64), so floats.Argsort may equally be used.  Returns the sample

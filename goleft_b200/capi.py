@@ -8,6 +8,8 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import time
+from concurrent.futures import ThreadPoolExecutor
 from typing import Optional, Tuple
 
 import numpy as np
@@ -196,6 +198,8 @@ _proto("gl_depth_format_chunk", C.c_int, C.c_char_p, C.c_int64, C.c_int64, C.c_i
 _proto("gl_free_text", None, _vp)
 _proto("gl_multidepth_begin", C.c_int, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_double)
 _proto("gl_multidepth_count", C.c_int, _vp)
+_proto("gl_multidepth_merge", C.c_int, _vp, C.POINTER(_vp), C.c_int32)
+_proto("gl_multidepth_adopt_sites", C.c_int, _vp, _vp)
 _proto("gl_multidepth_sites", C.c_int, _vp, _vp, _vp, C.c_int64, _i64p)
 _proto("gl_multidepth_blocks", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
        _vp, _vp, _vp, C.c_int64, _i64p)
@@ -1435,6 +1439,16 @@ class Ctx:
     def multidepth_count(self):
         self._ck(lib.gl_multidepth_count(self.h))
 
+    def multidepth_merge(self, sources):
+        """Add the pass-1 counters, site bits and counted samples of every context in `sources` (None stands for a null
+        handle) into this one's."""
+        arr = (_vp * max(len(sources), 1))(*[None if s is None else s.h for s in sources])
+        self._ck(lib.gl_multidepth_merge(self.h, arr, len(sources)))
+
+    def multidepth_adopt_sites(self, src):
+        """Copy src's site and sufficient bits and its class runs into this context."""
+        self._ck(lib.gl_multidepth_adopt_sites(self.h, None if src is None else src.h))
+
     def multidepth_sites(self):
         n = C.c_int64(0)
         self._ck(lib.gl_multidepth_sites(self.h, None, None, 0, C.byref(n)))
@@ -1481,6 +1495,76 @@ class Ctx:
             self.multidepth_sums(i)
         _, q, val, ok = self.multidepth_result(bs.size, S)
         return multidepth_text(chrom, bs, be, S, q, val, ok)
+
+    @staticmethod
+    def multidepth_sharded(ctxs, chrom: str, contig_len: int, adders, mincov: int = 7, min_samples: float = 0.5,
+                           max_skip: int = 10, min_size: int = 15, window: int = 10_000_000, chunk: int = 0, parts: bool = False):
+        """The whole tool for one contig with the cohort split over several contexts: adders[k] are context k's samples
+        (adders[k][j](ctx) adds one sample's segments to the open region, once per pass), numbered in context order.  Each
+        context runs its passes on a thread of its own; ctxs[0] merges the others' counts and finds the sites, the host makes
+        the blocks once, every other context adopts ctxs[0]'s sites, and each sample's columns come from its own context.
+        Returns the rows after the header line, or (rows, parts) with parts=True: the runs, blocks, sums / q / val /
+        certified (n_blocks x S), the phase times in ms (pass 2 includes each context's gl_multidepth_result; gather is
+        the host's column copy) and the bytes the merge moved."""
+        if len(ctxs) < 1 or len(ctxs) != len(adders):
+            raise ValueError("multidepth_sharded: one list of adders per context")
+        n = [len(a) for a in adders]
+        S = sum(n)
+        first = [sum(n[:k]) for k in range(len(n))]
+        t = [time.perf_counter()]
+
+        def each(pool, fn):
+            if len(ctxs) == 1:                                  # one context: on the calling thread, as Ctx.multidepth
+                fn(0)
+            else:
+                for f in [pool.submit(fn, k) for k in range(len(ctxs))]:
+                    f.result()
+            t.append(time.perf_counter())
+
+        def pass1(k):
+            c = ctxs[k]
+            c.multidepth_begin(contig_len, S, mincov, min_samples)
+            for add in adders[k]:
+                c.depth_begin(0, contig_len)
+                add(c)
+                c.multidepth_count()
+
+        def pass2(k):
+            c = ctxs[k]
+            if k:
+                c.multidepth_adopt_sites(ctxs[0])
+            c.multidepth_set_blocks(bs, be, bn)
+            for j, add in enumerate(adders[k]):
+                c.depth_begin(0, contig_len)
+                add(c)
+                c.multidepth_sums(first[k] + j)
+            res[k] = c.multidepth_result(bs.size, S)
+
+        res = [None] * len(ctxs)
+        with ThreadPoolExecutor(len(ctxs)) as pool:
+            each(pool, pass1)
+            if len(ctxs) > 1:
+                ctxs[0].multidepth_merge(ctxs[1:])
+            t.append(time.perf_counter())
+            rs, rc = ctxs[0].multidepth_sites()
+            t.append(time.perf_counter())
+            bs, be, bn = multidepth_blocks(rs, rc, contig_len, S, max_skip, min_size, window, chunk)
+            t.append(time.perf_counter())
+            each(pool, pass2)
+        sums, q, val, ok = res[0]                           # each sample's columns from the context that summed it
+        for k in range(1, len(ctxs)):
+            cols = slice(first[k], first[k] + n[k])
+            for dst, src in zip((sums, q, val, ok), res[k]):
+                dst[:, cols] = src[:, cols]
+        t.append(time.perf_counter())
+        rows = multidepth_text(chrom, bs, be, S, q, val, ok)
+        if not parts:
+            return rows
+        words = (contig_len + 4095) // 4096 * 128
+        ms = {k: (t[i + 1] - t[i]) * 1e3 for i, k in enumerate(("pass1", "merge", "sites", "blocks_host", "pass2"))}
+        ms["gather"] = (t[6] - t[5]) * 1e3
+        return rows, dict(runs=(rs, rc), blocks=(bs, be, bn), sums=sums, q=q, val=val, certified=ok, ms=ms,
+                          merge_bytes=(len(ctxs) - 1) * words * 68)
 
     # ---- dcnv
     def dcnv_normalize(self, x: np.ndarray, inds, c0: int = 0, c1: Optional[int] = None, block_cols: int = 0):

@@ -27,8 +27,10 @@ struct MdState {
     int64_t min_samples = 0;
     int32_t counted = 0, summed = 0;
     bool sites_done = false;
+    bool merged = false;                         // pass-1 state given to another context (gl_multidepth_merge)
     int64_t n_runs = 0;
     gl_buf ge, pos, cnt, site, suf, depth, run_s, run_c, cta_cnt, small;
+    gl_buf stage[2];                             // gl_multidepth_merge: a source's chunk, [counters | site bits]
     // blocks
     int64_t nb = 0, n_pairs = 0;
     gl_buf blk, pair_ptr, pair_blk, slots, tmp, sums, q, val, cert, walk_list;
@@ -63,6 +65,27 @@ __global__ void __launch_bounds__(256) md_accum_kernel(const unsigned* __restric
             const int k = 8 * j + 2 * h;
             u[h] += ((g >> k) & 1u) | (((g >> (k + 1)) & 1u) << 16);   // two uint16 counters per word, < 65536: no carry
         }
+        c4[j] = v;
+    }
+}
+
+// one 32-base word per thread: another context's pass-1 state, staged on this device, folded in.  cnt[x] += staged_cnt[x]
+// on the two uint16 counters of each 32-bit lane: every counter is at most the samples its context counted, and the merged
+// contexts count at most S <= 65535 samples together, so no sum carries into the other half.
+__global__ void __launch_bounds__(256) md_merge_kernel(const unsigned short* __restrict__ staged_cnt, const unsigned* __restrict__ staged_site,
+                                                       unsigned short* __restrict__ cnt, unsigned* __restrict__ site, long long words) {
+    const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= words) return;
+    const unsigned p = staged_site[w];
+    if (p) site[w] |= p;
+    const uint4* s4 = reinterpret_cast<const uint4*>(staged_cnt + w * 32);
+    uint4* c4 = reinterpret_cast<uint4*>(cnt + w * 32);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+        const uint4 a = s4[j];
+        if (!(a.x | a.y | a.z | a.w)) continue;
+        uint4 v = c4[j];
+        v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
         c4[j] = v;
     }
 }
@@ -238,6 +261,42 @@ int md_need(gl_ctx* ctx, const char* who) {
     return GL_OK;
 }
 
+// two contexts of one run: begun with the same contig, cohort and thresholds
+bool md_same_run(const MdState* a, const MdState* b) {
+    return a->L == b->L && a->S == b->S && a->mincov == b->mincov && a->min_samples == b->min_samples;
+}
+
+// gl_multidepth_merge's chunk, in 32-base words: GL_MD_MERGE_CHUNK_BASES (rounded up to 32 bases), else 2^24 bases, so the
+// two staging buffers take 2 x 35.7 MB of the destination
+int64_t md_merge_chunk_words() {
+    const char* v = getenv("GL_MD_MERGE_CHUNK_BASES");
+    const long long b = v ? atoll(v) : 0;
+    return b > 0 ? (b + 31) / 32 : (int64_t(1) << 24) / 32;
+}
+
+// events of one call, destroyed on every return path (a pending event is released once it completes)
+struct MdEvents {
+    std::vector<cudaEvent_t> ev;
+    ~MdEvents() { for (cudaEvent_t e : ev) cudaEventDestroy(e); }
+    // a new event on the current device
+    cudaError_t make(cudaEvent_t* e) {
+        const cudaError_t r = cudaEventCreateWithFlags(e, cudaEventDisableTiming);
+        if (r == cudaSuccess) ev.push_back(*e);
+        return r;
+    }
+};
+
+// dst->stream waits for everything queued on src->stream so far (the two may be on different devices)
+int md_after(gl_ctx* dst, gl_ctx* src, cudaStream_t dst_stream, MdEvents& evs) {
+    cudaEvent_t e;
+    GL_CHECK(gl_use(src));
+    GL_CUDA(dst, evs.make(&e));
+    GL_CUDA(dst, cudaEventRecord(e, src->stream));
+    GL_CHECK(gl_use(dst));
+    GL_CUDA(dst, cudaStreamWaitEvent(dst_stream, e, 0));
+    return GL_OK;
+}
+
 // the open depth region must be the whole contig of the multidepth run
 int md_region_ok(gl_ctx* ctx, const char* who) {
     MdState* m = st(ctx);
@@ -253,7 +312,8 @@ void md_free(gl_ctx* ctx) {
     MdState* m = st(ctx);
     if (!m) return;
     for (gl_buf* b : {&m->ge, &m->pos, &m->cnt, &m->site, &m->suf, &m->depth, &m->run_s, &m->run_c, &m->cta_cnt, &m->small, &m->blk,
-                      &m->pair_ptr, &m->pair_blk, &m->slots, &m->tmp, &m->sums, &m->q, &m->val, &m->cert, &m->walk_list})
+                      &m->pair_ptr, &m->pair_blk, &m->slots, &m->tmp, &m->sums, &m->q, &m->val, &m->cert, &m->walk_list,
+                      &m->stage[0], &m->stage[1]})
         md_buf_free(*b);
     delete m;
     ctx->md = nullptr;
@@ -275,7 +335,7 @@ int gl_multidepth_begin(gl_ctx* ctx, int64_t contig_len, int32_t n_samples, int3
     const int64_t tiles = (contig_len + kTileBases - 1) / kTileBases;
     const int64_t bases = tiles * kTileBases;                 // the tile core writes whole tiles
     m->counted = m->summed = 0;
-    m->sites_done = m->blocks_set = false;
+    m->sites_done = m->blocks_set = m->merged = false;
     m->n_runs = m->nb = m->n_pairs = m->walked = m->certified = 0;
     m->L = contig_len; m->words = bases / 32; m->tiles = tiles;
     m->S = n_samples; m->mincov = mincov;
@@ -295,6 +355,7 @@ int gl_multidepth_count(gl_ctx* ctx) {
     GL_CHECK(md_need(ctx, "gl_multidepth_count"));
     GL_CHECK(md_region_ok(ctx, "gl_multidepth_count"));
     MdState* m = st(ctx);
+    if (m->merged) return gl_fail(ctx, GL_ESTATE, "gl_multidepth_count: this context's counts were merged into another; adopt its sites");
     if (m->counted >= m->S) return gl_fail(ctx, GL_ESTATE, "gl_multidepth_count: all %d samples were counted already", m->S);
     gl_md_ep ep;
     ep.mode = 1;
@@ -319,7 +380,9 @@ int gl_multidepth_count(gl_ctx* ctx) {
 int gl_multidepth_sites(gl_ctx* ctx, int32_t* run_start, uint8_t* run_class, int64_t cap, int64_t* n_runs) {
     GL_CHECK(md_need(ctx, "gl_multidepth_sites"));
     MdState* m = st(ctx);
-    if (m->counted != m->S) return gl_fail(ctx, GL_ESTATE, "gl_multidepth_sites: %d of %d samples counted", m->counted, m->S);
+    if (m->merged) return gl_fail(ctx, GL_ESTATE, "gl_multidepth_sites: this context's counts were merged into another; adopt its sites");
+    if (!m->sites_done && m->counted != m->S)      // adopted sites (gl_multidepth_adopt_sites) stand for every sample
+        return gl_fail(ctx, GL_ESTATE, "gl_multidepth_sites: %d of %d samples counted", m->counted, m->S);
     if (!m->sites_done) {
         const long long words = m->words;
         const unsigned ctas = (unsigned)((words + kRunThreads - 1) / kRunThreads);
@@ -368,6 +431,104 @@ int gl_multidepth_sites(gl_ctx* ctx, int32_t* run_start, uint8_t* run_class, int
         if (run_class) GL_CUDA(ctx, cudaMemcpyAsync(run_class, m->run_c.p, (size_t)m->n_runs, cudaMemcpyDeviceToHost, ctx->stream));
     }
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
+}
+
+int gl_multidepth_merge(gl_ctx* dst, gl_ctx* const* src, int32_t n_src) {
+    GL_CHECK(md_need(dst, "gl_multidepth_merge"));
+    MdState* m = st(dst);
+    if (n_src < 0 || (n_src > 0 && !src)) return gl_fail(dst, GL_EINVAL, "gl_multidepth_merge: bad argument");
+    if (m->merged) return gl_fail(dst, GL_ESTATE, "gl_multidepth_merge: the destination's counts were merged into another context");
+    if (m->sites_done) return gl_fail(dst, GL_ESTATE, "gl_multidepth_merge: the destination has run its sites already");
+    int64_t total = m->counted;
+    for (int32_t i = 0; i < n_src; i++) {
+        gl_ctx* c = src[i];
+        if (!c) return gl_fail(dst, GL_EINVAL, "gl_multidepth_merge: source %d is null", i);
+        if (c == dst) return gl_fail(dst, GL_EINVAL, "gl_multidepth_merge: source %d is the destination", i);
+        for (int32_t j = 0; j < i; j++)
+            if (src[j] == c) return gl_fail(dst, GL_EINVAL, "gl_multidepth_merge: source %d repeats source %d", i, j);
+        const MdState* o = st(c);
+        if (!o) return gl_fail(dst, GL_ESTATE, "gl_multidepth_merge: source %d has not called gl_multidepth_begin", i);
+        if (!md_same_run(m, o))
+            return gl_fail(dst, GL_EINVAL, "gl_multidepth_merge: source %d was begun with another contig length, sample count, mincov or minSamples", i);
+        if (o->merged) return gl_fail(dst, GL_ESTATE, "gl_multidepth_merge: source %d was merged already", i);
+        if (o->sites_done) return gl_fail(dst, GL_ESTATE, "gl_multidepth_merge: source %d has run its sites", i);
+        total += o->counted;
+    }
+    if (total > m->S)
+        return gl_fail(dst, GL_ESTATE, "gl_multidepth_merge: %lld samples counted in all, more than the run's %d", (long long)total, m->S);
+    if (n_src == 0) return GL_OK;
+    // Each source's counters and site bits come over in chunks (cudaMemcpyPeerAsync: NVLink, through the host, or within
+    // one device) into two staging buffers on dst's copy stream; md_merge_kernel folds chunk k in on dst's stream while
+    // chunk k + 1 arrives.  ev_copy[b]: staging buffer b holds its chunk; ev_used[b]: the kernel has read it.
+    const int64_t cw = std::min(md_merge_chunk_words(), m->words);
+    for (gl_buf& b : m->stage) GL_CHECK(gl_buf_reserve(dst, b, (size_t)cw * 68));
+    MdEvents evs;
+    cudaEvent_t ev_copy[2], ev_used[2];
+    for (int b = 0; b < 2; b++) {
+        GL_CUDA(dst, evs.make(&ev_copy[b]));
+        GL_CUDA(dst, evs.make(&ev_used[b]));
+    }
+    int64_t k = 0;
+    for (int32_t i = 0; i < n_src; i++) {
+        gl_ctx* c = src[i];
+        const MdState* o = st(c);
+        GL_CHECK(md_after(dst, c, dst->copy_stream, evs));     // the source's last md_accum_kernel
+        for (int64_t off = 0; off < m->words; off += cw, k++) {
+            const int64_t n = std::min(cw, m->words - off);
+            const int b = (int)(k & 1);
+            char* stg = static_cast<char*>(m->stage[b].p);
+            if (k >= 2) GL_CUDA(dst, cudaStreamWaitEvent(dst->copy_stream, ev_used[b], 0));
+            GL_CUDA(dst, cudaMemcpyPeerAsync(stg, dst->device, static_cast<const char*>(o->cnt.p) + off * 64, c->device, (size_t)n * 64,
+                                             dst->copy_stream));
+            GL_CUDA(dst, cudaMemcpyPeerAsync(stg + cw * 64, dst->device, static_cast<const char*>(o->site.p) + off * 4, c->device,
+                                             (size_t)n * 4, dst->copy_stream));
+            GL_CUDA(dst, cudaEventRecord(ev_copy[b], dst->copy_stream));
+            GL_CUDA(dst, cudaStreamWaitEvent(dst->stream, ev_copy[b], 0));
+            {
+                gl_prof_scope prof(dst, "md_merge_kernel");
+                md_merge_kernel<<<(unsigned)((n + 255) / 256), 256, 0, dst->stream>>>(
+                    reinterpret_cast<const unsigned short*>(stg), reinterpret_cast<const unsigned*>(stg + cw * 64),
+                    static_cast<unsigned short*>(m->cnt.p) + off * 32, static_cast<unsigned*>(m->site.p) + off, n);
+            }
+            GL_LAUNCHED(dst, 1);
+            GL_CUDA(dst, cudaEventRecord(ev_used[b], dst->stream));
+        }
+    }
+    GL_CUDA(dst, cudaStreamSynchronize(dst->stream));
+    for (int32_t i = 0; i < n_src; i++) {
+        MdState* o = st(src[i]);
+        m->counted += o->counted;
+        o->merged = true;
+    }
+    return GL_OK;
+}
+
+int gl_multidepth_adopt_sites(gl_ctx* dst, gl_ctx* src) {
+    GL_CHECK(md_need(dst, "gl_multidepth_adopt_sites"));
+    MdState* m = st(dst);
+    if (!src) return gl_fail(dst, GL_EINVAL, "gl_multidepth_adopt_sites: null source");
+    if (src == dst) return gl_fail(dst, GL_EINVAL, "gl_multidepth_adopt_sites: the source is the destination");
+    const MdState* o = st(src);
+    if (!o) return gl_fail(dst, GL_ESTATE, "gl_multidepth_adopt_sites: the source has not called gl_multidepth_begin");
+    if (!md_same_run(m, o))
+        return gl_fail(dst, GL_EINVAL, "gl_multidepth_adopt_sites: the source was begun with another contig length, sample count, mincov or minSamples");
+    if (!o->sites_done) return gl_fail(dst, GL_ESTATE, "gl_multidepth_adopt_sites: the source has not run gl_multidepth_sites");
+    GL_CHECK(gl_buf_reserve(dst, m->run_s, (size_t)std::max<int64_t>(o->n_runs, 1) * 4));
+    GL_CHECK(gl_buf_reserve(dst, m->run_c, (size_t)std::max<int64_t>(o->n_runs, 1)));
+    MdEvents evs;
+    GL_CHECK(md_after(dst, src, dst->stream, evs));           // md_runs_write_kernel may still be queued there
+    GL_CUDA(dst, cudaMemcpyPeerAsync(m->site.p, dst->device, o->site.p, src->device, (size_t)m->words * 4, dst->stream));
+    GL_CUDA(dst, cudaMemcpyPeerAsync(m->suf.p, dst->device, o->suf.p, src->device, (size_t)m->words * 4, dst->stream));
+    if (o->n_runs > 0) {
+        GL_CUDA(dst, cudaMemcpyPeerAsync(m->run_s.p, dst->device, o->run_s.p, src->device, (size_t)o->n_runs * 4, dst->stream));
+        GL_CUDA(dst, cudaMemcpyPeerAsync(m->run_c.p, dst->device, o->run_c.p, src->device, (size_t)o->n_runs, dst->stream));
+    }
+    GL_CUDA(dst, cudaStreamSynchronize(dst->stream));
+    m->n_runs = o->n_runs;
+    m->sites_done = true;
+    m->merged = false;
+    m->blocks_set = false;
     return GL_OK;
 }
 

@@ -537,10 +537,29 @@ int  gl_indexsplit_chunks(const double* tile_sum, const int64_t* out_ptr, int32_
  *   gl_multidepth_result  : blocks x S arrays, row-major by block (any may be NULL).
  *   gl_multidepth_stats   : blocks, cells that took the float64 chain, cells certified, minSamples.
  *   gl_multidepth_text    : host-only: the rows after the header ("chrom\tstart\tend" + "\t%.2f" per sample), certified cells
- *                           printed from q, the others from val; made on `threads` of the host pool (0 = all).  gl_free_text. */
+ *                           printed from q, the others from val; made on `threads` of the host pool (0 = all).  gl_free_text.
+ * One run over several contexts (any devices, or several contexts on one device): each context is begun with the same
+ * (L, S, mincov, min_samples) and counts its own samples in pass 1; then
+ *   gl_multidepth_merge   : adds the per-base counters of every src into dst's and ORs their site bits into dst's
+ *                           (md_merge_kernel on dst's device; the state comes over with cudaMemcpyPeerAsync in chunks of
+ *                           GL_MD_MERGE_CHUNK_BASES, default 2^24, through two staging buffers), and adds their counted samples
+ *                           to dst's.  Returns when the merge is done.  GL_EINVAL: a null, repeated or differently begun source,
+ *                           or dst among the sources.  GL_ESTATE: a context not begun, or one that has run its sites or been
+ *                           merged already, or more than S samples counted in all.  A merged source refuses
+ *                           gl_multidepth_count, gl_multidepth_sites and another merge (GL_ESTATE) until it adopts sites.
+ *   gl_multidepth_sites   : on dst, once it holds every sample's counts.
+ *   gl_multidepth_adopt_sites : copies src's site and sufficient bits and its class runs into dst.  src must have run
+ *                           gl_multidepth_sites (else GL_ESTATE) and dst must have been begun with the same parameters (else
+ *                           GL_EINVAL).  dst then behaves as if it had run its sites: gl_multidepth_sites returns the same
+ *                           runs, and gl_multidepth_set_blocks, gl_multidepth_sums (with the cohort's sample numbers) and
+ *                           gl_multidepth_result work as on one context.  Each context's result holds the columns of the
+ *                           samples it summed; the others stay 0.
+ * A context that calls neither behaves as a one-context run. */
 int  gl_multidepth_begin(gl_ctx* ctx, int64_t contig_len, int32_t n_samples, int32_t mincov, double min_samples);
 int  gl_multidepth_count(gl_ctx* ctx);
+int  gl_multidepth_merge(gl_ctx* dst, gl_ctx* const* src, int32_t n_src);
 int  gl_multidepth_sites(gl_ctx* ctx, int32_t* run_start, uint8_t* run_class, int64_t cap, int64_t* n_runs);
+int  gl_multidepth_adopt_sites(gl_ctx* dst, gl_ctx* src);
 int  gl_multidepth_blocks(const int32_t* run_start, const uint8_t* run_class, int64_t n_runs, int64_t contig_len, int32_t n_samples,
                           int64_t chunk, int64_t max_skip, int64_t min_size, int64_t window, int64_t* blk_start, int64_t* blk_end,
                           int64_t* blk_sites, int64_t cap, int64_t* n_blocks);

@@ -1665,86 +1665,193 @@ static int cmd_indexcov(int argc, char** argv) {
 // ------------------------------------------------------------------------------------------------ covstats
 // V1 + V2 (covstats.go:122-220): gl_bam_covstats samples the records and computes the reference's Stats on the device;
 // a file it cannot take (GL_ESTATE), or GL_GPU_FEED=0, goes through gl_bam_covstats_host, with the same tail.
+//
+// --gpus N: one worker per GPU claims BAMs in argument order from a shared counter (a BAM the device refuses costs several
+// times more on the host route, so the dealing is dynamic).  A worker holds at most one BAM claimed ahead: it opens it before
+// it samples the current one, and starts reading its first batch (gl_bam_covstats_prefetch) as soon as the current one's
+// sampling call has consumed its own prefetch, so that the read overlaps the rest of the current BAM's work (the --hist
+// tail, the .bai read for the mapped counts, the commit).  The main thread commits the
+// rows in argument order; the first BAM that fails, in that order, ends the run as the sequential loop would, after the
+// workers have finished their current call and been joined.
+struct CsJob {
+    gl_bam* bh = nullptr;
+    bool done = false;
+    int code = 0;                           // exit code of this BAM's failure (0: none) and its message
+    std::string msg;
+    gl_covstats st;
+    std::vector<double> H;
+    std::string names, not_found;
+    long long genome = 0;
+    unsigned long long mapped = 0;
+};
+
 static int cmd_covstats(int argc, char** argv) {
     // the header is printed before the arguments are parsed (covstats.go:224-226)
     printf("coverage\tinsert_mean\tinsert_sd\tinsert_5th\tinsert_95th\ttemplate_mean\ttemplate_sd\tpct_unmapped\tpct_bad_reads\tpct_duplicate\tpct_proper_pair\tread_length\tbam\tsample\n");
-    std::string nstr = "1000000", regions, fasta, hist;
+    std::string nstr = "1000000", regions, fasta, hist, gpus = "0";
     ArgParser ap;
     ap.prog = "goleft covstats";
     ap.add("n", 'n', &nstr); ap.add("regions", 'r', &regions); ap.add("fasta", 'f', &fasta); ap.add("hist", 0, &hist);
+    ap.add("gpus", 0, &gpus);                       // extension: GPUs to use (0 = every visible one); the BAMs are dealt to them
     ap.parse(argc, argv);
     if (ap.positional.empty()) ap.fail("bams is required");
     const int N = atoi(nstr.c_str());
-    gl_ctx* ctx = open_ctx(0, "goleft covstats");
-    for (const std::string& bam : ap.positional) {
-        gl_bam* bh = nullptr;
+    const int kSkip = 100000;
+    const std::vector<std::string>& bams = ap.positional;
+    const size_t S = bams.size();
+    const GpuPlan gp = resolve_gpus(gpus, S, "goleft covstats");
+    std::vector<CsJob> jobs(S);
+    std::mutex mu;
+    std::condition_variable cv;
+    std::string ctx_err;                            // a worker that could not create its context
+    size_t next_claim = 0, fail_at = S;             // no BAM after the first known failure is claimed
+    auto claim = [&]() -> size_t {
+        std::lock_guard<std::mutex> lk(mu);
+        if (next_claim >= fail_at || !ctx_err.empty()) return S;
+        return next_claim++;
+    };
+    auto finish = [&](size_t i) {
+        std::lock_guard<std::mutex> lk(mu);
+        jobs[i].done = true;
+        if (jobs[i].code) fail_at = std::min(fail_at, i);
+        cv.notify_all();
+    };
+    auto open = [&](size_t i) {
         char oerr[512] = {0};
-        if (gl_bam_open(bam.c_str(), &bh, oerr, sizeof oerr) != GL_OK) fatal(1, "%s", oerr);
-        const glhts::BamHeader& hdr = bh->f.header;
-        gl_covstats st;
-        std::vector<double> H;
+        if (gl_bam_open(bams[i].c_str(), &jobs[i].bh, oerr, sizeof oerr) != GL_OK) { jobs[i].code = 1; jobs[i].msg = oerr; jobs[i].bh = nullptr; }
+    };
+    // BAM i on worker context c: everything but the output
+    auto run = [&](gl_ctx* c, size_t i, gl_bam* ahead) {
+        CsJob& J = jobs[i];
+        if (J.code) return;
+        const std::string& bam = bams[i];
+        gl_bam* bh = J.bh;
+        gl_covstats& st = J.st;
         auto sample = [&](bool device) {
-            int rc = device ? gl_bam_covstats(ctx, bh, N, 100000, &st, nullptr, 0) : gl_bam_covstats_host(ctx, bh, N, 100000, &st, nullptr, 0);
-            if (rc == GL_ERANGE && st.h_len > 0 && !hist.empty()) {              // H is wanted: the second call of the two
-                H.resize((size_t)st.h_len);
-                rc = device ? gl_bam_covstats(ctx, bh, N, 100000, &st, H.data(), st.h_len) : gl_bam_covstats_host(ctx, bh, N, 100000, &st, H.data(), st.h_len);
+            int rc = device ? gl_bam_covstats(c, bh, N, kSkip, &st, nullptr, 0) : gl_bam_covstats_host(c, bh, N, kSkip, &st, nullptr, 0);
+            if (rc == GL_ERANGE && st.h_len > 0 && !hist.empty()) {              // H is wanted: the tail over the samples this call left
+                const int32_t *rl = nullptr, *ins = nullptr, *tm = nullptr;
+                std::vector<int32_t> v;
+                if (device) {
+                    const int32_t *d_rl = nullptr, *d_ins = nullptr, *d_tm = nullptr;
+                    if ((rc = gl_bam_covstats_samples(c, &d_rl, &d_ins, &d_tm)) != GL_OK) return rc;
+                    v.resize((size_t)(st.n_read_len + 2 * st.n_insert));
+                    if (st.n_read_len && (rc = gl_memcpy_d2h(c, v.data(), d_rl, st.n_read_len * 4)) != GL_OK) return rc;
+                    if (st.n_insert && ((rc = gl_memcpy_d2h(c, v.data() + st.n_read_len, d_ins, st.n_insert * 4)) != GL_OK ||
+                                        (rc = gl_memcpy_d2h(c, v.data() + st.n_read_len + st.n_insert, d_tm, st.n_insert * 4)) != GL_OK)) return rc;
+                    rl = v.data(); ins = rl + st.n_read_len; tm = ins + st.n_insert;
+                } else if ((rc = gl_bam_covstats_host_samples(bh, &rl, &ins, &tm)) != GL_OK) return rc;
+                gl_covstats t = st;
+                J.H.resize((size_t)st.h_len);
+                rc = gl_covstats_tail(c, rl, st.n_read_len, ins, st.n_insert, tm, st.n_insert, &t, J.H.data(), st.h_len);
             } else if (rc == GL_ERANGE && st.h_len > 0) rc = GL_OK;              // the row does not print H
             return rc;
         };
         int rc = SegSource::gpu_feed() ? sample(true) : GL_ESTATE;
         if (rc == GL_ESTATE) rc = sample(false);
-        if (rc == GL_EINVAL && st.n_insert > 0 && st.n_insert < 3) fatal(2, "panic: runtime error: index out of range (covstats madFilter needs at least 3 insert sizes)");
-        if (rc == GL_ERANGE) fatal(2, "panic: runtime error: makeslice: len out of range (%s)", gl_last_error(ctx));
-        if (rc != GL_OK) fatal(1, "%s", gl_last_error(ctx));
-        std::string names;
-        for (auto& s : hdr.sample_names()) names += (names.empty() ? "" : ",") + s;
-        if (names.empty()) names = "<no-read-groups>";
+        // a prefetch that cannot start (no pinned memory) leaves the read to the call, which reports its own failures
+        if (ahead && SegSource::gpu_feed()) (void)gl_bam_covstats_prefetch(c, ahead, N, kSkip);
+        if (rc == GL_EINVAL && st.n_insert > 0 && st.n_insert < 3) { J.code = 2; J.msg = "panic: runtime error: index out of range (covstats madFilter needs at least 3 insert sizes)"; return; }
+        if (rc == GL_ERANGE) { J.code = 2; J.msg = std::string("panic: runtime error: makeslice: len out of range (") + gl_last_error(c) + ")"; return; }
+        if (rc != GL_OK) { J.code = 1; J.msg = gl_last_error(c); return; }
+        const glhts::BamHeader& hdr = bh->f.header;
+        for (auto& s : hdr.sample_names()) J.names += (J.names.empty() ? "" : ",") + s;
+        if (J.names.empty()) J.names = "<no-read-groups>";
         glhts::BaiIndex bai;
         bool have_idx = false;
         if (ends_with(bam, ".bam")) {
             std::string be = glhts::bai_read(bai_path(bam), bai);
-            if (!be.empty()) fatal(1, "%s", be.c_str());
+            if (!be.empty()) { J.code = 1; J.msg = be; return; }
             have_idx = true;
         }
+        for (size_t r = 0; r < hdr.refs.size(); r++) {                              // covstats.go:256-267
+            J.genome += hdr.refs[r].length;
+            if (have_idx) {
+                if (r >= bai.has_stats.size() || !bai.has_stats[r]) {
+                    if (hdr.refs[r].name.find("random") == std::string::npos && hdr.refs[r].length > 10000) J.not_found += (J.not_found.empty() ? "" : ",") + hdr.refs[r].name;
+                    continue;
+                }
+                J.mapped += bai.mapped[r];
+            }
+        }
+    };
+    std::vector<std::thread> th = start_workers(gp, [&](int g) {
+        gl_ctx* c = nullptr;
+        if (gl_ctx_create(g % gp.n_dev, &c) != GL_OK) {
+            std::lock_guard<std::mutex> lk(mu);
+            if (ctx_err.empty()) ctx_err = gl_last_error(nullptr);
+            cv.notify_all();
+            return;
+        }
+        size_t cur = claim();
+        if (cur < S) open(cur);
+        while (cur < S) {
+            const size_t nxt = claim();
+            if (nxt < S) open(nxt);
+            run(c, cur, nxt < S ? jobs[nxt].bh : nullptr);
+            if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
+            jobs[cur].bh = nullptr;
+            finish(cur);
+            cur = nxt;
+            bool stop;
+            { std::lock_guard<std::mutex> lk(mu); stop = cur > fail_at || !ctx_err.empty(); }
+            if (stop && cur < S) {                 // a BAM before it failed: it will never be committed
+                if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
+                jobs[cur].bh = nullptr;
+                break;
+            }
+        }
+        gl_ctx_destroy(c);
+    });
+    // the commit: rows in argument order.  stop() ends the claiming and joins the workers before a message ends the run.
+    auto stop = [&]() {
+        { std::lock_guard<std::mutex> lk(mu); fail_at = 0; }
+        for (std::thread& t : th) t.join();
+        th.clear();
+    };
+    long long region_genome = -1;
+    for (size_t i = 0; i < S; i++) {
+        {
+            std::unique_lock<std::mutex> lk(mu);
+            cv.wait(lk, [&] { return jobs[i].done || !ctx_err.empty(); });
+        }
+        CsJob& J = jobs[i];
+        if (!J.done) { stop(); fatal(1, "goleft covstats: %s", ctx_err.c_str()); }
+        if (J.code) { stop(); fatal(J.code, "%s", J.msg.c_str()); }
+        const std::string& bam = bams[i];
+        const gl_covstats& st = J.st;
         const double pBad = st.proportion_bad, pDup = st.proportion_duplicate, pProper = st.proportion_properly_paired, pUnmapped = st.proportion_unmapped;
         const double rlMean = st.read_length_mean, insMean = st.insert_mean, insSd = st.insert_sd, tMean = st.template_mean, tSd = st.template_sd;
         const int pct5 = st.insert_pct5, pct95 = st.insert_pct95, maxRead = st.max_read_length;
         if (!hist.empty()) {                                                        // Stats.H (covstats.go:202-217), one line per entry
-            const std::string hp = hist + "." + names + ".template_hist.tsv";
+            const std::string hp = hist + "." + J.names + ".template_hist.tsv";
             FILE* hf = fopen(hp.c_str(), "w");
-            if (!hf) fatal(1, "open %s: %s", hp.c_str(), strerror(errno));
-            for (size_t j = 0; j < H.size(); j++) fprintf(hf, "%lld\t%s\n", (long long)maxRead + (long long)j, go_float("%.6g", H[j]).c_str());
+            if (!hf) { const int e = errno; stop(); fatal(1, "open %s: %s", hp.c_str(), strerror(e)); }
+            for (size_t j = 0; j < J.H.size(); j++) fprintf(hf, "%lld\t%s\n", (long long)maxRead + (long long)j, go_float("%.6g", J.H[j]).c_str());
             fclose(hf);
         }
-        long long genome = 0;
-        unsigned long long mapped = 0;
-        std::string not_found;
-        for (size_t r = 0; r < hdr.refs.size(); r++) {                              // covstats.go:256-267
-            genome += hdr.refs[r].length;
-            if (have_idx) {
-                if (r >= bai.has_stats.size() || !bai.has_stats[r]) {
-                    if (hdr.refs[r].name.find("random") == std::string::npos && hdr.refs[r].length > 10000) not_found += (not_found.empty() ? "" : ",") + hdr.refs[r].name;
-                    continue;
+        if (!J.not_found.empty()) fprintf(stderr, "chromosomes: %s not found in %s\n", J.not_found.c_str(), bam.c_str());
+        long long genome = J.genome;
+        if (!regions.empty()) {                                                     // covstats.go:36-55, read once
+            if (region_genome < 0) {
+                gzFile f = gzopen(regions.c_str(), "rb");
+                if (!f) stop();                                                     // read_lines ends the run with the open error
+                else gzclose(f);
+                region_genome = 0;
+                for (const std::string& ln : read_lines(regions, true)) {
+                    size_t t1 = ln.find('\t');
+                    if (t1 == std::string::npos) continue;
+                    size_t t2 = ln.find('\t', t1 + 1);
+                    region_genome += atoll(ln.c_str() + t2 + 1) - atoll(ln.c_str() + t1 + 1);
                 }
-                mapped += bai.mapped[r];
             }
+            genome = region_genome;
         }
-        if (!not_found.empty()) fprintf(stderr, "chromosomes: %s not found in %s\n", not_found.c_str(), bam.c_str());
-        if (!regions.empty()) {                                                     // covstats.go:36-55
-            genome = 0;
-            for (const std::string& ln : read_lines(regions, true)) {
-                size_t t1 = ln.find('\t');
-                if (t1 == std::string::npos) continue;
-                size_t t2 = ln.find('\t', t1 + 1);
-                genome += atoll(ln.c_str() + t2 + 1) - atoll(ln.c_str() + t1 + 1);
-            }
-        }
-        const double coverage = (1 - pBad) * (double)mapped * rlMean / (double)genome;     // covstats.go:277
+        const double coverage = (1 - pBad) * (double)J.mapped * rlMean / (double)genome;     // covstats.go:277
         printf("%.2f\t%.2f\t%.2f\t%d\t%d\t%.2f\t%.2f\t%.2f\t%.1f\t%.1f\t%.1f\t%d\t%s\t%s\n", coverage, insMean, insSd, pct5, pct95, tMean, tSd,
-               100 * pUnmapped, 100 * pBad, 100 * pDup, 100 * pProper, maxRead, bam.c_str(), names.c_str());
-        gl_bam_close(bh);
+               100 * pUnmapped, 100 * pBad, 100 * pDup, 100 * pProper, maxRead, bam.c_str(), J.names.c_str());
     }
-    gl_ctx_destroy(ctx);
+    stop();
     return 0;
 }
 

@@ -480,6 +480,15 @@ type Stats struct {
 	H                                    []float64
 	// OnDevice tells whether the records were sampled on the GPU (false: the file went through the host sampler)
 	OnDevice bool
+	// Prefetched tells whether the first batch came from PrefetchBamStats
+	Prefetched bool
+}
+
+// PrefetchBamStats starts reading the first batch of next for a later BamStats(next, n, skipReads) on this Ctx and returns at
+// once, so that the read overlaps the BAM sampled before it.  A file the GPU would refuse gets no prefetch (BamStats then
+// takes the host sampler); the prefetch is dropped when next is closed or another prefetch starts.
+func (c *Ctx) PrefetchBamStats(next *Bam, n, skipReads int) error {
+	return c.err(C.gl_bam_covstats_prefetch(c.h, next.h, C.int32_t(n), C.int32_t(skipReads)))
 }
 
 // BamStats replaces covstats.BamStats(br, n, skipReads) (covstats/covstats.go:122-220): the records are sampled on the
@@ -516,6 +525,6 @@ func (c *Ctx) BamStats(b *Bam, n, skipReads int) (Stats, error) {
 		ReadLengthMean: float64(st.read_length_mean), ReadLengthMedian: float64(st.read_length_median),
 		ProportionBad: float64(st.proportion_bad), ProportionUnmapped: float64(st.proportion_unmapped),
 		ProportionProperlyPaired: float64(st.proportion_properly_paired), ProportionDuplicate: float64(st.proportion_duplicate),
-		MaxReadLength: int(st.max_read_length), H: h[:int(st.h_len)], OnDevice: st.path == 1,
+		MaxReadLength: int(st.max_read_length), H: h[:int(st.h_len)], OnDevice: st.path == 1, Prefetched: st.prefetched == 1,
 	}, nil
 }

@@ -131,6 +131,7 @@ _proto("gl_format_g3_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_bincount_i32", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp)
 _proto("gl_bam_covstats", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
 _proto("gl_bam_covstats_host", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
+_proto("gl_bam_covstats_prefetch", C.c_int, _vp, _vp, C.c_int32, C.c_int32)
 _proto("gl_bam_covstats_samples", C.c_int, _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp))
 _proto("gl_bam_covstats_host_samples", C.c_int, _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_vp))
 _proto("gl_covstats_tail", C.c_int, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp, C.c_int64, _vp, _vp, C.c_int64)
@@ -799,13 +800,13 @@ class CovStats(C.Structure):
                 [(k, C.c_int64) for k in ("n_unmapped", "k", "n_bad", "n_dup", "n_proper", "n_read_len", "n_insert", "n_records_read", "h_len",
                                           "bytes_in", "bytes_out")] +
                 [(k, C.c_double) for k in ("read_s", "inflate_s", "index_s", "fields_s", "cut_s", "tail_s", "wall_s")] +
-                [("n_batches", C.c_int32), ("_pad", C.c_int32)])
+                [("n_batches", C.c_int32), ("prefetched", C.c_int32)])
     STATS = ("insert_mean", "insert_sd", "insert_pct5", "insert_pct95", "template_mean", "template_sd", "read_length_mean", "read_length_median",
              "proportion_bad", "proportion_unmapped", "proportion_properly_paired", "proportion_duplicate", "max_read_length")
     COUNTERS = ("n_unmapped", "k", "n_bad", "n_dup", "n_proper", "n_read_len", "n_insert", "n_records_read")
 
     def as_dict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_ if k != "_pad"}
+        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 def _covstats_two_call(ctx, fn, st=None):
@@ -838,6 +839,12 @@ def bam_covstats(ctx: "Ctx", bam: Bam, n: int, skip: int = 100000, samples: bool
             ctx._ck(lib.gl_memcpy_d2h(ctx.h, _ptr(a), p.value, k * 4))
         out.append(a)
     return st, H, tuple(out)
+
+
+def bam_covstats_prefetch(ctx: "Ctx", bam: Bam, n: int, skip: int = 100000):
+    """start reading bam's first batch for a later bam_covstats(ctx, bam, n, skip) and return at once; a file the device would
+    refuse gets no prefetch (bam_covstats reports it)"""
+    ctx._ck(lib.gl_bam_covstats_prefetch(ctx.h, bam.h, n, skip))
 
 
 def bam_covstats_host(ctx: Optional["Ctx"], bam: Bam, n: int, skip: int = 100000, samples: bool = False):

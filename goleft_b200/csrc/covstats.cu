@@ -175,14 +175,6 @@ constexpr int64_t kLaterBatch = int64_t(64) << 20;     // compressed bytes per b
 constexpr int64_t kMaxTail = int64_t(64) << 20;        // the unplaced tail is one unit: one thread walks it
 constexpr int kEvents = 7;
 
-struct CsState {
-    gl_buf comp, infl, rec, hist;                      // compressed + tables, inflated stream, per-record arrays, histogram
-    gl_buf s_len, s_ins, s_tmpl;                       // the samples, file order
-    void* pin[2] = {nullptr, nullptr};
-    size_t pin_cap[2] = {0, 0};
-    cudaEvent_t ev[kEvents] = {};
-};
-
 // what the helper thread makes of one batch: the compressed bytes of units [i0, i1) in pinned memory, the member table and
 // the units' positions in the batch's inflated stream
 struct Batch {
@@ -193,6 +185,24 @@ struct Batch {
     std::vector<int64_t> comp_off, out_off;
     std::vector<long long> unit_pos;
     const char* err = nullptr;
+};
+
+// gl_bam_covstats_prefetch: the first batch of `b` for a later gl_bam_covstats(ctx, b, n, skip), read by `f` into pin[2]
+struct Prefetch {
+    gl_bam* b = nullptr;
+    int32_t n = 0, skip = 0;
+    std::vector<uint64_t> bound;
+    Batch B;
+    std::future<void> f;
+};
+
+struct CsState {
+    gl_buf comp, infl, rec, hist;                      // compressed + tables, inflated stream, per-record arrays, histogram
+    gl_buf s_len, s_ins, s_tmpl;                       // the samples, file order
+    void* pin[3] = {nullptr, nullptr, nullptr};        // [0], [1]: a call's batches; [2]: the prefetched first batch
+    size_t pin_cap[3] = {0, 0, 0};
+    cudaEvent_t ev[kEvents] = {};
+    Prefetch pf;
 };
 
 void load_batch(int fd, const std::vector<uint64_t>& bound, Batch& B) {
@@ -232,6 +242,62 @@ void load_batch(int fd, const std::vector<uint64_t>& bound, Batch& B) {
         if (!B.unit_pos.empty() && p < B.unit_pos.back()) { B.err = "index offsets are not in file order"; return; }
         B.unit_pos.push_back(p);
     }
+}
+
+// unit boundaries of the whole file, as virtual offsets in file order: the first record, every reference's chunk range and
+// linear-index offsets, end of file.  The last unit is the unplaced tail.  Returns why the device cannot take the file, or
+// an empty string.
+std::string cs_bounds(glhts::BamFile& F, std::vector<uint64_t>& bound) {
+    bound.clear();
+    if (!F.has_index || F.fd() < 0) return "no index";
+    if (F.rec_skip() > 65535) return "the header ends a 64 KB member";
+    const uint64_t v_first = ((uint64_t)F.rec_member() << 16) | F.rec_skip(), v_eof = (uint64_t)F.file_size() << 16;
+    for (size_t t = 0; t < F.bai.ioffsets.size(); t++) {
+        const uint64_t vbeg = t < F.bai.ref_beg.size() ? F.bai.ref_beg[t] : 0, vend = t < F.bai.ref_end.size() ? F.bai.ref_end[t] : 0;
+        if (vbeg == 0 || vend <= vbeg) {
+            for (uint64_t v : F.bai.ioffsets[t]) if (v) return "the index has no chunk range for reference " + std::to_string(t);
+            continue;
+        }
+        bound.push_back(vbeg); bound.push_back(vend);
+        for (uint64_t v : F.bai.ioffsets[t]) if (v > vbeg && v < vend) bound.push_back(v);
+    }
+    bound.push_back(v_first); bound.push_back(v_eof);
+    std::sort(bound.begin(), bound.end());
+    bound.erase(std::unique(bound.begin(), bound.end()), bound.end());
+    if (bound.front() != v_first || bound.back() != v_eof) return "index offsets outside the file's records";
+    return "";
+}
+
+// compressed bytes of the first batch (sized to the sample) and of the later ones; GL_COVSTATS_BATCH_BYTES sets both
+void cs_batch_bytes(int32_t n, int32_t skip, int64_t& first, int64_t& later) {
+    first = std::min<int64_t>(std::max<int64_t>(((int64_t)skip + 3 * (int64_t)n) * 40, int64_t(8) << 20), int64_t(192) << 20);
+    later = kLaterBatch;
+    if (const char* v = getenv("GL_COVSTATS_BATCH_BYTES")) { const long long x = atoll(v); if (x > 0) first = later = x; }
+}
+
+// units [i0, i1) of the batch that starts at i0: as many as fit the byte bound, at least one.  Returns why the device cannot
+// take the batch, or nullptr.
+const char* cs_plan(const glhts::BamFile& F, const std::vector<uint64_t>& bound, size_t i0, int64_t bytes, Batch& B) {
+    const size_t n_bound = bound.size();
+    size_t i1 = i0 + 1;
+    while (i1 + 1 < n_bound && (int64_t)(bound[i1 + 1] >> 16) - (int64_t)(bound[i0] >> 16) <= bytes) i1++;
+    B.i0 = i0; B.i1 = i1;
+    B.c0 = (int64_t)(bound[i0] >> 16);
+    const int64_t c1 = std::min<int64_t>(F.file_size(), (int64_t)(bound[i1] >> 16) + 65536 + 64);
+    if (i1 == n_bound - 1 && c1 - (int64_t)(bound[i1 - 1] >> 16) > kMaxTail) return "the sample reaches a large unplaced tail";
+    if (c1 - B.c0 > (int64_t(1) << 31)) return "a unit of more than 2 GB";
+    B.nbytes = (size_t)(c1 - B.c0);
+    return nullptr;
+}
+
+int cs_state(gl_ctx* ctx, CsState*& S) {
+    if (!ctx->cs) {
+        CsState* N = new CsState();
+        ctx->cs = N;
+        for (auto& e : N->ev) GL_CUDA(ctx, cudaEventCreate(&e));
+    }
+    S = static_cast<CsState*>(ctx->cs);
+    return GL_OK;
 }
 
 int pin_reserve(gl_ctx* ctx, CsState* S, int k, size_t bytes) {
@@ -288,9 +354,18 @@ int device_counts(gl_ctx* ctx, CsState* S, const int32_t* d_v, int64_t n, glcs::
 
 }  // namespace
 
+void cs_prefetch_drop(gl_ctx* ctx) {
+    CsState* S = static_cast<CsState*>(ctx->cs);
+    if (!S || !S->pf.b) return;
+    if (S->pf.f.valid()) S->pf.f.wait();
+    S->pf.b->cs_pf = nullptr;
+    S->pf = Prefetch();
+}
+
 void cs_free(gl_ctx* ctx) {
     CsState* S = static_cast<CsState*>(ctx->cs);
     if (!S) return;
+    cs_prefetch_drop(ctx);
     for (gl_buf* b : {&S->comp, &S->infl, &S->rec, &S->hist, &S->s_len, &S->s_ins, &S->s_tmpl}) if (b->p) cudaFree(b->p);
     for (void* p : S->pin) if (p) cudaFreeHost(p);
     for (cudaEvent_t e : S->ev) if (e) cudaEventDestroy(e);
@@ -306,62 +381,46 @@ int gl_bam_covstats(gl_ctx* ctx, gl_bam* b, int32_t n, int32_t skip, gl_covstats
     memset(out, 0, sizeof *out);
     out->path = 1;
     const double t_wall = now_s();
-    if (!ctx->cs) {
-        CsState* N = new CsState();
-        ctx->cs = N;
-        for (auto& e : N->ev) GL_CUDA(ctx, cudaEventCreate(&e));
-    }
-    CsState* S = static_cast<CsState*>(ctx->cs);
+    CsState* S = nullptr;
+    GL_CHECK(cs_state(ctx, S));
     glhts::BamFile& F = b->f;
-    if (!F.has_index || F.fd() < 0) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: no index");
-
-    // ---- unit boundaries of the whole file, as virtual offsets in file order: the first record, every reference's chunk
-    // range and linear-index offsets, end of file.  The last unit is the unplaced tail.
     std::vector<uint64_t> bound;
-    if (F.rec_skip() > 65535) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: the header ends a 64 KB member");
-    const uint64_t v_first = ((uint64_t)F.rec_member() << 16) | F.rec_skip(), v_eof = (uint64_t)F.file_size() << 16;
-    for (size_t t = 0; t < F.bai.ioffsets.size(); t++) {
-        const uint64_t vbeg = t < F.bai.ref_beg.size() ? F.bai.ref_beg[t] : 0, vend = t < F.bai.ref_end.size() ? F.bai.ref_end[t] : 0;
-        if (vbeg == 0 || vend <= vbeg) {
-            for (uint64_t v : F.bai.ioffsets[t]) if (v) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: the index has no chunk range for reference %zu", t);
-            continue;
-        }
-        bound.push_back(vbeg); bound.push_back(vend);
-        for (uint64_t v : F.bai.ioffsets[t]) if (v > vbeg && v < vend) bound.push_back(v);
+    Batch bat[2];
+    // a prefetch of this handle: consumed when it was made for this n and skip, discarded otherwise
+    const bool pre = S->pf.b == b && S->pf.n == n && S->pf.skip == skip;
+    if (pre) {
+        const double t0 = now_s();
+        S->pf.f.wait();
+        out->read_s += now_s() - t0;
+        bound = std::move(S->pf.bound);
+        bat[0] = std::move(S->pf.B);
+        out->prefetched = 1;
     }
-    bound.push_back(v_first); bound.push_back(v_eof);
-    std::sort(bound.begin(), bound.end());
-    bound.erase(std::unique(bound.begin(), bound.end()), bound.end());
-    if (bound.front() != v_first || bound.back() != v_eof) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: index offsets outside the file's records");
+    if (S->pf.b == b) cs_prefetch_drop(ctx);
+    if (!pre) {
+        const std::string e = cs_bounds(F, bound);
+        if (!e.empty()) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: %s", e.c_str());
+    }
     const size_t n_bound = bound.size();
 
     long long g0 = 0, e0 = 0, first = 0;                 // lengths and inserts so far; file index of the next batch's first record
     unsigned long long ctr[7] = {0, 0, 0, 0, 0, 0, 0};
     bool cut = false;
     if (n > 0 && n_bound >= 2) {
-        int64_t batch_first = std::min<int64_t>(std::max<int64_t>(((int64_t)skip + 3 * (int64_t)n) * 40, int64_t(8) << 20), int64_t(192) << 20), batch_later = kLaterBatch;
-        if (const char* v = getenv("GL_COVSTATS_BATCH_BYTES")) { const long long x = atoll(v); if (x > 0) batch_first = batch_later = x; }
-        // units [i0, i1) of the batch that starts at i0: as many as fit the byte bound, at least one
+        int64_t batch_first, batch_later;
+        cs_batch_bytes(n, skip, batch_first, batch_later);
         auto plan = [&](size_t i0, int64_t bytes, Batch& B) -> int {
-            size_t i1 = i0 + 1;
-            while (i1 + 1 < n_bound && (int64_t)(bound[i1 + 1] >> 16) - (int64_t)(bound[i0] >> 16) <= bytes) i1++;
-            B.i0 = i0; B.i1 = i1;
-            B.c0 = (int64_t)(bound[i0] >> 16);
-            const int64_t c1 = std::min<int64_t>(F.file_size(), (int64_t)(bound[i1] >> 16) + 65536 + 64);
-            if (i1 == n_bound - 1 && c1 - (int64_t)(bound[i1 - 1] >> 16) > kMaxTail) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: the sample reaches a large unplaced tail");
-            if (c1 - B.c0 > (int64_t(1) << 31)) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: a unit of more than 2 GB");
-            B.nbytes = (size_t)(c1 - B.c0);
-            return GL_OK;
+            const char* e = cs_plan(F, bound, i0, bytes, B);
+            return e ? gl_fail(ctx, GL_ESTATE, "gl_bam_covstats: %s", e) : GL_OK;
         };
-        Batch bat[2];
         std::future<void> pending;
         // the helper thread must be joined on every return path: it writes into this frame and into pinned memory
         struct Join { std::future<void>& f; ~Join() { if (f.valid()) f.wait(); } } join{pending};
         int cur = 0;
-        GL_CHECK(plan(0, batch_first, bat[0]));
-        GL_CHECK(pin_reserve(ctx, S, 0, bat[0].nbytes + 256));
-        bat[0].h = static_cast<uint8_t*>(S->pin[0]);
-        {
+        if (!pre) {
+            GL_CHECK(plan(0, batch_first, bat[0]));
+            GL_CHECK(pin_reserve(ctx, S, 0, bat[0].nbytes + 256));
+            bat[0].h = static_cast<uint8_t*>(S->pin[0]);
             const double t0 = now_s();
             load_batch(F.fd(), bound, bat[0]);
             out->read_s += now_s() - t0;
@@ -515,6 +574,30 @@ int gl_bam_covstats_samples(gl_ctx* ctx, const int32_t** d_read_len, const int32
     CsState* S = static_cast<CsState*>(ctx->cs);
     if (!S) return gl_fail(ctx, GL_ESTATE, "gl_bam_covstats_samples: no gl_bam_covstats call on this ctx");
     *d_read_len = static_cast<const int32_t*>(S->s_len.p); *d_insert = static_cast<const int32_t*>(S->s_ins.p); *d_tmpl = static_cast<const int32_t*>(S->s_tmpl.p);
+    return GL_OK;
+}
+
+int gl_bam_covstats_prefetch(gl_ctx* ctx, gl_bam* next, int32_t n, int32_t skip) {
+    GL_CHECK(gl_use(ctx));
+    if (!next) return gl_fail(ctx, GL_EINVAL, "gl_bam_covstats_prefetch: null argument");
+    CsState* S = nullptr;
+    GL_CHECK(cs_state(ctx, S));
+    cs_prefetch_drop(ctx);
+    if (next->cs_pf) cs_prefetch_drop(next->cs_pf);       // made on another ctx
+    if (n <= 0) return GL_OK;
+    // a file the device would refuse gets no prefetch: gl_bam_covstats reports it
+    Prefetch& P = S->pf;
+    if (!cs_bounds(next->f, P.bound).empty() || P.bound.size() < 2) { P.bound.clear(); return GL_OK; }
+    int64_t batch_first, batch_later;
+    cs_batch_bytes(n, skip, batch_first, batch_later);
+    if (cs_plan(next->f, P.bound, 0, batch_first, P.B)) { P = Prefetch(); return GL_OK; }
+    const int rc = pin_reserve(ctx, S, 2, P.B.nbytes + 256);
+    if (rc != GL_OK) { P = Prefetch(); return rc; }
+    P.B.h = static_cast<uint8_t*>(S->pin[2]);
+    P.b = next; P.n = n; P.skip = skip;
+    next->cs_pf = ctx;
+    const int fd = next->f.fd();
+    P.f = std::async(std::launch::async, [fd, &P] { load_batch(fd, P.bound, P.B); });
     return GL_OK;
 }
 

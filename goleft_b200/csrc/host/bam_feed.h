@@ -82,5 +82,8 @@ std::string bam_covstats_sample(BamFile& f, int n, int skip, CovstatsSample& out
 
 }  // namespace glhts
 
-// the C ABI's opaque BAM handle (feeder_api.cpp, bamgpu.cu)
-struct gl_bam { glhts::BamFile f; glhts::ContigSegs segs; glhts::CovstatsSample cs; };
+struct gl_ctx;
+// the C ABI's opaque BAM handle (feeder_api.cpp, bamgpu.cu).  cs_pf: the ctx whose covstats prefetch reads this file.
+struct gl_bam { glhts::BamFile f; glhts::ContigSegs segs; glhts::CovstatsSample cs; gl_ctx* cs_pf = nullptr; };
+// covstats.cu: join and forget ctx's covstats prefetch, if any
+void cs_prefetch_drop(gl_ctx* ctx);

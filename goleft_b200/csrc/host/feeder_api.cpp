@@ -89,7 +89,10 @@ int gl_bam_open(const char* path, gl_bam** out, char* err, int64_t err_cap) {
     return GL_OK;
 }
 
-void gl_bam_close(gl_bam* b) { delete b; }
+void gl_bam_close(gl_bam* b) {
+    if (b && b->cs_pf) cs_prefetch_drop(b->cs_pf);
+    delete b;
+}
 
 int gl_bam_info(const gl_bam* b, int32_t* n_refs, int32_t* has_index) {
     if (!b) return GL_EINVAL;

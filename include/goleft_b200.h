@@ -729,7 +729,8 @@ typedef struct {
     /* seconds.  Device route: read = pread not hidden behind device work, inflate .. cut = device time of the phases (CUDA
      * events).  Host route: read_s is read + inflate + the record walk together.  tail_s: histograms + the Stats arithmetic. */
     double read_s, inflate_s, index_s, fields_s, cut_s, tail_s, wall_s;
-    int32_t n_batches, _pad;
+    int32_t n_batches;
+    int32_t prefetched;           /* 1: the first batch came from gl_bam_covstats_prefetch */
 } gl_covstats;
 
 /* Sampled on the device: BGZF inflate, record index, per-record fields, cut + compaction and the three histograms are
@@ -739,6 +740,15 @@ typedef struct {
  * unplaced tail): call gl_bam_covstats_host.  GL_EINVAL with out->n_insert of 1 or 2, and GL_ERANGE with a message about
  * H's length, are the two places the reference panics. */
 int  gl_bam_covstats(gl_ctx* ctx, gl_bam* b, int32_t n, int32_t skip, gl_covstats* out, double* H, int64_t h_cap);
+/* Starts reading the first batch of `next` for a later gl_bam_covstats(ctx, next, n, skip) and returns at once: the same
+ * planning as the call, then a library thread preads the batch into a third pinned slot of the ctx (the two a call uses stay
+ * free).  A file the device would refuse gets no prefetch and GL_OK: the call reports it.  Only argument errors and
+ * allocation failures are returned.  The first gl_bam_covstats on this ctx with this handle, n and skip starts from that
+ * batch (out->prefetched = 1; its read_s counts only the wait that was not hidden); the results are the same bits as without
+ * a prefetch.  It is discarded (its thread joined) by a gl_bam_covstats on this handle with another n or skip, a new
+ * prefetch, gl_bam_close of the handle and gl_ctx_destroy; calls on other handles leave it in place.  One slot per ctx:
+ * prefetch BAM i+1 once the call on BAM i has returned. */
+int  gl_bam_covstats_prefetch(gl_ctx* ctx, gl_bam* next, int32_t n, int32_t skip);
 /* The last gl_bam_covstats on this ctx: its samples in file order, on the device (out->n_read_len, n_insert, n_insert
  * values), valid until the next call. */
 int  gl_bam_covstats_samples(gl_ctx* ctx, const int32_t** d_read_len, const int32_t** d_insert, const int32_t** d_tmpl);

@@ -249,25 +249,49 @@ struct SegSource {
         if (whole_ref && gpu_feed()) {
             gl_bam_segments g;
             const int rc = gl_bam_decode_device(ctx, &bam, tid, Q, &s, &e, &n, &g);
-            if (rc == GL_OK) {
-                on_device = true;
-                one.wall_s = g.wall_s; one.inflate_s = g.inflate_s; one.parse_s = g.parse_s;
-                one.n_records = g.n_records; one.bytes_in = g.bytes_in; one.bytes_out = g.bytes_out;
-                if (gpu_fed) ++*gpu_fed;
-            } else {
-                view(nullptr, nullptr, 0);
-                if (rc != GL_ESTATE) glck(ctx, rc, "gl_bam_decode_device");    // GL_ESTATE: not possible on the device for this reference
-            }
+            if (device_result(ctx, rc, g, "gl_bam_decode_device", one) && gpu_fed) ++*gpu_fed;
         }
         if (!on_device) {
             std::string err = bam.f.decode(tid, beg, end, Q, threads, want, host, &one);
             if (!err.empty()) fatal(1, "%s", err.c_str());
             if (host.format == 32) { s = host.start.data(); e = host.end.data(); n = host.n; }
         }
-        if (st) {
-            st->wall_s += one.wall_s; st->inflate_s += one.inflate_s; st->parse_s += one.parse_s;
-            st->n_records += one.n_records; st->bytes_in += one.bytes_in; st->bytes_out += one.bytes_out;
+        add_stats(st, one);
+    }
+
+    // The segments of reference tid whose blocks meet one of the intervals [beg[i], end[i]), decoded on the device from only
+    // the BGZF members the index's bin query names; they stay on the device.  False, with nothing fetched, where the GPU
+    // feeder cannot serve them (GL_GPU_FEED=0, a preloaded BAM, or GL_ESTATE from the library): the caller uses fetch().
+    bool fetch_regions(gl_ctx* ctx, gl_bam& bam, int tid, const std::vector<int64_t>& beg, const std::vector<int64_t>& end, int Q,
+                       glhts::DecodeStats* st) {
+        view(nullptr, nullptr, 0);
+        if (tid < 0 || whole || !gpu_feed()) return false;
+        glhts::DecodeStats one;
+        gl_bam_segments g;
+        const int rc = gl_bam_decode_device_regions(ctx, &bam, tid, beg.data(), end.data(), (int64_t)beg.size(), Q, &s, &e, &n, &g);
+        if (!device_result(ctx, rc, g, "gl_bam_decode_device_regions", one)) return false;
+        add_stats(st, one);
+        return true;
+    }
+
+    // a device decode's outcome: on GL_OK the arrays are on the device and its statistics go to one; GL_ESTATE (not possible
+    // on the device for this reference) leaves nothing; any other code is fatal
+    bool device_result(gl_ctx* ctx, int rc, const gl_bam_segments& g, const char* what, glhts::DecodeStats& one) {
+        if (rc != GL_OK) {
+            view(nullptr, nullptr, 0);
+            if (rc != GL_ESTATE) glck(ctx, rc, what);
+            return false;
         }
+        on_device = true;
+        one.wall_s = g.wall_s; one.inflate_s = g.inflate_s; one.parse_s = g.parse_s;
+        one.n_records = g.n_records; one.bytes_in = g.bytes_in; one.bytes_out = g.bytes_out;
+        return true;
+    }
+
+    static void add_stats(glhts::DecodeStats* st, const glhts::DecodeStats& one) {
+        if (!st) return;
+        st->wall_s += one.wall_s; st->inflate_s += one.inflate_s; st->parse_s += one.parse_s;
+        st->n_records += one.n_records; st->bytes_in += one.bytes_in; st->bytes_out += one.bytes_out;
     }
 
     void add(gl_ctx* ctx) const {
@@ -521,18 +545,32 @@ struct DepthEngine {
         long long lo = regions[ks[0]].s, hi = regions[ks[0]].e;
         for (size_t k : ks) { lo = std::min(lo, regions[k].s); hi = std::max(hi, regions[k].e); }
         const long long span_s = lo / W * W;
-        src.fetch(ctx, gbam, tid(job.chrom), span_s, hi, o.Q, o.threads, 32, false, &job.dec, &job.gpu_fed);   // int32: the interval sums and the per-line slices want arrays
-        const double tg = now_s();
+        const int t = tid(job.chrom);
         int64_t nw = 0, nr = 0;
         auto format_one = [&](size_t k, const int64_t* ws, int64_t nw_, const int32_t* rs_, const uint8_t* rc_, int64_t nr_) {
             emit(regions[k].chrom, regions[k].s, regions[k].e, ws, nw_, rs_, rc_, nr_, &(*sh.out_hd)[k], &(*sh.out_ca)[k]);
         };
         bool batched = ks.size() > 1 && hi - span_s < (1LL << 30) - 2 * (long long)W;
+        // The GPU feeder reads only the members the lines' bin queries name.  Its blocks are those that meet a line, in BAM
+        // order: what one pass over the span needs, or a single line's pass, but not the per-line slices of sorted arrays.
+        bool dev = false;
+        if (batched || ks.size() == 1) {
+            std::vector<int64_t> lb, le;
+            for (size_t k : ks) { lb.push_back(regions[k].s); le.push_back(regions[k].e); }
+            dev = src.fetch_regions(ctx, gbam, t, lb, le, o.Q, &job.dec);
+        }
+        if (!dev) src.fetch(ctx, gbam, t, span_s, hi, o.Q, o.threads, 32, false, &job.dec, &job.gpu_fed);   // int32: the interval sums and the per-line slices want arrays
+        const double tg = now_s();
         if (batched) {
             reduce_to_host(src, span_s, hi, 0, nw, nr);
             int32_t path = 0;
             batched = gl_depth_last_path(ctx, &path) == GL_OK && (path == 1 || src.n == 0);   // the interval sums want the fused path's cell index
+            if (!batched && dev) {                                             // per-line passes slice sorted host arrays
+                dev = false;
+                src.fetch(ctx, gbam, t, span_s, hi, o.Q, o.threads, 32, false, &job.dec, &job.gpu_fed);
+            }
         }
+        if (dev) job.gpu_fed++;
         if (!batched) {
             // per-line passes over the slice of segments that can reach the line (the arrays are sorted by start)
             const int32_t maxlen = std::max<int32_t>(src.host.max_len, 1);
@@ -540,6 +578,11 @@ struct DepthEngine {
             SegSource line;
             for (size_t k : ks) {
                 if (regions[k].e - regions[k].s >= (1LL << 30)) fatal(1, "BED region longer than 2^30-1 bases: %s", regions[k].chrom.c_str());
+                if (src.on_device) {                                           // one line, its blocks from the GPU feeder
+                    reduce_to_host(src, regions[k].s, regions[k].e, 0, nw, nr);
+                    format_one(k, sums.data(), nw, rstart.data(), rclass.data(), nr);
+                    continue;
+                }
                 int64_t a = 0, b = src.n;
                 if (sorted && src.n > 0) {
                     a = std::lower_bound(src.s, src.s + src.n, (int32_t)std::max<long long>(regions[k].s - maxlen, INT32_MIN)) - src.s;

@@ -160,6 +160,8 @@ _proto("gl_bam_info", C.c_int, _vp, _i32p, _i32p)
 _proto("gl_bam_ref", C.c_int, _vp, C.c_int32, C.POINTER(C.c_char_p), _i64p, _i64p)
 _proto("gl_bam_decode", C.c_int, _vp, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
 _proto("gl_bam_decode_device", C.c_int, _vp, _vp, C.c_int32, C.c_int32, C.POINTER(_vp), C.POINTER(_vp), _i64p, _vp)
+_proto("gl_bam_decode_device_regions", C.c_int, _vp, _vp, C.c_int32, _vp, _vp, C.c_int64, C.c_int32, C.POINTER(_vp), C.POINTER(_vp), _i64p, _vp)
+_proto("gl_bam_region_chunks", C.c_int, _vp, C.c_int32, _vp, _vp, C.c_int64, _vp, _vp, C.c_int64, _i64p)
 _proto("gl_bgzf_inflate_device", C.c_int, _vp, _vp, _vp, _vp, C.c_int64, _vp, _vp)
 _proto("gl_bai_read", C.c_int, C.c_char_p, C.POINTER(_vp), _vp, C.c_int64)
 _proto("gl_bai_n_refs", C.c_int, _vp, _i32p, _u64p)
@@ -778,6 +780,45 @@ def bam_decode_device(ctx: "Ctx", bam: Bam, tid: int, min_mapq: int = 1):
     o = _BamSegments()
     ps, pe, n = _vp(), _vp(), C.c_int64(0)
     rc = lib.gl_bam_decode_device(ctx.h, bam.h, tid, min_mapq, C.byref(ps), C.byref(pe), C.byref(n), C.byref(o))
+    return _device_segments(ctx, rc, o, ps, pe, n)
+
+
+def bam_decode_device_regions(ctx: "Ctx", bam: Bam, tid: int, beg, end, min_mapq: int = 1):
+    """The GPU feeder over a region query: the blocks of reference tid's passing records that meet one of the intervals
+    [beg[i], end[i]), in BAM order, decoded from only the BGZF members the index's bins name -> the dict bam_decode_device
+    gives; GlError(GL_ESTATE) when the device cannot do it."""
+    b_ = np.ascontiguousarray(beg, np.int64)
+    e_ = np.ascontiguousarray(end, np.int64)
+    if b_.shape != e_.shape or b_.ndim != 1:
+        raise ValueError("beg and end must be 1-D arrays of one length")
+    o = _BamSegments()
+    ps, pe, n = _vp(), _vp(), C.c_int64(0)
+    rc = lib.gl_bam_decode_device_regions(ctx.h, bam.h, tid, _ptr(b_) if b_.size else None, _ptr(e_) if e_.size else None, b_.size, min_mapq,
+                                          C.byref(ps), C.byref(pe), C.byref(n), C.byref(o))
+    return _device_segments(ctx, rc, o, ps, pe, n)
+
+
+def bam_region_chunks(bam: Bam, tid: int, beg, end):
+    """(vb, ve) uint64 arrays: the virtual-offset ranges a region query of the intervals [beg[i], end[i]) on reference tid
+    reads (gl_bam_region_chunks; host only)"""
+    b_ = np.ascontiguousarray(beg, np.int64)
+    e_ = np.ascontiguousarray(end, np.int64)
+    if b_.shape != e_.shape or b_.ndim != 1:
+        raise ValueError("beg and end must be 1-D arrays of one length")
+    args = (bam.h, tid, _ptr(b_) if b_.size else None, _ptr(e_) if e_.size else None, b_.size)
+    n = C.c_int64(0)
+    rc = lib.gl_bam_region_chunks(*args, None, None, 0, C.byref(n))
+    if rc == GL_ERANGE:
+        vb, ve = np.empty(n.value, np.uint64), np.empty(n.value, np.uint64)
+        rc = lib.gl_bam_region_chunks(*args, _ptr(vb), _ptr(ve), n.value, C.byref(n))
+    else:
+        vb, ve = np.zeros(0, np.uint64), np.zeros(0, np.uint64)
+    if rc != GL_OK:
+        raise GlError(rc, "gl_bam_region_chunks")
+    return vb, ve
+
+
+def _device_segments(ctx, rc, o, ps, pe, n):
     if rc != GL_OK:
         raise GlError(rc, lib.gl_last_error(ctx.h).decode())
     out = {"n": n.value, "units": o.units, "max_len": o.max_len, "n_records": o.n_records, "n_pass": o.n_pass, "bytes_in": o.bytes_in,

@@ -191,7 +191,7 @@ std::string BamFile::open(const std::string& p, bool with_index) {
         struct stat s2;
         if (stat(ip.c_str(), &s2) != 0) continue;
         BaiIndex b;
-        if (bai_read(ip, b).empty()) { bai = std::move(b); has_index = true; break; }
+        if (bai_read(ip, b).empty()) { bai = std::move(b); has_index = true; index_path = ip; break; }
     }
     return "";
 }

@@ -43,7 +43,7 @@ public:
     bool has_index = false;
     BamHeader header;
     BaiIndex bai;
-    std::string path;
+    std::string path, index_path;               // index_path: the .bai that was loaded
     // M/=/X blocks of the records of reference `tid` that pass the samtools-depth filter (glbam::depth_counts) and can
     // overlap [beg, end).  want: 0 = choose (packed8 unless the blocks are long), 8, 32.  Needs the index.
     std::string decode(int tid, int64_t beg, int64_t end, int min_mapq, int threads, int want, ContigSegs& out, DecodeStats* st);
@@ -84,6 +84,15 @@ std::string bam_covstats_sample(BamFile& f, int n, int skip, CovstatsSample& out
 
 struct gl_ctx;
 // the C ABI's opaque BAM handle (feeder_api.cpp, bamgpu.cu).  cs_pf: the ctx whose covstats prefetch reads this file.
-struct gl_bam { glhts::BamFile f; glhts::ContigSegs segs; glhts::CovstatsSample cs; gl_ctx* cs_pf = nullptr; };
+// bins: the index's binning section, read again from index_path on the first region query (bins_read), so that only
+// handles that query pay for it.
+struct gl_bam {
+    glhts::BamFile f; glhts::ContigSegs segs; glhts::CovstatsSample cs; gl_ctx* cs_pf = nullptr;
+    std::vector<glhts::BaiBins> bins; bool bins_read = false;
+};
+// The virtual-offset ranges that hold every record of reference tid overlapping one of the intervals [beg[i], end[i])
+// (glhts::bai_region_chunks over b's index).  "" or an error: no index, or its binning section cannot be read.
+std::string gl_bam_plan_regions(gl_bam& b, int tid, const int64_t* beg, const int64_t* end, int64_t n,
+                                std::vector<std::pair<uint64_t, uint64_t>>& out);
 // covstats.cu: join and forget ctx's covstats prefetch, if any
 void cs_prefetch_drop(gl_ctx* ctx);

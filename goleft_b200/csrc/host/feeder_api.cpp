@@ -17,6 +17,21 @@ static void put_err(char* err, int64_t cap, const std::string& m) {
     err[n] = 0;
 }
 
+std::string gl_bam_plan_regions(gl_bam& b, int tid, const int64_t* beg, const int64_t* end, int64_t n,
+                                std::vector<std::pair<uint64_t, uint64_t>>& out) {
+    out.clear();
+    if (!b.f.has_index) return "no index";
+    if (!b.bins_read) {
+        glhts::BaiIndex again;
+        const std::string e = glhts::bai_read(b.f.index_path, again, &b.bins);
+        if (!e.empty()) { b.bins.clear(); return e; }
+        b.bins_read = true;
+    }
+    if (tid < 0 || tid >= (int)b.bins.size() || tid >= (int)b.f.bai.ioffsets.size()) return "";
+    glhts::bai_region_chunks(b.bins[(size_t)tid], b.f.bai.ioffsets[(size_t)tid], beg, end, n, out);
+    return "";
+}
+
 extern "C" {
 
 int gl_bam_decode_segments(const char* path, int32_t min_mapq, int32_t threads, int32_t only_tid, gl_segset** out,
@@ -125,6 +140,20 @@ int gl_bam_decode(gl_bam* b, int32_t tid, int64_t beg, int64_t end, int32_t min_
     out->n_records = st.n_records; out->n_pass = st.n_pass; out->bytes_in = st.bytes_in; out->bytes_out = st.bytes_out;
     out->inflate_s = st.inflate_s; out->parse_s = st.parse_s; out->wall_s = st.wall_s; out->units = st.units;
     out->max_len = b->segs.max_len;
+    return GL_OK;
+}
+
+int gl_bam_region_chunks(const gl_bam* b, int32_t tid, const int64_t* beg, const int64_t* end, int64_t n, uint64_t* vb, uint64_t* ve,
+                         int64_t cap, int64_t* n_out) {
+    if (!b || !n_out || n < 0 || (n > 0 && (!beg || !end)) || cap < 0 || (cap > 0 && (!vb || !ve))) return GL_EINVAL;
+    *n_out = 0;
+    if (!b->f.has_index) return GL_ESTATE;
+    if (tid < 0 || tid >= (int32_t)b->f.header.refs.size()) return GL_EINVAL;
+    std::vector<std::pair<uint64_t, uint64_t>> r;
+    if (!gl_bam_plan_regions(const_cast<gl_bam&>(*b), tid, beg, end, n, r).empty()) return GL_ESTATE;   // fills the handle's bin cache
+    *n_out = (int64_t)r.size();
+    if ((int64_t)r.size() > cap) return GL_ERANGE;
+    for (size_t i = 0; i < r.size(); i++) { vb[i] = r[i].first; ve[i] = r[i].second; }
     return GL_OK;
 }
 

@@ -120,7 +120,7 @@ std::vector<std::string> BamHeader::sample_names() const {
 }
 
 // ---------------------------------------------------------------------------------------------- BAI
-std::string bai_read(const std::string& path, BaiIndex& out) {
+std::string bai_read(const std::string& path, BaiIndex& out, std::vector<BaiBins>* bins) {
     FILE* f = fopen(path.c_str(), "rb");
     if (!f) return "cannot open " + path;
     std::vector<uint8_t> b;
@@ -138,9 +138,11 @@ std::string bai_read(const std::string& path, BaiIndex& out) {
     out.has_stats.assign((size_t)n_ref, 0);
     out.ref_beg.assign((size_t)n_ref, 0);
     out.ref_end.assign((size_t)n_ref, 0);
+    if (bins) bins->assign((size_t)n_ref, BaiBins());
     for (int32_t r = 0; r < n_ref; r++) {
         if (off + 4 > b.size()) return "truncated BAI: " + path;
         const int32_t n_bin = rdi32(b.data() + off); off += 4;
+        std::vector<std::pair<uint32_t, size_t>> at;                       // (bin, offset of its chunk list) when bins are kept
         for (int32_t k = 0; k < n_bin; k++) {
             if (off + 8 > b.size()) return "truncated BAI: " + path;
             const uint32_t bin = rd32(b.data() + off);
@@ -152,6 +154,7 @@ std::string bai_read(const std::string& path, BaiIndex& out) {
                 out.unmapped[r] = rd64(b.data() + off + 24);
                 out.has_stats[r] = 1;
             } else {
+                if (bins) at.emplace_back(bin, off - 4);
                 for (int32_t c = 0; c < n_chunk; c++) {
                     const uint64_t cb = rd64(b.data() + off + 16 * (size_t)c), ce = rd64(b.data() + off + 16 * (size_t)c + 8);
                     if (out.ref_beg[r] == 0 || cb < out.ref_beg[r]) out.ref_beg[r] = cb;
@@ -159,6 +162,20 @@ std::string bai_read(const std::string& path, BaiIndex& out) {
                 }
             }
             off += 16 * (size_t)n_chunk;
+        }
+        if (bins) {
+            BaiBins& B = (*bins)[(size_t)r];
+            std::sort(at.begin(), at.end());
+            for (const auto& bo : at) {
+                const int32_t n_chunk = rdi32(b.data() + bo.second);
+                B.bin.push_back(bo.first);
+                B.first.push_back((uint32_t)B.cb.size());
+                for (int32_t c = 0; c < n_chunk; c++) {
+                    B.cb.push_back(rd64(b.data() + bo.second + 4 + 16 * (size_t)c));
+                    B.ce.push_back(rd64(b.data() + bo.second + 12 + 16 * (size_t)c));
+                }
+            }
+            B.first.push_back((uint32_t)B.cb.size());
         }
         if (off + 4 > b.size()) return "truncated BAI: " + path;
         const int32_t n_intv = rdi32(b.data() + off); off += 4;
@@ -169,6 +186,60 @@ std::string bai_read(const std::string& path, BaiIndex& out) {
     }
     out.n_no_coor = (off + 8 <= b.size()) ? rd64(b.data() + off) : 0;
     return "";
+}
+
+void bai_region_chunks(const BaiBins& bins, const std::vector<uint64_t>& lin, const int64_t* beg, const int64_t* end, int64_t n,
+                       std::vector<std::pair<uint64_t, uint64_t>>& out) {
+    out.clear();
+    const int64_t kMax = int64_t(1) << 29;                             // BAI bins cover [0, 2^29)
+    constexpr int64_t kBins = 37450;                                   // ((1 << 18) - 1) / 7 + 1: the stats pseudo-bin and up are not bins
+    auto find = [&](int64_t k) -> int64_t {                            // index of bin k with chunks, or -1
+        const auto it = std::lower_bound(bins.bin.begin(), bins.bin.end(), (uint32_t)k);
+        if (it == bins.bin.end() || *it != (uint32_t)k) return -1;
+        const size_t j = (size_t)(it - bins.bin.begin());
+        return bins.first[j + 1] > bins.first[j] ? (int64_t)j : -1;
+    };
+    // per bin: the loosest cut of the intervals naming it (smallest min_off, largest max_off)
+    std::vector<uint64_t> lo_of, hi_of;
+    std::vector<uint32_t> named;
+    for (int64_t i = 0; i < n; i++) {
+        const int64_t b = std::max<int64_t>(beg[i], 0), e = std::min<int64_t>(end[i], kMax);
+        if (e <= b) continue;
+        if (lo_of.empty()) { lo_of.assign(kBins, UINT64_MAX); hi_of.assign(kBins, 0); }
+        const uint64_t min_off = lin.empty() ? 0 : lin[(size_t)std::min<int64_t>(b >> 14, (int64_t)lin.size() - 1)];
+        // max_off: the first chunk of the nearest bin with chunks to the right of the interval (its records start at or
+        // after e, and so does every record after them); moving right, a first child goes up to its parent
+        uint64_t max_off = UINT64_MAX;
+        for (int64_t k = 4681 + ((e - 1) >> 14) + 1;; k++) {
+            if (k >= kBins) k = 0;
+            while (k % 8 == 1) k = (k - 1) >> 3;
+            if (k == 0) break;
+            const int64_t j = find(k);
+            if (j < 0) continue;
+            max_off = *std::min_element(bins.cb.begin() + bins.first[(size_t)j], bins.cb.begin() + bins.first[(size_t)j + 1]);
+            break;
+        }
+        static const int kFirst[6] = {0, 1, 9, 73, 585, 4681}, kShift[6] = {29, 26, 23, 20, 17, 14};
+        for (int l = 0; l < 6; l++)                                    // reg2bins: every level, the bins [b, e - 1] touches
+            for (int64_t k = kFirst[l] + (b >> kShift[l]); k <= kFirst[l] + ((e - 1) >> kShift[l]); k++) {
+                if (lo_of[(size_t)k] == UINT64_MAX && hi_of[(size_t)k] == 0) named.push_back((uint32_t)k);
+                lo_of[(size_t)k] = std::min(lo_of[(size_t)k], min_off);
+                hi_of[(size_t)k] = std::max(hi_of[(size_t)k], max_off);
+            }
+    }
+    for (uint32_t k : named) {
+        const int64_t j = find(k);
+        if (j < 0) continue;
+        for (uint32_t c = bins.first[(size_t)j]; c < bins.first[(size_t)j + 1]; c++)
+            if (bins.ce[c] > lo_of[k] && bins.cb[c] < hi_of[k] && bins.ce[c] > bins.cb[c]) out.emplace_back(bins.cb[c], bins.ce[c]);
+    }
+    std::sort(out.begin(), out.end());
+    size_t m = 0;
+    for (size_t i = 0; i < out.size(); i++) {
+        if (m > 0 && out[i].first <= out[m - 1].second) out[m - 1].second = std::max(out[m - 1].second, out[i].second);
+        else out[m++] = out[i];
+    }
+    out.resize(m);
 }
 
 // ---------------------------------------------------------------------------------------------- CRAI

@@ -4,6 +4,7 @@
 #pragma once
 #include <stdint.h>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace glhts {
@@ -48,7 +49,24 @@ struct BaiIndex {
     std::vector<uint64_t> ref_beg, ref_end;              // virtual-offset range of the reference's records (min chunk begin /
                                                          // max chunk end over its bins; 0 = no records)
 };
-std::string bai_read(const std::string& path, BaiIndex& out);
+// One reference's binning index (SAM spec 5.2): the chunks of every bin but the stats pseudo-bin, bins in ascending order;
+// bin[i]'s chunks are [cb, ce)[first[i] .. first[i+1]).
+struct BaiBins {
+    std::vector<uint32_t> bin, first;
+    std::vector<uint64_t> cb, ce;
+};
+// bins (may be null): also keep every reference's binning index.  Most callers only want the linear index and the stats
+// bin, and a WGS index's chunks are several MB, so they are dropped unless asked for.
+std::string bai_read(const std::string& path, BaiIndex& out, std::vector<BaiBins>* bins = nullptr);
+// The virtual-offset ranges a query of intervals [beg[i], end[i]) on one reference has to read, as htslib's BAI query
+// (hts_itr_query) picks them: the chunks of every bin reg2bins (SAM spec 5.3) names for an interval, less those that end
+// at or before min_off, the linear-index offset of the interval's first 16 KB tile (past the linear index: its last entry),
+// and those that begin at or after max_off, the first chunk of the nearest bin with chunks to the right of the interval
+// (htslib's walk: right along the leaves, up to the parent at a first child).  A bin several intervals name keeps the
+// chunks any of them would keep between its smallest min_off and its largest max_off.  Sorted by begin, overlapping or
+// touching ranges merged.  Empty intervals name no bins.
+void bai_region_chunks(const BaiBins& bins, const std::vector<uint64_t>& lin, const int64_t* beg, const int64_t* end, int64_t n,
+                       std::vector<std::pair<uint64_t, uint64_t>>& out);
 
 // ---------------------------------------------------------------------------------------------- CRAI
 // .crai (gzip'd text, 6 tab columns) -> per reference slices; sizes = the 16 KB pseudo-tiles indexcov uses for

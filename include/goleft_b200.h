@@ -334,6 +334,25 @@ int  gl_bam_decode(gl_bam* b, int32_t tid, int64_t beg, int64_t end, int32_t min
  * (no usable index, a member or record the device code rejects): use gl_bam_decode. */
 int  gl_bam_decode_device(gl_ctx* ctx, gl_bam* b, int32_t tid, int32_t min_mapq, const int32_t** d_start, const int32_t** d_end, int64_t* n,
                           gl_bam_segments* stats);
+/* Region queries of an indexed BAM: only the BGZF members that hold records overlapping a set of intervals of one reference.
+ * gl_bam_region_chunks (host only): the virtual-offset ranges [vb[i], ve[i]) such a query reads, as htslib's BAI query
+ *   picks them — the chunks of every bin reg2bins (SAM spec 5.3) names for an interval [beg[i], end[i]), less the chunks
+ *   ending at or before the linear-index offset of the interval's first 16 KB tile (the last entry past the linear index)
+ *   and those beginning at or after the first chunk of the nearest bin with chunks right of the interval — sorted,
+ *   overlapping or touching ranges merged.  The intervals may be in any order, overlap, be empty or reach past the
+ *   contig.  The handle reads its index's bins on the first query (gl_bam_open does not keep them).  *n_out = the number
+ *   of ranges; GL_ERANGE when it exceeds cap; GL_ESTATE: no index; GL_EINVAL: a null pointer, n < 0 or tid not in the header.
+ * gl_bam_decode_device_regions: gl_bam_decode_device over those ranges.  *d_start / *d_end (ctx-owned, valid until the next
+ *   decode call on this ctx) hold the M/=/X blocks of the passing records that intersect at least one interval, whole
+ *   (not clipped), in BAM order: records in file order, each record's blocks ascending.  stats: bytes_in = compressed bytes
+ *   read, n_records = records of tid parsed in the ranges.  When the ranges cover half the reference's compressed bytes
+ *   or more, the whole reference is read as one range.  GL_ESTATE wherever gl_bam_decode_device gives it: use
+ *   gl_bam_decode. */
+int  gl_bam_region_chunks(const gl_bam* b, int32_t tid, const int64_t* beg, const int64_t* end, int64_t n, uint64_t* vb, uint64_t* ve,
+                          int64_t cap, int64_t* n_out);
+int  gl_bam_decode_device_regions(gl_ctx* ctx, gl_bam* b, int32_t tid, const int64_t* beg, const int64_t* end, int64_t n,
+                                  int32_t min_mapq, const int32_t** d_start, const int32_t** d_end, int64_t* n_seg,
+                                  gl_bam_segments* stats);
 /* BGZF inflate ON THE GPU (inflate.cu): one warp per BGZF member, thousands in flight — the stage the reference's samtools
  * children (and this library's host feeder) spend their time in.  Block b = d_comp[comp_off[b], comp_off[b+1]) (the whole
  * member) -> d_out[out_off[b], out_off[b+1]), out_off from the members' ISIZE fields; d_status[b] != 0: malformed or

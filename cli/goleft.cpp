@@ -192,11 +192,20 @@ static std::vector<std::thread> start_workers(const GpuPlan& p, const std::funct
     return th;
 }
 
-// the index of an input (indexcov.go:500-510): x.bam.bai, else x.bai; a .bai names itself
+// the index of an input (indexcov.go:500-510): a .bai or .csi names itself; else the first of x.bam.bai, x.bai, x.bam.csi,
+// x.csi that exists (BamFile::open's order), and when none does the x.bai whose read error the caller reports
 static std::string bai_path(const std::string& b) {
-    std::string p = ends_with(b, ".bai") ? b : b + ".bai";
-    if (!file_exists(p)) p = b.substr(0, b.size() - 4) + (ends_with(b, ".bai") ? "" : ".bai");
-    return p;
+    if (ends_with(b, ".csi")) return b;
+    if (ends_with(b, ".bai")) return file_exists(b) ? b : b.substr(0, b.size() - 4);
+    for (const std::string& p : glhts::index_candidates(b)) if (file_exists(p)) return p;
+    return b.substr(0, b.size() - 4) + ".bai";
+}
+
+// indexcov and indexsplit size 16384-base tiles: a CSI whose tiles are wider cannot give them
+static void refuse_wide_csi(const glhts::BaiIndex& idx, const std::string& path, const char* prog) {
+    if (idx.is_csi && idx.min_shift > 14)
+        fatal(1, "%s: %s is a CSI with min_shift %d: its tiles are wider than the 16384 bases indexcov sizes (min_shift 14 or less is needed)",
+              prog, path.c_str(), idx.min_shift);
 }
 
 // CRAM pseudo-tile sizes of every reference of a .crai (crai.go:56-127), concatenated; ref_ptr[r] is where reference r's begin
@@ -495,13 +504,16 @@ struct DepthEngine {
     }
 
     // ---- .fai mode: one contig.  The GPU pass covers at most 2^30-1 bases; longer contigs go in whole-chunk pieces
-    //      whose texts concatenate (chunk edges are run breaks anyway).
+    //      whose texts concatenate (chunk edges are run breaks anyway).  The GPU feeder decodes a whole contig, or each piece
+    //      of a longer one as a region query of [ps, pe) (only a CSI can index past 2^29); the host feeder is the fallback.
     void run_contig(DepthJob& job) {
         const long long kMaxPass = ((1LL << 30) - 1) / o.step * o.step;
         const char* c = job.chrom.c_str();
         for (long long ps = 0; ps < job.len; ps += kMaxPass) {
             const long long pe = std::min(job.len, ps + kMaxPass);
-            src.fetch(ctx, gbam, tid(job.chrom), ps, pe, o.Q, o.threads, 0, ps == 0 && pe == job.len, &job.dec, &job.gpu_fed);
+            const bool whole_ref = ps == 0 && pe == job.len;
+            if (!whole_ref && src.fetch_regions(ctx, gbam, tid(job.chrom), {ps}, {pe}, o.Q, &job.dec)) job.gpu_fed++;
+            else src.fetch(ctx, gbam, tid(job.chrom), ps, pe, o.Q, o.threads, 0, whole_ref, &job.dec, &job.gpu_fed);
             const double tg = now_s();
             const bool dtext = !o.stats && job.chrom.size() <= 64;
             if (dtext && src.on_device) {                                      // segments already on the device (GPU feeder)
@@ -704,7 +716,7 @@ static int cmd_depth(int argc, char** argv) {
             usable = any;
         }
         if (!usable) {
-            fprintf(stderr, "goleft depth: no usable .bai next to %s: decoding the whole file (index it for -c / --bed to read only what they need)\n", bam.c_str());
+            fprintf(stderr, "goleft depth: no usable index (.bai or .csi) next to %s: decoding the whole file (index it for -c / --bed to read only what they need)\n", bam.c_str());
             int thr = o.threads > 0 ? o.threads : (int)std::max(1u, std::thread::hardware_concurrency());
             int only = -1;
             if (!chrom.empty()) for (size_t i = 0; i < probe.header.refs.size(); i++) if (probe.header.refs[i].name == chrom) only = (int)i;
@@ -1374,10 +1386,13 @@ static int cmd_indexcov(int argc, char** argv) {
         }
         read_err[i] = glhts::bai_read(bai_path(b), idx[i]);
         if (!read_err[i].empty()) return;
-        if (ends_with(b, ".bai")) names[i] = short_name(b, true, nullptr);
+        if (ends_with(b, ".bai") || ends_with(b, ".csi")) names[i] = short_name(b, true, nullptr);
         else { glhts::BamHeader h; read_err[i] = glhts::bam_read_header(b, h); if (read_err[i].empty()) names[i] = short_name(b, false, &h); }
     });
-    for (size_t i = 0; i < S; i++) if (!read_err[i].empty()) fatal(1, "%s", read_err[i].c_str());
+    for (size_t i = 0; i < S; i++) {
+        if (!read_err[i].empty()) fatal(1, "%s", read_err[i].c_str());
+        if (!ends_with(bams[i], ".crai")) refuse_wide_csi(idx[i], bai_path(bams[i]), "indexcov");
+    }
 
     ic_mark("read indexes");
     // ---- GPUs (SURVEY 8(e): samples are independent through I5 -> sample-sharded over the GPUs; the rows need every sample
@@ -2021,6 +2036,7 @@ static int cmd_indexsplit(int argc, char** argv) {
             glhts::BaiIndex bai;
             std::string e = glhts::bai_read(bai_path(b), bai);
             if (!e.empty()) fatal(1, "%s", e.c_str());
+            refuse_wide_csi(bai, bai_path(b), "indexsplit");
             const size_t nr = bai.ioffsets.size();
             std::vector<uint64_t> voff;
             std::vector<int64_t> rp(nr + 1, 0);

@@ -158,6 +158,7 @@ _proto("gl_bam_open", C.c_int, C.c_char_p, C.POINTER(_vp), _vp, C.c_int64)
 _proto("gl_bam_close", None, _vp)
 _proto("gl_bam_info", C.c_int, _vp, _i32p, _i32p)
 _proto("gl_bam_ref", C.c_int, _vp, C.c_int32, C.POINTER(C.c_char_p), _i64p, _i64p)
+_proto("gl_bam_index", C.c_int, _vp, C.POINTER(C.c_char_p), _i32p, _i32p, _i32p)
 _proto("gl_bam_decode", C.c_int, _vp, C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
 _proto("gl_bam_decode_device", C.c_int, _vp, _vp, C.c_int32, C.c_int32, C.POINTER(_vp), C.POINTER(_vp), _i64p, _vp)
 _proto("gl_bam_decode_device_regions", C.c_int, _vp, _vp, C.c_int32, _vp, _vp, C.c_int64, C.c_int32, C.POINTER(_vp), C.POINTER(_vp), _i64p, _vp)
@@ -166,6 +167,7 @@ _proto("gl_bgzf_inflate_device", C.c_int, _vp, _vp, _vp, _vp, C.c_int64, _vp, _v
 _proto("gl_bai_read", C.c_int, C.c_char_p, C.POINTER(_vp), _vp, C.c_int64)
 _proto("gl_bai_n_refs", C.c_int, _vp, _i32p, _u64p)
 _proto("gl_bai_ref", C.c_int, _vp, C.c_int32, C.POINTER(_vp), _i64p, _u64p, _u64p, _i32p)
+_proto("gl_bai_geometry", C.c_int, _vp, _i32p, _i32p, _i32p)
 _proto("gl_bai_free", None, _vp)
 _proto("gl_pack_segments16_bound", C.c_int64, C.c_int64)
 _proto("gl_pack_segments16", C.c_int, _vp, _vp, C.c_int64, _vp, _vp, _vp, C.c_int64, _i64p)
@@ -744,6 +746,11 @@ class Bam:
         n, hi = C.c_int32(0), C.c_int32(0)
         lib.gl_bam_info(h, C.byref(n), C.byref(hi))
         self.has_index = bool(hi.value)
+        self.index_path, self.index_geometry = None, None      # the .bai / .csi loaded, and its (min_shift, depth, is_csi)
+        if self.has_index:
+            ip, ms, dp, ic = C.c_char_p(), C.c_int32(0), C.c_int32(0), C.c_int32(0)
+            if lib.gl_bam_index(h, C.byref(ip), C.byref(ms), C.byref(dp), C.byref(ic)) == GL_OK:
+                self.index_path, self.index_geometry = ip.value.decode(), (ms.value, dp.value, bool(ic.value))
         self.refs = []
         for tid in range(n.value):
             name, ln, nm = C.c_char_p(), C.c_int64(0), C.c_int64(0)
@@ -925,6 +932,8 @@ def crai_make_sizes(start, span, nbytes) -> np.ndarray:
 
 
 def bai_read(path: str):
+    """A BAI or CSI -> dict(ioffsets (16 KB linear index per reference; rebuilt from the bins for a CSI), mapped, unmapped,
+    has_stats, n_no_coor, min_shift, depth, is_csi); GlError on a file that is neither, or a malformed one."""
     h = _vp()
     err = C.create_string_buffer(512)
     rc = lib.gl_bai_read(path.encode(), C.byref(h), C.cast(err, _vp), 512)
@@ -933,12 +942,15 @@ def bai_read(path: str):
     try:
         n, nc = C.c_int32(0), C.c_uint64(0)
         lib.gl_bai_n_refs(h, C.byref(n), C.byref(nc))
-        out = {"ioffsets": [], "mapped": [], "unmapped": [], "n_no_coor": nc.value}
+        ms, dp, ic = C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        lib.gl_bai_geometry(h, C.byref(ms), C.byref(dp), C.byref(ic))
+        out = {"ioffsets": [], "mapped": [], "unmapped": [], "has_stats": [], "n_no_coor": nc.value, "min_shift": ms.value,
+               "depth": dp.value, "is_csi": bool(ic.value)}
         for tid in range(n.value):
             p, k, m, u, hs = _vp(), C.c_int64(0), C.c_uint64(0), C.c_uint64(0), C.c_int32(0)
             lib.gl_bai_ref(h, tid, C.byref(p), C.byref(k), C.byref(m), C.byref(u), C.byref(hs))
             out["ioffsets"].append(np.ctypeslib.as_array(C.cast(p, _u64p), (k.value,)).copy() if k.value else np.zeros(0, np.uint64))
-            out["mapped"].append(m.value); out["unmapped"].append(u.value)
+            out["mapped"].append(m.value); out["unmapped"].append(u.value); out["has_stats"].append(bool(hs.value))
         return out
     finally:
         lib.gl_bai_free(h)

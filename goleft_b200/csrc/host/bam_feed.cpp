@@ -184,10 +184,7 @@ std::string BamFile::open(const std::string& p, bool with_index) {
     }
     if (!done) return "truncated BAM header: " + p;
     if (!with_index) return "";
-    std::string cand[2] = {p + ".bai", p};
-    if (p.size() > 4 && p.compare(p.size() - 4, 4, ".bam") == 0) cand[1] = p.substr(0, p.size() - 4) + ".bai"; else cand[1].clear();
-    for (const std::string& ip : cand) {
-        if (ip.empty()) continue;
+    for (const std::string& ip : index_candidates(p)) {
         struct stat s2;
         if (stat(ip.c_str(), &s2) != 0) continue;
         BaiIndex b;
@@ -200,14 +197,16 @@ std::string BamFile::decode(int tid, int64_t beg, int64_t end, int min_mapq, int
     const double t_wall = now_s();
     out = ContigSegs();
     if (fd_ < 0) return "BAM not open";
-    if (!has_index) return "no .bai index for " + path;
+    if (!has_index) return "no .bai or .csi index for " + path;
     if (tid < 0 || tid >= (int)header.refs.size() || tid >= (int)bai.ioffsets.size()) return "";
     const std::vector<uint64_t>& lin = bai.ioffsets[(size_t)tid];
     const int64_t ref_len = header.refs[(size_t)tid].length;
     if (beg < 0) beg = 0;
     if (end > ref_len) end = ref_len;
     if (lin.empty() || end <= beg) return "";
-    const int64_t t0 = beg >> 14;
+    // past a BAI's linear index no record reaches the region; a CSI's rebuilt one ends at the last tile a bin starts in, and
+    // a record that starts before it may reach further: start from its last entry
+    const int64_t t0 = bai.is_csi ? std::min<int64_t>(beg >> 14, (int64_t)lin.size() - 1) : beg >> 14;
     if (t0 >= (int64_t)lin.size()) return "";                        // no record reaches the region
     const int64_t t1 = std::min<int64_t>((int64_t)lin.size() - 1, (end - 1) >> 14);
     // ---- units: cut at linear-index offsets (each is the first record overlapping a 16 KB tile: record-aligned)

@@ -37,13 +37,13 @@ public:
     BamFile() {}
     ~BamFile();
     BamFile(const BamFile&) = delete;
-    // opens path and parses its header; with_index: also loads path + ".bai" (or path with .bam replaced by .bai), and
-    // has_index tells whether one was found
+    // opens path and parses its header; with_index: also loads the first index of index_candidates(path) that reads (a BAI
+    // or a CSI), and has_index tells whether one was found
     std::string open(const std::string& path, bool with_index = true);
     bool has_index = false;
     BamHeader header;
     BaiIndex bai;
-    std::string path, index_path;               // index_path: the .bai that was loaded
+    std::string path, index_path;               // index_path: the .bai or .csi that was loaded
     // M/=/X blocks of the records of reference `tid` that pass the samtools-depth filter (glbam::depth_counts) and can
     // overlap [beg, end).  want: 0 = choose (packed8 unless the blocks are long), 8, 32.  Needs the index.
     std::string decode(int tid, int64_t beg, int64_t end, int min_mapq, int threads, int want, ContigSegs& out, DecodeStats* st);

@@ -1,5 +1,6 @@
 // feeder_api.cpp — C ABI over the host readers (hts_io): the segment feeder that replaces the
-// `samtools depth` child's decode + filter (depth/depth.go:45) and biogo's BAI reader (indexcov.go:514).
+// `samtools depth` child's decode + filter (depth/depth.go:45) and biogo's BAI reader (indexcov.go:514), which
+// here reads CSI too.
 #include <string.h>
 #include <string>
 #include <vector>
@@ -28,7 +29,7 @@ std::string gl_bam_plan_regions(gl_bam& b, int tid, const int64_t* beg, const in
         b.bins_read = true;
     }
     if (tid < 0 || tid >= (int)b.bins.size() || tid >= (int)b.f.bai.ioffsets.size()) return "";
-    glhts::bai_region_chunks(b.bins[(size_t)tid], b.f.bai.ioffsets[(size_t)tid], beg, end, n, out);
+    glhts::bai_region_chunks(b.bins[(size_t)tid], b.f.bai.ioffsets[(size_t)tid], b.f.bai.min_shift, b.f.bai.depth, beg, end, n, out);
     return "";
 }
 
@@ -92,6 +93,14 @@ int gl_bai_ref(const gl_bai* b, int32_t tid, const uint64_t** ioffsets, int64_t*
     return GL_OK;
 }
 
+int gl_bai_geometry(const gl_bai* b, int32_t* min_shift, int32_t* depth, int32_t* is_csi) {
+    if (!b) return GL_EINVAL;
+    if (min_shift) *min_shift = b->b.min_shift;
+    if (depth) *depth = b->b.depth;
+    if (is_csi) *is_csi = b->b.is_csi ? 1 : 0;
+    return GL_OK;
+}
+
 void gl_bai_free(gl_bai* b) { delete b; }
 
 // ---- index-guided parallel feeder (bam_feed.h)
@@ -113,6 +122,16 @@ int gl_bam_info(const gl_bam* b, int32_t* n_refs, int32_t* has_index) {
     if (!b) return GL_EINVAL;
     if (n_refs) *n_refs = (int32_t)b->f.header.refs.size();
     if (has_index) *has_index = b->f.has_index ? 1 : 0;
+    return GL_OK;
+}
+
+int gl_bam_index(const gl_bam* b, const char** path, int32_t* min_shift, int32_t* depth, int32_t* is_csi) {
+    if (!b) return GL_EINVAL;
+    if (!b->f.has_index) return GL_ESTATE;
+    if (path) *path = b->f.index_path.c_str();
+    if (min_shift) *min_shift = b->f.bai.min_shift;
+    if (depth) *depth = b->f.bai.depth;
+    if (is_csi) *is_csi = b->f.bai.is_csi ? 1 : 0;
     return GL_OK;
 }
 

@@ -1,4 +1,4 @@
-// hts_io.cpp — BAI / CRAI / FAI readers, the BAM header's sample names and a BGZF writer (see hts_io.h).
+// hts_io.cpp — BAI / CSI / CRAI / FAI readers, the BAM header's sample names and a BGZF writer (see hts_io.h).
 #include "hts_io.h"
 #include <stdio.h>
 #include <string.h>
@@ -119,16 +119,12 @@ std::vector<std::string> BamHeader::sample_names() const {
     return names;
 }
 
-// ---------------------------------------------------------------------------------------------- BAI
-std::string bai_read(const std::string& path, BaiIndex& out, std::vector<BaiBins>* bins) {
-    FILE* f = fopen(path.c_str(), "rb");
-    if (!f) return "cannot open " + path;
-    std::vector<uint8_t> b;
-    uint8_t tmp[1 << 16];
-    size_t got;
-    while ((got = fread(tmp, 1, sizeof tmp, f)) > 0) b.insert(b.end(), tmp, tmp + got);
-    fclose(f);
-    if (b.size() < 8 || memcmp(b.data(), "BAI\1", 4) != 0) return "not a BAI file: " + path;
+// ---------------------------------------------------------------------------------------------- BAI / CSI
+namespace {
+
+// the BAI layout (SAM spec 5.2), b starting with its magic
+std::string bai_parse(const std::vector<uint8_t>& b, const std::string& path, BaiIndex& out, std::vector<BaiBins>* bins) {
+    out.min_shift = 14; out.depth = 5; out.is_csi = false;
     size_t off = 4;
     const int32_t n_ref = rdi32(b.data() + off); off += 4;
     if (n_ref < 0) return "corrupt BAI: " + path;
@@ -188,29 +184,210 @@ std::string bai_read(const std::string& path, BaiIndex& out, std::vector<BaiBins
     return "";
 }
 
-void bai_region_chunks(const BaiBins& bins, const std::vector<uint64_t>& lin, const int64_t* beg, const int64_t* end, int64_t n,
-                       std::vector<std::pair<uint64_t, uint64_t>>& out) {
+// a BGZF file (concatenated gzip members) inflated whole; false when a member is malformed or cut short
+bool gunzip_all(const std::vector<uint8_t>& in, std::vector<uint8_t>& out) {
+    z_stream zs;
+    memset(&zs, 0, sizeof zs);
+    if (inflateInit2(&zs, 15 + 16) != Z_OK) return false;
+    zs.next_in = const_cast<Bytef*>(in.data());
+    zs.avail_in = (uInt)in.size();
+    uint8_t buf[1 << 16];
+    bool ok = true;
+    for (;;) {
+        zs.next_out = buf;
+        zs.avail_out = sizeof buf;
+        const int rc = inflate(&zs, Z_NO_FLUSH);
+        out.insert(out.end(), buf, buf + (sizeof buf - zs.avail_out));
+        if (rc == Z_STREAM_END) {
+            if (zs.avail_in == 0) break;
+            if (inflateReset(&zs) != Z_OK) { ok = false; break; }
+        } else if (rc != Z_OK) {                                           // Z_BUF_ERROR: the input ends inside a member
+            ok = false;
+            break;
+        }
+    }
+    inflateEnd(&zs);
+    return ok;
+}
+
+inline int64_t bin_first(int level) { return ((int64_t(1) << (3 * level)) - 1) / 7; }   // the first bin of a level (CSIv1)
+
+// No BAM record starts at or past 2^31 (positions are int32): bins whose first base lies there take no part in the linear
+// index, which keeps it at most 2^17 entries whatever the geometry.
+constexpr int64_t kBamPosEnd = int64_t(1) << 31;
+
+// The 16 KB linear index of one reference of a CSI, rebuilt from its bins' loffsets.  bots: (the bin's first tile at
+// 2^min_shift granularity, its loffset) of every real bin with loffset != 0.
+//   F[x] = the smallest loffset of the bins whose first tile is x; a tile no bin starts in takes the value of the nearest
+//   known tile to its left, leading unknown tiles the first known value; F has max x + 1 entries.
+//   min_shift <= 14: lin[t] = F[t << (14 - min_shift)], ceil(|F| / 2^(14 - min_shift)) entries;
+//   min_shift >  14: lin[t] = F[t >> (min_shift - 14)], |F| << (min_shift - 14) entries (at most 2^17).
+// Why this is safe: an indexer that follows htslib fills its 2^min_shift-tile linear index (every tile a record overlaps
+// takes the first such record; gaps take the value on their left) and sets each bin's loffset to that index at the bin's
+// first tile.  So F equals that filled index at every tile some bin starts in, and is never above it elsewhere, because the
+// filled index does not decrease.  Every entry is therefore a record start at or before the first record that overlaps the
+// tile: the host feeder, the device decode and the region planner may start there (and cut parse units there) without
+// dropping a record.  With min_shift > 14 one wide tile's value stands for each 16 KB tile inside it: still such a bound.
+std::vector<uint64_t> csi_linear(std::vector<std::pair<int64_t, uint64_t>>& bots, int min_shift) {
+    std::vector<uint64_t> lin;
+    if (bots.empty()) return lin;
+    std::sort(bots.begin(), bots.end());
+    size_t m = 0;
+    for (size_t i = 0; i < bots.size(); i++)                          // one entry per tile: sorted, so the first is the smallest
+        if (m == 0 || bots[i].first != bots[m - 1].first) bots[m++] = bots[i];
+    bots.resize(m);
+    const int64_t n_f = bots.back().first + 1;
+    size_t j = 0;                                                      // F at increasing tiles x: a walk over bots
+    auto F = [&](int64_t x) -> uint64_t {
+        while (j + 1 < bots.size() && bots[j + 1].first <= x) j++;
+        return bots[j].first <= x ? bots[j].second : bots[0].second;
+    };
+    if (min_shift <= 14) {
+        const int s = 14 - min_shift;
+        const int64_t n = (n_f + (int64_t(1) << s) - 1) >> s;
+        lin.resize((size_t)n);
+        for (int64_t t = 0; t < n; t++) lin[(size_t)t] = F(t << s);
+    } else {
+        const int d = min_shift - 14;
+        const int64_t cap = kBamPosEnd >> 14;
+        const int64_t n = d >= 17 ? cap : std::min<int64_t>(n_f << d, cap);
+        lin.resize((size_t)n);
+        for (int64_t t = 0; t < n; t++) lin[(size_t)t] = F(t >> d);
+    }
+    return lin;
+}
+
+// the CSIv1 layout, b inflated and starting with its magic:
+//   "CSI\1" min_shift:i32 depth:i32 l_aux:i32 aux[l_aux] n_ref:i32
+//   per ref: n_bin:i32, per bin: bin:u32 loffset:u64 n_chunk:i32 (beg:u64 end:u64)[n_chunk];  [n_no_coor:u64]
+// The stats pseudo-bin ((1 << (3 depth + 3)) - 1) / 7 + 1 holds (ref_beg, ref_end), (mapped, unmapped), as BAI's 0x924a.
+std::string csi_parse(const std::vector<uint8_t>& b, const std::string& path, BaiIndex& out, std::vector<BaiBins>* bins) {
+    const std::string trunc = "truncated CSI: " + path, bad = "corrupt CSI: " + path;
+    if (b.size() < 16 || memcmp(b.data(), "CSI\1", 4) != 0) return "not a BAI or CSI file: " + path;
+    const int32_t min_shift = rdi32(b.data() + 4), depth = rdi32(b.data() + 8), l_aux = rdi32(b.data() + 12);
+    // bin numbers up to the pseudo-bin fit 32 bits for depth <= 10, and the addressable range 2^(min_shift + 3 depth) an int64
+    if (min_shift < 0 || depth < 0 || depth > 10 || min_shift + 3 * depth > 62)
+        return "unsupported CSI geometry (min_shift " + std::to_string(min_shift) + ", depth " + std::to_string(depth) + "): " + path;
+    if (l_aux < 0) return bad;
+    size_t off = 16;
+    if (off + (size_t)l_aux + 4 > b.size()) return trunc;
+    off += (size_t)l_aux;                                              // a tabix header: read past, not used
+    const int32_t n_ref = rdi32(b.data() + off); off += 4;
+    if (n_ref < 0) return bad;
+    out.min_shift = min_shift; out.depth = depth; out.is_csi = true;
+    out.ioffsets.assign((size_t)n_ref, {});
+    out.mapped.assign((size_t)n_ref, 0);
+    out.unmapped.assign((size_t)n_ref, 0);
+    out.has_stats.assign((size_t)n_ref, 0);
+    out.ref_beg.assign((size_t)n_ref, 0);
+    out.ref_end.assign((size_t)n_ref, 0);
+    if (bins) bins->assign((size_t)n_ref, BaiBins());
+    const int64_t n_real = bin_first(depth + 1);                      // bins 0 .. n_real - 1 are real
+    const uint32_t stats_bin = (uint32_t)(n_real + 1);
+    for (int32_t r = 0; r < n_ref; r++) {
+        if (off + 4 > b.size()) return trunc;
+        const int32_t n_bin = rdi32(b.data() + off); off += 4;
+        if (n_bin < 0) return bad;
+        std::vector<std::pair<uint32_t, size_t>> at;                   // (bin, offset of its chunk list) when bins are kept
+        std::vector<std::pair<int64_t, uint64_t>> bots;
+        for (int32_t k = 0; k < n_bin; k++) {
+            if (off + 16 > b.size()) return trunc;
+            const uint32_t bin = rd32(b.data() + off);
+            const uint64_t loff = rd64(b.data() + off + 4);
+            const int32_t n_chunk = rdi32(b.data() + off + 12);
+            off += 16;
+            if (n_chunk < 0 || off + 16 * (size_t)n_chunk > b.size()) return trunc;
+            if (bin == stats_bin && n_chunk == 2) {
+                out.mapped[r] = rd64(b.data() + off + 16);
+                out.unmapped[r] = rd64(b.data() + off + 24);
+                out.has_stats[r] = 1;
+            } else if ((int64_t)bin < n_real) {
+                if (bins) at.emplace_back(bin, off - 4);
+                for (int32_t c = 0; c < n_chunk; c++) {
+                    const uint64_t cb = rd64(b.data() + off + 16 * (size_t)c), ce = rd64(b.data() + off + 16 * (size_t)c + 8);
+                    if (out.ref_beg[r] == 0 || cb < out.ref_beg[r]) out.ref_beg[r] = cb;
+                    if (ce > out.ref_end[r]) out.ref_end[r] = ce;
+                }
+                int l = 0;
+                while (l < depth && (int64_t)bin >= bin_first(l + 1)) l++;
+                const int64_t bot = ((int64_t)bin - bin_first(l)) << (3 * (depth - l));
+                if (loff != 0 && (bot << min_shift) < kBamPosEnd) bots.emplace_back(bot, loff);
+            }                                                          // other ids (a pseudo-bin of another shape) are no bins
+            off += 16 * (size_t)n_chunk;
+        }
+        if (bins) {
+            BaiBins& B = (*bins)[(size_t)r];
+            std::sort(at.begin(), at.end());
+            for (const auto& bo : at) {
+                const int32_t n_chunk = rdi32(b.data() + bo.second);
+                B.bin.push_back(bo.first);
+                B.first.push_back((uint32_t)B.cb.size());
+                for (int32_t c = 0; c < n_chunk; c++) {
+                    B.cb.push_back(rd64(b.data() + bo.second + 4 + 16 * (size_t)c));
+                    B.ce.push_back(rd64(b.data() + bo.second + 12 + 16 * (size_t)c));
+                }
+            }
+            B.first.push_back((uint32_t)B.cb.size());
+        }
+        out.ioffsets[r] = csi_linear(bots, min_shift);
+    }
+    out.n_no_coor = (off + 8 <= b.size()) ? rd64(b.data() + off) : 0;
+    return "";
+}
+
+}  // namespace
+
+std::string bai_read(const std::string& path, BaiIndex& out, std::vector<BaiBins>* bins) {
+    FILE* f = fopen(path.c_str(), "rb");
+    if (!f) return "cannot open " + path;
+    std::vector<uint8_t> b;
+    uint8_t tmp[1 << 16];
+    size_t got;
+    while ((got = fread(tmp, 1, sizeof tmp, f)) > 0) b.insert(b.end(), tmp, tmp + got);
+    fclose(f);
+    if (b.size() >= 8 && memcmp(b.data(), "BAI\1", 4) == 0) return bai_parse(b, path, out, bins);
+    if (b.size() < 2 || b[0] != 0x1f || b[1] != 0x8b) return "not a BAI or CSI file: " + path;
+    std::vector<uint8_t> raw;
+    if (!gunzip_all(b, raw)) return "truncated or corrupt CSI: " + path;
+    return csi_parse(raw, path, out, bins);
+}
+
+std::vector<std::string> index_candidates(const std::string& p) {
+    const bool bam = p.size() > 4 && p.compare(p.size() - 4, 4, ".bam") == 0;
+    const std::string stem = bam ? p.substr(0, p.size() - 4) : std::string();
+    std::vector<std::string> c;
+    c.push_back(p + ".bai");
+    if (bam) c.push_back(stem + ".bai");
+    c.push_back(p + ".csi");
+    if (bam) c.push_back(stem + ".csi");
+    return c;
+}
+
+void bai_region_chunks(const BaiBins& bins, const std::vector<uint64_t>& lin, int min_shift, int depth, const int64_t* beg,
+                       const int64_t* end, int64_t n, std::vector<std::pair<uint64_t, uint64_t>>& out) {
     out.clear();
-    const int64_t kMax = int64_t(1) << 29;                             // BAI bins cover [0, 2^29)
-    constexpr int64_t kBins = 37450;                                   // ((1 << 18) - 1) / 7 + 1: the stats pseudo-bin and up are not bins
+    // the bins cover [0, 2^(min_shift + 3 depth)) (BAI: 2^29); no BAM record starts at or past 2^31
+    const int64_t kMax = std::min<int64_t>(int64_t(1) << (min_shift + 3 * depth), kBamPosEnd);
+    const int64_t kBins = bin_first(depth + 1) + 1;                    // the stats pseudo-bin and up are not bins (BAI: 37450)
+    const int64_t kLeaf = bin_first(depth);                            // the first leaf (BAI: 4681)
     auto find = [&](int64_t k) -> int64_t {                            // index of bin k with chunks, or -1
         const auto it = std::lower_bound(bins.bin.begin(), bins.bin.end(), (uint32_t)k);
         if (it == bins.bin.end() || *it != (uint32_t)k) return -1;
         const size_t j = (size_t)(it - bins.bin.begin());
         return bins.first[j + 1] > bins.first[j] ? (int64_t)j : -1;
     };
-    // per bin: the loosest cut of the intervals naming it (smallest min_off, largest max_off)
-    std::vector<uint64_t> lo_of, hi_of;
-    std::vector<uint32_t> named;
+    // (bin, min_off, max_off) for every interval that names the bin; a bin keeps the loosest cut (smallest min_off,
+    // largest max_off)
+    struct Named { uint32_t bin; uint64_t lo, hi; };
+    std::vector<Named> named;
     for (int64_t i = 0; i < n; i++) {
         const int64_t b = std::max<int64_t>(beg[i], 0), e = std::min<int64_t>(end[i], kMax);
         if (e <= b) continue;
-        if (lo_of.empty()) { lo_of.assign(kBins, UINT64_MAX); hi_of.assign(kBins, 0); }
         const uint64_t min_off = lin.empty() ? 0 : lin[(size_t)std::min<int64_t>(b >> 14, (int64_t)lin.size() - 1)];
         // max_off: the first chunk of the nearest bin with chunks to the right of the interval (its records start at or
         // after e, and so does every record after them); moving right, a first child goes up to its parent
         uint64_t max_off = UINT64_MAX;
-        for (int64_t k = 4681 + ((e - 1) >> 14) + 1;; k++) {
+        for (int64_t k = kLeaf + ((e - 1) >> min_shift) + 1;; k++) {
             if (k >= kBins) k = 0;
             while (k % 8 == 1) k = (k - 1) >> 3;
             if (k == 0) break;
@@ -219,19 +396,22 @@ void bai_region_chunks(const BaiBins& bins, const std::vector<uint64_t>& lin, co
             max_off = *std::min_element(bins.cb.begin() + bins.first[(size_t)j], bins.cb.begin() + bins.first[(size_t)j + 1]);
             break;
         }
-        static const int kFirst[6] = {0, 1, 9, 73, 585, 4681}, kShift[6] = {29, 26, 23, 20, 17, 14};
-        for (int l = 0; l < 6; l++)                                    // reg2bins: every level, the bins [b, e - 1] touches
-            for (int64_t k = kFirst[l] + (b >> kShift[l]); k <= kFirst[l] + ((e - 1) >> kShift[l]); k++) {
-                if (lo_of[(size_t)k] == UINT64_MAX && hi_of[(size_t)k] == 0) named.push_back((uint32_t)k);
-                lo_of[(size_t)k] = std::min(lo_of[(size_t)k], min_off);
-                hi_of[(size_t)k] = std::max(hi_of[(size_t)k], max_off);
-            }
+        for (int l = 0; l <= depth; l++) {                             // reg2bins: every level, the bins [b, e - 1] touches
+            const int shift = min_shift + 3 * (depth - l);
+            for (int64_t k = bin_first(l) + (b >> shift); k <= bin_first(l) + ((e - 1) >> shift); k++)
+                named.push_back(Named{(uint32_t)k, min_off, max_off});
+        }
     }
-    for (uint32_t k : named) {
-        const int64_t j = find(k);
+    std::sort(named.begin(), named.end(), [](const Named& x, const Named& y) { return x.bin < y.bin; });
+    for (size_t a = 0; a < named.size();) {
+        size_t z = a;
+        uint64_t lo = UINT64_MAX, hi = 0;
+        for (; z < named.size() && named[z].bin == named[a].bin; z++) { lo = std::min(lo, named[z].lo); hi = std::max(hi, named[z].hi); }
+        const int64_t j = find(named[a].bin);
+        a = z;
         if (j < 0) continue;
         for (uint32_t c = bins.first[(size_t)j]; c < bins.first[(size_t)j + 1]; c++)
-            if (bins.ce[c] > lo_of[k] && bins.cb[c] < hi_of[k] && bins.ce[c] > bins.cb[c]) out.emplace_back(bins.cb[c], bins.ce[c]);
+            if (bins.ce[c] > lo && bins.cb[c] < hi && bins.ce[c] > bins.cb[c]) out.emplace_back(bins.cb[c], bins.ce[c]);
     }
     std::sort(out.begin(), out.end());
     size_t m = 0;

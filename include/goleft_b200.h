@@ -305,9 +305,11 @@ int  gl_segset_ref(const gl_segset* s, int32_t tid, const char** name, int64_t* 
                    const int32_t** end, int64_t* n);
 void gl_segset_free(gl_segset* s);
 /* Index-guided parallel feeder: what `samtools depth -r chr:b-e` gives the reference (depth/depth.go:116,152) — only
- * the BGZF blocks of the requested reference range are read (BAI linear index -> record-aligned virtual offsets); the
+ * the BGZF blocks of the requested reference range are read (16 KB linear index -> record-aligned virtual offsets); the
  * range is cut into units at those offsets and every host-pool thread inflates and parses its own units.
- * gl_bam_open also loads path + ".bai" (or .bam -> .bai); decoding needs that index.
+ * gl_bam_open also loads the BAM's index, the first of x.bam.bai, x.bai, x.bam.csi, x.csi that reads (so a BAM with both
+ * keeps its BAI; a CSI is what a contig past 2^29 bases needs); decoding needs that index.
+ * gl_bam_index: the file that was loaded and its binning geometry (BAI: min_shift 14, depth 5); GL_ESTATE: no index.
  * gl_bam_decode: the M/=/X blocks of the records of `tid` that pass the filter and can overlap [beg,end), as
  *   format 8  : packed8 words  (a0 = int32 anchors[n], a1 = uint8 dstart[64 n], a2 = uint8 len[64 n]; n blocks), or
  *   format 32 : (a0 = int32 start[n], a1 = int32 end[n]) sorted by start,
@@ -323,6 +325,7 @@ typedef struct {
 int  gl_bam_open(const char* path, gl_bam** out, char* err, int64_t err_cap);
 void gl_bam_close(gl_bam* b);
 int  gl_bam_info(const gl_bam* b, int32_t* n_refs, int32_t* has_index);
+int  gl_bam_index(const gl_bam* b, const char** path, int32_t* min_shift, int32_t* depth, int32_t* is_csi);
 int  gl_bam_ref(const gl_bam* b, int32_t tid, const char** name, int64_t* length, int64_t* n_mapped /* -1: no stats bin */);
 int  gl_bam_decode(gl_bam* b, int32_t tid, int64_t beg, int64_t end, int32_t min_mapq, int32_t threads, int32_t want_format,
                    gl_bam_segments* out, char* err, int64_t err_cap);
@@ -335,9 +338,11 @@ int  gl_bam_decode(gl_bam* b, int32_t tid, int64_t beg, int64_t end, int32_t min
 int  gl_bam_decode_device(gl_ctx* ctx, gl_bam* b, int32_t tid, int32_t min_mapq, const int32_t** d_start, const int32_t** d_end, int64_t* n,
                           gl_bam_segments* stats);
 /* Region queries of an indexed BAM: only the BGZF members that hold records overlapping a set of intervals of one reference.
- * gl_bam_region_chunks (host only): the virtual-offset ranges [vb[i], ve[i]) such a query reads, as htslib's BAI query
- *   picks them — the chunks of every bin reg2bins (SAM spec 5.3) names for an interval [beg[i], end[i]), less the chunks
- *   ending at or before the linear-index offset of the interval's first 16 KB tile (the last entry past the linear index)
+ * gl_bam_region_chunks (host only): the virtual-offset ranges [vb[i], ve[i]) such a query reads, as htslib's index query
+ *   picks them — the chunks of every bin reg2bins (SAM spec 5.3, at the index's min_shift and depth: a BAI's 6 levels or a
+ *   CSI's depth + 1) names for an interval [beg[i], end[i]), less the chunks
+ *   ending at or before the linear-index offset of the interval's first 16 KB tile (the last entry past the linear index;
+ *   for a CSI the index rebuilt from its bins' loffsets, never past the first record overlapping the tile)
  *   and those beginning at or after the first chunk of the nearest bin with chunks right of the interval — sorted,
  *   overlapping or touching ranges merged.  The intervals may be in any order, overlap, be empty or reach past the
  *   contig.  The handle reads its index's bins on the first query (gl_bam_open does not keep them).  *n_out = the number
@@ -359,13 +364,18 @@ int  gl_bam_decode_device_regions(gl_ctx* ctx, gl_bam* b, int32_t tid, const int
  * unsupported member (fall back to zlib).  Device pointers; asynchronous on the ctx stream. */
 int  gl_bgzf_inflate_device(gl_ctx* ctx, const uint8_t* d_comp, const int64_t* d_comp_off, const int64_t* d_out_off, int64_t n_blocks,
                             uint8_t* d_out, int32_t* d_status);
-/* BAI: per-reference linear index (16 KB tiles) + the 0x924a stats bin (indexcov/types.go:19,45-58),
- * what indexcov takes from biogo's bam.ReadIndex (indexcov/indexcov.go:514). */
+/* BAI or CSI (told apart by content: a BAI starts with "BAI\1", a CSI is BGZF holding "CSI\1"): per-reference linear index
+ * (16 KB tiles) + the stats pseudo-bin (BAI's 0x924a, indexcov/types.go:19,45-58), what indexcov takes from biogo's
+ * bam.ReadIndex (indexcov/indexcov.go:514), which reads BAI only.  A CSI has no linear index: it is rebuilt at 16 KB tiles
+ * from the bins' loffsets, a record-aligned lower bound of the first record overlapping each tile (DESIGN §1.6).  A CSI
+ * whose min_shift or depth would overflow the bin or position arithmetic is refused.
+ * gl_bai_geometry: min_shift, depth (BAI: 14, 5) and whether the file was a CSI. */
 typedef struct gl_bai gl_bai;
 int  gl_bai_read(const char* path, gl_bai** out, char* err, int64_t err_cap);
 int  gl_bai_n_refs(const gl_bai* b, int32_t* n_refs, uint64_t* n_no_coor);
 int  gl_bai_ref(const gl_bai* b, int32_t tid, const uint64_t** ioffsets, int64_t* n_intv, uint64_t* mapped,
                 uint64_t* unmapped, int32_t* has_stats);
+int  gl_bai_geometry(const gl_bai* b, int32_t* min_shift, int32_t* depth, int32_t* is_csi);
 void gl_bai_free(gl_bai* b);
 
 /* CRAM index: one reference's slices (alignment start, span, slice bytes) -> 16 KB pseudo-tile sizes

@@ -17,6 +17,8 @@
 #   tests/golden/ref_emdepth_gotest.txt                  `go test ./emdepth` (its TestBig fails: it expects CN 8, the code gives 9)
 #   tests/golden/ref_indexcov_pca{8,4}.ped               goleft indexcov --fai on the .bai cohorts of tests/golden/make_pca_cohort.py
 #   tests/golden/ref_cnveval_<case>_<mode>.txt           cnveval stdout on the sets of tests/golden/make_cnveval_sets.py
+#   tests/golden/ref_csi_<bam>.bam.{bai,csi}, ref_csi_<bam>.m12.bam.csi
+#                                                        samtools index -b / -c / -c -m 12 of depth/test/t.bam and hla.bam
 #
 # This image has neither toolchain (`go version`, `samtools --version`: command not found), so the files cannot be made
 # here; until they exist every report says "bit-exact vs the restated oracle, parity unpinned".  tests/test_reference_goldens.py
@@ -65,6 +67,16 @@ printf 'nothing_here\t12345\t0\t60\t61\n' >> "$TMP/t.fa.fai"
 for f in depth callable; do [[ -e "$TMP/empty_500.nothing_here.$f.bed" ]] && cp "$TMP/empty_500.nothing_here.$f.bed" "$OUT/ref_empty_500.$f.bed"; done
 
 cp "$TMP/t.fa.fai" "$OUT/ref_t.fai"
+# samtools-written indexes of the same BAMs, a BAI and CSIs at min_shift 14 and 12, for tests/test_csi_goldens.py: the
+# library's CSI reader against the BAI of one file (every CSI the other tests read comes from tests/csi_bams.py)
+for B in "$T/t.bam" "$T/hla.bam"; do
+  [[ -e "$B" ]] || continue
+  n=$(basename "$B" .bam)
+  cp "$B" "$TMP/$n.bam"
+  samtools index -b "$TMP/$n.bam" "$OUT/ref_csi_$n.bam.bai"
+  samtools index -c "$TMP/$n.bam" "$OUT/ref_csi_$n.bam.csi"
+  samtools index -c -m 12 "$TMP/$n.bam" "$OUT/ref_csi_$n.m12.bam.csi"
+done
 IC="$REF/indexcov/test-data"
 if [[ -e "$IC/sample_issue_27_0001.bam" ]]; then
   "$G" indexcov -d "$TMP/ic27" "$IC/sample_issue_27_0001.bam"

@@ -8,7 +8,10 @@
  *   2. deflate: workers take runs of 64 blocks, regenerate the cells under them, compress
  *   3. index  : virtual offset of every record -> bins + 16 KB linear index + the 37450 stats bin (SAM spec 5.2)
  * then the compressed blocks are written in order.
- *   gls_write_bam(path, n_contigs, names[], lengths[], seed_index[], coverage, read_len, threads) -> 0 / -1      */
+ *   gls_write_bam(path, n_contigs, names[], lengths[], seed_index[], coverage, read_len, threads) -> 0 / -1      (path.bai)
+ *   gls_write_bam_csi(the same arguments)                                                                       (path.csi)
+ * The CSI (CSIv1, min_shift 14, depth 5) holds the BAI's bins and chunks, each bin's loffset the 16 KB linear index at
+ * the bin's first tile, the stats as the pseudo-bin 37450, BGZF-compressed.                                        */
 #define _GNU_SOURCE
 #include <pthread.h>
 #include <stdio.h>
@@ -198,8 +201,8 @@ static void brun(BJob* J, int threads) {
 
 static int cmp_bin(const void* a, const void* b) { return ((const bin_t*)a)->bin - ((const bin_t*)b)->bin; }
 
-int gls_write_bam(const char* path, int n_contigs, const char** names, const int64_t* lengths, const int* seed_index,
-                  double coverage, int read_len, int threads) {
+static int write_bam(const char* path, int n_contigs, const char** names, const int64_t* lengths, const int* seed_index,
+                     double coverage, int read_len, int threads, int csi) {
     if (n_contigs <= 0 || read_len < 20 || read_len > 250) return -1;
     BJob J;
     memset(&J, 0, sizeof J);
@@ -247,11 +250,13 @@ int gls_write_bam(const char* path, int n_contigs, const char** names, const int
 
     /* ---- index: sequential over records (sizes only; cheap next to the deflate pass) */
     char ipath[4096];
-    snprintf(ipath, sizeof ipath, "%s.bai", path);
+    snprintf(ipath, sizeof ipath, csi ? "%s.csi" : "%s.bai", path);
     FILE* fi = fopen(ipath, "wb");
     if (!fi) return -1;
     bbuf ix = {0};
-    bb_put(&ix, "BAI\1", 4); put32(&ix, (uint32_t)n_contigs);
+    if (csi) { bb_put(&ix, "CSI\1", 4); put32(&ix, 14); put32(&ix, 5); put32(&ix, 0); }     /* min_shift, depth, l_aux */
+    else bb_put(&ix, "BAI\1", 4);
+    put32(&ix, (uint32_t)n_contigs);
     gls_read* rd = (gls_read*)malloc(sizeof(gls_read) * GLS_MAX_CELL_READS);
     uint64_t* pk = (uint64_t*)malloc(8 * (size_t)GLS_MAX_CELL_READS);
 #define VOFF(so) ((((uint64_t)J.coff[(so) / BLK]) << 16) | (uint64_t)((so) % BLK))
@@ -304,24 +309,54 @@ int gls_write_bam(const char* path, int n_contigs, const char** names, const int
         qsort(bins, (size_t)nbins, sizeof(bin_t), cmp_bin);
         put32(&ix, (uint32_t)(nbins + (have ? 1 : 0)));
         for (int k = 0; k < nbins; k++) {
-            put32(&ix, (uint32_t)bins[k].bin); put32(&ix, (uint32_t)bins[k].n);
+            put32(&ix, (uint32_t)bins[k].bin);
+            if (csi) {                                                       /* loffset: the linear index at the bin's first tile */
+                static const int first[6] = {0, 1, 9, 73, 585, 4681};
+                int l = 5;
+                while (bins[k].bin < first[l]) l--;
+                const int64_t bot = (int64_t)(bins[k].bin - first[l]) << (3 * (5 - l));
+                const uint64_t lo = bot < lin_n ? lin[bot] : 0;
+                put32(&ix, (uint32_t)lo); put32(&ix, (uint32_t)(lo >> 32));
+            }
+            put32(&ix, (uint32_t)bins[k].n);
             for (int c = 0; c < bins[k].n; c++) { put32(&ix, (uint32_t)bins[k].ch[c].beg); put32(&ix, (uint32_t)(bins[k].ch[c].beg >> 32)); put32(&ix, (uint32_t)bins[k].ch[c].end); put32(&ix, (uint32_t)(bins[k].ch[c].end >> 32)); }
             free(bins[k].ch);
         }
         if (have) {
-            put32(&ix, 37450); put32(&ix, 2);
+            put32(&ix, 37450);
+            if (csi) { put32(&ix, 0); put32(&ix, 0); }
+            put32(&ix, 2);
             const uint64_t q[4] = {ref_beg, ref_end, n_mapped, n_unmapped};
             for (int k = 0; k < 4; k++) { put32(&ix, (uint32_t)q[k]); put32(&ix, (uint32_t)(q[k] >> 32)); }
         }
-        put32(&ix, (uint32_t)lin_n);
-        for (int64_t k = 0; k < lin_n; k++) { put32(&ix, (uint32_t)lin[k]); put32(&ix, (uint32_t)(lin[k] >> 32)); }
+        if (!csi) {                                                          /* a CSI has no linear index */
+            put32(&ix, (uint32_t)lin_n);
+            for (int64_t k = 0; k < lin_n; k++) { put32(&ix, (uint32_t)lin[k]); put32(&ix, (uint32_t)(lin[k] >> 32)); }
+        }
         free(lin); free(bins); free(bin_slot);
     }
     put32(&ix, 0); put32(&ix, 0);                                    /* n_no_coor */
-    fwrite(ix.p, 1, ix.len, fi);
+    if (csi) {                                                       /* BGZF, then the EOF block */
+        uint8_t* out = (uint8_t*)malloc(0x10000 + 64);
+        for (size_t o = 0; o < ix.len; o += BLK) fwrite(out, 1, bgzf_compress_block(ix.p + o, ix.len - o < BLK ? ix.len - o : BLK, out), fi);
+        fwrite(out, 1, bgzf_compress_block(NULL, 0, out), fi);
+        free(out);
+    } else {
+        fwrite(ix.p, 1, ix.len, fi);
+    }
     fclose(fi);
     free(ix.p); free(rd); free(pk); free(h.p); free(text.p);
     free(J.C); free(J.cell_base); free(J.cell_off); free(J.cell_reads); free(J.cblk); free(J.clen); free(J.coff);
     pthread_mutex_destroy(&J.mu);
     return 0;
+}
+
+int gls_write_bam(const char* path, int n_contigs, const char** names, const int64_t* lengths, const int* seed_index,
+                  double coverage, int read_len, int threads) {
+    return write_bam(path, n_contigs, names, lengths, seed_index, coverage, read_len, threads, 0);
+}
+
+int gls_write_bam_csi(const char* path, int n_contigs, const char** names, const int64_t* lengths, const int* seed_index,
+                      double coverage, int read_len, int threads) {
+    return write_bam(path, n_contigs, names, lengths, seed_index, coverage, read_len, threads, 1);
 }

@@ -28,21 +28,23 @@ def _lib():
     lib.gls_segments.restype = C.c_int
     lib.gls_segments.argtypes = [C.c_int64, C.c_double, C.c_int, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                  C.c_void_p, C.c_int64, C.POINTER(C.c_int64)]
-    lib.gls_write_bam.restype = C.c_int
-    lib.gls_write_bam.argtypes = [C.c_char_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.POINTER(C.c_int), C.c_double,
-                                  C.c_int, C.c_int]
+    for fn in (lib.gls_write_bam, lib.gls_write_bam_csi):
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_char_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.POINTER(C.c_int), C.c_double, C.c_int, C.c_int]
     return lib
 
 
-def write_bam(path, contigs, coverage=30.0, read_len=150, threads=0):
+def write_bam(path, contigs, coverage=30.0, read_len=150, threads=0, index="bai"):
     """contigs = [(name, length, contig_index)] -> path + path.bai holding EVERY read of the recipe (the filter is the
-    decoder's job); segments(length, contig_index) are exactly what `samtools depth -Q 1` would count from it."""
+    decoder's job); segments(length, contig_index) are exactly what `samtools depth -Q 1` would count from it.
+    index="csi": path.csi (min_shift 14, depth 5) instead of path.bai; the BAM is the same."""
     lib = _lib()
     n = len(contigs)
     names = (C.c_char_p * n)(*[c[0].encode() for c in contigs])
     lens = (C.c_int64 * n)(*[c[1] for c in contigs])
     seeds = (C.c_int * n)(*[c[2] for c in contigs])
-    rc = lib.gls_write_bam(path.encode(), n, names, lens, seeds, coverage, read_len, threads or (os.cpu_count() or 1))
+    fn = {"bai": lib.gls_write_bam, "csi": lib.gls_write_bam_csi}[index]
+    rc = fn(path.encode(), n, names, lens, seeds, coverage, read_len, threads or (os.cpu_count() or 1))
     if rc != 0:
         raise RuntimeError("gls_write_bam failed")
 

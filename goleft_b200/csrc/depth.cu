@@ -356,8 +356,17 @@ __device__ __forceinline__ void clear_warp_region(int* region, int lane) {
     for (int j = 0; j < kElems / 128; j++) reinterpret_cast<int4*>(region)[lane + 32 * j] = make_int4(0, 0, 0, 0);
 }
 
+// Inclusive scan over the warp's 32 lanes.  shfl.up's predicate says whether the source lane exists, so a step is a SHFL
+// and a predicated add; `if (lane >= o) v += t` compiles to a SHFL, a SEL and an add.
+__device__ __forceinline__ int warp_incl_scan(int v) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1)
+        asm("{\n\t.reg .s32 t;\n\t.reg .pred p;\n\tshfl.sync.up.b32 t|p, %0, %1, 0, -1;\n\t@p add.s32 %0, %0, t;\n\t}" : "+r"(v) : "r"(o));
+    return v;
+}
+
 // BPT bases per thread (16 or 32), WARPS warps per CTA, BPT * 32 * WARPS == kTile.  32 bases per thread halves the work
-// that is paid per thread and tile (warp scan, class check, window loop, run claim, barrier) — K_fused8 uses <32, 4>.
+// that is paid per thread and tile (warp scans, class check, window sums, run claim, barrier) — K_fused8 uses <32, 4>.
 // kSliceInTile (K_fused8): the depth slice goes over the warp's own region of s_tile instead of s_depth (unused, may be
 // null), and the region is cleared when the core is done with it.  The caller must then hold every warp at a barrier
 // between the core and the next tile's atomics.
@@ -387,12 +396,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     }
 #pragma unroll
     for (int k = 1; k < BPT; k++) x[k] += x[k - 1];
-    int inc = x[BPT - 1];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(kFull, inc, o);
-        if (lane >= o) inc += t;
-    }
+    const int inc = warp_incl_scan(x[BPT - 1]);
     const int lane_excl = inc - x[BPT - 1];
     if (lane == 31) s_warp_tot[warp] = inc;
     // depth[k] = tbase + x[k], tbase known only after the barrier: take min / max / sum of the x[k] now, while other
@@ -510,7 +514,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     int* const s_slice = kSliceInTile ? s_tile : s_depth;
     int* sw = s_slice + warp * kWElems;
     int* stb = s_tbase + warp * 32;
-    const bool need_slice = slow_runs || p.do_windows;       // warp-uniform
+    const bool need_slice = slow_runs || slow_win;           // warp-uniform; the fast window path works from registers
     if (need_slice) {
         __syncwarp();
 #pragma unroll
@@ -551,12 +555,7 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
             }
             mask &= (nv >= BPT) ? (BPT == 32 ? 0xffffffffu : 0xffffu) : ((1u << nv) - 1u);
             const int c = __popc(mask);
-            int ci = c;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t = __shfl_up_sync(kFull, ci, o);
-                if (lane >= o) ci += t;
-            }
+            const int ci = warp_incl_scan(c);
             lane_rank = ci - c;
             warp_cnt = __shfl_sync(kFull, ci, 31);
         }
@@ -566,34 +565,45 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
 
     // ---- window partial sums of this warp's 512 bases
     if (fast_win) {
-        // The sum of the warp's depths left of an edge at offset el * BPT + cu is, summed over the lanes j: all BPT depths
-        // of lane j (s16) for j < el, plus base j of lane el for j < cu — one LDS from the slice plus lane el's tbase by
-        // SHFL, no per-lane select.
-        // Each lane keeps what it has contributed so far (counted), so one REDUX of the differences gives the window's part
-        // in this warp (< 2^32 since depth < 2^22), and lane 0 issues one 64-bit red per window.
-        const int s16 = BPT * tbase + xsum;
-        const unsigned a0 = (unsigned)p.rs + (unsigned)warp_base;     // absolute, < 2^32
+        // With W >= BPT a thread's BPT bases hold at most one window edge that is not on its first base, and cu of them
+        // lie left of it (cu = 0: none).  lx = sum of x[k] for k < cu, from the g8 group sums plus one partial group.
+        const unsigned a = (unsigned)p.rs + (unsigned)idx0;              // absolute, < 2^32
         const unsigned uW = (unsigned)p.W;
-        // iw = a0 / W without a division: q = hi32(a0 * floor(2^32/W)) is the quotient or one less
-        unsigned iw = __umulhi(a0, p.W_inv);
-        unsigned rem = a0 - iw * uW;
+        // iw = a / W without a division: q = hi32(a * floor(2^32/W)) is the quotient or one less, because
+        // a * floor(2^32/W) > a * 2^32 / W - a and a < 2^32
+        unsigned iw = __umulhi(a, p.W_inv);
+        unsigned rem = a - iw * uW;
         if (rem >= uW) { iw++; rem -= uW; }
-        if (rem >= uW) { iw++; rem -= uW; }
-        unsigned edge = uW - rem;                                     // offset of the next window edge in the warp, in (0, W]
-        int counted = 0;
-#pragma unroll 1
-        for (; edge < (unsigned)kWElems; edge += uW, iw++) {         // edges inside the warp
-            const int el = (int)(edge / BPT);                         // lane holding the edge (warp-uniform)
-            const int cu = (int)(edge % BPT);                         // bases of that lane left of the edge (warp-uniform)
-            const int d = sw[swz_elem_t<BPT>(el * BPT + (lane & (BPT - 1)))] + __shfl_sync(kFull, tbase, el);
-            const int cur = (lane < el ? s16 : 0) + (lane < cu ? d : 0);
-            const unsigned tot = (unsigned)__reduce_add_sync(kFull, cur - counted);
-            counted = cur;
-            if (lane == 0) atomicAdd(p.win_sum + ((long long)iw - p.w0), (unsigned long long)tot);
+        const int cu = uW - rem < (unsigned)BPT ? (int)(uW - rem) : 0;
+        const int gi = cu >> 3, r = cu & 7;
+        int lx = 0;
+#pragma unroll
+        for (int g = 0; g + 1 < BPT / 8; g++) lx += g < gi ? g8[g] : 0;
+#pragma unroll
+        for (int j = 0; j < 7; j++) {
+            int v = x[j];
+#pragma unroll
+            for (int g = 1; g < BPT / 8; g++) v = gi == g ? x[8 * g + j] : v;
+            lx += j < r ? v : 0;
         }
-        // the window that runs past the warp's end (or ends exactly at it) gets the rest of the warp
-        const unsigned tot = (unsigned)__reduce_add_sync(kFull, s16 - counted);
-        if (lane == 0) atomicAdd(p.win_sum + ((long long)iw - p.w0), (unsigned long long)tot);
+        // An edge lane holds one window edge: inside its bases (cu > 0, it ends window iw) or on its first base (it ends
+        // window iw - 1; on lane 0 that is the warp's start, not an edge).  c = the warp's depth sum left of the edge, so a
+        // window's part in this warp is c minus the c of the edge lane before it (0 for the first), and the window that
+        // runs past the warp's end (or ends exactly at it) gets the warp's total minus the last c.  Every partial sum is
+        // < 2^32 because depth < 2^22 on this path, so unsigned 32-bit arithmetic is exact.
+        const unsigned s16 = (unsigned)(BPT * tbase + xsum);
+        const unsigned si = (unsigned)warp_incl_scan((int)s16);          // the lanes' depth sums, inclusive (mod 2^32)
+        const unsigned total = __shfl_sync(kFull, si, 31);
+        const bool at_start = rem == 0 && lane > 0;
+        const bool edge = cu > 0 || at_start;
+        const unsigned c = si - s16 + (unsigned)(cu * tbase + lx);
+        const unsigned M = __ballot_sync(kFull, edge);
+        const unsigned before = M & ((1u << lane) - 1u);
+        const unsigned cprev = __shfl_sync(kFull, c, before ? 31 - __clz(before) : 0);
+        unsigned long long* const ws = p.win_sum + ((long long)iw - p.w0);
+        if (edge) atomicAdd(ws - (at_start ? 1 : 0), (unsigned long long)(c - (before ? cprev : 0u)));
+        if (lane == (M ? 31 - __clz(M) : 0))                              // lane 0 without edges: c = 0, cu = 0
+            atomicAdd(ws + (cu > 0 ? 1 : 0), (unsigned long long)(total - c));
     } else if (slow_win) {
         // General path from this warp's smem slice: any W, min, ragged end, depth up to 2^31.
         const unsigned a0 = (unsigned)p.rs + (unsigned)warp_base;
@@ -1106,7 +1116,7 @@ __global__ void __launch_bounds__(256) depth_tileidx8_kernel(const ScanParams p)
 struct P8Regs { unsigned d, l; int anchor; };
 
 // K_fused8 runs 128-thread CTAs whose threads own 32 consecutive bases each (tile_core<32, 4>): the work that is paid per
-// thread and tile — warp scan, class check, window loop, run claim, barrier — is spread over twice the bases of the
+// thread and tile — warp scans, class check, window sums, run claim, barrier — is spread over twice the bases of the
 // 16-per-thread core (ncu, round 1: 568 warp instructions per thread and tile = 35.5 per base, issue-bound).
 constexpr int kF8Threads = 128;
 constexpr int kF8Warps = kF8Threads / 32;

@@ -100,6 +100,10 @@ struct ArgParser {
     std::vector<std::string> positional;
     void add(const std::string& lng, char sht, std::string* v, bool required = false) { specs.push_back({lng, sht, false, v, nullptr, required, false}); }
     void addb(const std::string& lng, char sht, bool* v) { specs.push_back({lng, sht, true, nullptr, v, false, false}); }
+    bool given(const std::string& lng) const {
+        for (const Spec& s : specs) if (s.lng == lng) return s.seen;
+        return false;
+    }
     [[noreturn]] void fail(const std::string& msg) const {
         fprintf(stderr, "Usage: %s [options] ...\nerror: %s\n", prog.c_str(), msg.c_str());
         exit(255);                                         // functional-tests.sh:40-42
@@ -190,6 +194,19 @@ static std::vector<std::thread> start_workers(const GpuPlan& p, const std::funct
             fn(g);
         });
     return th;
+}
+
+// whether a BAM's index can be seeked with: a stub index (stats bin but an empty / all-zero linear index for a reference that
+// has reads) cannot, and such a BAM is decoded whole
+static bool index_usable(const glhts::BamFile& f) {
+    bool usable = f.has_index;
+    for (size_t r = 0; usable && r < f.bai.ioffsets.size(); r++) {
+        if (!f.bai.has_stats[r] || f.bai.mapped[r] + f.bai.unmapped[r] == 0) continue;
+        bool any = false;
+        for (uint64_t v : f.bai.ioffsets[r]) if (v) { any = true; break; }
+        usable = any;
+    }
+    return usable;
 }
 
 // the index of an input (indexcov.go:500-510): a .bai or .csi names itself; else the first of x.bam.bai, x.bai, x.bam.csi,
@@ -707,15 +724,7 @@ static int cmd_depth(int argc, char** argv) {
         glhts::BamFile probe;
         std::string e = probe.open(bam);
         if (!e.empty()) fatal(1, "%s", e.c_str());
-        bool usable = probe.has_index;
-        // a stub index (stats bin but an empty / all-zero linear index for a reference that has reads) cannot be seeked with
-        for (size_t r = 0; usable && r < probe.bai.ioffsets.size(); r++) {
-            if (!probe.bai.has_stats[r] || probe.bai.mapped[r] + probe.bai.unmapped[r] == 0) continue;
-            bool any = false;
-            for (uint64_t v : probe.bai.ioffsets[r]) if (v) { any = true; break; }
-            usable = any;
-        }
-        if (!usable) {
+        if (!index_usable(probe)) {
             fprintf(stderr, "goleft depth: no usable index (.bai or .csi) next to %s: decoding the whole file (index it for -c / --bed to read only what they need)\n", bam.c_str());
             int thr = o.threads > 0 ? o.threads : (int)std::max(1u, std::thread::hardware_concurrency());
             int only = -1;
@@ -1914,14 +1923,310 @@ static int cmd_covstats(int argc, char** argv) {
 }
 
 // ------------------------------------------------------------------------------------------------ depthwed
+// getNameFromFile (depthwed.go:37-46): the file's base name without a trailing .gz, then .bed, then .depth
+static std::string wed_name(const std::string& path) {
+    std::string nm = path.substr(path.find_last_of('/') == std::string::npos ? 0 : path.find_last_of('/') + 1);
+    for (const char* suf : {".gz", ".bed", ".depth"}) if (ends_with(nm, suf)) nm = nm.substr(0, nm.size() - strlen(suf));
+    return nm;
+}
+
+static void append_int(std::string& out, long long v) {
+    char b[24];
+    int n = 0;
+    unsigned long long u = v < 0 ? 0ull - (unsigned long long)v : (unsigned long long)v;
+    do { b[n++] = (char)('0' + u % 10); u /= 10; } while (u);
+    if (v < 0) out.push_back('-');
+    while (n) out.push_back(b[--n]);
+}
+
+// The matrix rows as depthwed.go:69-75 prints them: chrom, start, end, then every sample's cell(g, s), tab-separated.  Blocks
+// of rows are formatted on the host pool, a batch of blocks at a time, and written in order.
+template <class Pos, class Cell>
+static void wed_write(FILE* f, int64_t G, size_t S, const std::vector<std::string>& chroms, const int32_t* oc, const Pos* os, const Pos* oe,
+                      const Cell& cell) {
+    const int64_t kRows = 4096;
+    const int64_t nb = (G + kRows - 1) / kRows;
+    glhost::ThreadPool& pool = glhost::ThreadPool::global();
+    const int64_t batch = 2 * (int64_t)pool.size();
+    std::vector<std::string> txt((size_t)std::min<int64_t>(batch, std::max<int64_t>(nb, 1)));
+    for (int64_t b0 = 0; b0 < nb; b0 += batch) {
+        const int64_t b1 = std::min(nb, b0 + batch);
+        pool.run(b1 - b0, [&](int64_t t, int) {
+            std::string& out = txt[(size_t)t];
+            out.clear();
+            const int64_t g0 = (b0 + t) * kRows, g1 = std::min(G, g0 + kRows);
+            for (int64_t g = g0; g < g1; g++) {
+                out += chroms[(size_t)oc[g]];
+                out.push_back('\t'); append_int(out, (long long)os[g]);
+                out.push_back('\t'); append_int(out, (long long)oe[g]);
+                for (size_t s = 0; s < S; s++) { out.push_back('\t'); append_int(out, (long long)cell(g, s)); }
+                out.push_back('\n');
+            }
+        });
+        for (int64_t t = 0; t < b1 - b0; t++) fwrite(txt[(size_t)t].data(), 1, txt[(size_t)t].size(), f);
+    }
+}
+
+// depthwed from BAMs: the matrix `goleft depth --prefix <base> -w W -Q Q [-c chrom] -r ref.fa x.bam` for every BAM, then
+// `goleft depthwed -s SIZE <base>[.chrom].depth.bed ...` print, with no text in between.  The rows are the .fai windows
+// [iW, min((i+1)W, len)) of every contig (or -c); the groups come from gl_depthwed_plan once, with a device map from window
+// to group.  One worker per GPU claims the BAMs in argument order and opens the next while it reduces the current one: per
+// contig (in passes of at most 2^30 - 1 bases) fetch, gl_depth_reduce, gl_depthwed_add_column into the sample's int64
+// column on the device; the finished column comes home once, as int32 cells (int64 when a group sum does not fit).  The main
+// thread takes the BAMs' messages in argument order, and the first that failed ends the run before anything is printed.
+namespace {
+
+struct WedJob {
+    gl_bam* bh = nullptr;
+    bool whole = false;                     // no usable index: the file is decoded whole
+    bool done = false;
+    int code = 0;                           // exit code of this BAM's failure (0: none) and its message
+    std::string msg, note;                  // note: a line for stderr
+    std::vector<int64_t> wide;              // the column as int64 when a group sum does not fit int32
+    glhts::DecodeStats dec;
+    int gpu_fed = 0;
+    double gpu_s = 0, d2h_s = 0;
+};
+
+struct WedContig { std::string name; long long len; int64_t w0; };
+
+}  // namespace
+
+static int wed_bams(const ArgParser& ap, long long size, const std::string& w, const std::string& q, const std::string& reference,
+                    const std::string& chrom, const std::string& procs, const std::string& gpus, bool timing) {
+    const double t_start = now_s();
+    const std::vector<std::string>& bams = ap.positional;
+    const size_t S = bams.size();
+    if (reference.empty()) ap.fail("--reference is required with BAM inputs");
+    const int W = atoi(w.c_str()), Q = atoi(q.c_str()), threads = std::max(0, atoi(procs.c_str()));
+    if (W <= 0) ap.fail("windowsize must be > 0");
+    const long long step = std::max(1LL, 10000000LL / W) * W;                // depth.go:132
+    const long long kMaxPass = ((1LL << 30) - 1) / step * step;
+    if (kMaxPass == 0) fatal(1, "goleft depthwed: windowsize %d is above the 2^30 - 1 bases of one pass", W);
+
+    // rows: the .fai contigs goleft depth walks (cmd_depth), their windows numbered across the genome
+    std::vector<WedContig> contigs;
+    int64_t R = 0;
+    for (const std::string& ln : read_lines(reference + ".fai", true)) {
+        size_t t1 = ln.find('\t');
+        if (t1 == std::string::npos) continue;
+        std::string c = ln.substr(0, t1);
+        if (!chrom.empty() && c != chrom) continue;
+        const long long len = atoll(ln.c_str() + t1 + 1);
+        if (len <= 0) continue;
+        contigs.push_back({c, len, R});
+        R += (len + W - 1) / W;
+    }
+    // groups, planned contig by contig (a group never crosses a contig)
+    std::vector<std::string> names;
+    std::vector<int32_t> oc, grp_of((size_t)R);
+    std::vector<int64_t> os, oe;
+    {
+        std::vector<int64_t> rs, re, first;
+        std::vector<int32_t> cid;
+        for (size_t c = 0; c < contigs.size(); c++) {
+            const WedContig& k = contigs[c];
+            const int64_t n = (k.len + W - 1) / W;
+            rs.resize((size_t)n); re.resize((size_t)n); first.resize((size_t)n + 1); cid.assign((size_t)n, (int32_t)c);
+            for (int64_t i = 0; i < n; i++) { rs[(size_t)i] = i * W; re[(size_t)i] = std::min<int64_t>((i + 1) * W, k.len); }
+            const size_t g0 = os.size();
+            os.resize(g0 + (size_t)n); oe.resize(os.size()); oc.resize(os.size());
+            int64_t ng = 0;
+            if (gl_depthwed_plan(rs.data(), re.data(), cid.data(), n, size, first.data(), os.data() + g0, oe.data() + g0, oc.data() + g0, n, &ng) != GL_OK)
+                fatal(1, "gl_depthwed_plan: %s", gl_last_error(nullptr));
+            os.resize(g0 + (size_t)ng); oe.resize(os.size()); oc.resize(os.size());
+            if (os.size() > (size_t)INT32_MAX) fatal(1, "goleft depthwed: more than 2^31 - 1 output rows");
+            for (int64_t g = 0; g < ng; g++)
+                std::fill(grp_of.begin() + (k.w0 + first[(size_t)g]), grp_of.begin() + (k.w0 + first[(size_t)g + 1]), (int32_t)(g0 + (size_t)g));
+            names.push_back(k.name);
+        }
+    }
+    const int64_t G = (int64_t)os.size();
+    std::string header = "#chrom\tstart\tend";
+    const std::string sfx = chrom.empty() ? "" : "." + chrom;                 // depth.go:378-389
+    for (const std::string& b : bams) {
+        std::string base = b.substr(b.find_last_of('/') == std::string::npos ? 0 : b.find_last_of('/') + 1);
+        base = base.substr(0, base.size() - 4);                               // every input ends in .bam
+        header += "\t" + wed_name(base + sfx + ".depth.bed");
+    }
+    if (G == 0) {                                   // no windows (-c names no .fai contig): the header alone, once every BAM opens
+        for (const std::string& b : bams) {
+            glhts::BamFile f;
+            const std::string e = f.open(b);
+            if (!e.empty()) fatal(1, "%s", e.c_str());
+        }
+        printf("%s\n", header.c_str());
+        return 0;
+    }
+
+    const GpuPlan gp = resolve_gpus(gpus, S, "goleft depthwed");
+    std::vector<int32_t> m32((size_t)S * (size_t)G);                          // sample-major: column s at [s * G, (s + 1) * G)
+    std::vector<WedJob> jobs(S);
+    std::mutex mu;
+    std::condition_variable cv;
+    std::string ctx_err;                            // a worker that could not create its context or its buffers
+    size_t next_claim = 0, fail_at = S;             // no BAM after the first known failure is claimed
+    auto claim = [&]() -> size_t {
+        std::lock_guard<std::mutex> lk(mu);
+        if (next_claim >= fail_at || !ctx_err.empty()) return S;
+        return next_claim++;
+    };
+    auto finish = [&](size_t i) {
+        std::lock_guard<std::mutex> lk(mu);
+        jobs[i].done = true;
+        if (jobs[i].code) fail_at = std::min(fail_at, i);
+        cv.notify_all();
+    };
+    auto open = [&](size_t i) {
+        WedJob& J = jobs[i];
+        char oerr[512] = {0};
+        if (gl_bam_open(bams[i].c_str(), &J.bh, oerr, sizeof oerr) != GL_OK) { J.code = 1; J.msg = oerr; J.bh = nullptr; return; }
+        if (!index_usable(J.bh->f)) {
+            J.whole = true;
+            J.note = "goleft depthwed: no usable index (.bai or .csi) next to " + bams[i] + ": decoding the whole file";
+        }
+    };
+    struct Dev { gl_ctx* c = nullptr; int32_t* map = nullptr; int64_t* col = nullptr; int32_t* col32 = nullptr; int32_t* ovf = nullptr; };
+    // BAM i on one worker's device: its column into m32 (or J.wide)
+    auto run = [&](Dev& d, size_t i) {
+        WedJob& J = jobs[i];
+        if (J.code) return;
+        gl_ctx* c = d.c;
+        gl_bam& bam = *J.bh;
+        glhts::SegmentSet whole;
+        SegSource src;
+        std::map<std::string, int> tid_of;
+        for (size_t r = 0; r < bam.f.header.refs.size(); r++) tid_of[bam.f.header.refs[r].name] = (int)r;
+        if (J.whole) {
+            const double t0 = now_s();
+            int only = -1;
+            if (!chrom.empty()) { auto it = tid_of.find(chrom); if (it != tid_of.end()) only = it->second; }
+            const int thr = threads > 0 ? threads : (int)std::max(1u, std::thread::hardware_concurrency());
+            const std::string e = glhts::bam_decode_segments(bams[i], Q, thr, only, whole);
+            if (!e.empty()) { J.code = 1; J.msg = e; return; }
+            src.whole = &whole;
+            J.dec.wall_s += now_s() - t0;
+        }
+        glck(c, gl_depthwed_column_begin(c, d.col, G), "gl_depthwed_column_begin");
+        for (const WedContig& k : contigs) {
+            auto it = tid_of.find(k.name);
+            if (it == tid_of.end()) continue;                                 // not in the BAM: every window is 0
+            const int tid = it->second;
+            for (long long ps = 0; ps < k.len; ps += kMaxPass) {              // as goleft depth's run_contig
+                const long long pe = std::min(k.len, ps + kMaxPass);
+                const bool whole_ref = ps == 0 && pe == k.len;
+                if (!whole_ref && src.fetch_regions(c, bam, tid, {ps}, {pe}, Q, &J.dec)) J.gpu_fed++;
+                else src.fetch(c, bam, tid, ps, pe, Q, threads, 0, whole_ref, &J.dec, &J.gpu_fed);
+                const double tg = now_s();
+                glck(c, gl_depth_begin(c, ps, pe), "gl_depth_begin");
+                src.add(c);
+                glck(c, gl_depth_reduce(c, W, 4, 0, step), "gl_depth_reduce");
+                glck(c, gl_depthwed_add_column(c, k.w0 + ps / W, d.map, d.col), "gl_depthwed_add_column");
+                J.gpu_s += now_s() - tg;
+            }
+        }
+        const double t0 = now_s();
+        glck(c, gl_depthwed_column_i32(c, d.col, G, d.col32, d.ovf), "gl_depthwed_column_i32");
+        int32_t ovf = 0;
+        if (G) glck(c, gl_memcpy_d2h(c, m32.data() + i * (size_t)G, d.col32, G * 4), "gl_memcpy_d2h");
+        glck(c, gl_memcpy_d2h(c, &ovf, d.ovf, 4), "gl_memcpy_d2h");
+        if (ovf) {
+            J.wide.resize((size_t)G);
+            glck(c, gl_memcpy_d2h(c, J.wide.data(), d.col, G * 8), "gl_memcpy_d2h");
+        }
+        J.d2h_s = now_s() - t0;
+    };
+    std::vector<std::thread> th = start_workers(gp, [&](int g) {
+        Dev d;
+        auto dev_fail = [&](const char* what) {
+            std::lock_guard<std::mutex> lk(mu);
+            if (ctx_err.empty()) ctx_err = std::string(what) + ": " + gl_last_error(d.c);
+            cv.notify_all();
+        };
+        if (gl_ctx_create(g % gp.n_dev, &d.c) != GL_OK) { dev_fail("gl_ctx_create"); return; }
+        void *pm = nullptr, *pc = nullptr, *p32 = nullptr, *po = nullptr;
+        if (gl_dev_alloc(d.c, std::max<int64_t>(R, 1) * 4, &pm) != GL_OK || gl_dev_alloc(d.c, std::max<int64_t>(G, 1) * 8, &pc) != GL_OK ||
+            gl_dev_alloc(d.c, std::max<int64_t>(G, 1) * 4, &p32) != GL_OK || gl_dev_alloc(d.c, 16, &po) != GL_OK ||
+            (R > 0 && gl_memcpy_h2d(d.c, pm, grp_of.data(), R * 4) != GL_OK)) {
+            dev_fail("goleft depthwed");
+        } else {
+            d.map = static_cast<int32_t*>(pm); d.col = static_cast<int64_t*>(pc); d.col32 = static_cast<int32_t*>(p32); d.ovf = static_cast<int32_t*>(po);
+            size_t cur = claim();
+            if (cur < S) open(cur);
+            while (cur < S) {
+                const size_t nxt = claim();
+                if (nxt < S) open(nxt);
+                run(d, cur);
+                if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
+                jobs[cur].bh = nullptr;
+                finish(cur);
+                cur = nxt;
+                bool stop;
+                { std::lock_guard<std::mutex> lk(mu); stop = cur > fail_at || !ctx_err.empty(); }
+                if (stop && cur < S) {                 // a BAM before it failed: it will never be committed
+                    if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
+                    jobs[cur].bh = nullptr;
+                    break;
+                }
+            }
+        }
+        for (void* p : {pm, pc, p32, po}) if (p) gl_dev_free(d.c, p);
+        gl_ctx_destroy(d.c);
+    });
+    auto stop = [&]() {
+        { std::lock_guard<std::mutex> lk(mu); fail_at = 0; }
+        for (std::thread& t : th) t.join();
+        th.clear();
+    };
+    for (size_t i = 0; i < S; i++) {
+        {
+            std::unique_lock<std::mutex> lk(mu);
+            cv.wait(lk, [&] { return jobs[i].done || !ctx_err.empty(); });
+        }
+        WedJob& J = jobs[i];
+        if (!J.done) { stop(); fatal(1, "goleft depthwed: %s", ctx_err.c_str()); }
+        if (!J.note.empty()) fprintf(stderr, "%s\n", J.note.c_str());
+        if (J.code) { stop(); fatal(J.code, "%s", J.msg.c_str()); }
+    }
+    stop();
+    const double t_fmt = now_s();
+    printf("%s\n", header.c_str());
+    wed_write(stdout, G, S, names, oc.data(), os.data(), oe.data(), [&](int64_t g, size_t s) -> long long {
+        const WedJob& J = jobs[s];
+        return J.wide.empty() ? (long long)m32[s * (size_t)G + (size_t)g] : (long long)J.wide[(size_t)g];
+    });
+    fflush(stdout);
+    if (timing) {
+        double dec = 0, gpu = 0, d2h = 0; long long rec = 0, bin = 0; int fed = 0;
+        for (const WedJob& J : jobs) { dec += J.dec.wall_s; gpu += J.gpu_s; d2h += J.d2h_s; rec += J.dec.n_records; bin += J.dec.bytes_in; fed += J.gpu_fed; }
+        fprintf(stderr, "{\"goleft_depthwed_timing\": {\"wall_s\": %.4f, \"gpus\": %d, \"samples\": %zu, \"windows\": %lld, \"rows\": %lld, "
+                        "\"decode_wall_s_sum\": %.4f, \"reduce_column_s_sum\": %.4f, \"d2h_s_sum\": %.4f, \"format_s\": %.4f, "
+                        "\"records\": %lld, \"bgzf_bytes_in\": %lld, \"gpu_fed_passes\": %d}}\n",
+                now_s() - t_start, gp.G, S, (long long)R, (long long)G, dec, gpu, d2h, now_s() - t_fmt, rec, bin, fed);
+    }
+    return 0;
+}
+
 static int cmd_depthwed(int argc, char** argv) {
-    std::string size;
+    std::string size, w = "250", q = "1", reference, chrom, procs = "0", gpus = "0", bed;
+    bool timing = false;
     ArgParser ap;
     ap.prog = "goleft depthwed";
     ap.add("size", 's', &size, true);
+    // extension: BAM inputs, with goleft depth's options and defaults
+    ap.add("windowsize", 'w', &w); ap.add("q", 'Q', &q); ap.add("reference", 'r', &reference); ap.add("chrom", 'c', &chrom);
+    ap.add("processes", 'p', &procs); ap.add("gpus", 0, &gpus); ap.addb("timing", 0, &timing);
+    ap.add("bed", 'b', &bed);
     ap.parse(argc, argv);
     if (ap.positional.empty()) ap.fail("beds is required");
     const long long sz = atoll(size.c_str());
+    size_t n_bam = 0;
+    for (const std::string& p : ap.positional) n_bam += ends_with(p, ".bam");
+    if (n_bam && n_bam < ap.positional.size()) ap.fail("inputs must be all BAMs or all depth.bed files");
+    if (ap.given("bed")) ap.fail("--bed is not supported: BAM inputs are windowed over the .fai contigs of --reference");
+    if (n_bam) return wed_bams(ap, sz, w, q, reference, chrom, procs, gpus, timing);
+    for (const char* f : {"windowsize", "q", "reference", "chrom", "processes", "gpus", "timing"})
+        if (ap.given(f)) ap.fail(std::string("--") + f + " needs BAM inputs");
     const size_t S = ap.positional.size();
     std::vector<std::string> chroms;
     std::map<std::string, int> chrom_id;
@@ -1932,10 +2237,7 @@ static int cmd_depthwed(int argc, char** argv) {
     size_t R = 0;
     std::string header = "#chrom\tstart\tend";
     for (size_t f = 0; f < S; f++) {
-        std::string nm = ap.positional[f];                                          // getNameFromFile (depthwed.go:37-46)
-        nm = nm.substr(nm.find_last_of('/') == std::string::npos ? 0 : nm.find_last_of('/') + 1);
-        for (const char* suf : {".gz", ".bed", ".depth"}) if (ends_with(nm, suf)) nm = nm.substr(0, nm.size() - strlen(suf));
-        header += "\t" + nm;
+        header += "\t" + wed_name(ap.positional[f]);
         std::vector<std::string> lines = read_lines(ap.positional[f], true);
         if (f == 0) { R = lines.size(); means.resize(S * R); depth32.resize(S * R); }
         else if (lines.size() != R) fatal(2, "panic: not all files have same number of records");
@@ -1978,15 +2280,9 @@ static int cmd_depthwed(int argc, char** argv) {
         glck(ctx, gl_depthwed_aggregate(ctx, means.data(), (int32_t)S, (int64_t)R, starts.data(), ends.data(), cid.data(), sz, os.data(), oe.data(),
                                         oc.data(), out.data(), (int64_t)R, &n_out), "gl_depthwed_aggregate");
     }
-    std::string row;
-    char num[32];
-    for (int64_t g = 0; g < n_out; g++) {
-        row = chroms[oc[g]];
-        snprintf(num, sizeof num, "\t%d\t%d", os[g], oe[g]); row += num;
-        for (size_t s = 0; s < S; s++) { snprintf(num, sizeof num, "\t%lld", have32 ? (long long)out32[(size_t)g * S + s] : (long long)out[(size_t)g * S + s]); row += num; }
-        row += "\n";
-        fwrite(row.data(), 1, row.size(), stdout);
-    }
+    wed_write(stdout, n_out, S, chroms, oc.data(), os.data(), oe.data(), [&](int64_t g, size_t s) -> long long {
+        return have32 ? (long long)out32[(size_t)g * S + s] : (long long)out[(size_t)g * S + s];
+    });
     gl_ctx_destroy(ctx);
     return 0;
 }

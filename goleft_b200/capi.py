@@ -141,6 +141,11 @@ _proto("gl_depthwed_aggregate_device", C.c_int, _vp, _vp, C.c_int32, C.c_int64, 
 _proto("gl_depthwed_aggregate_i32", C.c_int, _vp, _vp, C.c_int32, C.c_int64, _vp, _vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _i64p)
 _proto("gl_depthwed_aggregate_i32_device", C.c_int, _vp, _vp, C.c_int32, C.c_int64, _vp, C.c_int64, C.c_int64, _vp, _vp)
 _proto("gl_depthwed_aggregate_i32_p2p", C.c_int, _vp, _vp, C.c_int32, C.c_int64, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int64, C.c_int32, _vp)
+_proto("gl_depthwed_plan", C.c_int, _vp, _vp, _vp, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp, C.c_int64, _i64p)
+_proto("gl_depthwed_cells", C.c_int, _vp, _vp, _vp, C.c_int64, _vp, C.c_int64, _vp)
+_proto("gl_depthwed_column_begin", C.c_int, _vp, _vp, C.c_int64)
+_proto("gl_depthwed_add_column", C.c_int, _vp, C.c_int64, _vp, _vp)
+_proto("gl_depthwed_column_i32", C.c_int, _vp, _vp, C.c_int64, _vp, _vp)
 _proto("gl_ipc_export", C.c_int, _vp, _vp, _vp)
 _proto("gl_ipc_open", C.c_int, _vp, _vp, C.POINTER(_vp))
 _proto("gl_ipc_close", C.c_int, _vp, _vp)
@@ -476,6 +481,20 @@ PLOT_DEPTH, PLOT_PLAIN = 0, 1
 def _ck0(rc: int):
     if rc != GL_OK:
         raise GlError(rc, lib.gl_last_error(None).decode())
+
+
+def depthwed_plan(starts, ends, chrom_id, size: int):
+    """gl_depthwed_plan (host only): (grp_first [n+1], out_start, out_end, out_chrom) of the groups depthwed.go:117-157 makes"""
+    starts, ends, chrom_id = _as(starts, np.int64), _as(ends, np.int64), _as(chrom_id, np.int32)
+    R = starts.size
+    assert ends.size == R and chrom_id.size == R
+    cap = max(R, 1)
+    first, o_s, o_e, o_c = np.empty(cap + 1, np.int64), np.empty(cap, np.int64), np.empty(cap, np.int64), np.empty(cap, np.int32)
+    n = C.c_int64(0)
+    _ck0(lib.gl_depthwed_plan(_ptr(starts), _ptr(ends), _ptr(chrom_id), R, size, _ptr(first), _ptr(o_s), _ptr(o_e), _ptr(o_c), cap,
+                              C.byref(n)))
+    k = n.value
+    return first[:k + 1], o_s[:k], o_e[:k], o_c[:k]
 
 
 def plot_select_host(vals, off, lens):
@@ -1465,6 +1484,32 @@ class Ctx:
                                       d_out_ptr: int, d_overflow: DevBuf):
         self._ck(lib.gl_depthwed_aggregate_i32_device(self.h, d_depth.ptr, S, R, d_grp.ptr if d_grp is not None else None, g_begin, g_end,
                                                       d_out_ptr, d_overflow.ptr))
+
+    def depthwed_cells(self, sums, lens, grp_of=None, n_groups: Optional[int] = None) -> np.ndarray:
+        """int64 cells of explicit windows (sums[i] depth over lens[i] bases) as `goleft depth` then `depthwed` make them,
+        summed per group grp_of[i] (None: one cell per window)"""
+        sums, lens = _as(sums, np.int64), _as(lens, np.int64)
+        assert sums.size == lens.size
+        if grp_of is not None:
+            grp_of = _as(grp_of, np.int32)
+            assert grp_of.size == sums.size
+            n_groups = int(grp_of.max()) + 1 if n_groups is None and grp_of.size else int(n_groups or 0)
+        else:
+            n_groups = sums.size
+        out = np.empty(max(n_groups, 1), np.int64)
+        self._ck(lib.gl_depthwed_cells(self.h, _ptr(sums), _ptr(lens), sums.size, _ptr(grp_of) if grp_of is not None else None, n_groups,
+                                       _ptr(out)))
+        return out[:n_groups]
+
+    def depthwed_column_begin(self, d_col: DevBuf, n_groups: int):
+        self._ck(lib.gl_depthwed_column_begin(self.h, d_col.ptr, n_groups))
+
+    def depthwed_add_column(self, w0: int, d_grp_of: DevBuf, d_col: DevBuf):
+        """asynchronous: the last gl_depth_reduce's window cells added into d_col[d_grp_of[w0 + k]]"""
+        self._ck(lib.gl_depthwed_add_column(self.h, w0, d_grp_of.ptr, d_col.ptr))
+
+    def depthwed_column_i32(self, d_col: DevBuf, n_groups: int, d_col32: DevBuf, d_overflow: DevBuf):
+        self._ck(lib.gl_depthwed_column_i32(self.h, d_col.ptr, n_groups, d_col32.ptr, d_overflow.ptr))
 
     def ipc_export(self, buf: DevBuf) -> bytes:
         h = (C.c_uint8 * 64)()

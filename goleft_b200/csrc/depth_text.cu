@@ -74,19 +74,27 @@ __device__ __forceinline__ unsigned long long scaled_round64(unsigned long long 
     return (unsigned long long)q;
 }
 
-// "%.4g" of a finite double 0 <= q < 1e15 (and q == 0 or q >= 1e-15): appends to t, returns the new length
-__device__ __forceinline__ int put_g4(unsigned char* t, int len, double q) {
-    if (q == 0.0) { t[len++] = '0'; return len; }
+// The four significant digits of "%.4g" of a finite double 0 < q < 1e15, q >= 1e-15: the text's value is N * 10^(e10-3)
+// with 1000 <= N <= 9999.  The text kernel prints them and the depthwed cell kernel rounds them, so both read one rounding.
+__device__ __forceinline__ unsigned long long g4_digits(double q, int& e10) {
     const unsigned long long bits = (unsigned long long)__double_as_longlong(q);
     const int ex = (int)((bits >> 52) & 0x7ff);
     const unsigned long long frac = bits & ((1ull << 52) - 1);
     const unsigned long long m = ex ? (frac | (1ull << 52)) : frac;
     const int e2 = ex ? ex - 1075 : -1074;
-    int e10 = (int)floor(log10(q));
+    e10 = (int)floor(log10(q));
     unsigned long long N = scaled_round64(m, e2, 3 - e10);
     if (N < 1000) { e10--; N = scaled_round64(m, e2, 3 - e10); }            // estimate one too high
     else if (N > 10000) { e10++; N = scaled_round64(m, e2, 3 - e10); }      // one too low
     if (N >= 10000) { N = 1000; e10++; }                                    // 9999.5.. rounds up to the next decade
+    return N;
+}
+
+// "%.4g" of a finite double 0 <= q < 1e15 (and q == 0 or q >= 1e-15): appends to t, returns the new length
+__device__ __forceinline__ int put_g4(unsigned char* t, int len, double q) {
+    if (q == 0.0) { t[len++] = '0'; return len; }
+    int e10;
+    const unsigned long long N = g4_digits(q, e10);
     int dig[4];
     dig[0] = (int)(N / 1000); dig[1] = (int)(N / 100 % 10); dig[2] = (int)(N / 10 % 10); dig[3] = (int)(N % 10);
     const int nd = dig[3] ? 4 : (dig[2] ? 3 : (dig[1] ? 2 : 1));             // significant digits after stripping zeros
@@ -122,6 +130,72 @@ __device__ __forceinline__ int put_class(unsigned char* t, int len, int cls) {
                    : cls == GL_CALLABLE ? "CALLABLE" : "EXCESSIVE_COVERAGE";
     for (int k = 0; nm[k]; k++) t[len++] = (unsigned char)nm[k];
     return len;
+}
+
+// ------------------------------------------------------------------------------------------------ depthwed cells
+// The cell depthwed.go:103 makes of a depth.bed row, int(0.5 + ParseFloat("%.4g" of q)), without the text: the text's value
+// is N * 10^(e10-3), so the cell is floor(N * 10^(e10-3) + 1/2) in integers, ties up.  That is exactly what Go computes:
+// a value with a fractional part is below 1000 and a multiple of 10^-4 or zero, so 0.5 + it truncates to the same integer.
+__device__ __forceinline__ unsigned long long g4_cell(double q) {
+    if (q == 0.0) return 0;
+    int e10;
+    const unsigned long long N = g4_digits(q, e10);
+    unsigned long long p = 1;
+    for (int k = e10 > 3 ? e10 - 3 : 3 - e10; k > 0; k--) p *= 10;          // 10^|e10-3|, at most 10^19
+    return e10 >= 3 ? N * p : (N + p / 2) / p;
+}
+
+struct CellParams {
+    long long n;                              // windows
+    // implicit windows of the last reduce (sum == null): window i = [max(rs, (wb+i)W), min(re, (wb+i+1)W))
+    long long rs, re, wb;
+    int W;
+    const unsigned long long* win_sum;
+    const long long* sum; const long long* len;   // explicit windows
+    const int* grp_of; long long g0;          // window i adds into col[grp_of[g0 + i]]; grp_of == null: col[i]
+    unsigned long long* col;
+};
+
+// One thread per window.  Consecutive windows of one group are summed in the warp (a segmented suffix scan over the runs of
+// equal group ids) and each run's first lane adds the run's sum with one 64-bit atomic: a group of SIZE/W windows costs
+// about SIZE/W/32 atomics per column, not one per window.  Any map is accepted; a group split into several runs gets one
+// atomic per run.
+__global__ void __launch_bounds__(256) depthwed_cells_kernel(const CellParams p) {
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    unsigned long long v = 0;
+    long long key = -1;
+    if (i < p.n) {
+        long long sum, len;
+        if (p.sum) { sum = p.sum[i]; len = p.len[i]; }
+        else {
+            sum = (long long)p.win_sum[i];
+            len = min(p.re, (p.wb + i + 1) * (long long)p.W) - max(p.rs, (p.wb + i) * (long long)p.W);
+        }
+        // depth.go:181-189, as bed_rows_kernel: 0 for an empty cache or zero length, else float64 sum / float64(len)
+        v = g4_cell((sum <= 0 || len <= 0) ? 0.0 : __ddiv_rn((double)sum, (double)len));
+        key = p.grp_of ? (long long)p.grp_of[p.g0 + i] : i;
+    }
+    const long long knext = __shfl_down_sync(0xffffffffu, key, 1);
+    bool ends = lane == 31 || knext != key;                                   // the lane's run ends here
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_down_sync(0xffffffffu, v, o);
+        const bool ey = __shfl_down_sync(0xffffffffu, ends, o);
+        if (!ends && lane + o < 32) { v += y; ends = ey; }
+    }
+    const long long kprev = __shfl_up_sync(0xffffffffu, key, 1);
+    if (key >= 0 && v != 0 && (lane == 0 || kprev != key)) atomicAdd(p.col + key, v);
+}
+
+int launch_cells(gl_ctx* ctx, const CellParams& p) {
+    if (p.n <= 0) return GL_OK;
+    {
+        gl_prof_scope prof(ctx, "depthwed_cells_kernel");
+        depthwed_cells_kernel<<<(unsigned)((p.n + 255) / 256), 256, 0, ctx->stream>>>(p);
+    }
+    GL_LAUNCHED(ctx, 1);
+    return GL_OK;
 }
 
 __global__ void __launch_bounds__(kRowsPerBlock) bed_rows_kernel(const TextParams p) {
@@ -376,6 +450,60 @@ int gl_depth_format_rows(gl_ctx* ctx, const char* chrom, const int32_t* row_s, c
     GL_CUDA(ctx, cudaMemcpyAsync(out, ctx->text_out[0].p, (size_t)total, cudaMemcpyDeviceToHost, ctx->stream));
     GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return GL_OK;
+}
+
+int gl_depthwed_cells(gl_ctx* ctx, const int64_t* sums, const int64_t* lens, int64_t n, const int32_t* grp_of, int64_t n_groups, int64_t* out) {
+    GL_CHECK(gl_use(ctx));
+    if (n < 0 || !out || (n > 0 && (!sums || !lens)) || (grp_of ? n_groups < 0 : n_groups != n))
+        return gl_fail(ctx, GL_EINVAL, "gl_depthwed_cells: bad argument");
+    for (int64_t i = 0; i < n; i++) {
+        if (grp_of && (grp_of[i] < 0 || grp_of[i] >= n_groups)) return gl_fail(ctx, GL_EINVAL, "gl_depthwed_cells: grp_of[%lld] out of range", (long long)i);
+        if (sums[i] > 0 && lens[i] > 0 && (sums[i] >= (int64_t(1) << 53) || lens[i] >= (int64_t(1) << 31) || (double)sums[i] / (double)lens[i] >= 1e15))
+            return gl_fail(ctx, GL_ERANGE, "gl_depthwed_cells: window %lld: sum %lld over %lld bases is out of range", (long long)i,
+                           (long long)sums[i], (long long)lens[i]);
+    }
+    if (n_groups == 0) return GL_OK;
+    gl_scratch tmp(ctx);
+    long long *d_sum, *d_len;
+    int* d_grp = nullptr;
+    unsigned long long* d_out;
+    GL_CHECK(tmp.upload(d_sum, reinterpret_cast<const long long*>(sums), (size_t)n));
+    GL_CHECK(tmp.upload(d_len, reinterpret_cast<const long long*>(lens), (size_t)n));
+    if (grp_of) GL_CHECK(tmp.upload(d_grp, reinterpret_cast<const int*>(grp_of), (size_t)n));
+    GL_CHECK(tmp.alloc(d_out, (size_t)n_groups));
+    GL_CUDA(ctx, cudaMemsetAsync(d_out, 0, (size_t)n_groups * 8, ctx->stream));
+    CellParams p;
+    memset(&p, 0, sizeof p);
+    p.n = n; p.sum = d_sum; p.len = d_len; p.grp_of = d_grp; p.col = d_out;
+    GL_CHECK(launch_cells(ctx, p));
+    GL_CUDA(ctx, cudaMemcpyAsync(out, d_out, (size_t)n_groups * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    GL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return GL_OK;
+}
+
+int gl_depthwed_column_begin(gl_ctx* ctx, int64_t* d_col, int64_t n_groups) {
+    GL_CHECK(gl_use(ctx));
+    if (n_groups < 0 || (n_groups > 0 && !d_col)) return gl_fail(ctx, GL_EINVAL, "gl_depthwed_column_begin: bad argument");
+    if (n_groups) GL_CUDA(ctx, cudaMemsetAsync(d_col, 0, (size_t)n_groups * 8, ctx->stream));
+    return GL_OK;
+}
+
+int gl_depthwed_add_column(gl_ctx* ctx, int64_t w0, const int32_t* d_grp_of, int64_t* d_col) {
+    GL_CHECK(gl_use(ctx));
+    GL_CHECK(depth_resolve(ctx));
+    if (!ctx->depth_reduced) return gl_fail(ctx, GL_ESTATE, "gl_depthwed_add_column: call gl_depth_reduce first");
+    if (w0 < 0 || !d_grp_of || !d_col) return gl_fail(ctx, GL_EINVAL, "gl_depthwed_add_column: bad argument");
+    const int W = ctx->red.W;
+    if (ctx->n_windows > 0 && ctx->rs % W != 0)
+        return gl_fail(ctx, GL_EINVAL, "gl_depthwed_add_column: region start %lld is not a multiple of the window size", (long long)ctx->rs);
+    CellParams p;
+    memset(&p, 0, sizeof p);
+    p.n = ctx->n_windows;
+    p.rs = ctx->rs; p.re = ctx->re; p.wb = ctx->rs / W; p.W = W;
+    p.win_sum = static_cast<const unsigned long long*>(ctx->win_sum_p);
+    p.grp_of = reinterpret_cast<const int*>(d_grp_of); p.g0 = w0;
+    p.col = reinterpret_cast<unsigned long long*>(d_col);
+    return launch_cells(ctx, p);
 }
 
 }  // extern "C"

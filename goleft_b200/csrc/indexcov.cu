@@ -1170,20 +1170,68 @@ int gl_bincount_i32(gl_ctx* ctx, const int32_t* v, int64_t n, int32_t lo, int32_
     return GL_OK;
 }
 
+}  // extern "C"
+
 // groups of consecutive rows per output line (depthwed.go:117-157): sequential in the row order, O(R) on the host
-static int64_t depthwed_groups(int64_t R, const int32_t* starts, const int32_t* ends, const int32_t* chrom_id, int64_t size,
+template <class Pos>
+static int64_t depthwed_groups(int64_t R, const Pos* starts, const Pos* ends, const int32_t* chrom_id, int64_t size,
                                std::vector<int64_t>& grp) {
     grp.clear();
     int64_t r = 0;
     while (r < R) {
         grp.push_back(r);
-        const int32_t chrom = chrom_id[r], st = starts[r];
-        int32_t en = ends[r];
+        const int32_t chrom = chrom_id[r];
+        const int64_t st = starts[r];
+        int64_t en = ends[r];
         r++;
-        while (r < R && (int64_t)en - st < size && chrom_id[r] == chrom) { en = ends[r]; r++; }
+        while (r < R && en - st < size && chrom_id[r] == chrom) { en = ends[r]; r++; }
     }
     grp.push_back(R);
     return (int64_t)grp.size() - 1;
+}
+
+// a depthwed column (int64 group sums) narrowed to int32; *overflow = 1 when a sum does not fit
+__global__ void __launch_bounds__(256) depthwed_narrow_kernel(const long long* __restrict__ col, long long n, int* __restrict__ out,
+                                                             int* __restrict__ overflow) {
+    const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (i >= n) return;
+    const long long v = col[i];
+    if (v > 2147483647ll || v < -2147483648ll) *overflow = 1;
+    out[i] = (int)v;
+}
+
+extern "C" {
+
+int gl_depthwed_plan(const int64_t* starts, const int64_t* ends, const int32_t* chrom_id, int64_t R, int64_t size, int64_t* grp_first,
+                     int64_t* out_start, int64_t* out_end, int32_t* out_chrom, int64_t cap, int64_t* n_groups) {
+    if (R < 0 || size <= 0 || !n_groups || (R > 0 && (!starts || !ends || !chrom_id)))
+        return gl_fail(nullptr, GL_EINVAL, "gl_depthwed_plan: bad argument");
+    std::vector<int64_t> grp;
+    const int64_t ng = depthwed_groups(R, starts, ends, chrom_id, size, grp);
+    *n_groups = ng;
+    if (ng > cap) return gl_fail(nullptr, GL_ERANGE, "gl_depthwed_plan: %lld groups > cap %lld", (long long)ng, (long long)cap);
+    for (int64_t g = 0; g <= ng; g++) {
+        if (grp_first) grp_first[g] = grp[g];
+        if (g == ng) break;
+        if (out_start) out_start[g] = starts[grp[g]];
+        if (out_end) out_end[g] = ends[grp[g + 1] - 1];
+        if (out_chrom) out_chrom[g] = chrom_id[grp[g]];
+    }
+    return GL_OK;
+}
+
+int gl_depthwed_column_i32(gl_ctx* ctx, const int64_t* d_col, int64_t n_groups, int32_t* d_col32, int32_t* d_overflow) {
+    GL_CHECK(gl_use(ctx));
+    if (n_groups < 0 || !d_overflow || (n_groups > 0 && (!d_col || !d_col32))) return gl_fail(ctx, GL_EINVAL, "gl_depthwed_column_i32: bad argument");
+    GL_CUDA(ctx, cudaMemsetAsync(d_overflow, 0, 4, ctx->stream));
+    if (n_groups == 0) return GL_OK;
+    {
+        gl_prof_scope prof(ctx, "depthwed_narrow_kernel");
+        depthwed_narrow_kernel<<<(unsigned)((n_groups + 255) / 256), 256, 0, ctx->stream>>>(reinterpret_cast<const long long*>(d_col), n_groups,
+                                                                                             d_col32, d_overflow);
+    }
+    GL_LAUNCHED(ctx, 1);
+    return GL_OK;
 }
 
 int gl_depthwed_aggregate_device(gl_ctx* ctx, const double* d_means, int32_t S, int64_t R, const int64_t* d_grp, int64_t n_out,

@@ -826,6 +826,34 @@ int  gl_depthwed_aggregate_i32_device(gl_ctx* ctx, const int32_t* d_depth, int32
 int  gl_depthwed_aggregate_i32_p2p(gl_ctx* ctx, const int32_t* d_depth, int32_t S, int64_t R, const int64_t* d_grp, int64_t g_begin,
                                    int64_t g_end, int32_t* const* d_dst, int32_t world, int64_t row_stride, int32_t col_off,
                                    int32_t* d_overflow);
+
+/* depthwed from BAMs (`goleft depthwed -r ref.fa *.bam`): the matrix straight from the window sums, with no depth.bed text.
+ * The cell of a window of `sum` depth over `len` bases is what `goleft depth` prints and depthwed.go:103 parses back,
+ * int(0.5 + ParseFloat("%.4g" of float64(sum)/float64(len))), computed on the device from the four digits N and exponent e10
+ * the depth.bed text kernel prints (one shared helper): floor(N * 10^(e10-3) + 1/2) in integers, ties up.  A window with
+ * sum <= 0 or len <= 0 is 0.  Cells are summed per group into int64.
+ *
+ * Group planner, host only (depthwed.go:117-157): R window rows (start, end, chrom_id) in file order and SIZE -> *n_groups
+ * output rows; grp_first[g] = the first row of group g (grp_first has room for cap + 1: grp_first[n] = R), and out_start /
+ * out_end / out_chrom the group's line.  Any output may be NULL.  GL_ERANGE with *n_groups set when cap is too small.
+ * gl_depthwed_aggregate* group their rows the same way. */
+int  gl_depthwed_plan(const int64_t* starts, const int64_t* ends, const int32_t* chrom_id, int64_t R, int64_t size, int64_t* grp_first,
+                      int64_t* out_start, int64_t* out_end, int32_t* out_chrom, int64_t cap, int64_t* n_groups);
+/* Explicit windows (synchronous): out[grp_of[i]] = the sum of the cells of windows i (sums[i] depth over lens[i] bases) in
+ * group grp_of[i] in [0, n_groups); out is overwritten.  grp_of NULL: out[i] = window i's cell (n_groups = n).  A window with
+ * sum > 0 and len > 0 needs sum < 2^53, len < 2^31 and sum / len < 1e15 (GL_ERANGE otherwise). */
+int  gl_depthwed_cells(gl_ctx* ctx, const int64_t* sums, const int64_t* lens, int64_t n, const int32_t* grp_of, int64_t n_groups,
+                       int64_t* out);
+/* Device column, ASYNCHRONOUS on the ctx stream.  gl_depthwed_column_begin zeroes d_col[n_groups] (int64).
+ * gl_depthwed_add_column adds the cells of the last gl_depth_reduce's windows into it: window k of the region is window
+ * w0 + k of the column's window list and goes to group d_grp_of[w0 + k] (a device int32 map that covers those windows).  The
+ * region start must be a multiple of W.  Calls accumulate, so a contig reduced in passes (each at most 2^30 - 1 bases) adds
+ * one call per pass, and a group that straddles two passes gets both parts; the passes are ordered on the ctx stream.
+ * gl_depthwed_column_i32 narrows d_col into d_col32 and sets *d_overflow (a device int it zeroes first) to 1 when a group
+ * sum does not fit int32 (then read d_col itself). */
+int  gl_depthwed_column_begin(gl_ctx* ctx, int64_t* d_col, int64_t n_groups);
+int  gl_depthwed_add_column(gl_ctx* ctx, int64_t w0, const int32_t* d_grp_of, int64_t* d_col);
+int  gl_depthwed_column_i32(gl_ctx* ctx, const int64_t* d_col, int64_t n_groups, int32_t* d_col32, int32_t* d_overflow);
 /* peer memory between the per-GPU processes of one box: export a gl_dev_alloc allocation as a 64-byte handle, open another
  * rank's handle as a device pointer usable by kernels of this ctx (cudaIpc*; the link is NVLink / NVSwitch) */
 int  gl_ipc_export(gl_ctx* ctx, void* d_ptr, uint8_t handle64[64]);

@@ -245,6 +245,7 @@ _proto("gl_indexcov_pca", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.
 _proto("gl_indexcov_pca_device", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int64, C.c_int32, _vp, _vp, _i32p, _vp)
 _proto("gl_indexcov_pca_phases", C.c_int, _vp, C.POINTER(C.c_double))
 _proto("gl_pca_tridiag_top", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, _vp)
+_proto("gl_sym_tridiag", C.c_int, _vp, _vp, C.c_int32, _vp, _vp, _vp, _vp, C.c_int32, _vp)
 _proto("gl_dcnv_svd", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_double, C.c_int64, _vp, _vp, _i32p, _i64p)
 _proto("gl_dcnv_svd_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, C.c_int32, C.c_double, _vp, _vp, _i32p, _i64p)
 _proto("gl_dcnv_svd_phases", C.c_int, _vp, C.POINTER(C.c_double))
@@ -1795,6 +1796,23 @@ class Ctx:
         t = (C.c_double * 3)()
         self._ck(lib.gl_indexcov_pca_phases(self.h, t))
         return dict(zip(("upload", "gram", "eigen"), list(t)))
+
+    def sym_tridiag(self, a: np.ndarray, u: Optional[np.ndarray] = None):
+        """(d[n], e[n-1], tau[n-2], reflectors n x n, Q u or None) of the symmetric n x n float64 matrix a: the device
+        tridiagonalisation indexcov's PCA and dcnv --svd share (gl_sym_tridiag); u: k x n vectors of T"""
+        a = _as(a, np.float64)
+        if a.ndim != 2 or a.shape[0] != a.shape[1]:
+            raise ValueError("sym_tridiag: a must be square")
+        n = a.shape[0]
+        d, e, tau = np.empty(n, np.float64), np.empty(max(n - 1, 0), np.float64), np.empty(max(n - 2, 0), np.float64)
+        refl = np.empty((n, n), np.float64)
+        if u is not None:
+            u = np.array(u, np.float64, order="C", copy=True)
+            if u.ndim != 2 or u.shape[1] != n:
+                raise ValueError("sym_tridiag: u must be k x n")
+        k = 0 if u is None else u.shape[0]
+        self._ck(lib.gl_sym_tridiag(self.h, _ptr(a), n, _ptr(d), _ptr(e), _ptr(tau), _ptr(refl), k, _ptr(u)))
+        return d, e, tau, refl, u
 
     # ---- multi-GPU
     def comm_init(self, id128: bytes, rank: int, world: int):

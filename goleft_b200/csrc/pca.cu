@@ -442,4 +442,22 @@ int gl_indexcov_pca_phases(gl_ctx* ctx, double* t3) {
     return GL_OK;
 }
 
+int gl_sym_tridiag(gl_ctx* ctx, const double* a, int32_t n, double* d, double* e, double* tau, double* refl, int32_t k, double* u) {
+    GL_CHECK(gl_use(ctx));
+    if (n < 1 || k < 0 || !a || !d || (n > 1 && !e) || (n > 2 && !tau) || !refl || (k > 0 && !u))
+        return gl_fail(ctx, GL_EINVAL, "gl_sym_tridiag: bad argument (n = %d, k = %d)", n, k);
+    if (n > 65535) return gl_fail(ctx, GL_EINVAL, "gl_sym_tridiag: n = %d; at most 65535", n);
+    gl_scratch tmp(ctx);
+    double* d_A;
+    GL_CHECK(tmp.upload(d_A, a, (size_t)n * n));
+    SymTridiag tri;
+    GL_CHECK(sym_tridiag(ctx, d_A, n, tri));
+    std::copy(tri.d.begin(), tri.d.end(), d);
+    std::copy(tri.e.begin(), tri.e.begin() + (n - 1), e);
+    std::copy(tri.tau.begin(), tri.tau.begin() + std::max(0, n - 2), tau);
+    std::copy(tri.hA.begin(), tri.hA.end(), refl);
+    if (k > 0) tri.back_transform(u, k);
+    return GL_OK;
+}
+
 }  // extern "C"

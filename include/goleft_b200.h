@@ -451,7 +451,13 @@ int  gl_indexcov_xnorm(gl_ctx* ctx, float* depths, const int32_t* lens, int32_t 
  *   gl_indexcov_pca_device : the same on a device-resident X; d_x and ld must be multiples of 16 bytes.  The outputs are host.
  *   gl_indexcov_pca_phases : seconds of the last call: upload, Gram + centring, eigenvectors + projections.
  *   gl_pca_tridiag_top     : host-only: the k largest eigenvalues w (descending) of the symmetric tridiagonal (d[n], e[n-1])
- *                            and, when z is not NULL, unit eigenvectors (column j at z[j*n]), as gl_indexcov_pca finds them. */
+ *                            and, when z is not NULL, unit eigenvectors (column j at z[j*n]), as gl_indexcov_pca finds them.
+ *   gl_sym_tridiag         : the device Householder tridiagonalisation gl_indexcov_pca and gl_dcnv_svd share, on the symmetric
+ *                            row-major n x n matrix a (host): T = tridiag(e, d, e) = Q^T a Q with Q = H_0 H_1 ... H_{n-3},
+ *                            H_j = I - tau[j] v_j v_j^T.  Returns d[n], e[n-1], tau[n-2] (0: no reflector) and refl (n x n, the
+ *                            device matrix after the reduction: row j holds v_j from column j + 1, v_j[0] = 1).  k > 0: the k
+ *                            vectors of T in u (vector j at u[j*n]) become Q u in place, as both callers take them back.  The
+ *                            same a gives the same bits.  1 <= n <= 65535, k >= 0; e, tau, u may be NULL when they hold nothing. */
 int  gl_indexcov_pca8(const float* d, int64_t n, uint8_t* out);
 int  gl_indexcov_pca(gl_ctx* ctx, const uint8_t* x, int64_t ld, int32_t S, int64_t D, int32_t k, double* proj, double* sv,
                      int32_t* k_out, int64_t* gram);
@@ -463,6 +469,7 @@ int  gl_indexcov_pca_phases(gl_ctx* ctx, double* t3);
  * normalised `vars` (indexcov.go:787-789), the "variance explained" of component k. */
 int  gl_indexcov_pca_total(const uint8_t* x, int64_t ld, int32_t S, int64_t D, double* total);
 int  gl_pca_tridiag_top(const double* d, const double* e, int32_t n, int32_t k, double* w, double* z);
+int  gl_sym_tridiag(gl_ctx* ctx, const double* a, int32_t n, double* d, double* e, double* tau, double* refl, int32_t k, double* u);
 
 /* ---------------------------------------------------------------- indexcov charts (plot.cu; DESIGN §1.14)
  * A chart's lines are drawn into an INDEX IMAGE: W x H uint32 over its data area (row 0 at the top), 0 where no line passes,

@@ -25,8 +25,8 @@ def _zt_z(x):
     return z.T @ z, kept
 
 
-@pytest.mark.parametrize("S,n", [(1, 1000), (2, 5000), (3, 2 ** 20 + 7), (8, 100_003), (33, 50_001), (128, 70_000),
-                                 (257, 20_011), (2504, 3_001)])
+@pytest.mark.parametrize("S,n", [(1, 1000), (2, 5000), (3, 2 ** 20 + 7), (8, 100_003), (33, 50_001), (63, 30_011), (65, 30_013),
+                                 (128, 70_000), (257, 20_011), (2504, 3_001)])
 def test_gram_against_numpy(ctx, S, n):
     rng = np.random.default_rng(S)
     x = _cohort(rng, n, S, const_every=97)
@@ -73,10 +73,11 @@ def _planted(rng, n, S, k):
     return np.maximum(x, 0.0)
 
 
-@pytest.mark.parametrize("k", [0, 1, 5, 20])
-def test_planted_batch_effects_against_oracle(ctx, k):
-    rng = np.random.default_rng(100 + k)
-    n, S = 30_000, 64
+@pytest.mark.parametrize("S,n,k", [pytest.param(64, 30_000, k, id=str(k)) for k in (0, 1, 5, 20)] +
+                         [pytest.param(1000, 6_000, k, id="1000-%d" % k) for k in (0, 1, 5, 20)] +
+                         [pytest.param(2504, 1_200, 5, id="wide-2504-5")])  # S > n: rank 1200, a null space of 1304
+def test_planted_batch_effects_against_oracle(ctx, S, n, k):
+    rng = np.random.default_rng(100 + k if S == 64 else [S, k])
     x = _planted(rng, n, S, k)
     z, kept, m, sd = osv.zscore(x)
     s = osv.singular_values(z, S)

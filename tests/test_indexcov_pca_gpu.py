@@ -10,11 +10,18 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("S,D,fill", [(1, 1, None), (3, 7, None), (7, 300, None), (33, 32768, None), (33, 32769, None),
-                                      (33, 65537, 255), (128, 100003, None), (1000, 2 ** 17 + 5, None)])
+                                      (33, 65537, 255), (127, 20011, None), (128, 100003, None), (129, 30011, None),
+                                      (257, 50021, None), (1000, 2 ** 17 + 5, None),
+                                      # 36 tiles: pca_run's split gives kc = 32768, the kKMax limit, at 132 SMs and at 114,
+                                      # so eight of each tile's nine CTAs sum 32768 columns of 255^2: 2,130,739,200 < 2^31
+                                      (1000, 2 ** 18 + 5, 255)])
 def test_gram_exact(ctx, S, D, fill):
     rng = np.random.default_rng(S * 7 + D)
     x = np.full((S, D), fill, np.uint8) if fill is not None else rng.integers(0, 256, (S, D), dtype=np.uint8)
     _, _, _, g = ctx.indexcov_pca(x, want_gram=True)
+    if fill is not None:
+        assert np.array_equal(g, np.full((S, S), fill * fill * D, np.int64))
+        return
     xf = x.astype(np.float64)
     assert np.array_equal(g, (xf @ xf.T).astype(np.int64))            # every partial sum is an integer below 2^53
 
@@ -71,7 +78,7 @@ def _check(ctx, x):
     return proj, sv, k
 
 
-@pytest.mark.parametrize("S", [3, 4, 5, 6, 7, 100, 1000])
+@pytest.mark.parametrize("S", [3, 4, 5, 6, 7, 100, 1000, 2504])
 @pytest.mark.parametrize("kind", ["noise", "planted"])
 def test_pca_against_oracle(ctx, S, kind):
     rng = np.random.default_rng(S + (0 if kind == "noise" else 1000))

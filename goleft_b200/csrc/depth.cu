@@ -41,6 +41,14 @@ constexpr int kMaxBatches = 8;
 constexpr int kLenSlots = 1024;
 constexpr int kFlagWords = 16 + kLenSlots;
 
+// Programmatic dependent launch (sm_90): the packed8 reduce's kernels are launched with programmatic stream serialization
+// (launch_chained), so each may start while the kernel before it drains.  A chained kernel lets its successor launch at
+// its top and waits for its predecessor (complete, memory visible) before it touches anything an earlier kernel writes or
+// reads.  Every CTA waits before it exits: a grid that finished without waiting could complete before its predecessor,
+// and its successor's wait would then no longer cover the predecessor.  Outside a chained launch both are no-ops.
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
 __device__ __forceinline__ int4 ld_stream_int4(const int4* p) {
     int4 r;
     asm volatile("ld.global.nc.L1::no_allocate.v4.s32 {%0,%1,%2,%3}, [%4];"
@@ -316,7 +324,7 @@ struct ScanParams {
     int* tmp_start;               // [run_cap] run starts in claim order
     unsigned char* tmp_class;     // [run_cap]
     long long run_cap;
-    uint64_t* header;             // [0]=runs claimed (= n_runs) [2]=max_depth [3]=fused path rejected
+    uint64_t* header;             // [0]=runs claimed (= n_runs) [2]=max_depth [3]=fused path rejected (1) / packed8 rejected (p8_tag)
     uint64_t* chunk_runs;         // [num_tiles*8] per 512-base warp chunk: (claim offset << 32) | count
     unsigned* super_cnt;          // [num_tiles*8/64+1] run starts per 64 chunks
     int* depth_out;               // optional per-base output (debug/parity), else null
@@ -332,6 +340,8 @@ struct ScanParams {
     unsigned W_inv;               // floor(2^32 / W): window index by multiplication (fast window path, W >= 16)
     int tile_begin, tile_end;     // K_fused8 processes these tiles (a streamed upload launches it once per arrived chunk)
     int idx_begin, idx_end;       // K_tileidx8 handles the anchor gaps i in [idx_begin, idx_end), i = -1 .. nb-1
+    long long zero_words;         // K_tileidx8: u64 words of scratch to zero first, all but header[3] (the reduce's first launch only)
+    uint64_t p8_tag;              // packed8: header[3] == p8_tag marks this reduce rejected (header[3] is never zeroed there)
     gl_md_ep md;                  // multidepth epilogue (mode 0: none)
 };
 
@@ -1078,38 +1088,49 @@ __global__ void __launch_bounds__(kScanThreads, 4) depth_fused_kernel(const Scan
 // ================================================================================================
 __device__ __forceinline__ long long floordiv_tile(long long x) { return x >> kTileShift; }   // arithmetic shift = floor
 
+// One-wave grid: each CTA strides over the gaps 256 at a time (the stride is uniform, so whole warps iterate together).
+// The reduce's first launch also zeroes the scratch the reduce accumulates into (header, super_cnt, window sums), after
+// its wait, because the previous reduce's kernels use the same words.  header[3] is left alone: this kernel's CTAs may
+// set it, so a rejection is told apart from a stale value by its tag (p8_tag).
 __global__ void __launch_bounds__(256) depth_tileidx8_kernel(const ScanParams p) {
-    const long long i = (long long)blockIdx.x * 256 + threadIdx.x + p.idx_begin;
+    pdl_launch_dependents();
+    pdl_wait();
+    const long long stride = (long long)gridDim.x * 256;
+    for (long long w = (long long)blockIdx.x * 256 + threadIdx.x; w < p.zero_words; w += stride)
+        if (w != 3) p.header[w] = 0;
     const int lane = threadIdx.x & 31;
     const int nb = p.p8_nblocks;
     const int T = p.num_tiles;
-    long long h0 = 1, h1 = 0, l0 = 1, l1 = 0;                               // empty ranges
-    if (i < p.idx_end) {
-        const long long lo_x = i >= 0 ? (long long)p.p8_anchors[i] : LLONG_MIN / 2;
-        const long long hi_x = i + 1 < nb ? (long long)p.p8_anchors[i + 1] : LLONG_MAX / 2;
-        if (lo_x > hi_x) p.header[3] = 1;                                   // unsorted anchors: the host falls back
-        else {
-            // boundaries x_k with lo_x < x_k <= hi_x, and the same for x_k - 255
-            h0 = max(0ll, floordiv_tile(lo_x - p.rs) + 1); h1 = min((long long)T, floordiv_tile(hi_x - p.rs));
-            l0 = max(0ll, floordiv_tile(lo_x - p.rs + 255) + 1); l1 = min((long long)T, floordiv_tile(hi_x - p.rs + 255));
+    for (long long i0 = (long long)blockIdx.x * 256 + p.idx_begin; i0 < p.idx_end; i0 += stride) {
+        const long long i = i0 + threadIdx.x;
+        long long h0 = 1, h1 = 0, l0 = 1, l1 = 0;                           // empty ranges
+        if (i < p.idx_end) {
+            const long long lo_x = i >= 0 ? (long long)p.p8_anchors[i] : LLONG_MIN / 2;
+            const long long hi_x = i + 1 < nb ? (long long)p.p8_anchors[i + 1] : LLONG_MAX / 2;
+            if (lo_x > hi_x) p.header[3] = p.p8_tag;                        // unsorted anchors: the host falls back
+            else {
+                // boundaries x_k with lo_x < x_k <= hi_x, and the same for x_k - 255
+                h0 = max(0ll, floordiv_tile(lo_x - p.rs) + 1); h1 = min((long long)T, floordiv_tile(hi_x - p.rs));
+                l0 = max(0ll, floordiv_tile(lo_x - p.rs + 255) + 1); l1 = min((long long)T, floordiv_tile(hi_x - p.rs + 255));
+            }
         }
-    }
-    const int v = (int)(i + 1);
-    // a gap without coverage (centromere, contig ends) spans many boundaries: the warp writes those together
-    const bool longr = (h1 - h0 > 2) || (l1 - l0 > 2);
-    unsigned m = __ballot_sync(kFull, longr);
-    if (!longr) {
-        for (long long k = h0; k <= h1; k++) p.tile_hi[k] = v;
-        for (long long k = l0; k <= l1; k++) p.tile_lo[k] = v;
-    }
-    while (m) {
-        const int src = __ffs(m) - 1;
-        m &= m - 1;
-        const long long a0 = __shfl_sync(kFull, h0, src), a1 = __shfl_sync(kFull, h1, src);
-        const long long b0 = __shfl_sync(kFull, l0, src), b1 = __shfl_sync(kFull, l1, src);
-        const int vv = __shfl_sync(kFull, v, src);
-        for (long long k = a0 + lane; k <= a1; k += 32) p.tile_hi[k] = vv;
-        for (long long k = b0 + lane; k <= b1; k += 32) p.tile_lo[k] = vv;
+        const int v = (int)(i + 1);
+        // a gap without coverage (centromere, contig ends) spans many boundaries: the warp writes those together
+        const bool longr = (h1 - h0 > 2) || (l1 - l0 > 2);
+        unsigned m = __ballot_sync(kFull, longr);
+        if (!longr) {
+            for (long long k = h0; k <= h1; k++) p.tile_hi[k] = v;
+            for (long long k = l0; k <= l1; k++) p.tile_lo[k] = v;
+        }
+        while (m) {
+            const int src = __ffs(m) - 1;
+            m &= m - 1;
+            const long long a0 = __shfl_sync(kFull, h0, src), a1 = __shfl_sync(kFull, h1, src);
+            const long long b0 = __shfl_sync(kFull, l0, src), b1 = __shfl_sync(kFull, l1, src);
+            const int vv = __shfl_sync(kFull, v, src);
+            for (long long k = a0 + lane; k <= a1; k += 32) p.tile_hi[k] = vv;
+            for (long long k = b0 + lane; k <= b1; k += 32) p.tile_lo[k] = vv;
+        }
     }
 }
 
@@ -1190,11 +1211,13 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
     int* const s_tile = s_buf + kF8Guard;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = gridDim.x;
-    if (p.header[3] != 0) return;                           // K_tileidx8 found unsorted anchors: the host falls back
+    pdl_launch_dependents();
 #pragma unroll
     for (int j = 0; j < kF8BPT / 4; j++) reinterpret_cast<int4*>(s_tile)[tid * (kF8BPT / 4) + j] = make_int4(0, 0, 0, 0);   // later tiles: cleared by the core
     if (tid < 2 * kF8Guard) s_buf[tid < kF8Guard ? tid : kTile + tid] = 0;   // the lead guard is cleared again after each tile's read
     if (tid < kF8Warps) s_carry[tid] = 0;
+    pdl_wait();
+    if (p.header[3] == p.p8_tag) return;                    // K_tileidx8 found unsorted anchors: the host falls back
     int tile = p.tile_begin + blockIdx.x;
     const int nb = p.p8_nblocks;                            // (clamps: garbage ranges of a rejected input stay in bounds)
     int lo = 0, hi = 0, lo2 = 0, hi2 = 0;
@@ -1228,36 +1251,42 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
 
 // K_gather: one warp per 512-base chunk moves its runs from claim order to position order.  The ordered offset
 // of a chunk is the number of runs that start before it: counts per 64 chunks + the chunk counts of its own group
-// (only chunks that have runs pay for the sum).
-__global__ void __launch_bounds__(256) depth_gather_runs_kernel(const uint64_t* __restrict__ header,
+// (only chunks that have runs pay for the sum).  Warps stride over the chunks, so any grid covers them.
+// header[3] == reject: the fast path was rejected (fused int32: 1; packed8: the reduce's tag).  hdr_out (packed8: the
+// ctx's mapped host header) receives the header's first four words, rejected or not.
+__global__ void __launch_bounds__(256) depth_gather_runs_kernel(const uint64_t* __restrict__ header, uint64_t reject,
+                                                               uint64_t* __restrict__ hdr_out,
                                                                const uint64_t* __restrict__ chunk_runs,
                                                                const unsigned* __restrict__ super_cnt, int chunks,
                                                                const int* __restrict__ tmp_start,
                                                                const unsigned char* __restrict__ tmp_class,
                                                                int* __restrict__ run_start, unsigned char* __restrict__ run_class,
                                                                long long cap) {
-    if (header[3] != 0) return;                                         // fused path was rejected
+    pdl_launch_dependents();
+    pdl_wait();
+    if (hdr_out && blockIdx.x == 0 && threadIdx.x < 4) hdr_out[threadIdx.x] = header[threadIdx.x];
+    if (header[3] == reject) return;
     const int lane = threadIdx.x & 31;
-    const int base = (blockIdx.x * 8 + (threadIdx.x >> 5)) * 32;        // each warp looks at 32 chunks (one coalesced load)
-    if (base >= chunks) return;
-    const uint64_t mine = (base + lane < chunks) ? chunk_runs[base + lane] : 0;
-    unsigned nz = __ballot_sync(kFull, (unsigned)mine != 0);
-    while (nz) {                                                        // warp-uniform: chunks that have runs
-        const int l = __ffs(nz) - 1;
-        nz &= nz - 1;
-        const int t = base + l;
-        const uint64_t w = __shfl_sync(kFull, mine, l);
-        const unsigned cnt = (unsigned)w;
-        const int st = t >> kSuperShift;
-        unsigned part = 0;
-        for (int k = lane; k < st; k += 32) part += super_cnt[k];
-        for (int k = (st << kSuperShift) + lane; k < t; k += 32) part += (unsigned)chunk_runs[k];
-        const long long dst = (long long)__reduce_add_sync(kFull, part);
-        const long long src = (long long)(w >> 32);
-        for (unsigned i = lane; i < cnt; i += 32) {
-            if (src + i < cap && dst + i < cap) {
-                run_start[dst + i] = tmp_start[src + i];
-                run_class[dst + i] = tmp_class[src + i];
+    for (int base = (blockIdx.x * 8 + (threadIdx.x >> 5)) * 32; base < chunks; base += gridDim.x * 256) {   // 32 chunks per warp (one coalesced load)
+        const uint64_t mine = (base + lane < chunks) ? chunk_runs[base + lane] : 0;
+        unsigned nz = __ballot_sync(kFull, (unsigned)mine != 0);
+        while (nz) {                                                    // warp-uniform: chunks that have runs
+            const int l = __ffs(nz) - 1;
+            nz &= nz - 1;
+            const int t = base + l;
+            const uint64_t w = __shfl_sync(kFull, mine, l);
+            const unsigned cnt = (unsigned)w;
+            const int st = t >> kSuperShift;
+            unsigned part = 0;
+            for (int k = lane; k < st; k += 32) part += super_cnt[k];
+            for (int k = (st << kSuperShift) + lane; k < t; k += 32) part += (unsigned)chunk_runs[k];
+            const long long dst = (long long)__reduce_add_sync(kFull, part);
+            const long long src = (long long)(w >> 32);
+            for (unsigned i = lane; i < cnt; i += 32) {
+                if (src + i < cap && dst + i < cap) {
+                    run_start[dst + i] = tmp_start[src + i];
+                    run_class[dst + i] = tmp_class[src + i];
+                }
             }
         }
     }
@@ -1469,12 +1498,38 @@ int accumulate_events(gl_ctx* ctx) {
 
 // The reduce's work is queued: send its header home behind it and leave the rest to depth_resolve (ctx->pend is filled in).
 // No wait here, so the next region's work queues up behind this one while the device is still busy.  The slot is
-// overwritten in stream order by the next reduce's header; depth_resolve only reads it after the latest ev_hdr.
+// overwritten in stream order by the next reduce's header; depth_resolve reads it behind an event it records itself.
+// (The packed8 path needs no copy: its K_gather stores the header through the slot's device alias.)
 int defer_header(gl_ctx* ctx) {
     GL_CUDA(ctx, cudaMemcpyAsync(ctx->hdr_host, ctx->scratch.p, 4 * sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    GL_CUDA(ctx, cudaEventRecord(ctx->ev_hdr, ctx->stream));
     ctx->pend.active = true;
     return GL_OK;
+}
+
+// One launch of the packed8 chain (K_tileidx8 -> K_fused8 -> K_gather, and on into the next reduce): programmatic stream
+// serialization lets the kernel launch and ramp up while the one before it drains; it waits at pdl_wait().
+template <class... Params, class... Args>
+int launch_chained(gl_ctx* ctx, void (*kernel)(Params...), unsigned grid, unsigned block, Args... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = ctx->stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    GL_CUDA(ctx, cudaLaunchKernelEx(&cfg, kernel, args...));
+    GL_LAUNCHED(ctx, 1);
+    return GL_OK;
+}
+
+// CTAs of a 256-thread kernel the device holds at once (a one-wave grid: every CTA is resident when the wait releases)
+int one_wave_256(gl_ctx* ctx, const void* kernel) {
+    int nblk = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, kernel, 256, 0) != cudaSuccess || nblk < 1) { cudaGetLastError(); nblk = 1; }
+    return ctx->sm_count * nblk;
 }
 
 constexpr int kP8ChunksMax = 32;
@@ -1537,7 +1592,8 @@ struct Reduce {
     char* tail = nullptr;
 };
 
-int reduce_begin(gl_ctx* ctx, const ReduceArgs& a, int warps, size_t zeroed_bytes, size_t tail_bytes, Reduce& r) {
+// zero_on_device: the path's first kernel zeroes the scratch itself (p.zero_words), with no memset in front of it
+int reduce_begin(gl_ctx* ctx, const ReduceArgs& a, int warps, size_t zeroed_bytes, size_t tail_bytes, Reduce& r, bool zero_on_device = false) {
     const int64_t len = ctx->re - ctx->rs;
     const int64_t w0 = ctx->rs / a.W;
     const bool want_min = a.do_windows && a.want_min;
@@ -1556,11 +1612,12 @@ int reduce_begin(gl_ctx* ctx, const ReduceArgs& a, int warps, size_t zeroed_byte
     ctx->win_sum_p = sbase + head_bytes;
     r.zeroed = sbase + head_bytes + win_bytes;
     r.tail = sbase + zero_bytes + run_bytes;
-    GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
+    if (!zero_on_device) GL_CUDA(ctx, cudaMemsetAsync(sbase, 0, zero_bytes, ctx->stream));
     if (want_min) GL_CUDA(ctx, cudaMemsetAsync(ctx->win_min.p, 0x7f, (size_t)r.n_windows * 4, ctx->stream));
 
     ScanParams& p = r.p;
     memset(&p, 0, sizeof p);
+    p.zero_words = zero_on_device ? (long long)(zero_bytes / 8) : 0;
     p.len = (int)len;
     p.rs = (int)ctx->rs;
     p.re = (int)ctx->re;
@@ -1596,11 +1653,22 @@ int reduce_begin(gl_ctx* ctx, const ReduceArgs& a, int warps, size_t zeroed_byte
 // is read, and leave the rest to depth_resolve.
 int reduce_end(gl_ctx* ctx, const Reduce& r, int path, int64_t w_sent) {
     const ScanParams& p = r.p;
-    if (p.do_runs) {
+    int* const run_start = static_cast<int*>(ctx->run_start.p);
+    unsigned char* const run_class = static_cast<unsigned char*>(ctx->run_class.p);
+    if (path == kPathPacked8) {
+        // always launched, as the last link of the chain: it also stores the header into the mapped host slot
+        static int gather_wave = 0;
+        if (gather_wave == 0) gather_wave = one_wave_256(ctx, reinterpret_cast<const void*>(depth_gather_runs_kernel));
+        const int chunks = p.do_runs ? (int)r.chunks : 0;
+        gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
+        GL_CHECK(launch_chained(ctx, depth_gather_runs_kernel, (unsigned)std::max<int64_t>(1, std::min<int64_t>((chunks + 255) / 256, gather_wave)), 256,
+                                (const uint64_t*)p.header, (uint64_t)p.p8_tag, ctx->hdr_dev, (const uint64_t*)p.chunk_runs,
+                                (const unsigned*)p.super_cnt, chunks, (const int*)p.tmp_start, (const unsigned char*)p.tmp_class,
+                                run_start, run_class, p.run_cap));
+    } else if (p.do_runs) {
         gl_prof_scope prof(ctx, "depth_gather_runs_kernel");
         depth_gather_runs_kernel<<<(unsigned)((r.chunks + 255) / 256), 256, 0, ctx->stream>>>(
-            p.header, p.chunk_runs, p.super_cnt, (int)r.chunks, p.tmp_start, p.tmp_class, static_cast<int*>(ctx->run_start.p),
-            static_cast<unsigned char*>(ctx->run_class.p), p.run_cap);
+            p.header, 1, nullptr, p.chunk_runs, p.super_cnt, (int)r.chunks, p.tmp_start, p.tmp_class, run_start, run_class, p.run_cap);
         GL_LAUNCHED(ctx, 1);
     }
     ctx->prefetched = false;
@@ -1627,6 +1695,11 @@ int reduce_end(gl_ctx* ctx, const Reduce& r, int path, int64_t w_sent) {
     ctx->pend.cells = p.batch[0].cell_hi;      // batch 0's cell_hi
     ctx->pend.origin = p.origin;
     ctx->pend.ncells = p.ncells;
+    ctx->pend.tag = p.p8_tag;
+    if (path == kPathPacked8) {
+        ctx->pend.active = true;
+        return GL_OK;
+    }
     return defer_header(ctx);
 }
 
@@ -1635,14 +1708,17 @@ int reduce_end(gl_ctx* ctx, const Reduce& r, int path, int64_t w_sent) {
 int reduce_packed8(gl_ctx* ctx, const ReduceArgs& a) {
     const size_t tile_tab = al256((size_t)(num_tiles_for(ctx->re - ctx->rs) + 1) * 4);
     Reduce r;
-    GL_CHECK(reduce_begin(ctx, a, kF8Warps, 0, 2 * tile_tab, r));      // tail: tile_lo | tile_hi
+    GL_CHECK(reduce_begin(ctx, a, kF8Warps, 0, 2 * tile_tab, r, true));   // tail: tile_lo | tile_hi; the first K_tileidx8 zeroes
     static int f8_ctas_per_sm = 0;                            // persistent grid: what fits on an SM (registers decide)
     if (f8_ctas_per_sm == 0) {
         int nblk = 0;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nblk, depth_fused8_kernel<false>, kF8Threads, 0) != cudaSuccess || nblk < 1) { cudaGetLastError(); nblk = 4; }
         f8_ctas_per_sm = nblk;
     }
+    static int tileidx_wave = 0;
+    if (tileidx_wave == 0) tileidx_wave = one_wave_256(ctx, reinterpret_cast<const void*>(depth_tileidx8_kernel));
     ScanParams& p = r.p;
+    p.p8_tag = ctx->p8_tag++;
     p.p8_anchors = ctx->p8.anchors;
     p.p8_ds = static_cast<const unsigned*>(ctx->p8.ds);
     p.p8_len = static_cast<const unsigned*>(ctx->p8.len);
@@ -1677,8 +1753,9 @@ int reduce_packed8(gl_ctx* ctx, const ReduceArgs& a) {
         p.idx_end = (int)(last ? nb : b1 - 1);
         if (p.idx_end > p.idx_begin) {
             gl_prof_scope prof(ctx, "depth_tileidx8_kernel");
-            depth_tileidx8_kernel<<<(unsigned)((p.idx_end - p.idx_begin + 255) / 256), 256, 0, ctx->stream>>>(p);
-            GL_LAUNCHED(ctx, 1);
+            GL_CHECK(launch_chained(ctx, depth_tileidx8_kernel, (unsigned)std::min<int64_t>(((int64_t)p.idx_end - p.idx_begin + 255) / 256, tileidx_wave),
+                                    256, (const ScanParams)p));
+            p.zero_words = 0;                                 // later chunks' launches must not zero again
         }
         // tiles whose end boundary is not beyond the last anchor on the device are complete
         int64_t t_ready = tiles;
@@ -1691,8 +1768,8 @@ int reduce_packed8(gl_ctx* ctx, const ReduceArgs& a) {
             p.tile_end = (int)t_ready;
             gl_prof_scope prof(ctx, "depth_fused8_kernel");
             auto k8 = p.md.mode ? depth_fused8_kernel<true> : depth_fused8_kernel<false>;   // the multidepth epilogue, or none
-            k8<<<(unsigned)std::min<int64_t>(t_ready - t_prev, (int64_t)ctx->sm_count * f8_ctas_per_sm), kF8Threads, 0, ctx->stream>>>(p);
-            GL_LAUNCHED(ctx, 1);
+            GL_CHECK(launch_chained(ctx, k8, (unsigned)std::min<int64_t>(t_ready - t_prev, (int64_t)ctx->sm_count * f8_ctas_per_sm), kF8Threads,
+                                    (const ScanParams)p));
         }
         if (early_sums && !last && t_ready > t_prev) {
             // windows that end at or before the last reduced tile's end are final: send them home on their own stream
@@ -1710,8 +1787,11 @@ int reduce_packed8(gl_ctx* ctx, const ReduceArgs& a) {
         b0 = b1;
     }
     ctx->p8.upload_pending = false;
-    GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));      // the packed staging buffer may be overwritten after this
-    return reduce_end(ctx, r, kPathPacked8, w_sent);
+    GL_CHECK(reduce_end(ctx, r, kPathPacked8, w_sent));
+    // words from the packed staging buffer (host adds): it may be overwritten after this.  Device words (the caller's own
+    // buffers) need no event, so consecutive resident reduces hold nothing but the chain's kernels.
+    if (ctx->p8.anchors == ctx->packed.p) GL_CUDA(ctx, cudaEventRecord(ctx->ev_used[0], ctx->stream));
+    return GL_OK;
 }
 
 inline bool general_path(int path) { return path == kPathHbmDiff || path == kPathEvents; }
@@ -1864,10 +1944,12 @@ int depth_resolve(gl_ctx* ctx) {
     while (ctx->pend.active) {
         const auto q = ctx->pend;
         ctx->pend.active = false;
+        GL_CUDA(ctx, cudaEventRecord(ctx->ev_hdr, ctx->stream));            // behind the pending reduce and its header
         GL_CUDA(ctx, cudaEventSynchronize(ctx->ev_hdr));
         if (q.d2h) GL_CUDA(ctx, cudaStreamSynchronize(ctx->d2h_stream));
-        const uint64_t* hdr = ctx->hdr_host;
-        if ((q.path == kPathPacked8 || q.path == kPathFused) && hdr[3] != 0) {   // packed8 anchors not sorted / int32 input not in BAM order
+        const volatile uint64_t* hdr = ctx->hdr_host;                       // packed8: written by the device through the mapping
+        // packed8 anchors not sorted (this reduce's tag) / int32 input not in BAM order
+        if (q.path == kPathPacked8 ? hdr[3] == q.tag : (q.path == kPathFused && hdr[3] != 0)) {
             ctx->prefetched = false;
             ctx->prefetched_runs = 0;
             GL_CHECK(run_reduce(ctx, q.args, q.path == kPathPacked8 ? kPathFused : kPathEvents));   // the next path down
@@ -1948,6 +2030,7 @@ int gl_depth_add_segments(gl_ctx* ctx, const int32_t* start, const int32_t* end,
     int32_t* d_s = static_cast<int32_t*>(ctx->store_s.p) + ctx->store_n;
     int32_t* d_e = static_cast<int32_t*>(ctx->store_e.p) + ctx->store_n;
     // a reduce of the previous region may still be queued and reading the store: the copies go after it
+    GL_CUDA(ctx, cudaEventRecord(ctx->ev_hdr, ctx->stream));
     GL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_hdr, 0));
     if (is_pinned_host(start) && is_pinned_host(end)) {
         GL_CUDA(ctx, cudaMemcpyAsync(d_s, start, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->copy_stream));

@@ -103,13 +103,17 @@ struct gl_ctx {
     int64_t* prefetch_sums = nullptr; int64_t prefetch_cap = 0; bool prefetched = false;   // one-call entries: window sums go home while the header is read
     int32_t* prefetch_run_start = nullptr; uint8_t* prefetch_run_class = nullptr; int64_t prefetch_run_cap = 0, prefetched_runs = 0;   // and the first runs
     // gl_depth_reduce only queues its work: the header (runs claimed, max depth, fast path rejected) travels into the pinned
-    // hdr_host behind ev_hdr, and depth_resolve reads it at the first result query, with what accepting or rerunning needs
-    uint64_t* hdr_host = nullptr;         // 4 words, pinned
+    // hdr_host (a copy, or on the packed8 path K_gather's store through hdr_dev), and depth_resolve reads it behind ev_hdr
+    // at the first result query, with what accepting or rerunning needs
+    uint64_t* hdr_host = nullptr;         // 4 words, pinned and mapped
+    uint64_t* hdr_dev = nullptr;          // hdr_host's device address
     cudaEvent_t ev_hdr = nullptr;
+    uint64_t p8_tag = 2;                  // the next packed8 reduce's rejection tag (never 0 or 1, never reused)
     struct { bool active = false;
              ReduceArgs args;
              int path = kPathNone; long long run_cap = 0; int64_t n_windows = 0;   // the path tried and its run capacity
              bool d2h = false;                                             // window sums also on their way home on d2h_stream
+             uint64_t tag = 0;                                             // packed8: header[3] == tag means rejected
              const int* flags = nullptr; const unsigned* cells = nullptr; int origin = 0, ncells = 0; } pend;
     gl_buf win_min;       // i32[n_windows]
     gl_buf run_start;     // i32[run_cap]

@@ -96,7 +96,8 @@ int gl_ctx_create(int device, gl_ctx** out) {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_used[i], cudaEventDisableTiming);
     }
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_hdr, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaHostAlloc(reinterpret_cast<void**>(&ctx->hdr_host), 4 * sizeof(uint64_t), cudaHostAllocDefault);
+    if (e == cudaSuccess) e = cudaHostAlloc(reinterpret_cast<void**>(&ctx->hdr_host), 4 * sizeof(uint64_t), cudaHostAllocMapped);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&ctx->hdr_dev), ctx->hdr_host, 0);
     if (e == cudaSuccess) {
         cudaDeviceProp prop;
         e = cudaGetDeviceProperties(&prop, device);

@@ -1182,20 +1182,25 @@ __device__ __forceinline__ P8Regs fused8_load(const ScanParams& p, int lo, int h
     return r;
 }
 
-__device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t0) {
-    const int sub = threadIdx.x & 15, lane = threadIdx.x & 31;
-    const int d0 = r.d & 0xff, d1 = d0 + ((r.d >> 8) & 0xff), d2 = d1 + ((r.d >> 16) & 0xff), d3 = d2 + (r.d >> 24);
-    int inc = d3;
+// Inclusive scan over each 16-lane half of the warp (one block's words), as warp_incl_scan: shfl.up within 16-lane
+// segments (c = 0x1000) says whether the source lane is in this lane's segment, so a step is a SHFL and a predicated add.
+__device__ __forceinline__ int half_warp_incl_scan(int v) {
 #pragma unroll
-    for (int o = 1; o < 16; o <<= 1) {
-        const int v = __shfl_up_sync(kFull, inc, o, 16);
-        if (sub >= o) inc += v;
-    }
+    for (int o = 1; o < 16; o <<= 1)
+        asm("{\n\t.reg .s32 t;\n\t.reg .pred p;\n\tshfl.sync.up.b32 t|p, %0, %1, 0x1000, -1;\n\t@p add.s32 %0, %0, t;\n\t}" : "+r"(v) : "r"(o));
+    return v;
+}
+
+__device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t0) {
     if (__ballot_sync(kFull, r.l != 0) == 0) return;        // no live slot in the whole warp (warp-uniform: no divergence)
+    const int lane = threadIdx.x & 31;
+    // byte k of a word, zero-extended: one PRMT (__byte_perm selector 0x444k) where a shift and a mask take two
+    const int d0 = r.d & 0xff, d1 = d0 + __byte_perm(r.d, 0, 0x4441), d2 = d1 + __byte_perm(r.d, 0, 0x4442), d3 = d2 + (r.d >> 24);
+    const int inc = half_warp_incl_scan(d3);
     const int base = r.anchor + inc - d3 - t0;              // tile-relative start of the slot before this thread's first
     fused_apply32(s_tile, base + d0, (int)(r.l & 0xff), lane);
-    fused_apply32(s_tile, base + d1, (int)((r.l >> 8) & 0xff), lane);
-    fused_apply32(s_tile, base + d2, (int)((r.l >> 16) & 0xff), lane);
+    fused_apply32(s_tile, base + d1, (int)__byte_perm(r.l, 0, 0x4441), lane);
+    fused_apply32(s_tile, base + d2, (int)__byte_perm(r.l, 0, 0x4442), lane);
     fused_apply32(s_tile, base + d3, (int)(r.l >> 24), lane);
 }
 

@@ -14,13 +14,14 @@
 // The device checks a fast path's eligibility itself and says so in the reduce's header; depth_resolve then reruns the
 // region on the next path down.
 //
-// Tile core (every path, DESIGN §1.3): 16 or 32 consecutive bases per thread (swizzled smem transpose), one thread-local
+// Tile core (every path, DESIGN §1.3): 16 or 64 consecutive bases per thread (swizzled smem transpose), one thread-local
 // + one warp scan, REDUX-based window sums (one LDS per lane and window edge), class runs detected on warp min/max with a
 // per-base slow path, runs claimed per tile with one atomic and put in position order by K_gather.
 // All arithmetic is integer; results are bit-exact against oracle/oracle_depth.c.
 #include "gl_common.cuh"
 #include <string.h>
 #include <chrono>
+#include <type_traits>
 
 extern "C" int glhost_pool_size(void);          // host/thread_pool.cpp: threads of the library's host pool
 
@@ -61,9 +62,12 @@ __device__ __forceinline__ int4 ld_stream_int4(const int4* p) {
 // consecutive chunks and for a warp whose lane l touches chunks 4l..4l+3 (the blocked layout).
 __device__ __forceinline__ int swz_chunk(int c) { return c ^ ((c >> 2) & 7); }
 __device__ __forceinline__ int swz_elem(int e) { return e ^ (((e >> 4) & 7) << 2); }   // == (swz_chunk(e>>2)<<2) | (e&3)
-// the same for a core whose threads own BPT consecutive bases (BPT/4 chunks): lane l touches chunks (BPT/4)l .. +BPT/4-1
-template <int BPT> __device__ __forceinline__ int swz_chunk_t(int c) { return BPT == 32 ? (c ^ ((c >> 3) & 7)) : (c ^ ((c >> 2) & 7)); }
-template <int BPT> __device__ __forceinline__ int swz_elem_t(int e) { return BPT == 32 ? (e ^ (((e >> 5) & 7) << 2)) : (e ^ (((e >> 4) & 7) << 2)); }
+// the same for a core whose threads own BPT consecutive bases (BPT/4 chunks): lane l touches chunks (BPT/4)l .. +BPT/4-1.
+// BPT 64: thread t's chunk j is 16t ^ (t & 7) ^ j, so the 8 lanes of each quarter-warp phase of an LDS/STS.128 hit chunks
+// (t & 7) ^ j mod 8, eight distinct bank groups; and the 64 bases of one thread are XORed with the constant (t & 7) << 2,
+// a permutation within each aligned group of 32, so 32 lanes reading 32 of them hit 32 banks.
+template <int BPT> __device__ __forceinline__ int swz_chunk_t(int c) { return BPT == 64 ? (c ^ ((c >> 4) & 7)) : (c ^ ((c >> 2) & 7)); }
+template <int BPT> __device__ __forceinline__ int swz_elem_t(int e) { return BPT == 64 ? (e ^ (((e >> 6) & 7) << 2)) : (e ^ (((e >> 4) & 7) << 2)); }
 
 // ================================================================================================
 // GENERAL path, K_scatter.  One thread = 4 segments (two 128-bit loads), 8 fire-and-forget reds.
@@ -325,7 +329,7 @@ struct ScanParams {
     unsigned char* tmp_class;     // [run_cap]
     long long run_cap;
     uint64_t* header;             // [0]=runs claimed (= n_runs) [2]=max_depth [3]=fused path rejected (1) / packed8 rejected (p8_tag)
-    uint64_t* chunk_runs;         // [num_tiles*8] per 512-base warp chunk: (claim offset << 32) | count
+    uint64_t* chunk_runs;         // [num_tiles*warps] per warp chunk of the core: (claim offset << 32) | count
     unsigned* super_cnt;          // [num_tiles*8/64+1] run starts per 64 chunks
     int* depth_out;               // optional per-base output (debug/parity), else null
     int num_tiles;
@@ -375,16 +379,37 @@ __device__ __forceinline__ int warp_incl_scan(int v) {
     return v;
 }
 
-// BPT bases per thread (16 or 32), WARPS warps per CTA, BPT * 32 * WARPS == kTile.  32 bases per thread halves the work
-// that is paid per thread and tile (warp scans, class check, window sums, run claim, barrier) — K_fused8 uses <32, 4>.
+// The window of a thread's first base a = rs + idx0 (iw = a / W, rem = a % W), and cu = the number of the thread's bpt
+// bases left of the next window edge when that edge falls inside them (0: none)
+__device__ __forceinline__ void window_edge(const ScanParams& p, int idx0, int bpt, unsigned& iw, unsigned& rem, int& cu) {
+    const unsigned a = (unsigned)p.rs + (unsigned)idx0;              // absolute, < 2^32
+    const unsigned uW = (unsigned)p.W;
+    // iw = a / W without a division: q = hi32(a * floor(2^32/W)) is the quotient or one less, because
+    // a * floor(2^32/W) > a * 2^32 / W - a and a < 2^32
+    iw = __umulhi(a, p.W_inv);
+    rem = a - iw * uW;
+    if (rem >= uW) { iw++; rem -= uW; }
+    cu = uW - rem < (unsigned)bpt ? (int)(uW - rem) : 0;
+}
+
+// Per-base run-start bits of one thread's bases
+__device__ __forceinline__ int mask_popc(unsigned m) { return __popc(m); }
+__device__ __forceinline__ int mask_popc(unsigned long long m) { return __popcll(m); }
+__device__ __forceinline__ int mask_ffs(unsigned m) { return __ffs(m); }
+__device__ __forceinline__ int mask_ffs(unsigned long long m) { return __ffsll((long long)m); }
+
+// BPT bases per thread (16 or 64), WARPS warps per CTA, BPT * 32 * WARPS == kTile.  64 bases per thread spreads the work
+// that is paid per thread and tile (warp scans, class check, window sums, run claim, barrier) over four times the bases
+// of the 16-base core — K_fused8 uses <64, 2>.
 // kSliceInTile (K_fused8): the depth slice goes over the warp's own region of s_tile instead of s_depth (unused, may be
 // null), and the region is cleared when the core is done with it.  The caller must then hold every warp at a barrier
 // between the core and the next tile's atomics.
 template <int BPT, int WARPS, bool kZeroAfterRead, bool kMD = false, bool kSliceInTile = false>
 __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__ s_tile, int* __restrict__ s_depth,
                                           const int* s_carry, int tile, int& acc_max) {
-    static_assert(BPT * 32 * WARPS == kTile, "tile shape");
+    static_assert(BPT * 32 * WARPS == kTile && (BPT == 16 || BPT == 64), "tile shape");
     constexpr int kWElems = BPT * 32;                         // bases per warp
+    using Mask = std::conditional_t<BPT == 64, unsigned long long, unsigned>;   // one bit per base of a thread
     __shared__ int s_warp_tot[WARPS];
     __shared__ int s_has_break;
     __shared__ int s_tbase[WARPS * 32];                       // depth before each thread's first base (slow paths)
@@ -397,35 +422,84 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     // ---- BPT consecutive differences per thread; thread-local inclusive scan; one warp scan
     // a thread's chunks: swz_chunk_t<BPT>(t * (BPT / 4) + j) == c0 ^ j for j < BPT / 4 (the XOR only reads bits of t)
     const int c0 = swz_chunk_t<BPT>(tid * (BPT / 4));
-    int x[BPT];
-#pragma unroll
-    for (int j = 0; j < BPT / 4; j++) {
-        const int4 q = reinterpret_cast<const int4*>(s_tile)[c0 ^ j];
-        x[4 * j] = q.x; x[4 * j + 1] = q.y; x[4 * j + 2] = q.z; x[4 * j + 3] = q.w;
-        if (kZeroAfterRead && !kSliceInTile) reinterpret_cast<int4*>(s_tile)[c0 ^ j] = make_int4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int k = 1; k < BPT; k++) x[k] += x[k - 1];
-    const int inc = warp_incl_scan(x[BPT - 1]);
-    const int lane_excl = inc - x[BPT - 1];
-    if (lane == 31) s_warp_tot[warp] = inc;
     // depth[k] = tbase + x[k], tbase known only after the barrier: take min / max / sum of the x[k] now, while other
     // warps are still arriving, and add tbase afterwards (the per-base depths are formed only where a slow path needs them)
-    int xmn = x[0], xmx = x[0];
-#pragma unroll
-    for (int k = 1; k + 1 < BPT; k += 2) {                    // three-input min / max (VIMNMX3)
-        xmn = __vimin3_s32(xmn, x[k], x[k + 1]);
-        xmx = __vimax3_s32(xmx, x[k], x[k + 1]);
-    }
-    xmn = min(xmn, x[BPT - 1]);
-    xmx = max(xmx, x[BPT - 1]);
+    int x[BPT];
     int g8[BPT / 8];                                          // sums of groups of 8 (the window path reuses them)
+    int xmn, xmx, xsum, xlast;
+    // the fast window path's terms (below); kSliceInTile finds them before the barrier
+    unsigned iw = 0, rem = 0;
+    int cu = 0, lx = 0;
+    if constexpr (kSliceInTile) {
+        // x[64] held across the barrier would cost ~40 registers (118 in all, 8 CTAs per SM), so the thread reads its
+        // differences in two halves of 32 and keeps only what the fast window path needs.  The differences stay in the
+        // warp's region of s_tile until the warp clears it, so a warp that needs x after the barrier scans them again.
+        // cu depends only on positions: lx is summed half by half, from the half's group sums and one partial group.
+        window_edge(p, idx0, BPT, iw, rem, cu);
+        xmn = INT_MAX; xmx = INT_MIN; xsum = 0;
+        int run = 0;
 #pragma unroll
-    for (int g = 0; g < BPT / 8; g++)
-        g8[g] = (x[8 * g] + x[8 * g + 1] + x[8 * g + 2]) + (x[8 * g + 3] + x[8 * g + 4] + x[8 * g + 5]) + (x[8 * g + 6] + x[8 * g + 7]);
-    int xsum = g8[0];
+        for (int h = 0; h < BPT / 32; h++) {
 #pragma unroll
-    for (int g = 1; g < BPT / 8; g++) xsum += g8[g];
+            for (int j = 0; j < 8; j++) {
+                const int4 q = reinterpret_cast<const int4*>(s_tile)[c0 ^ (8 * h + j)];
+                x[4 * j] = q.x; x[4 * j + 1] = q.y; x[4 * j + 2] = q.z; x[4 * j + 3] = q.w;
+            }
+            x[0] += run;
+#pragma unroll
+            for (int k = 1; k < 32; k++) x[k] += x[k - 1];
+            run = x[31];
+#pragma unroll
+            for (int k = 0; k < 32; k += 2) {                 // three-input min / max (VIMNMX3)
+                xmn = __vimin3_s32(xmn, x[k], x[k + 1]);
+                xmx = __vimax3_s32(xmx, x[k], x[k + 1]);
+            }
+#pragma unroll
+            for (int g = 0; g < 4; g++) {
+                g8[g] = (x[8 * g] + x[8 * g + 1] + x[8 * g + 2]) + (x[8 * g + 3] + x[8 * g + 4] + x[8 * g + 5]) + (x[8 * g + 6] + x[8 * g + 7]);
+                xsum += g8[g];
+            }
+            const int ch = min(max(cu - 32 * h, 0), 32);      // bases of this half left of the edge
+            const int gi = ch >> 3, r = ch & 7;
+#pragma unroll
+            for (int g = 0; g < 4; g++) lx += g < gi ? g8[g] : 0;
+#pragma unroll
+            for (int j = 0; j < 7; j++) {
+                int v = x[j];
+#pragma unroll
+                for (int g = 1; g < 4; g++) v = gi == g ? x[8 * g + j] : v;
+                lx += j < r ? v : 0;
+            }
+        }
+        xlast = run;
+    } else {
+#pragma unroll
+        for (int j = 0; j < BPT / 4; j++) {
+            const int4 q = reinterpret_cast<const int4*>(s_tile)[c0 ^ j];
+            x[4 * j] = q.x; x[4 * j + 1] = q.y; x[4 * j + 2] = q.z; x[4 * j + 3] = q.w;
+            if (kZeroAfterRead) reinterpret_cast<int4*>(s_tile)[c0 ^ j] = make_int4(0, 0, 0, 0);
+        }
+#pragma unroll
+        for (int k = 1; k < BPT; k++) x[k] += x[k - 1];
+        xmn = x[0], xmx = x[0];
+#pragma unroll
+        for (int k = 1; k + 1 < BPT; k += 2) {                // three-input min / max (VIMNMX3)
+            xmn = __vimin3_s32(xmn, x[k], x[k + 1]);
+            xmx = __vimax3_s32(xmx, x[k], x[k + 1]);
+        }
+        xmn = min(xmn, x[BPT - 1]);
+        xmx = max(xmx, x[BPT - 1]);
+#pragma unroll
+        for (int g = 0; g < BPT / 8; g++)
+            g8[g] = (x[8 * g] + x[8 * g + 1] + x[8 * g + 2]) + (x[8 * g + 3] + x[8 * g + 4] + x[8 * g + 5]) + (x[8 * g + 6] + x[8 * g + 7]);
+        xsum = g8[0];
+#pragma unroll
+        for (int g = 1; g < BPT / 8; g++) xsum += g8[g];
+        xlast = x[BPT - 1];
+    }
+    const int inc = warp_incl_scan(xlast);
+    const int lane_excl = inc - xlast;
+    if (lane == 31) s_warp_tot[warp] = inc;
     if (tid == 0) {
         // does a forced run break (multiple of run_break) fall inside this tile?  (absolute positions are < 2^32)
         int hb = 0;
@@ -443,16 +517,71 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     const int tbase = wbase + lane_excl;                      // depth at the base before this thread's first
 
     const int mn = tbase + xmn, mx = tbase + xmx;
-#define GL_D(k) (tbase + x[k])                                 /* depth of this thread's k-th base */
+    const bool full_warp = warp_base + kWElems <= p.len;   // false only at the region's ragged end
+    const int wmin = __reduce_min_sync(kFull, mn), wmax = __reduce_max_sync(kFull, mx);
+
+    const bool tile_has_break = s_has_break != 0;
+
+    // class(d) is monotone in d: the warp's bases plus the base before them are one class iff
+    // class(min) == class(max) — then no run starts here and all per-base class work is skipped.
+    bool slow_runs = false;
+    if (p.do_runs)
+        slow_runs = !full_warp || tile_has_break || warp_base == 0 ||
+                    cov_class(min(wmin, wbase), p.mincov, p.maxmean) != cov_class(max(wmax, wbase), p.mincov, p.maxmean);
+    constexpr int kFastDepth = kWElems > 1024 ? (1 << 21) : (1 << 22);   // kWElems * kFastDepth <= 2^32
+    const bool fast_win = p.do_windows && full_warp && p.W >= BPT && p.win_min == nullptr && wmax < kFastDepth;
+    const bool slow_win = p.do_windows && !fast_win;
+
+    // Depth by position: this warp's private slice of s_depth holds x[k] (depth relative to the thread's tbase), swizzled
+    // like s_tile (base e of the slice at sw[swz_elem_t<BPT>(e)]) so that both a lane storing its BPT/4 chunks and 32 lanes
+    // reading 32 consecutive bases of one thread are conflict-free; the threads' tbase go to s_tbase.  Storing x instead of
+    // depth saves BPT adds per thread; a reader adds the owner's tbase.  The slice uses the same chunks as the warp's region
+    // of s_tile, so a warp only ever touches its own kWElems elements of either buffer.  With kSliceInTile it overwrites
+    // that region, which is safe because no warp starts the next tile's atomics before the caller's barrier; otherwise a
+    // warp that leaves the core early may already be adding into s_tile, and the slice goes to s_depth.  With kSliceInTile
+    // x is not in registers: each thread scans its differences into the slice in place, and the per-base depths below
+    // are read from it (depth_out and the multidepth epilogues then need the slice too).
+    int* const s_slice = kSliceInTile ? s_tile : s_depth;
+    int* sw = s_slice + warp * kWElems;
+    int* stb = s_tbase + warp * 32;
+    const bool need_slice = slow_runs || slow_win || (kSliceInTile && (p.depth_out != nullptr || (kMD && p.md.mode != 0)));
+    if (need_slice) {
+        __syncwarp();
+        int run = 0;
+#pragma unroll
+        for (int j = 0; j < BPT / 4; j++) {
+            int4 q;
+            if constexpr (kSliceInTile) {
+                q = reinterpret_cast<const int4*>(s_slice)[c0 ^ j];
+                q.x += run; q.y += q.x; q.z += q.y; q.w += q.z;
+                run = q.w;
+            } else {
+                q = make_int4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
+            }
+            reinterpret_cast<int4*>(s_slice)[c0 ^ j] = q;
+        }
+        stb[lane] = tbase;
+        __syncwarp();
+    } else if (kSliceInTile) {
+        clear_warp_region<kWElems>(sw, lane);                 // every lane has read its differences (block barrier above)
+    }
+    // x[4j .. 4j+3]: from registers, or with kSliceInTile from the slice (a thread reads its own chunks: no bank conflict)
+    auto xq = [&](int j) -> int4 {
+        if constexpr (kSliceInTile) return reinterpret_cast<const int4*>(s_slice)[c0 ^ j];
+        else return make_int4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
+    };
+#define GL_D(q, i) (tbase + ((i) == 0 ? (q).x : (i) == 1 ? (q).y : (i) == 2 ? (q).z : (q).w))   /* depth of base 4j+i, q = xq(j) */
+
     if (p.depth_out) {
 #pragma unroll
         for (int j = 0; j < BPT / 4; j++) {
             const int idx = idx0 + 4 * j;
-            if (idx + 3 < p.len) reinterpret_cast<int4*>(p.depth_out + idx)[0] = make_int4(GL_D(4 * j), GL_D(4 * j + 1), GL_D(4 * j + 2), GL_D(4 * j + 3));
+            const int4 q = xq(j);
+            if (idx + 3 < p.len) reinterpret_cast<int4*>(p.depth_out + idx)[0] = make_int4(GL_D(q, 0), GL_D(q, 1), GL_D(q, 2), GL_D(q, 3));
             else {
-                if (idx < p.len) p.depth_out[idx] = GL_D(4 * j);
-                if (idx + 1 < p.len) p.depth_out[idx + 1] = GL_D(4 * j + 1);
-                if (idx + 2 < p.len) p.depth_out[idx + 2] = GL_D(4 * j + 2);
+                if (idx < p.len) p.depth_out[idx] = GL_D(q, 0);
+                if (idx + 1 < p.len) p.depth_out[idx + 1] = GL_D(q, 1);
+                if (idx + 2 < p.len) p.depth_out[idx + 2] = GL_D(q, 2);
             }
         }
     }
@@ -460,13 +589,17 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     if (kMD && p.md.mode == 1) {
         // pass 1: this sample's (d >= mincov) and (d > 0) bits, 16 bases per halfword
         const int nv = max(0, min(BPT, p.len - idx0));
-        unsigned ge = 0, pos = 0;
+        Mask ge = 0, pos = 0;
 #pragma unroll
-        for (int k = 0; k < BPT; k++) {
-            const int d = GL_D(k);
-            if (k < nv) {
-                ge |= (d >= p.md.mincov ? 1u : 0u) << k;
-                pos |= (d > 0 ? 1u : 0u) << k;
+        for (int j = 0; j < BPT / 4; j++) {
+            const int4 q = xq(j);
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const int k = 4 * j + i, d = GL_D(q, i);
+                if (k < nv) {
+                    ge |= (Mask)(d >= p.md.mincov ? 1u : 0u) << k;
+                    pos |= (Mask)(d > 0 ? 1u : 0u) << k;
+                }
             }
         }
 #pragma unroll
@@ -477,7 +610,9 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     } else if (kMD && p.md.mode == 2) {
         // pass 2: Σ d over the sufficient sites of every block that meets this warp's bases, one slot per (pair, 512-base chunk)
         const unsigned sw32 = p.md.suf[idx0 >> 5];
-        const unsigned sm = BPT == 32 ? sw32 : ((sw32 >> (idx0 & 31)) & 0xffffu);
+        Mask sm;
+        if constexpr (BPT == 64) sm = sw32 | ((Mask)p.md.suf[(idx0 >> 5) + 1] << 32);
+        else sm = (sw32 >> (idx0 & 31)) & 0xffffu;
         const int q0 = p.md.pair_ptr[tile], q1 = p.md.pair_ptr[tile + 1];
         for (int q = q0; q < q1; q++) {
             const int b = p.md.pair_blk[q];
@@ -485,72 +620,46 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
             unsigned long long part = 0;
             if (bs < warp_base + kWElems && be > warp_base) {          // warp-uniform
                 const int lo = min(max(bs - idx0, 0), BPT), hi = min(max(be - idx0, 0), BPT);
-                const unsigned rng = (hi >= 32 ? 0xffffffffu : ((1u << hi) - 1u)) & ~(lo >= 32 ? 0xffffffffu : ((1u << lo) - 1u));
-                const unsigned m = sm & rng;
+                const Mask rng = (hi >= BPT ? ~(Mask)0 : (((Mask)1 << hi) - 1u)) & ~(lo >= BPT ? ~(Mask)0 : (((Mask)1 << lo) - 1u));
+                const Mask m = sm & rng;
 #pragma unroll
-                for (int k = 0; k < BPT; k++)
-                    if ((m >> k) & 1u) part += (unsigned long long)(unsigned)GL_D(k);
+                for (int j = 0; j < BPT / 4; j++) {
+                    const int4 xj = xq(j);
+#pragma unroll
+                    for (int i = 0; i < 4; i++)
+                        if ((m >> (4 * j + i)) & 1u) part += (unsigned long long)(unsigned)GL_D(xj, i);
+                }
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(kFull, part, o);
             }
-            // slots are per 512-base chunk, so every path (8 warps x 16 bases/thread or 4 x 32) rewrites all eight of them
+            // slots are per 512-base chunk, so every path (8 warps x 16 bases/thread or 2 x 64) rewrites all eight of them
             if (lane == 0) {
 #pragma unroll
                 for (int h = 0; h < BPT / 16; h++) p.md.slots[(size_t)q * 8 + warp * (BPT / 16) + h] = h ? 0ull : part;
             }
         }
     }
-    const bool full_warp = warp_base + kWElems <= p.len;   // false only at the region's ragged end
-    const int wmin = __reduce_min_sync(kFull, mn), wmax = __reduce_max_sync(kFull, mx);
-
-    const bool tile_has_break = s_has_break != 0;
-
-    // class(d) is monotone in d: the warp's 512 bases plus the base before them are one class iff
-    // class(min) == class(max) — then no run starts here and all per-base class work is skipped.
-    bool slow_runs = false;
-    if (p.do_runs)
-        slow_runs = !full_warp || tile_has_break || warp_base == 0 ||
-                    cov_class(min(wmin, wbase), p.mincov, p.maxmean) != cov_class(max(wmax, wbase), p.mincov, p.maxmean);
-    const bool fast_win = p.do_windows && full_warp && p.W >= BPT && p.win_min == nullptr && wmax < (1 << 22);
-    const bool slow_win = p.do_windows && !fast_win;
-
-    // Depth by position: this warp's private slice of s_depth holds x[k] (depth relative to the thread's tbase), swizzled
-    // like s_tile (base e of the slice at sw[swz_elem_t<BPT>(e)]) so that both a lane storing its BPT/4 chunks and 32 lanes
-    // reading 32 consecutive bases of one thread are conflict-free; the threads' tbase go to s_tbase.  Storing x instead of
-    // depth saves BPT adds per thread; a reader adds the owner's tbase.  The slice uses the same chunks as the warp's region
-    // of s_tile, so a warp only ever touches its own kWElems elements of either buffer.  With kSliceInTile it overwrites
-    // that region, which is safe because no warp starts the next tile's atomics before the caller's barrier; otherwise a
-    // warp that leaves the core early may already be adding into s_tile, and the slice goes to s_depth.
-    int* const s_slice = kSliceInTile ? s_tile : s_depth;
-    int* sw = s_slice + warp * kWElems;
-    int* stb = s_tbase + warp * 32;
-    const bool need_slice = slow_runs || slow_win;           // warp-uniform; the fast window path works from registers
-    if (need_slice) {
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < BPT / 4; j++)
-            reinterpret_cast<int4*>(s_slice)[c0 ^ j] = make_int4(x[4 * j], x[4 * j + 1], x[4 * j + 2], x[4 * j + 3]);
-        stb[lane] = tbase;
-        __syncwarp();
-    } else if (kSliceInTile) {
-        clear_warp_region<kWElems>(sw, lane);                 // every lane has read its differences (block barrier above)
-    }
 
     // ---- run starts (slow path): one mask bit per base, rank inside the warp in position order
-    unsigned mask = 0;
+    Mask mask = 0;
     int lane_rank = 0, warp_cnt = 0;
     int maxd = full_warp ? wmax : 0;
     if (slow_runs || !full_warp) {
         const int nv = max(0, min(BPT, p.len - idx0));
         int cp = cov_class(tbase, p.mincov, p.maxmean);
 #pragma unroll
-        for (int k = 0; k < BPT; k++) {
-            if (k < nv) {
-                if (!full_warp) maxd = max(maxd, GL_D(k));
-                if (slow_runs) {
-                    const int c = cov_class(GL_D(k), p.mincov, p.maxmean);
-                    if (c != cp) mask |= 1u << k;
-                    cp = c;
+        for (int j = 0; j < BPT / 4; j++) {
+            const int4 q = xq(j);
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const int k = 4 * j + i;
+                if (k < nv) {
+                    if (!full_warp) maxd = max(maxd, GL_D(q, i));
+                    if (slow_runs) {
+                        const int c = cov_class(GL_D(q, i), p.mincov, p.maxmean);
+                        if (c != cp) mask |= (Mask)1 << k;
+                        cp = c;
+                    }
                 }
             }
         }
@@ -558,13 +667,13 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
             if (idx0 == 0) mask |= 1u;                        // the region's first base always starts a run
             if (tile_has_break) {
                 const unsigned a = (unsigned)p.rs + (unsigned)idx0;
-                // rare (one tile in 2441 at 10 Mb): unrolled, its 32 divisions were the register peak of every kernel here
+                // rare (one tile in 2441 at 10 Mb): unrolled, its BPT divisions were the register peak of every kernel here
 #pragma unroll 1
                 for (int k = 0; k < BPT; k++)
-                    if ((a + k) % p.run_break == 0) mask |= 1u << k;
+                    if ((a + k) % p.run_break == 0) mask |= (Mask)1 << k;
             }
-            mask &= (nv >= BPT) ? (BPT == 32 ? 0xffffffffu : 0xffffu) : ((1u << nv) - 1u);
-            const int c = __popc(mask);
+            mask &= (nv >= BPT) ? ~(Mask)0 : (((Mask)1 << nv) - 1u);
+            const int c = mask_popc(mask);
             const int ci = warp_incl_scan(c);
             lane_rank = ci - c;
             warp_cnt = __shfl_sync(kFull, ci, 31);
@@ -573,34 +682,28 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
     }
     acc_max = max(acc_max, maxd);                             // warp-uniform; the kernel publishes it once (flush_max)
 
-    // ---- window partial sums of this warp's 512 bases
+    // ---- window partial sums of this warp's bases
     if (fast_win) {
         // With W >= BPT a thread's BPT bases hold at most one window edge that is not on its first base, and cu of them
         // lie left of it (cu = 0: none).  lx = sum of x[k] for k < cu, from the g8 group sums plus one partial group.
-        const unsigned a = (unsigned)p.rs + (unsigned)idx0;              // absolute, < 2^32
-        const unsigned uW = (unsigned)p.W;
-        // iw = a / W without a division: q = hi32(a * floor(2^32/W)) is the quotient or one less, because
-        // a * floor(2^32/W) > a * 2^32 / W - a and a < 2^32
-        unsigned iw = __umulhi(a, p.W_inv);
-        unsigned rem = a - iw * uW;
-        if (rem >= uW) { iw++; rem -= uW; }
-        const int cu = uW - rem < (unsigned)BPT ? (int)(uW - rem) : 0;
-        const int gi = cu >> 3, r = cu & 7;
-        int lx = 0;
+        if constexpr (!kSliceInTile) {
+            window_edge(p, idx0, BPT, iw, rem, cu);
+            const int gi = cu >> 3, r = cu & 7;
 #pragma unroll
-        for (int g = 0; g + 1 < BPT / 8; g++) lx += g < gi ? g8[g] : 0;
+            for (int g = 0; g + 1 < BPT / 8; g++) lx += g < gi ? g8[g] : 0;
 #pragma unroll
-        for (int j = 0; j < 7; j++) {
-            int v = x[j];
+            for (int j = 0; j < 7; j++) {
+                int v = x[j];
 #pragma unroll
-            for (int g = 1; g < BPT / 8; g++) v = gi == g ? x[8 * g + j] : v;
-            lx += j < r ? v : 0;
+                for (int g = 1; g < BPT / 8; g++) v = gi == g ? x[8 * g + j] : v;
+                lx += j < r ? v : 0;
+            }
         }
         // An edge lane holds one window edge: inside its bases (cu > 0, it ends window iw) or on its first base (it ends
         // window iw - 1; on lane 0 that is the warp's start, not an edge).  c = the warp's depth sum left of the edge, so a
         // window's part in this warp is c minus the c of the edge lane before it (0 for the first), and the window that
         // runs past the warp's end (or ends exactly at it) gets the warp's total minus the last c.  Every partial sum is
-        // < 2^32 because depth < 2^22 on this path, so unsigned 32-bit arithmetic is exact.
+        // < 2^32 because depth < kFastDepth on this path, so unsigned 32-bit arithmetic is exact.
         const unsigned s16 = (unsigned)(BPT * tbase + xsum);
         const unsigned si = (unsigned)warp_incl_scan((int)s16);          // the lanes' depth sums, inclusive (mod 2^32)
         const unsigned total = __shfl_sync(kFull, si, 31);
@@ -672,9 +775,9 @@ __device__ __forceinline__ void tile_core(const ScanParams& p, int* __restrict__
         if (warp_cnt) {                                       // warp-uniform
             off = __shfl_sync(kFull, off, 0);
             long long rank = (long long)off + lane_rank;
-            unsigned m = mask;
+            Mask m = mask;
             while (m) {
-                const int k = __ffs(m) - 1;
+                const int k = mask_ffs(m) - 1;
                 m &= m - 1;
                 if (rank < p.run_cap) {
                     p.tmp_start[rank] = p.rs + idx0 + k;
@@ -1134,18 +1237,19 @@ __global__ void __launch_bounds__(256) depth_tileidx8_kernel(const ScanParams p)
     }
 }
 
-struct P8Regs { unsigned d, l; int anchor; };
+struct P8Regs { uint2 d, l; int anchor; };
 
-// K_fused8 runs 128-thread CTAs whose threads own 32 consecutive bases each (tile_core<32, 4>): the work that is paid per
-// thread and tile — warp scans, class check, window sums, run claim, barrier — is spread over twice the bases of the
-// 16-per-thread core (ncu, round 1: 568 warp instructions per thread and tile = 35.5 per base, issue-bound).
-constexpr int kF8Threads = 128;
+// K_fused8 runs 64-thread CTAs whose threads own 64 consecutive bases each (tile_core<64, 2>): the work that is paid per
+// thread and tile — warp scans, class check, window sums, run claim, barrier — is spread over four times the bases of the
+// 16-per-thread core (ncu, round 1: 568 warp instructions per thread and tile = 35.5 per base, issue-bound), and each
+// barrier waits for two warps.
+constexpr int kF8Threads = 64;
 constexpr int kF8Warps = kF8Threads / 32;
-constexpr int kF8BPT = kTile / kF8Threads;          // 32
-constexpr int kF8BlocksPerPass = kF8Threads / 16;   // a block is 16 lanes x 4 slots
+constexpr int kF8BPT = kTile / kF8Threads;          // 64
+constexpr int kF8BlocksPerPass = kF8Threads / 8;    // a block is 8 lanes x 8 slots
 
 // K_fused8's tile buffer has a guard band of kF8Guard entries on either side of the tile: s_tile[-32, 0) is the lead
-// guard, s_tile[4096, 4128) the trailing one.  swz_elem_t<32> maps each guard onto itself (it XORs bits 2-4 with bits 5-7,
+// guard, s_tile[4096, 4128) the trailing one.  swz_elem_t<64> maps each guard onto itself (it XORs bits 2-4 with bits 6-8,
 // which are 7 for [-32, 0) and 0 for [4096, 4128)), so one address expression covers the whole buffer.
 constexpr int kF8Guard = 32;
 
@@ -1170,38 +1274,51 @@ __device__ __forceinline__ void fused_apply32(int* s_tile, int a, int len, int l
     atomicAdd(s_tile + swz_elem_t<kF8BPT>(min(max(a + len, lo), hi)), -1);
 }
 
-// thread (tid) takes slots 4*(tid&15)..+3 of block lo + (tid>>4) + 8*pass
+// thread (tid) takes slots 8*(tid&7)..+7 of block lo + (tid>>3) + 8*pass: one uint2 of start deltas, one of lengths
 __device__ __forceinline__ P8Regs fused8_load(const ScanParams& p, int lo, int hi, int pass) {
-    P8Regs r = {0u, 0u, 0};
-    const int b = lo + (int)(threadIdx.x >> 4) + kF8BlocksPerPass * pass;
+    P8Regs r = {make_uint2(0u, 0u), make_uint2(0u, 0u), 0};
+    const int b = lo + (int)(threadIdx.x >> 3) + kF8BlocksPerPass * pass;
     if (b < hi) {
-        r.d = p.p8_ds[(size_t)b * 16 + (threadIdx.x & 15)];
-        r.l = p.p8_len[(size_t)b * 16 + (threadIdx.x & 15)];
+        r.d = reinterpret_cast<const uint2*>(p.p8_ds)[(size_t)b * 8 + (threadIdx.x & 7)];
+        r.l = reinterpret_cast<const uint2*>(p.p8_len)[(size_t)b * 8 + (threadIdx.x & 7)];
         r.anchor = p.p8_anchors[b];
     }
     return r;
 }
 
-// Inclusive scan over each 16-lane half of the warp (one block's words), as warp_incl_scan: shfl.up within 16-lane
-// segments (c = 0x1000) says whether the source lane is in this lane's segment, so a step is a SHFL and a predicated add.
-__device__ __forceinline__ int half_warp_incl_scan(int v) {
+// Inclusive scan over each 8-lane quarter of the warp (one block's words), as warp_incl_scan: shfl.up within 8-lane
+// segments (c = 0x1800) says whether the source lane is in this lane's segment, so a step is a SHFL and a predicated add.
+__device__ __forceinline__ int quarter_warp_incl_scan(int v) {
 #pragma unroll
-    for (int o = 1; o < 16; o <<= 1)
-        asm("{\n\t.reg .s32 t;\n\t.reg .pred p;\n\tshfl.sync.up.b32 t|p, %0, %1, 0x1000, -1;\n\t@p add.s32 %0, %0, t;\n\t}" : "+r"(v) : "r"(o));
+    for (int o = 1; o < 8; o <<= 1)
+        asm("{\n\t.reg .s32 t;\n\t.reg .pred p;\n\tshfl.sync.up.b32 t|p, %0, %1, 0x1800, -1;\n\t@p add.s32 %0, %0, t;\n\t}" : "+r"(v) : "r"(o));
     return v;
 }
 
 __device__ __forceinline__ void fused8_apply(const P8Regs& r, int* s_tile, int t0) {
-    if (__ballot_sync(kFull, r.l != 0) == 0) return;        // no live slot in the whole warp (warp-uniform: no divergence)
+    if (__ballot_sync(kFull, (r.l.x | r.l.y) != 0) == 0) return;   // no live slot in the whole warp (warp-uniform: no divergence)
     const int lane = threadIdx.x & 31;
-    // byte k of a word, zero-extended: one PRMT (__byte_perm selector 0x444k) where a shift and a mask take two
-    const int d0 = r.d & 0xff, d1 = d0 + __byte_perm(r.d, 0, 0x4441), d2 = d1 + __byte_perm(r.d, 0, 0x4442), d3 = d2 + (r.d >> 24);
-    const int inc = half_warp_incl_scan(d3);
-    const int base = r.anchor + inc - d3 - t0;              // tile-relative start of the slot before this thread's first
-    fused_apply32(s_tile, base + d0, (int)(r.l & 0xff), lane);
-    fused_apply32(s_tile, base + d1, (int)__byte_perm(r.l, 0, 0x4441), lane);
-    fused_apply32(s_tile, base + d2, (int)__byte_perm(r.l, 0, 0x4442), lane);
-    fused_apply32(s_tile, base + d3, (int)(r.l >> 24), lane);
+    // running sum of the thread's 8 start deltas; byte k of a word, zero-extended: one PRMT (__byte_perm selector 0x444k)
+    // where a shift and a mask take two
+    int d[8];
+    d[0] = r.d.x & 0xff;
+    d[1] = d[0] + __byte_perm(r.d.x, 0, 0x4441);
+    d[2] = d[1] + __byte_perm(r.d.x, 0, 0x4442);
+    d[3] = d[2] + (r.d.x >> 24);
+    d[4] = d[3] + (r.d.y & 0xff);
+    d[5] = d[4] + __byte_perm(r.d.y, 0, 0x4441);
+    d[6] = d[5] + __byte_perm(r.d.y, 0, 0x4442);
+    d[7] = d[6] + (r.d.y >> 24);
+    const int inc = quarter_warp_incl_scan(d[7]);
+    const int base = r.anchor + inc - d[7] - t0;            // tile-relative start of the slot before this thread's first
+    fused_apply32(s_tile, base + d[0], (int)(r.l.x & 0xff), lane);
+    fused_apply32(s_tile, base + d[1], (int)__byte_perm(r.l.x, 0, 0x4441), lane);
+    fused_apply32(s_tile, base + d[2], (int)__byte_perm(r.l.x, 0, 0x4442), lane);
+    fused_apply32(s_tile, base + d[3], (int)(r.l.x >> 24), lane);
+    fused_apply32(s_tile, base + d[4], (int)(r.l.y & 0xff), lane);
+    fused_apply32(s_tile, base + d[5], (int)__byte_perm(r.l.y, 0, 0x4441), lane);
+    fused_apply32(s_tile, base + d[6], (int)__byte_perm(r.l.y, 0, 0x4442), lane);
+    fused_apply32(s_tile, base + d[7], (int)(r.l.y >> 24), lane);
 }
 
 // K_fused8: persistent, software-pipelined like K_fused: while tile n runs its core, the packed words of tile n+1 (two
@@ -1254,9 +1371,9 @@ __global__ void __launch_bounds__(kF8Threads) depth_fused8_kernel(const ScanPara
     flush_max(p, acc_max);
 }
 
-// K_gather: one warp per 512-base chunk moves its runs from claim order to position order.  The ordered offset
-// of a chunk is the number of runs that start before it: counts per 64 chunks + the chunk counts of its own group
-// (only chunks that have runs pay for the sum).  Warps stride over the chunks, so any grid covers them.
+// K_gather: one warp per warp chunk of the core (512 bases; 2048 in K_fused8) moves its runs from claim order to position
+// order.  The ordered offset of a chunk is the number of runs that start before it: counts per 64 chunks + the chunk
+// counts of its own group (only chunks that have runs pay for the sum).  Warps stride over the chunks, so any grid covers them.
 // header[3] == reject: the fast path was rejected (fused int32: 1; packed8: the reduce's tag).  hdr_out (packed8: the
 // ctx's mapped host header) receives the header's first four words, rejected or not.
 __global__ void __launch_bounds__(256) depth_gather_runs_kernel(const uint64_t* __restrict__ header, uint64_t reject,

@@ -1013,9 +1013,31 @@ static void ic_plot_select(gl_ctx* c, const float* d_dep, size_t a, size_t b, co
     }
 }
 
-// round 2 on one GPU: the index images of its samples' lines, with the cohort's extents (img: every chart)
+// The path text of a vector chart (INDEXCOV_FMT; plot.cu): dataset j's bytes are text[pos[j] .. pos[j + 1]).
+struct IcPathText {
+    std::vector<int64_t> pos;
+    std::vector<char> text;
+};
+
+// gl_plot_path_*_size, the lengths home, then gl_plot_path_*_emit into a buffer of exactly that size and the text home
+template <class Size, class Emit>
+static void ic_path_text(gl_ctx* c, DevBufs& tmp, size_t n, const Size& size, const Emit& emit, IcPathText& pt) {
+    int64_t* d_len = tmp.alloc<int64_t>(n);
+    int64_t* d_pos = tmp.alloc<int64_t>(n + 1);
+    glck(c, size(d_len, d_pos), "gl_plot_path_*_size");
+    pt.pos.resize(n + 1);
+    glck(c, gl_memcpy_d2h(c, pt.pos.data(), d_pos, (int64_t)(n + 1) * 8), "gl_memcpy_d2h");
+    const int64_t total = pt.pos[n];
+    pt.text.resize((size_t)total);
+    char* d_txt = tmp.alloc<char>((size_t)total);
+    glck(c, emit(d_pos, total, d_txt), "gl_plot_path_*_emit");
+    glck(c, gl_memcpy_d2h(c, pt.text.data(), d_txt, total), "gl_memcpy_d2h");
+}
+
+// round 2 on one GPU: the index images of its samples' lines, with the cohort's extents (img: every chart), and with
+// vfmt >= 0 their depth charts' path text in (chart, sample) order
 static void ic_plot_raster(gl_ctx* c, const float* d_dep, size_t a, size_t b, const std::vector<int64_t>& sample_ptr, const IcSlices& sl,
-                           const IcPlots& pl, double r, uint32_t* img) {
+                           const IcPlots& pl, double r, uint32_t* img, int vfmt, IcPathText& pt) {
     const size_t S = sample_ptr.size() - 1, nk = b - a, nc = pl.q_of.size(), n = nc * nk;
     std::vector<int64_t> off, len, sel(n * 3);
     std::vector<int32_t> chart(n);
@@ -1027,11 +1049,77 @@ static void ic_plot_raster(gl_ctx* c, const float* d_dep, size_t a, size_t b, co
         chart[j] = (int32_t)ch; draw[j] = (uint32_t)(k + 1);
     }
     DevBufs tmp(c);
+    const int64_t* d_off = tmp.upload(off.data(), n);
+    const int64_t* d_sel = tmp.upload(sel.data(), n * 3);
+    const int32_t* d_chart = tmp.upload(chart.data(), n);
+    const double* d_xf = tmp.upload(pl.xf.data(), nc * 4);
     uint32_t* d_img = tmp.alloc<uint32_t>(nc * GL_PLOT_W * GL_PLOT_H);
-    glck(c, gl_plot_raster_series_device(c, d_dep, tmp.upload(off.data(), n), tmp.upload(sel.data(), n * 3), (double)GL_TILE_WIDTH,
-                                         tmp.upload(chart.data(), n), tmp.upload(draw.data(), n), (int32_t)n, tmp.upload(pl.xf.data(), nc * 4),
+    glck(c, gl_plot_raster_series_device(c, d_dep, d_off, d_sel, (double)GL_TILE_WIDTH, d_chart, tmp.upload(draw.data(), n), (int32_t)n, d_xf,
                                          (int32_t)nc, GL_PLOT_W, GL_PLOT_H, r, d_img), "gl_plot_raster_series_device");
     glck(c, gl_memcpy_d2h(c, img, d_img, (int64_t)(nc * GL_PLOT_W * GL_PLOT_H * 4)), "gl_memcpy_d2h");
+    if (vfmt < 0) return;
+    ic_path_text(c, tmp, n,
+                 [&](int64_t* d_len, int64_t* d_pos) {
+                     return gl_plot_path_series_size(c, d_dep, d_off, d_sel, (double)GL_TILE_WIDTH, d_chart, (int32_t)n, d_xf, (int32_t)nc,
+                                                     GL_PLOT_DEPTH, vfmt, d_len, d_pos);
+                 },
+                 [&](const int64_t* d_pos, int64_t total, char* d_txt) {
+                     return gl_plot_path_series_emit(c, d_dep, d_off, d_sel, (double)GL_TILE_WIDTH, d_chart, (int32_t)n, d_xf, (int32_t)nc,
+                                                     GL_PLOT_DEPTH, vfmt, d_pos, total, d_txt, total);
+                 },
+                 pt);
+}
+
+// the path text of explicit vertices (the ROC and sex charts), on GPU 0 as their rasters are
+static void ic_path_text_xy(gl_ctx* c, const std::vector<double>& x, const std::vector<double>& y, const std::vector<int64_t>& ptr,
+                            const std::vector<int32_t>& chart, const double* xf, size_t n_charts, int kind, int vfmt, IcPathText& pt) {
+    const size_t n = chart.size();
+    DevBufs tmp(c);
+    const double* d_x = tmp.upload(x.data(), x.size());
+    const double* d_y = tmp.upload(y.data(), y.size());
+    const int64_t* d_ptr = tmp.upload(ptr.data(), ptr.size());
+    const int32_t* d_chart = tmp.upload(chart.data(), n);
+    const double* d_xf = tmp.upload(xf, n_charts * 4);
+    ic_path_text(c, tmp, n,
+                 [&](int64_t* d_len, int64_t* d_pos) {
+                     return gl_plot_path_xy_size(c, d_x, d_y, d_ptr, d_chart, (int32_t)n, d_xf, (int32_t)n_charts, kind, vfmt, d_len, d_pos);
+                 },
+                 [&](const int64_t* d_pos, int64_t total, char* d_txt) {
+                     return gl_plot_path_xy_emit(c, d_x, d_y, d_ptr, d_chart, (int32_t)n, d_xf, (int32_t)n_charts, kind, vfmt, d_pos, total,
+                                                 d_txt, total);
+                 },
+                 pt);
+}
+
+// One vector chart file: its datasets' path text (data[d], len[d]) in draw order, each stroked in rgb[3 d ..].
+struct IcVecFile {
+    std::string path, xtitle, ytitle;
+    int kind = GL_PLOT_DEPTH;
+    double ext[4] = {0, 0, 0, 0};
+    double width = 0.8;
+    std::vector<uint8_t> rgb;
+    std::vector<const char*> data;
+    std::vector<int64_t> len;
+};
+
+// The vector charts (INDEXCOV_FMT): the files and the path text they point into.  vfmt < 0: none.
+struct IcVectors {
+    int vfmt = -1;
+    std::string ext;                                       // "svg" or "eps"
+    std::vector<IcPathText> depth;                         // per GPU: its samples' depth paths, in (chart, sample) order
+    IcPathText roc, sex;
+    std::vector<IcVecFile> files;
+    std::string file_of(const std::string& png) const { return png.substr(0, png.size() - 3) + ext; }   // plot.go:533-534
+};
+
+// every vector chart file, one pool task each
+static void ic_vectors_write(const IcVectors& vec) {
+    glhost::ThreadPool::global().run((int64_t)vec.files.size(), [&](int64_t t, int) {
+        const IcVecFile& f = vec.files[(size_t)t];
+        if (gl_plot_vector_write(f.path.c_str(), f.kind, vec.vfmt, f.ext, f.xtitle.c_str(), f.ytitle.c_str(), (int32_t)f.data.size(), f.rgb.data(),
+                                 f.width, f.data.data(), f.len.data()) != GL_OK)
+            fatal(1, "%s", gl_last_error(nullptr));
+    });
 }
 
 static void ic_write_png(const std::string& path, const uint32_t* img, const std::vector<uint8_t>& palette, int kind, const double* ext,
@@ -1086,9 +1174,11 @@ static void ic_write_text(const std::string& path, const std::string& text) {
     if (!f || fwrite(text.data(), 1, text.size(), f) != text.size() || fclose(f) != 0) fatal(1, "cannot write %s", path.c_str());
 }
 
+// With INDEXCOV_FMT, vec gets the list of vector chart files: the depth paths were made in phase B (vec.depth, one entry per
+// GPU, whose samples are [cut[g], cut[g + 1])); the ROC and sex paths are made here on GPU 0.
 static void ic_plots_write(gl_ctx* ctx, const std::string& base, const std::string& dir, const std::vector<const IcRef*>& kept,
                            const IcPlots& pl, const std::vector<std::vector<float>>& roc_vals, const std::vector<uint32_t>& depth_img,
-                           double r, size_t S, const IcReport& rep) {
+                           double r, size_t S, const IcReport& rep, const std::vector<size_t>& cut, IcVectors& vec) {
     const size_t kMaxSamples = 100;                                         // indexcov.go:528 maxSamples
     if (S > kMaxSamples)
         fprintf(stderr, "indexcov: creating only static (no interactive) plots for depth because # of samples %zu is > %zu\n", S, kMaxSamples);
@@ -1134,6 +1224,34 @@ static void ic_plots_write(gl_ctx* ctx, const std::string& base, const std::stri
     std::vector<uint32_t> roc_img(nc * img_n);
     if (nc) glck(ctx, gl_plot_raster_xy(ctx, x.data(), y.data(), ptr.data(), chart.data(), draw.data(), (int32_t)chart.size(), rp.xf.data(),
                                         (int32_t)nc, GL_PLOT_W, GL_PLOT_H, r, roc_img.data()), "gl_plot_raster_xy");
+    if (vec.vfmt >= 0) {
+        if (nc) ic_path_text_xy(ctx, x, y, ptr, chart, rp.xf.data(), nc, GL_PLOT_PLAIN, vec.vfmt, vec.roc);
+        const double w = gl_plot_line_width((int32_t)S);
+        for (size_t c = 0; c < nc; c++) {                                   // asPng's vector copies (plot.go:527-536)
+            const std::string& chrom = kept[pl.q_of[c]]->name;
+            IcVecFile d, o;
+            d.path = vec.file_of(base + "-depth-" + chrom + ".png"); d.kind = GL_PLOT_DEPTH; std::copy(&pl.ext[c * 4], &pl.ext[c * 4 + 4], d.ext);
+            d.xtitle = "position on " + chrom; d.ytitle = "scaled coverage"; d.width = w;
+            for (size_t g = 0; g + 1 < cut.size(); g++) {
+                const size_t nk = cut[g + 1] - cut[g];
+                for (size_t k = cut[g]; k < cut[g + 1]; k++) {
+                    const size_t j = c * nk + (k - cut[g]);
+                    const IcPathText& pt = vec.depth[g];
+                    d.data.push_back(pt.text.data() + pt.pos[j]); d.len.push_back(pt.pos[j + 1] - pt.pos[j]);
+                    d.rgb.insert(d.rgb.end(), &palette[3 * (k + 1)], &palette[3 * (k + 1)] + 3);
+                }
+            }
+            o.path = vec.file_of(base + "-roc-" + chrom + ".png"); o.kind = GL_PLOT_PLAIN; std::copy(&rp.ext[c * 4], &rp.ext[c * 4 + 4], o.ext);
+            o.xtitle = "scaled coverage for " + chrom; o.ytitle = "proportion of regions covered"; o.width = w;
+            for (size_t i = 0; i < chart.size(); i++) {
+                if ((size_t)chart[i] != c) continue;
+                o.data.push_back(vec.roc.text.data() + vec.roc.pos[i]); o.len.push_back(vec.roc.pos[i + 1] - vec.roc.pos[i]);
+                o.rgb.insert(o.rgb.end(), &palette[3 * draw[i]], &palette[3 * draw[i]] + 3);
+            }
+            vec.files.push_back(std::move(d));
+            vec.files.push_back(std::move(o));
+        }
+    }
     const std::string stem = base.substr(base.find_last_of('/') + 1);
     const std::string back = "<p><a href=\"index.html\">back to index</a></p>\n";
     glhost::ThreadPool::global().run((int64_t)(4 * nc), [&](int64_t t, int) {
@@ -1233,6 +1351,17 @@ static void ic_plots_write(gl_ctx* ctx, const std::string& base, const std::stri
         std::vector<uint8_t> png((size_t)n);
         if (gl_plot_png(rgb.data(), GL_PLOT_SQ_CW, GL_PLOT_SQ_CH, png.data(), n, &n) != GL_OK) fatal(1, "gl_plot_png failed");
         ic_write_text(base + "-sex.png", std::string(png.begin(), png.begin() + n));
+        if (vec.vfmt >= 0) {
+            ic_path_text_xy(ctx, sx, sy, sptr, schart, xf, 1, GL_PLOT_SQUARE, vec.vfmt, vec.sex);
+            IcVecFile f;
+            f.path = vec.file_of(base + "-sex.png"); f.kind = GL_PLOT_SQUARE; std::copy(e, e + 4, f.ext);
+            f.xtitle = k0 + " Copy Number"; f.ytitle = k1 + " Copy Number"; f.width = gl_plot_line_width((int32_t)schart.size());
+            for (size_t i = 0; i < schart.size(); i++) {
+                f.data.push_back(vec.sex.text.data() + vec.sex.pos[i]); f.len.push_back(vec.sex.pos[i + 1] - vec.sex.pos[i]);
+            }
+            f.rgb.assign(spal.begin() + 3, spal.end());
+            vec.files.push_back(std::move(f));
+        }
         body += "<p><img src=\"" + stem + "-sex.png\" alt=\"sex\"></p>\n";
     }
     std::vector<std::string> fg_names;
@@ -1341,6 +1470,10 @@ static int cmd_indexcov(int argc, char** argv) {
     bool noplots = false;
     ap.addb("noplots", 0, &noplots);                // extension: no charts; index.html only lists the outputs
     ap.parse(argc, argv);
+    // INDEXCOV_FMT (plot.go:527-536): every chart PNG gets a vector copy, X.svg for "svg" and X.eps for any other non-empty value
+    IcVectors vec;
+    if (const char* v = getenv("INDEXCOV_FMT"))
+        if (*v && !noplots) { vec.ext = strcmp(v, "svg") == 0 ? "svg" : "eps"; vec.vfmt = vec.ext == "svg" ? GL_PLOT_SVG : GL_PLOT_EPS; }
     std::vector<std::string> bams = ap.positional;
     if (bams.empty()) ap.fail("bam is required");
     std::vector<std::string> sexes_wanted;
@@ -1578,11 +1711,13 @@ static int cmd_indexcov(int argc, char** argv) {
     if (n_charts) {
         for (size_t c = 0; c < n_charts; c++) ic_plot_extent(pl, c, S, (double)GL_TILE_WIDTH);
         std::vector<std::vector<uint32_t>> part((size_t)G);
+        vec.depth.resize((size_t)G);
         run_on_gpus([&](int g) {
             const size_t a = cut[(size_t)g], b = cut[(size_t)g + 1];
             if (b == a) return;
             part[(size_t)g].resize(n_charts * img_n);
-            ic_plot_raster(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, pl, plot_r, part[(size_t)g].data());
+            ic_plot_raster(ctxs[(size_t)g], shard[(size_t)g].d_dep, a, b, sample_ptr, sl, pl, plot_r, part[(size_t)g].data(), vec.vfmt,
+                           vec.depth[(size_t)g]);
         });
         depth_img.assign(n_charts * img_n, 0);
         for (auto& p : part)
@@ -1710,8 +1845,12 @@ static int cmd_indexcov(int argc, char** argv) {
     ic_write_ped(base, names, sexes, bins, slopes, pcs, n_pc, mapped, unmapped);
     if (!noplots) {
         ic_plots_write(ctx, base, dir, kept, pl, roc_vals, depth_img, plot_r, S,
-                       IcReport{names, dep.data(), sl, sexes, mapped, unmapped, bins, pcs, n_pc, vars});
+                       IcReport{names, dep.data(), sl, sexes, mapped, unmapped, bins, pcs, n_pc, vars}, cut, vec);
         ic_mark("charts");
+        if (vec.vfmt >= 0) {
+            ic_vectors_write(vec);
+            ic_mark("vector");
+        }
     } else {                                                                // --noplots: a plain list of the outputs
         const std::string index_path = dir + "/index.html";
         FILE* ih = fopen(index_path.c_str(), "w");

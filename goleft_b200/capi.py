@@ -126,6 +126,19 @@ _proto("gl_plot_millions", C.c_int, C.c_double, C.c_char_p, C.c_int32)
 _proto("gl_plot_text", C.c_int, _vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_char_p, C.c_int32)
 _proto("gl_plot_compose", C.c_int, _vp, _vp, C.c_int32, C.c_int32, _vp, C.c_char_p, C.c_char_p, _vp)
 _proto("gl_plot_png", C.c_int, _vp, C.c_int32, C.c_int32, _vp, C.c_int64, _i64p)
+_proto("gl_plot_path_series_size", C.c_int, _vp, _vp, _vp, _vp, C.c_double, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp)
+_proto("gl_plot_path_series_emit", C.c_int, _vp, _vp, _vp, _vp, C.c_double, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp,
+       C.c_int64, _vp, C.c_int64)
+_proto("gl_plot_path_series_size_host", C.c_int, _vp, _vp, _vp, C.c_double, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp)
+_proto("gl_plot_path_series_emit_host", C.c_int, _vp, _vp, _vp, C.c_double, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp,
+       C.c_int64)
+_proto("gl_plot_path_xy_size", C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp)
+_proto("gl_plot_path_xy_emit", C.c_int, _vp, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, _vp, C.c_int64)
+_proto("gl_plot_path_xy_size_host", C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp)
+_proto("gl_plot_path_xy_emit_host", C.c_int, _vp, _vp, _vp, _vp, C.c_int32, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, C.c_int64)
+_proto("gl_plot_line_width", C.c_double, C.c_int32)
+_proto("gl_plot_vector_write", C.c_int, C.c_char_p, C.c_int32, C.c_int32, _vp, C.c_char_p, C.c_char_p, C.c_int32, _vp, C.c_double,
+       C.POINTER(C.c_char_p), _vp)
 _proto("gl_format_g3", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_g3_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_bincount_i32", C.c_int, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp)
@@ -476,7 +489,8 @@ def pca_tridiag_above(d, e, rel: float = 1e-12) -> np.ndarray:
 
 # ---- indexcov charts (plot.cu)
 PLOT_CW, PLOT_CH, PLOT_AX, PLOT_AY, PLOT_W, PLOT_H = 384, 288, 56, 8, 316, 244
-PLOT_DEPTH, PLOT_PLAIN = 0, 1
+PLOT_DEPTH, PLOT_PLAIN, PLOT_SQUARE = 0, 1, 2
+PLOT_SVG, PLOT_EPS = 0, 1
 
 
 def _ck0(rc: int):
@@ -533,6 +547,48 @@ def plot_raster_xy_host(x, y, ptr, chart, draw, xf, n_charts: int, W: int, H: in
     _ck0(lib.gl_plot_raster_xy_host(_ptr(x), _ptr(y), _ptr(ptr), _ptr(chart), _ptr(draw), chart.size, _ptr(xf), n_charts, W, H, r,
                                     _ptr(img)))
     return img
+
+
+def plot_path_series_host(vals, off, sel, mult: float, chart, xf, n_charts: int, kind: int, fmt: int, cap: Optional[int] = None):
+    """(len [n] int64, text bytes) of every dataset's path text (gl_plot_path_series_size_host + _emit_host); cap: the room
+    given to the emit (default: exactly the total)"""
+    vals, off, sel = _as(vals, np.float32), _as(off, np.int64), _as(sel, np.int64)
+    chart, xf = _as(chart, np.int32), _as(xf, np.float64)
+    n = chart.size
+    ln, pos = np.empty(max(n, 1), np.int64), np.empty(n + 1, np.int64)
+    _ck0(lib.gl_plot_path_series_size_host(_ptr(vals), _ptr(off), _ptr(sel), mult, _ptr(chart), n, _ptr(xf), n_charts, kind, fmt, _ptr(ln),
+                                           _ptr(pos)))
+    out = np.empty(max(int(pos[n]) if cap is None else cap, 1), np.uint8)
+    _ck0(lib.gl_plot_path_series_emit_host(_ptr(vals), _ptr(off), _ptr(sel), mult, _ptr(chart), n, _ptr(xf), n_charts, kind, fmt, _ptr(pos),
+                                           _ptr(out), int(pos[n]) if cap is None else cap))
+    return ln[:n].copy(), out[:int(pos[n])].tobytes()
+
+
+def plot_path_xy_host(x, y, ptr, chart, xf, n_charts: int, kind: int, fmt: int, cap: Optional[int] = None):
+    """(len [n] int64, text bytes) of every dataset's path text from explicit vertices (gl_plot_path_xy_size_host + _emit_host)"""
+    x, y, ptr = _as(x, np.float64), _as(y, np.float64), _as(ptr, np.int64)
+    chart, xf = _as(chart, np.int32), _as(xf, np.float64)
+    n = chart.size
+    ln, pos = np.empty(max(n, 1), np.int64), np.empty(n + 1, np.int64)
+    _ck0(lib.gl_plot_path_xy_size_host(_ptr(x), _ptr(y), _ptr(ptr), _ptr(chart), n, _ptr(xf), n_charts, kind, fmt, _ptr(ln), _ptr(pos)))
+    out = np.empty(max(int(pos[n]) if cap is None else cap, 1), np.uint8)
+    _ck0(lib.gl_plot_path_xy_emit_host(_ptr(x), _ptr(y), _ptr(ptr), _ptr(chart), n, _ptr(xf), n_charts, kind, fmt, _ptr(pos), _ptr(out),
+                                       int(pos[n]) if cap is None else cap))
+    return ln[:n].copy(), out[:int(pos[n])].tobytes()
+
+
+def plot_line_width(n_datasets: int) -> float:
+    return lib.gl_plot_line_width(n_datasets)
+
+
+def plot_vector_write(path: str, kind: int, fmt: int, ext4, xtitle: str, ytitle: str, rgb, width: float, texts):
+    """gl_plot_vector_write: texts[d] is dataset d's path text (bytes), rgb (n, 3) uint8 its colour"""
+    e, rgb = _as(ext4, np.float64), _as(rgb, np.uint8)
+    n = len(texts)
+    data = (C.c_char_p * max(n, 1))(*texts)
+    lens = np.array([len(t) for t in texts] or [0], np.int64)
+    _ck0(lib.gl_plot_vector_write(path.encode(), kind, fmt, _ptr(e), xtitle.encode(), ytitle.encode(), n, _ptr(rgb), width, data,
+                                  _ptr(lens)))
 
 
 def dcnv_chart_select_host(x):
@@ -1424,6 +1480,52 @@ class Ctx:
         finally:
             for b in bufs:
                 b.free()
+
+    def _paths(self, size, emit, arrs, n: int, cap: Optional[int]):
+        bufs = [DevBuf(self, max(16, a.nbytes)).upload(a) for a in arrs]
+        d_len, d_pos = DevBuf(self, max(16, n * 8)), DevBuf(self, (n + 1) * 8)
+        d_out = None
+        try:
+            size(bufs, d_len, d_pos)
+            self.sync()
+            ln, pos = d_len.download(np.int64, n), d_pos.download(np.int64, n + 1)
+            total = int(pos[n])
+            room = total if cap is None else cap
+            d_out = DevBuf(self, max(16, room))
+            emit(bufs, d_pos, total, d_out, room)
+            self.sync()
+            return ln, d_out.download(np.uint8, total).tobytes()
+        finally:
+            for b in bufs + [d_len, d_pos] + ([d_out] if d_out is not None else []):
+                b.free()
+
+    def plot_path_series(self, vals, off, sel, mult: float, chart, xf, n_charts: int, kind: int, fmt: int, cap: Optional[int] = None):
+        """the device path text of selected value series on host arrays: (len [n] int64, text bytes)"""
+        arrs = [_as(vals, np.float32), _as(off, np.int64), _as(sel, np.int64), _as(chart, np.int32), _as(xf, np.float64)]
+        n = arrs[3].size
+
+        def size(b, d_len, d_pos):
+            self._ck(lib.gl_plot_path_series_size(self.h, b[0].ptr, b[1].ptr, b[2].ptr, mult, b[3].ptr, n, b[4].ptr, n_charts, kind, fmt,
+                                                  d_len.ptr, d_pos.ptr))
+
+        def emit(b, d_pos, total, d_out, room):
+            self._ck(lib.gl_plot_path_series_emit(self.h, b[0].ptr, b[1].ptr, b[2].ptr, mult, b[3].ptr, n, b[4].ptr, n_charts, kind, fmt,
+                                                  d_pos.ptr, total, d_out.ptr, room))
+        return self._paths(size, emit, arrs, n, cap)
+
+    def plot_path_xy(self, x, y, ptr, chart, xf, n_charts: int, kind: int, fmt: int, cap: Optional[int] = None):
+        """the device path text of explicit vertices on host arrays: (len [n] int64, text bytes)"""
+        arrs = [_as(x, np.float64), _as(y, np.float64), _as(ptr, np.int64), _as(chart, np.int32), _as(xf, np.float64)]
+        n = arrs[3].size
+
+        def size(b, d_len, d_pos):
+            self._ck(lib.gl_plot_path_xy_size(self.h, b[0].ptr, b[1].ptr, b[2].ptr, b[3].ptr, n, b[4].ptr, n_charts, kind, fmt, d_len.ptr,
+                                              d_pos.ptr))
+
+        def emit(b, d_pos, total, d_out, room):
+            self._ck(lib.gl_plot_path_xy_emit(self.h, b[0].ptr, b[1].ptr, b[2].ptr, b[3].ptr, n, b[4].ptr, n_charts, kind, fmt, d_pos.ptr,
+                                              total, d_out.ptr, room))
+        return self._paths(size, emit, arrs, n, cap)
 
     def plot_raster_xy(self, x, y, ptr, chart, draw, xf, n_charts: int, W: int, H: int, r: float) -> np.ndarray:
         x, y, ptr = _as(x, np.float64), _as(y, np.float64), _as(ptr, np.int64)

@@ -16,13 +16,22 @@
 // round-to-nearest step in the order written in plot_rule.cuh: explicit _rn intrinsics on the device, plain operations on
 // the host (the library is built with --fmad=false and no host FMA), so the host mirror and numpy restate the device bit
 // for bit.
+//
+// The vector charts (INDEXCOV_FMT, indexcov/plot.go:527-536) are the same charts in points (72 per inch, 0.75 per pixel):
+// vertex (x, y) of a dataset is at Xpt = 0.75 (AX + (x - xmin) sx), Ypt = 0.75 (AY + (H - (y - ymin) sy)), one float64
+// round-to-nearest step per operation in that order (EPS: y = 0.75 CH - Ypt), written as printf("%.2f") by the f2 token
+// rule (host/f2_token.h).  pl_path_kernel makes every dataset's path text on the device in two passes: the byte length of
+// each dataset, then, at the offsets an exclusive scan of those lengths gives, the text itself.
 #include "gl_common.cuh"
 #include "plot_rule.cuh"
+#include "ll_scan.cuh"
+#include "host/f2_token.h"
 #include "host/font5x7.h"
 #include "host/thread_pool.h"
 #include <zlib.h>
 #include <math.h>
 #include <string.h>
+#include <array>
 
 namespace {
 
@@ -165,6 +174,169 @@ int raster_device(gl_ctx* ctx, const Src& src, const int32_t* d_chart, const uin
     return GL_OK;
 }
 
+// ---- path text
+constexpr int kPathThreads = 256;
+constexpr int kVertexMax = 2 * glf2::kTok + 16;       // the longest vertex token: " L x y" or "x y lineto\n"
+
+// the canvas of a chart kind, in pixels, and the output format
+struct Canvas {
+    double ax, ay, h, ch;
+    bool eps;
+};
+
+bool canvas_of(int32_t kind, int32_t fmt, Canvas& cv) {
+    if (kind < GL_PLOT_DEPTH || kind > GL_PLOT_SQUARE || (fmt != GL_PLOT_SVG && fmt != GL_PLOT_EPS)) return false;
+    const bool sq = kind == GL_PLOT_SQUARE;
+    cv = Canvas{(double)GL_PLOT_AX, (double)GL_PLOT_AY, (double)(sq ? GL_PLOT_SQ_H : GL_PLOT_H), (double)(sq ? GL_PLOT_SQ_CH : GL_PLOT_CH),
+                fmt == GL_PLOT_EPS};
+    return true;
+}
+
+// The text of vertex j of dataset d into t (kVertexMax bytes of room): SVG "M x y" (j == 0) or " L x y"; EPS "x y moveto\n"
+// or "x y lineto\n".  Returns its length, or 0 when a coordinate is not finite or its "%.2f" does not fit a token.
+template <class Src>
+__host__ __device__ inline int vertex_text(const Src& src, int64_t d, int64_t j, const double* f, const Canvas& cv, unsigned char* t) {
+    using glplot::p_add; using glplot::p_sub;
+    double x, y;
+    src.xy(d, j, x, y);
+    const double X = p_mul(0.75, p_add(cv.ax, p_mul(p_sub(x, f[0]), f[1])));
+    double Y = p_mul(0.75, p_add(cv.ay, p_sub(cv.h, p_mul(p_sub(y, f[2]), f[3]))));
+    if (cv.eps) Y = p_sub(p_mul(0.75, cv.ch), Y);
+    if (!isfinite(X) || !isfinite(Y)) return 0;
+    unsigned char tx[glf2::kTok], ty[glf2::kTok];
+    const int lx = glf2::token(X, tx), ly = glf2::token(Y, ty);
+    if (!lx || !ly) return 0;
+    int n = 0;
+    auto put = [&](const char* s) { while (*s) t[n++] = (unsigned char)*s++; };
+    if (!cv.eps) put(j ? " L " : "M ");
+    for (int k = 0; k < lx; k++) t[n++] = tx[k];
+    t[n++] = ' ';
+    for (int k = 0; k < ly; k++) t[n++] = ty[k];
+    if (cv.eps) put(j ? " lineto\n" : " moveto\n");
+    return n;
+}
+
+// Pass 1 (pos == nullptr): len[d] = the bytes of dataset d's path text, 0 when it is not written (fewer than 2 vertices, as
+// the raster draws nothing then, or a vertex vertex_text rejects).  Pass 2: the text at out + pos[d]; no byte is written at
+// or past min(pos[d + 1], cap), so a pos that does not match pass 1 cannot write out of bounds.
+template <class Src>
+__global__ void __launch_bounds__(kPathThreads) pl_path_kernel(Src src, const int32_t* __restrict__ chart, const double* __restrict__ xf,
+                                                               Canvas cv, long long* __restrict__ len, const long long* __restrict__ pos,
+                                                               unsigned char* __restrict__ out, long long cap) {
+    __shared__ long long s_w[kPathThreads / 32];
+    const int64_t d = blockIdx.x;
+    const int64_t m = src.count(d);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const double* f = xf + 4 * (int64_t)chart[d];
+    unsigned char t[kVertexMax];
+    if (!pos) {
+        long long sum = 0;
+        bool bad = false;
+        for (int64_t j = threadIdx.x; j < m && m >= 2; j += blockDim.x) {
+            const int n = vertex_text(src, d, j, f, cv, t);
+            bad |= n == 0;
+            sum += n;
+        }
+        bad = __syncthreads_or(bad);
+        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        if (lane == 0) s_w[warp] = sum;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            for (int w = 1; w < kPathThreads / 32; w++) sum += s_w[w];
+            len[d] = (m < 2 || bad) ? 0 : sum;
+        }
+        return;
+    }
+    const long long end = min(pos[d + 1], cap);
+    if (pos[d] >= end) return;
+    long long base = pos[d];
+    for (int64_t j0 = 0; j0 < m; j0 += blockDim.x) {
+        const int64_t j = j0 + threadIdx.x;
+        const int n = j < m ? vertex_text(src, d, j, f, cv, t) : 0;
+        int inc = n;                                   // block-wide exclusive scan of the vertex lengths
+        for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+        __syncthreads();                               // s_w of the previous chunk has been read
+        if (lane == 31) s_w[warp] = inc;
+        __syncthreads();
+        long long at = base + inc - n, tot = 0;
+        for (int w = 0; w < kPathThreads / 32; w++) { if (w < warp) at += s_w[w]; tot += s_w[w]; }
+        for (int k = 0; k < n && at + k < end; k++) out[at + k] = t[k];
+        base += tot;
+    }
+}
+
+template <class Src>
+int path_size_device(gl_ctx* ctx, const Src& src, const int32_t* d_chart, int32_t n, const double* d_xf, const Canvas& cv, int64_t* d_len,
+                     int64_t* d_pos) {
+    if (n > 0) {
+        gl_prof_scope prof(ctx, "pl_path_kernel");
+        pl_path_kernel<<<(unsigned)n, kPathThreads, 0, ctx->stream>>>(src, d_chart, d_xf, cv, reinterpret_cast<long long*>(d_len), nullptr,
+                                                                      nullptr, 0);
+        GL_LAUNCHED(ctx, 1);
+    }
+    ll_scan_kernel<<<1, 1024, 0, ctx->stream>>>(reinterpret_cast<const long long*>(d_len), reinterpret_cast<long long*>(d_pos), n);
+    GL_LAUNCHED(ctx, 1);
+    return GL_OK;
+}
+
+template <class Src>
+int path_emit_device(gl_ctx* ctx, const char* fn, const Src& src, const int32_t* d_chart, int32_t n, const double* d_xf, const Canvas& cv,
+                     const int64_t* d_pos, int64_t total, char* d_out, int64_t cap) {
+    if (total < 0 || cap < 0 || (cap > 0 && !d_out)) return gl_fail(ctx, GL_EINVAL, "%s: bad argument", fn);
+    if (total > cap) return gl_fail(ctx, GL_ERANGE, "%s: path text is %lld bytes, buffer holds %lld", fn, (long long)total, (long long)cap);
+    if (n == 0 || total == 0) return GL_OK;
+    gl_prof_scope prof(ctx, "pl_path_kernel");
+    pl_path_kernel<<<(unsigned)n, kPathThreads, 0, ctx->stream>>>(src, d_chart, d_xf, cv, nullptr, reinterpret_cast<const long long*>(d_pos),
+                                                                  reinterpret_cast<unsigned char*>(d_out), (long long)cap);
+    GL_LAUNCHED(ctx, 1);
+    return GL_OK;
+}
+
+// host mirror: one pool task per dataset
+template <class Src>
+void path_size_host(const Src& src, const int32_t* chart, int32_t n, const double* xf, const Canvas& cv, int64_t* len, int64_t* pos) {
+    glhost::ThreadPool::global().run(n, [&](int64_t d, int) {
+        const int64_t m = src.count(d);
+        unsigned char t[kVertexMax];
+        int64_t sum = 0;
+        for (int64_t j = 0; j < m && m >= 2; j++) {
+            const int k = vertex_text(src, d, j, xf + 4 * chart[d], cv, t);
+            if (!k) { sum = 0; break; }
+            sum += k;
+        }
+        len[d] = m < 2 ? 0 : sum;
+    });
+    pos[0] = 0;
+    for (int32_t d = 0; d < n; d++) pos[d + 1] = pos[d] + len[d];
+}
+
+template <class Src>
+int path_emit_host(const char* fn, const Src& src, const int32_t* chart, int32_t n, const double* xf, const Canvas& cv, const int64_t* pos,
+                   char* out, int64_t cap) {
+    for (int32_t d = 0; d < n; d++)
+        if (pos[d + 1] < pos[d] || pos[0] != 0) return gl_fail(nullptr, GL_EINVAL, "%s: pos is not a scan of the lengths", fn);
+    if (pos[n] > cap) return gl_fail(nullptr, GL_ERANGE, "%s: path text is %lld bytes, buffer holds %lld", fn, (long long)pos[n], (long long)cap);
+    if (pos[n] > 0 && !out) return gl_fail(nullptr, GL_EINVAL, "%s: bad argument", fn);
+    glhost::ThreadPool::global().run(n, [&](int64_t d, int) {
+        if (pos[d + 1] == pos[d]) return;
+        const int64_t m = src.count(d);
+        unsigned char t[kVertexMax];
+        int64_t at = pos[d];
+        for (int64_t j = 0; j < m; j++) {
+            const int k = vertex_text(src, d, j, xf + 4 * chart[d], cv, t);
+            for (int i = 0; i < k && at < pos[d + 1]; i++) out[at++] = (char)t[i];
+        }
+    });
+    return GL_OK;
+}
+
+int path_args(gl_ctx* ctx, const char* fn, const void* a, const void* b, const void* c, const int32_t* chart, int32_t n, const double* xf,
+              int32_t n_charts, int32_t kind, int32_t fmt, Canvas& cv) {
+    if (n < 0 || n_charts < 0 || (n > 0 && (!a || !b || !c || !chart || !xf)) || !canvas_of(kind, fmt, cv))
+        return gl_fail(ctx, GL_EINVAL, "%s: bad argument", fn);
+    return GL_OK;
+}
+
 // ---- the frame
 constexpr int kGlyphW = 6;             // 5 columns and a blank one
 
@@ -223,6 +395,104 @@ std::string plain_label(double v, double step) {
     return b;
 }
 
+// ---- the vector document (header, frame, paths, trailer)
+std::string f2(double v) {
+    char b[64];
+    snprintf(b, sizeof b, "%.2f", v);
+    return b;
+}
+
+std::string svg_escape(const char* s) {
+    std::string o;
+    for (; *s; s++) {
+        const unsigned char c = (unsigned char)*s;
+        if (c == '&') o += "&amp;";
+        else if (c == '<') o += "&lt;";
+        else if (c == '>') o += "&gt;";
+        else if (c == '"') o += "&quot;";
+        else if (c < 0x20) o += '?';                   // not allowed in XML 1.0 text
+        else o += (char)c;
+    }
+    return o;
+}
+
+std::string ps_string(const char* s) {
+    std::string o = "(";
+    for (; *s; s++) {
+        const unsigned char c = (unsigned char)*s;
+        if (c == '(' || c == ')' || c == '\\') { o += '\\'; o += (char)c; }
+        else if (c < 0x20 || c >= 0x7F) { char b[8]; snprintf(b, sizeof b, "\\%03o", c); o += b; }
+        else o += (char)c;
+    }
+    return o + ")";
+}
+
+// Everything before the paths: the header, the white page, the axes and ticks as strokes, the labels and titles as text.
+// Positions are gl_plot_compose's, in points: the tick values are its ticks at their exact (not pixel-rounded) places.
+std::string vector_head(int32_t kind, const Canvas& cv, const double* xf, const char* xtitle, const char* ytitle) {
+    const bool sq = kind == GL_PLOT_SQUARE;
+    const double W = sq ? GL_PLOT_SQ_W : GL_PLOT_W, CW = sq ? GL_PLOT_SQ_CW : GL_PLOT_CW, H = cv.h, CH = cv.ch, AX = cv.ax, AY = cv.ay;
+    const double pw = CW * 0.75, ph = CH * 0.75;
+    auto px = [&](double x) { return f2(0.75 * x); };
+    auto py = [&](double y) { return f2(cv.eps ? ph - 0.75 * y : 0.75 * y); };
+    std::vector<double> xt, yt;
+    nice_ticks(xf[0], xf[0] + W / xf[1], xt);
+    if (kind == GL_PLOT_DEPTH) yt = {0.0, 0.5, 1.0, 1.5, 2.0};
+    else nice_ticks(xf[2], xf[2] + H / xf[3], yt);
+    const double xstep = xt.size() > 1 ? xt[1] - xt[0] : 0, ystep = yt.size() > 1 ? yt[1] - yt[0] : 0;
+    // (x0, y0)-(x1, y1) strokes and (x, y, anchor: 0 start, 1 middle, 2 end, rotated, text) labels, in pixels
+    std::vector<std::array<double, 4>> lines = {{AX, AY, AX, AY + H}, {AX, AY + H, AX + W, AY + H}};
+    struct Label { double x, y; int anchor; bool rot; std::string s; };
+    std::vector<Label> labels;
+    for (double t : xt) {
+        const double X = (t - xf[0]) * xf[1];
+        if (!(X >= 0 && X <= W)) continue;
+        lines.push_back({AX + X, AY + H, AX + X, AY + H + 4});
+        labels.push_back({AX + X, AY + H + 14, 1, false, kind == GL_PLOT_DEPTH ? millions(t) : plain_label(t, xstep)});
+    }
+    for (double t : yt) {
+        const double Y = H - (t - xf[2]) * xf[3];
+        if (!(Y >= 0 && Y <= H)) continue;
+        lines.push_back({AX - 5, AY + Y, AX, AY + Y});
+        char b[64];
+        if (kind == GL_PLOT_DEPTH) snprintf(b, sizeof b, "%.1f", t);
+        else snprintf(b, sizeof b, "%s", plain_label(t, ystep).c_str());
+        labels.push_back({AX - 8, AY + Y + 3.5, 2, false, b});
+    }
+    labels.push_back({AX + W / 2, CH - 3, 1, false, xtitle});
+    labels.push_back({10, AY + H / 2, 1, true, ytitle});
+    std::string o;
+    if (!cv.eps) {
+        const std::string w = std::to_string((int)pw), h = std::to_string((int)ph);
+        o += "<?xml version=\"1.0\" encoding=\"UTF-8\"?>\n<svg xmlns=\"http://www.w3.org/2000/svg\" version=\"1.1\" width=\"" + w + "pt\" height=\"" + h +
+             "pt\" viewBox=\"0 0 " + w + " " + h + "\">\n";
+        o += "<rect x=\"0\" y=\"0\" width=\"100%\" height=\"100%\" fill=\"#ffffff\"/>\n";
+        for (auto& l : lines)
+            o += "<path d=\"M " + px(l[0]) + " " + py(l[1]) + " L " + px(l[2]) + " " + py(l[3]) + "\" stroke=\"#000000\" stroke-width=\"0.75\" fill=\"none\"/>\n";
+        static const char* anchor[3] = {"start", "middle", "end"};
+        for (auto& l : labels) {
+            o += "<text font-family=\"Helvetica, Arial, sans-serif\" font-size=\"7\" fill=\"#000000\" text-anchor=\"" + std::string(anchor[l.anchor]) + "\" ";
+            if (l.rot) o += "transform=\"translate(" + px(l.x) + " " + py(l.y) + ") rotate(-90)\" x=\"0\" y=\"0\">";
+            else o += "x=\"" + px(l.x) + "\" y=\"" + py(l.y) + "\">";
+            o += svg_escape(l.s.c_str()) + "</text>\n";
+        }
+        return o;
+    }
+    char b[256];
+    snprintf(b, sizeof b, "%%!PS-Adobe-3.0 EPSF-3.0\n%%%%BoundingBox: 0 0 %d %d\n%%%%Creator: goleft indexcov\n%%%%EndComments\n", (int)pw, (int)ph);
+    o += b;
+    o += "1 setgray newpath 0 0 moveto " + f2(pw) + " 0 lineto " + f2(pw) + " " + f2(ph) + " lineto 0 " + f2(ph) + " lineto closepath fill\n";
+    o += "1 setlinejoin 1 setlinecap\n0 setgray 0.75 setlinewidth\n";
+    for (auto& l : lines) o += "newpath " + px(l[0]) + " " + py(l[1]) + " moveto " + px(l[2]) + " " + py(l[3]) + " lineto stroke\n";
+    o += "/Helvetica findfont 7 scalefont setfont\n";
+    for (auto& l : labels) {
+        const std::string s = ps_string(l.s.c_str()), shift = l.anchor == 0 ? "" : l.anchor == 1 ? "dup stringwidth pop 2 div neg 0 rmoveto " : "dup stringwidth pop neg 0 rmoveto ";
+        if (l.rot) o += "gsave " + px(l.x) + " " + py(l.y) + " translate 90 rotate 0 0 moveto " + s + " " + shift + "show grestore\n";
+        else o += px(l.x) + " " + py(l.y) + " moveto " + s + " " + shift + "show\n";
+    }
+    return o;
+}
+
 void be32(uint8_t* p, uint32_t v) { p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v; }
 
 }  // namespace
@@ -275,8 +545,7 @@ int gl_plot_transform(const double* ext4, int32_t W, int32_t H, double* xf4) {
 }
 
 double gl_plot_line_radius(int32_t n_datasets) {
-    const double w = n_datasets > 30 ? 0.65 : 0.8;           // plot.go:508-511, points
-    return std::max(0.5, w * 96.0 / 72.0 / 2.0);
+    return std::max(0.5, gl_plot_line_width(n_datasets) * 96.0 / 72.0 / 2.0);
 }
 
 int gl_plot_raster_series_device(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_sel3, double mult,
@@ -327,6 +596,119 @@ int gl_plot_raster_xy_host(const double* x, const double* y, const int64_t* ptr,
     if (n > 0 && !ptr) return gl_fail(nullptr, GL_EINVAL, "gl_plot_raster_xy_host: bad argument");
     GL_CHECK(check_charts_host("gl_plot_raster_xy_host", chart, n, n_charts));
     raster_host(XySrc{x, y, ptr}, chart, draw, n, xf4, n_charts, W, H, r, img);
+    return GL_OK;
+}
+
+int gl_plot_path_series_size(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_sel3, double mult, const int32_t* d_chart,
+                             int32_t n, const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, int64_t* d_len, int64_t* d_pos) {
+    GL_CHECK(gl_use(ctx));
+    Canvas cv;
+    GL_CHECK(path_args(ctx, "gl_plot_path_series_size", d_vals, d_off, d_sel3, d_chart, n, d_xf4, n_charts, kind, fmt, cv));
+    if ((n > 0 && !d_len) || !d_pos) return gl_fail(ctx, GL_EINVAL, "gl_plot_path_series_size: bad argument");
+    return path_size_device(ctx, SeriesSrc{d_vals, d_off, d_sel3, mult}, d_chart, n, d_xf4, cv, d_len, d_pos);
+}
+
+int gl_plot_path_series_emit(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_sel3, double mult, const int32_t* d_chart,
+                             int32_t n, const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* d_pos, int64_t total,
+                             char* d_out, int64_t cap) {
+    GL_CHECK(gl_use(ctx));
+    Canvas cv;
+    GL_CHECK(path_args(ctx, "gl_plot_path_series_emit", d_vals, d_off, d_sel3, d_chart, n, d_xf4, n_charts, kind, fmt, cv));
+    if (!d_pos) return gl_fail(ctx, GL_EINVAL, "gl_plot_path_series_emit: bad argument");
+    return path_emit_device(ctx, "gl_plot_path_series_emit", SeriesSrc{d_vals, d_off, d_sel3, mult}, d_chart, n, d_xf4, cv, d_pos, total, d_out, cap);
+}
+
+int gl_plot_path_series_size_host(const float* vals, const int64_t* off, const int64_t* sel3, double mult, const int32_t* chart, int32_t n,
+                                  const double* xf4, int32_t n_charts, int32_t kind, int32_t fmt, int64_t* len, int64_t* pos) {
+    Canvas cv;
+    GL_CHECK(path_args(nullptr, "gl_plot_path_series_size_host", vals, off, sel3, chart, n, xf4, n_charts, kind, fmt, cv));
+    if ((n > 0 && !len) || !pos) return gl_fail(nullptr, GL_EINVAL, "gl_plot_path_series_size_host: bad argument");
+    GL_CHECK(check_charts_host("gl_plot_path_series_size_host", chart, n, n_charts));
+    path_size_host(SeriesSrc{vals, off, sel3, mult}, chart, n, xf4, cv, len, pos);
+    return GL_OK;
+}
+
+int gl_plot_path_series_emit_host(const float* vals, const int64_t* off, const int64_t* sel3, double mult, const int32_t* chart, int32_t n,
+                                  const double* xf4, int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* pos, char* out, int64_t cap) {
+    Canvas cv;
+    GL_CHECK(path_args(nullptr, "gl_plot_path_series_emit_host", vals, off, sel3, chart, n, xf4, n_charts, kind, fmt, cv));
+    if (!pos) return gl_fail(nullptr, GL_EINVAL, "gl_plot_path_series_emit_host: bad argument");
+    GL_CHECK(check_charts_host("gl_plot_path_series_emit_host", chart, n, n_charts));
+    return path_emit_host("gl_plot_path_series_emit_host", SeriesSrc{vals, off, sel3, mult}, chart, n, xf4, cv, pos, out, cap);
+}
+
+int gl_plot_path_xy_size(gl_ctx* ctx, const double* d_x, const double* d_y, const int64_t* d_ptr, const int32_t* d_chart, int32_t n,
+                         const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, int64_t* d_len, int64_t* d_pos) {
+    GL_CHECK(gl_use(ctx));
+    Canvas cv;
+    GL_CHECK(path_args(ctx, "gl_plot_path_xy_size", d_x, d_y, d_ptr, d_chart, n, d_xf4, n_charts, kind, fmt, cv));
+    if ((n > 0 && !d_len) || !d_pos) return gl_fail(ctx, GL_EINVAL, "gl_plot_path_xy_size: bad argument");
+    return path_size_device(ctx, XySrc{d_x, d_y, d_ptr}, d_chart, n, d_xf4, cv, d_len, d_pos);
+}
+
+int gl_plot_path_xy_emit(gl_ctx* ctx, const double* d_x, const double* d_y, const int64_t* d_ptr, const int32_t* d_chart, int32_t n,
+                         const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* d_pos, int64_t total, char* d_out,
+                         int64_t cap) {
+    GL_CHECK(gl_use(ctx));
+    Canvas cv;
+    GL_CHECK(path_args(ctx, "gl_plot_path_xy_emit", d_x, d_y, d_ptr, d_chart, n, d_xf4, n_charts, kind, fmt, cv));
+    if (!d_pos) return gl_fail(ctx, GL_EINVAL, "gl_plot_path_xy_emit: bad argument");
+    return path_emit_device(ctx, "gl_plot_path_xy_emit", XySrc{d_x, d_y, d_ptr}, d_chart, n, d_xf4, cv, d_pos, total, d_out, cap);
+}
+
+int gl_plot_path_xy_size_host(const double* x, const double* y, const int64_t* ptr, const int32_t* chart, int32_t n, const double* xf4,
+                              int32_t n_charts, int32_t kind, int32_t fmt, int64_t* len, int64_t* pos) {
+    Canvas cv;
+    GL_CHECK(path_args(nullptr, "gl_plot_path_xy_size_host", x, y, ptr, chart, n, xf4, n_charts, kind, fmt, cv));
+    if ((n > 0 && !len) || !pos) return gl_fail(nullptr, GL_EINVAL, "gl_plot_path_xy_size_host: bad argument");
+    GL_CHECK(check_charts_host("gl_plot_path_xy_size_host", chart, n, n_charts));
+    path_size_host(XySrc{x, y, ptr}, chart, n, xf4, cv, len, pos);
+    return GL_OK;
+}
+
+int gl_plot_path_xy_emit_host(const double* x, const double* y, const int64_t* ptr, const int32_t* chart, int32_t n, const double* xf4,
+                              int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* pos, char* out, int64_t cap) {
+    Canvas cv;
+    GL_CHECK(path_args(nullptr, "gl_plot_path_xy_emit_host", x, y, ptr, chart, n, xf4, n_charts, kind, fmt, cv));
+    if (!pos) return gl_fail(nullptr, GL_EINVAL, "gl_plot_path_xy_emit_host: bad argument");
+    GL_CHECK(check_charts_host("gl_plot_path_xy_emit_host", chart, n, n_charts));
+    return path_emit_host("gl_plot_path_xy_emit_host", XySrc{x, y, ptr}, chart, n, xf4, cv, pos, out, cap);
+}
+
+double gl_plot_line_width(int32_t n_datasets) {
+    return n_datasets > 30 ? 0.65 : 0.8;                      // plot.go:508-511, points
+}
+
+int gl_plot_vector_write(const char* path, int32_t kind, int32_t fmt, const double* ext4, const char* xtitle, const char* ytitle, int32_t n,
+                         const uint8_t* rgb, double width, const char* const* data, const int64_t* len) {
+    Canvas cv;
+    double xf[4];
+    if (!path || !ext4 || !xtitle || !ytitle || n < 0 || (n > 0 && (!rgb || !data || !len)) || !(width > 0) || !canvas_of(kind, fmt, cv))
+        return gl_fail(nullptr, GL_EINVAL, "gl_plot_vector_write: bad argument");
+    for (int32_t d = 0; d < n; d++)
+        if (len[d] < 0 || (len[d] > 0 && !data[d])) return gl_fail(nullptr, GL_EINVAL, "gl_plot_vector_write: dataset %d: bad text", d);
+    const bool sq = kind == GL_PLOT_SQUARE;
+    GL_CHECK(gl_plot_transform(ext4, sq ? GL_PLOT_SQ_W : GL_PLOT_W, sq ? GL_PLOT_SQ_H : GL_PLOT_H, xf));
+    FILE* f = fopen(path, "wb");
+    if (!f) return gl_fail(nullptr, GL_EINVAL, "gl_plot_vector_write: cannot create %s", path);
+    bool ok = true;
+    auto put = [&](const std::string& s) { ok = ok && fwrite(s.data(), 1, s.size(), f) == s.size(); };
+    put(vector_head(kind, cv, xf, xtitle, ytitle));
+    const std::string w = f2(width);
+    for (int32_t d = 0; d < n; d++) {
+        if (len[d] == 0) continue;
+        const uint8_t* c = rgb + 3 * (size_t)d;
+        char pre[96];
+        if (cv.eps) snprintf(pre, sizeof pre, "%.4f %.4f %.4f setrgbcolor %s setlinewidth newpath\n", c[0] / 255.0, c[1] / 255.0, c[2] / 255.0, w.c_str());
+        else snprintf(pre, sizeof pre, "<path d=\"");
+        put(pre);
+        ok = ok && fwrite(data[d], 1, (size_t)len[d], f) == (size_t)len[d];
+        if (cv.eps) put("stroke\n");
+        else { char post[96]; snprintf(post, sizeof post, "\" stroke=\"#%02x%02x%02x\" stroke-width=\"%s\" fill=\"none\"/>\n", c[0], c[1], c[2], w.c_str()); put(post); }
+    }
+    put(cv.eps ? "showpage\n%%EOF\n" : "</svg>\n");
+    ok = fclose(f) == 0 && ok;
+    if (!ok) return gl_fail(nullptr, GL_EINVAL, "gl_plot_vector_write: cannot write %s", path);
     return GL_OK;
 }
 

@@ -498,7 +498,26 @@ int  gl_sym_tridiag(gl_ctx* ctx, const double* a, int32_t n, double* d, double* 
  *       in KB/MB; GL_PLOT_PLAIN: nice ticks on both axes; GL_PLOT_SQUARE: the same on the square canvas (rgb and img then
  *       have its sizes).  ext4 as gl_plot_transform takes it.
  *   gl_plot_png     : host-only: the PNG of W x H RGB8 pixels: filter 0 on every row, one IDAT.  out == NULL: *len = the
- *       room needed. */
+ *       room needed.
+ *
+ * The vector charts (INDEXCOV_FMT): the same charts in points, 0.75 pt per pixel (depth, ROC: 288 x 216 pt; sex: 432 x 432).
+ * Vertex (x, y) of a dataset on chart c with xf4 = {xmin, sx, ymin, sy} is at Xpt = 0.75 * (AX + (x - xmin) * sx),
+ * Ypt = 0.75 * (AY + (H - (y - ymin) * sy)), each operation one float64 round-to-nearest step in that order; GL_PLOT_EPS
+ * writes 0.75 * CH - Ypt (y up).  AX, AY, H and CH are those of `kind`'s canvas.  Each coordinate is the exact
+ * printf("%.2f") of its value.  A dataset's PATH TEXT is, for vertices 0..m-1: GL_PLOT_SVG "M x y" then " L x y" per
+ * vertex (the d attribute of one <path>); GL_PLOT_EPS "x y moveto\n" then "x y lineto\n" per vertex.  It is empty when the
+ * chart's PNG draws nothing for the dataset (fewer than 2 vertices) or a coordinate is not finite or needs more than 16
+ * bytes of text.  Datasets are concatenated in input order.
+ *   gl_plot_path_series_size : queued on the ctx stream: d_len[d] = the bytes of dataset d's path text (series source as
+ *       in gl_plot_raster_series_device) and d_pos[0..n] their exclusive scan (d_pos[n] = the total).
+ *   gl_plot_path_series_emit : queued: the text of dataset d at d_out + d_pos[d].  total = d_pos[n] as the caller read it;
+ *       total > cap is GL_ERANGE.  No byte is written at or past min(d_pos[d + 1], cap).
+ *   gl_plot_path_xy_size / _emit : the same for explicit float64 vertices (device arrays, as gl_plot_raster_xy's).
+ *   ..._host : the mirrors, on host arrays (emit: pos[n] > cap is GL_ERANGE).
+ *   gl_plot_line_width : the stroke width in points: 0.8, or 0.65 above 30 datasets (plot.go:508-511).
+ *   gl_plot_vector_write : host-only: writes the document to `path`: header, white page, axes, ticks, tick labels and
+ *       titles at gl_plot_compose's places (labels as text: SVG escapes & < > ", PostScript strings escape ( ) \), then one
+ *       path per dataset with len[d] > 0, in order: data[d][0..len[d]) stroked in rgb[3*d..] with `width` points. */
 #define GL_PLOT_CW 384
 #define GL_PLOT_CH 288
 #define GL_PLOT_AX 56
@@ -534,6 +553,29 @@ int  gl_plot_text(uint8_t* rgb, int32_t CW, int32_t CH, int32_t x, int32_t y, co
 int  gl_plot_compose(const uint32_t* img, const uint8_t* palette, int32_t n_pal, int32_t kind, const double* ext4, const char* xtitle,
                      const char* ytitle, uint8_t* rgb);
 int  gl_plot_png(const uint8_t* rgb, int32_t W, int32_t H, uint8_t* out, int64_t cap, int64_t* len);
+#define GL_PLOT_SVG 0
+#define GL_PLOT_EPS 1
+int  gl_plot_path_series_size(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_sel3, double mult, const int32_t* d_chart,
+                              int32_t n, const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, int64_t* d_len, int64_t* d_pos);
+int  gl_plot_path_series_emit(gl_ctx* ctx, const float* d_vals, const int64_t* d_off, const int64_t* d_sel3, double mult, const int32_t* d_chart,
+                              int32_t n, const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* d_pos, int64_t total,
+                              char* d_out, int64_t cap);
+int  gl_plot_path_series_size_host(const float* vals, const int64_t* off, const int64_t* sel3, double mult, const int32_t* chart, int32_t n,
+                                   const double* xf4, int32_t n_charts, int32_t kind, int32_t fmt, int64_t* len, int64_t* pos);
+int  gl_plot_path_series_emit_host(const float* vals, const int64_t* off, const int64_t* sel3, double mult, const int32_t* chart, int32_t n,
+                                   const double* xf4, int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* pos, char* out, int64_t cap);
+int  gl_plot_path_xy_size(gl_ctx* ctx, const double* d_x, const double* d_y, const int64_t* d_ptr, const int32_t* d_chart, int32_t n,
+                          const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, int64_t* d_len, int64_t* d_pos);
+int  gl_plot_path_xy_emit(gl_ctx* ctx, const double* d_x, const double* d_y, const int64_t* d_ptr, const int32_t* d_chart, int32_t n,
+                          const double* d_xf4, int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* d_pos, int64_t total, char* d_out,
+                          int64_t cap);
+int  gl_plot_path_xy_size_host(const double* x, const double* y, const int64_t* ptr, const int32_t* chart, int32_t n, const double* xf4,
+                               int32_t n_charts, int32_t kind, int32_t fmt, int64_t* len, int64_t* pos);
+int  gl_plot_path_xy_emit_host(const double* x, const double* y, const int64_t* ptr, const int32_t* chart, int32_t n, const double* xf4,
+                               int32_t n_charts, int32_t kind, int32_t fmt, const int64_t* pos, char* out, int64_t cap);
+double gl_plot_line_width(int32_t n_datasets);
+int  gl_plot_vector_write(const char* path, int32_t kind, int32_t fmt, const double* ext4, const char* xtitle, const char* ytitle, int32_t n,
+                          const uint8_t* rgb, double width, const char* const* data, const int64_t* len);
 
 /* indexsplit (indexsplit/indexsplit.go:92-115): amount of cohort data per 16 KB tile = sum over the S samples, in path
  * order, of float64(size)/1e9 — bit-identical to the reference's sequential adds.  sizes: every sample's tile sizes

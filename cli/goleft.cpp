@@ -2711,6 +2711,9 @@ static int cmd_samplename(int argc, char** argv) {
 // `dcnv --svd PCT` (also --svd=PCT, before the positionals; DESIGN §1.13) then removes the cohort's leading components from
 // the normalised matrix (gl_dcnv_svd, row blocks sized to device memory) and logs "variance:" with the removed ones' shares.
 // PCT must be finite and >= 0, else exit 255 as go-arg's flag errors.
+// `dcnv --chunk W` (also --chunk=W; DESIGN §1.9) debiases with the reference's unreached ChunkDebiaser in place of the
+// moving median: the GC-sorted rows are cut into chunks spanning at most W of GC (gl_dcnv_chunk_slices), and each sample's
+// values in a chunk are divided by their median there (gl_dcnv_normalize_chunked).  W must be finite and > 0, else exit 255.
 namespace {
 
 struct DcnvRow { const char* p; size_t n; };                 // one line, without its "\n"
@@ -2960,10 +2963,25 @@ void dcnv_charts(gl_ctx* ctx, const double* X, size_t R, size_t S, const std::ve
 
 static int cmd_dcnv(int argc, char** argv) {
     double svd_pct = -1;                                         // --svd PCT; < 0: off
+    double chunk_w = 0;                                          // --chunk W; 0: off (the moving median of 9)
     bool noplots = false;                                        // --noplots (extension, as in indexcov): no chart files
-    for (bool more = true; more && argc >= 2;) {                 // the flags, in either order, before the positionals
+    for (bool more = true; more && argc >= 2;) {                 // the flags, in any order, before the positionals
         more = false;
-        if (strcmp(argv[1], "--noplots") == 0) {
+        if (strncmp(argv[1], "--chunk", 7) == 0 && (argv[1][7] == 0 || argv[1][7] == '=')) {
+            ArgParser ap;
+            ap.prog = "goleft dcnv";
+            const int used = argv[1][7] == '=' ? 1 : 2;
+            if (used == 2 && argc < 3) ap.fail("missing value for --chunk");
+            const std::string v = used == 1 ? argv[1] + 8 : argv[2];
+            char* endp = nullptr;
+            const double w = strtod(v.c_str(), &endp);
+            if (v.empty() || *endp) ap.fail("error processing chunk: strconv.ParseFloat: parsing \"" + v + "\": invalid syntax");
+            if (!std::isfinite(w) || !(w > 0)) ap.fail("chunk must be a finite number > 0");
+            chunk_w = w;
+            more = true;
+            argc -= used;
+            argv += used;
+        } else if (strcmp(argv[1], "--noplots") == 0) {
             noplots = more = true;
             argc -= 1;
             argv += 1;
@@ -3011,7 +3029,8 @@ static int cmd_dcnv(int argc, char** argv) {
     const std::vector<int64_t>& ends = mx.ends;
     const std::vector<std::pair<const char*, size_t>>& chrom = mx.chrom;
     for (int64_t& v : starts) v = std::max<int64_t>(v, 250);
-    if (R < 5) fatal(2, "panic: runtime error: index out of range (%zu data rows; the moving median needs 5)", R);
+    if (chunk_w > 0 && R < 1) fatal(2, "panic: runtime error: index out of range [0] with length 0 (no data rows)");
+    if (chunk_w == 0 && R < 5) fatal(2, "panic: runtime error: index out of range (%zu data rows; the moving median needs 5)", R);
     mark("parse");
 
     // ---- GC of every row, a contig at a time: Faidx.Stats(chrom, start - 250, end)
@@ -3054,10 +3073,24 @@ static int cmd_dcnv(int argc, char** argv) {
     // ---- debias + normalise on the GPU, in place
     const char* bc = getenv("GL_DCNV_BLOCK_COLS");
     std::vector<double> med(S);
-    const int rc = gl_dcnv_normalize(ctx, X.data(), (int64_t)R, (int64_t)S, inds.data(), 0, (int32_t)S, bc ? atoi(bc) : 0, X.data(), (int64_t)S, med.data());
-    if (rc == GL_ERANGE) fatal(2, "panic: runtime error: index out of range: %s", gl_last_error(ctx));
-    glck(ctx, rc, "gl_dcnv_normalize");
-    mark("normalize");
+    if (chunk_w > 0) {                                           // the chunks over the GC values in sorted order
+        std::vector<double> v(R);
+        for (size_t i = 0; i < R; i++) v[i] = gc[(size_t)inds[i]];
+        int64_t n_chunks = 0;
+        glck(ctx, gl_dcnv_chunk_slices(v.data(), (int64_t)R, chunk_w, nullptr, 0, &n_chunks), "gl_dcnv_chunk_slices");
+        std::vector<int64_t> ptr((size_t)n_chunks + 1);
+        glck(ctx, gl_dcnv_chunk_slices(v.data(), (int64_t)R, chunk_w, ptr.data(), n_chunks + 1, &n_chunks), "gl_dcnv_chunk_slices");
+        const int rc = gl_dcnv_normalize_chunked(ctx, X.data(), (int64_t)R, (int64_t)S, inds.data(), ptr.data(), n_chunks, 0, (int32_t)S,
+                                                 bc ? atoi(bc) : 0, X.data(), (int64_t)S, med.data());
+        if (rc == GL_ERANGE) fatal(2, "panic: runtime error: index out of range: %s", gl_last_error(ctx));
+        glck(ctx, rc, "gl_dcnv_normalize_chunked");
+        mark("normalize (chunk)");
+    } else {
+        const int rc = gl_dcnv_normalize(ctx, X.data(), (int64_t)R, (int64_t)S, inds.data(), 0, (int32_t)S, bc ? atoi(bc) : 0, X.data(), (int64_t)S, med.data());
+        if (rc == GL_ERANGE) fatal(2, "panic: runtime error: index out of range: %s", gl_last_error(ctx));
+        glck(ctx, rc, "gl_dcnv_normalize");
+        mark("normalize (median 9)");
+    }
     if (svd_pct >= 0) {
         std::vector<double> sv(S);
         int32_t n_removed = 0;

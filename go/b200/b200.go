@@ -321,6 +321,36 @@ func (c *Ctx) Dcnv(depths []float64, gcs []float64, samples int) ([]float64, err
 	return medians, c.err(rc)
 }
 
+// DcnvChunk is Dcnv with ChunkDebiaser.Debias (dcnv/debiaser/debiaser.go:125-170, ScoreWindow = window) in place of the
+// moving median, over the rows in GC order (`goleft dcnv --chunk W`): the sorted rows are cut into chunks spanning at most
+// window of GC, and each sample's values in a chunk are divided by their median there when it is > 0.  window must be
+// finite and > 0.  Returns the sample medians of the later NormalizeBySampleMedian.
+func (c *Ctx) DcnvChunk(depths []float64, gcs []float64, samples int, window float64) ([]float64, error) {
+	n := len(gcs)
+	inds := make([]int64, n)
+	if C.gl_go_argsort_f64((*C.double)(&gcs[0]), C.int64_t(n), (*C.int64_t)(&inds[0])) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_go_argsort_f64 failed")
+	}
+	sorted := make([]float64, n)
+	for i, j := range inds {
+		sorted[i] = gcs[j]
+	}
+	var nChunks C.int64_t
+	if C.gl_dcnv_chunk_slices((*C.double)(&sorted[0]), C.int64_t(n), C.double(window), nil, 0, &nChunks) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_dcnv_chunk_slices: window must be finite and > 0")
+	}
+	ptr := make([]int64, int(nChunks)+1)
+	if C.gl_dcnv_chunk_slices((*C.double)(&sorted[0]), C.int64_t(n), C.double(window), (*C.int64_t)(&ptr[0]), C.int64_t(len(ptr)),
+		&nChunks) != C.GL_OK {
+		return nil, fmt.Errorf("goleft_b200: gl_dcnv_chunk_slices failed")
+	}
+	medians := make([]float64, samples)
+	d := (*C.double)(unsafe.Pointer(&depths[0]))
+	rc := C.gl_dcnv_normalize_chunked(c.h, d, C.int64_t(n), C.int64_t(samples), (*C.int64_t)(&inds[0]), (*C.int64_t)(&ptr[0]), nChunks,
+		0, C.int32_t(samples), 0, d, C.int64_t(samples), (*C.double)(&medians[0]))
+	return medians, c.err(rc)
+}
+
 // DcnvSVD replaces scalers.ZScore.Scale + debiaser.SVD{MinVariancePct}.Debias + ZScore.UnScale (dcnv/scalers/scalers.go:25-56,
 // dcnv/debiaser/debiaser.go:173-200) on the normalised n x S row-major matrix `depths`, in place: rows whose values are all
 // equal are left as they are, the leading components whose share of the singular values is above minPct (at most 15) are

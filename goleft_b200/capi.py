@@ -235,6 +235,11 @@ _proto("gl_multidepth_text", C.c_int, C.c_char_p, _vp, _vp, C.c_int64, C.c_int32
 _proto("gl_go_argsort_f64", C.c_int, _vp, C.c_int64, _vp)
 _proto("gl_dcnv_normalize_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int32, _vp, C.c_int64, _vp)
 _proto("gl_dcnv_normalize", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_int64, _vp)
+_proto("gl_dcnv_chunk_slices", C.c_int, _vp, C.c_int64, C.c_double, _vp, C.c_int64, _i64p)
+_proto("gl_dcnv_normalize_chunked_device", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, _vp,
+       C.c_int64, _vp)
+_proto("gl_dcnv_normalize_chunked", C.c_int, _vp, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _vp,
+       C.c_int64, _vp)
 _proto("gl_format_f2", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_f2_device", C.c_int, _vp, _vp, C.c_int64, _vp)
 _proto("gl_format_f2_host", C.c_int, _vp, C.c_int64, _vp)
@@ -384,6 +389,20 @@ def go_argsort(v) -> np.ndarray:
     if rc != GL_OK:
         raise GlError(rc, "gl_go_argsort_f64: bad arguments")
     return inds
+
+
+def dcnv_chunk_slices(gc_sorted, w: float) -> np.ndarray:
+    """Host-only: ChunkDebiaser's chunks of the GC values in sorted order, as CSR offsets (ptr[0] = 0, ptr[-1] = n)."""
+    v = _as(gc_sorted, np.float64)
+    nc = C.c_int64(0)
+    rc = lib.gl_dcnv_chunk_slices(_ptr(v), v.size, float(w), None, 0, C.byref(nc))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_dcnv_chunk_slices: bad arguments (n >= 1, w finite and > 0)")
+    ptr = np.empty(nc.value + 1, np.int64)
+    rc = lib.gl_dcnv_chunk_slices(_ptr(v), v.size, float(w), _ptr(ptr), ptr.size, C.byref(nc))
+    if rc != GL_OK:
+        raise GlError(rc, "gl_dcnv_chunk_slices: failed")
+    return ptr
 
 
 def format_f2_host(vals) -> np.ndarray:
@@ -1789,6 +1808,24 @@ class Ctx:
     def dcnv_normalize_device(self, d_x: DevBuf, n: int, ld: int, d_inds: DevBuf, c0: int, c1: int, d_out: DevBuf, ld_out: int,
                               d_medians: DevBuf):
         self._ck(lib.gl_dcnv_normalize_device(self.h, d_x.ptr, n, ld, d_inds.ptr, c0, c1, d_out.ptr, ld_out, d_medians.ptr))
+
+    def dcnv_normalize_chunked(self, x: np.ndarray, inds, chunk_ptr, c0: int = 0, c1: Optional[int] = None, block_cols: int = 0):
+        """dcnv_normalize with ChunkDebiaser's chunks (chunk_ptr, from dcnv_chunk_slices) in place of the moving median"""
+        x = np.ascontiguousarray(x, np.float64)
+        n, S = x.shape
+        c1 = S if c1 is None else c1
+        inds, chunk_ptr = _as(inds, np.int64), _as(chunk_ptr, np.int64)
+        out, med = np.empty((n, c1 - c0), np.float64), np.empty(c1 - c0, np.float64)
+        self._ck(lib.gl_dcnv_normalize_chunked(self.h, _ptr(x), n, S, _ptr(inds), _ptr(chunk_ptr), chunk_ptr.size - 1, c0, c1, block_cols,
+                                               _ptr(out), c1 - c0, _ptr(med)))
+        return out, med
+
+    def dcnv_normalize_chunked_device(self, d_x: DevBuf, n: int, ld: int, d_inds: DevBuf, chunk_ptr, c0: int, c1: int, d_out: DevBuf,
+                                      ld_out: int, d_medians: DevBuf):
+        """chunk_ptr is a host array"""
+        chunk_ptr = _as(chunk_ptr, np.int64)
+        self._ck(lib.gl_dcnv_normalize_chunked_device(self.h, d_x.ptr, n, ld, d_inds.ptr, _ptr(chunk_ptr), chunk_ptr.size - 1, c0, c1,
+                                                      d_out.ptr, ld_out, d_medians.ptr))
 
     def format_f2(self, vals: np.ndarray) -> np.ndarray:
         vals = _as(vals, np.float64)

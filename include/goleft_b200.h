@@ -674,6 +674,23 @@ int  gl_dcnv_normalize_device(gl_ctx* ctx, const double* d_x, int64_t n, int64_t
                               double* d_out, int64_t ld_out, double* d_medians);
 int  gl_dcnv_normalize(gl_ctx* ctx, const double* x, int64_t n, int64_t ld, const int64_t* inds, int32_t c0, int32_t c1, int32_t block_cols,
                        double* out, int64_t ld_out, double* medians);
+/* dcnv --chunk W (DESIGN §1.9): ChunkDebiaser.Debias in place of the moving median, over the GC-sorted rows.
+ *   gl_dcnv_chunk_slices : host-only: with v = the GC values in sorted order (v[i] = gc[inds[i]]), the chunks start at 0 and
+ *                        at every i where v[i] - v0 > w (float64), v0 = v[the chunk's first row].  ptr[0] = 0, ptr[*n_chunks]
+ *                        = n.  *n_chunks is always set; ptr NULL only sizes (cap entries of room, >= *n_chunks + 1, else
+ *                        GL_ERANGE).  n >= 1; w finite and > 0, else GL_EINVAL.
+ *   gl_dcnv_normalize_chunked[_device] : as gl_dcnv_normalize[_device], with the chunks chunk_ptr[0 .. n_chunks] (a HOST
+ *                        array in both; 0 = ptr[0] < ptr[1] < ... < ptr[n_chunks] = n) in place of the moving median: per
+ *                        sample and chunk, with sorted = the chunk's values ascending and k = its leading exact zeros (0
+ *                        when a value is negative), median = sorted[(len - k) / 2] (the index is into the whole chunk); when
+ *                        median > 0 every value of the chunk is divided by it, else the chunk is left as it is.  Then the
+ *                        same sample median and GL_ERANGE for an all-zero sample.  n >= 1.  The host entry streams blocks of
+ *                        block_cols columns (0: as many as fit, 24 bytes per cell and 8 per chunk and sample). */
+int  gl_dcnv_chunk_slices(const double* gc_sorted, int64_t n, double w, int64_t* ptr, int64_t cap, int64_t* n_chunks);
+int  gl_dcnv_normalize_chunked_device(gl_ctx* ctx, const double* d_x, int64_t n, int64_t ld, const int64_t* d_inds, const int64_t* chunk_ptr,
+                                      int64_t n_chunks, int32_t c0, int32_t c1, double* d_out, int64_t ld_out, double* d_medians);
+int  gl_dcnv_normalize_chunked(gl_ctx* ctx, const double* x, int64_t n, int64_t ld, const int64_t* inds, const int64_t* chunk_ptr, int64_t n_chunks,
+                               int32_t c0, int32_t c1, int32_t block_cols, double* out, int64_t ld_out, double* medians);
 int  gl_format_f2(gl_ctx* ctx, const double* vals, int64_t n, uint8_t* tokens);
 int  gl_format_f2_device(gl_ctx* ctx, const double* d_vals, int64_t n, uint8_t* d_tokens);
 int  gl_format_f2_host(const double* vals, int64_t n, uint8_t* tokens);

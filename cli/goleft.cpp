@@ -196,6 +196,97 @@ static std::vector<std::thread> start_workers(const GpuPlan& p, const std::funct
     return th;
 }
 
+// A cohort's BAMs run by one worker per GPU and committed in argument order (covstats and depthwed from BAMs).  A worker
+// claims the BAMs in argument order and opens the one after its current BAM before it runs the current one, so that the open
+// overlaps the run.  No BAM after the first known failure is claimed, and one claimed ahead of a failure is closed without
+// running.  The main thread takes the jobs in order with wait(i), and stop() joins the workers before a failure ends the run,
+// so the failure reported is the first in argument order.
+struct BamJob {
+    gl_bam* bh = nullptr;
+    bool done = false;
+    int code = 0;                           // exit code of this BAM's failure (0: none) and its message
+    std::string msg;
+};
+
+template <class Job> struct BamQueue {
+    const std::vector<std::string>& bams;
+    std::vector<Job> jobs;
+    std::mutex mu;
+    std::condition_variable cv;
+    std::string setup_err;                  // the first worker that could not be set up: the message that ends the run
+    size_t next_claim = 0, fail_at;         // no BAM after the first known failure is claimed
+    std::vector<std::thread> th;
+
+    explicit BamQueue(const std::vector<std::string>& b) : bams(b), jobs(b.size()), fail_at(b.size()) {}
+    ~BamQueue() { stop(); }
+
+    // Worker g: state = setup(g, err), where a message in err ends the run; run(state, i, next) for each BAM i it claims that
+    // opened, next being the BAM opened after it (or null); teardown(state) at its end, set up or not.
+    template <class Setup, class Run, class Teardown> void start(const GpuPlan& gp, Setup setup, Run run, Teardown teardown) {
+        th = start_workers(gp, [this, setup, run, teardown](int g) {
+            std::string err;
+            auto st = setup(g, err);
+            if (!err.empty()) {
+                std::lock_guard<std::mutex> lk(mu);
+                if (setup_err.empty()) setup_err = err;
+                cv.notify_all();
+            }
+            const size_t S = jobs.size();
+            for (size_t cur = err.empty() ? claim() : S; cur < S;) {
+                if (behind(cur)) { close(cur); break; }
+                const size_t nxt = claim();
+                if (!jobs[cur].code) run(st, cur, nxt < S ? jobs[nxt].bh : nullptr);
+                close(cur);
+                std::lock_guard<std::mutex> lk(mu);
+                jobs[cur].done = true;
+                if (jobs[cur].code) fail_at = std::min(fail_at, cur);
+                cv.notify_all();
+                cur = nxt;
+            }
+            teardown(st);
+        });
+    }
+
+    // the next BAM, opened (a failed open is its job's failure), or jobs.size() once claiming has ended
+    size_t claim() {
+        size_t i;
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            if (next_claim >= fail_at || !setup_err.empty()) return jobs.size();
+            i = next_claim++;
+        }
+        char oerr[512] = {0};
+        if (gl_bam_open(bams[i].c_str(), &jobs[i].bh, oerr, sizeof oerr) != GL_OK) { jobs[i].code = 1; jobs[i].msg = oerr; jobs[i].bh = nullptr; }
+        return i;
+    }
+
+    // whether BAM i will never be committed: a BAM before it failed, or a worker could not be set up
+    bool behind(size_t i) {
+        std::lock_guard<std::mutex> lk(mu);
+        return i > fail_at || !setup_err.empty();
+    }
+
+    void close(size_t i) {
+        if (jobs[i].bh) gl_bam_close(jobs[i].bh);
+        jobs[i].bh = nullptr;
+    }
+
+    // job i once its worker is done with it; a worker that could not be set up ends the run here instead
+    Job& wait(size_t i) {
+        std::unique_lock<std::mutex> lk(mu);
+        cv.wait(lk, [&] { return jobs[i].done || !setup_err.empty(); });
+        if (!jobs[i].done) { lk.unlock(); stop(); fatal(1, "%s", setup_err.c_str()); }
+        return jobs[i];
+    }
+
+    // ends the claiming and joins the workers
+    void stop() {
+        { std::lock_guard<std::mutex> lk(mu); fail_at = 0; }
+        for (std::thread& t : th) t.join();
+        th.clear();
+    }
+};
+
 // whether a BAM's index can be seeked with: a stub index (stats bin but an empty / all-zero linear index for a reference that
 // has reads) cannot, and such a BAM is decoded whole
 static bool index_usable(const glhts::BamFile& f) {
@@ -207,6 +298,25 @@ static bool index_usable(const glhts::BamFile& f) {
         usable = any;
     }
     return usable;
+}
+
+// A BAM without a usable index cannot be seeked, so it is decoded once, whole, on `threads` host threads: reference `only`, or
+// every reference for -1, into `whole`, which a SegSource then views.  True when it was, after `note` (when given) went to
+// stderr; err then holds a failed decode's message.  False, with nothing decoded, for a BAM whose index can be used.
+static bool decode_unindexed(const glhts::BamFile& f, const std::string& path, int Q, int threads, int only, glhts::SegmentSet& whole,
+                             std::string& err, const char* note = nullptr) {
+    if (index_usable(f)) return false;
+    if (note) fprintf(stderr, "%s\n", note);
+    err = glhts::bam_decode_segments(path, Q, threads, only, whole);
+    return true;
+}
+
+// The bases of one pass over a contig: whole `step` chunks within the 2^30 - 1 bases the GPU reduces at once.  A window wider
+// than that leaves no pass, and ends the run.
+static long long pass_length(long long step, int W, const char* prog) {
+    const long long n = ((1LL << 30) - 1) / step * step;
+    if (n == 0) fatal(1, "%s: windowsize %d is above the 2^30 - 1 bases of one pass", prog, W);
+    return n;
 }
 
 // the index of an input (indexcov.go:500-510): a .bai or .csi names itself; else the first of x.bam.bai, x.bai, x.bam.csi,
@@ -300,6 +410,15 @@ struct SegSource {
         return true;
     }
 
+    // One pass [ps, pe) over reference tid, of length len: a region query on the GPU feeder when the pass is not the whole
+    // reference and the feeder serves it (only a CSI can index past 2^29), else fetch().  A GPU-fed pass counts in *gpu_fed.
+    void fetch_pass(gl_ctx* ctx, gl_bam& bam, int tid, long long ps, long long pe, long long len, int Q, int threads,
+                    glhts::DecodeStats* st, int* gpu_fed) {
+        const bool whole_ref = ps == 0 && pe == len;
+        if (!whole_ref && fetch_regions(ctx, bam, tid, {ps}, {pe}, Q, st)) ++*gpu_fed;
+        else fetch(ctx, bam, tid, ps, pe, Q, threads, 0, whole_ref, st, gpu_fed);
+    }
+
     // a device decode's outcome: on GL_OK the arrays are on the device and its statistics go to one; GL_ESTATE (not possible
     // on the device for this reference) leaves nothing; any other code is fatal
     bool device_result(gl_ctx* ctx, int rc, const gl_bam_segments& g, const char* what, glhts::DecodeStats& one) {
@@ -391,6 +510,7 @@ namespace {
 struct DepthOpts {
     int W = 250, maxmean = 0, Q = 1, mincov = 4, threads = 0;
     long long step = 10000000;
+    long long pass = 0;                             // .fai mode: the bases of one GPU pass (pass_length)
     bool stats = false;
     std::string reference;
 };
@@ -520,17 +640,12 @@ struct DepthEngine {
         job.ca.append(tbuf_ca.data(), (size_t)cl);
     }
 
-    // ---- .fai mode: one contig.  The GPU pass covers at most 2^30-1 bases; longer contigs go in whole-chunk pieces
-    //      whose texts concatenate (chunk edges are run breaks anyway).  The GPU feeder decodes a whole contig, or each piece
-    //      of a longer one as a region query of [ps, pe) (only a CSI can index past 2^29); the host feeder is the fallback.
+    // ---- .fai mode: one contig, in passes of o.pass bases whose texts concatenate (chunk edges are run breaks anyway)
     void run_contig(DepthJob& job) {
-        const long long kMaxPass = ((1LL << 30) - 1) / o.step * o.step;
         const char* c = job.chrom.c_str();
-        for (long long ps = 0; ps < job.len; ps += kMaxPass) {
-            const long long pe = std::min(job.len, ps + kMaxPass);
-            const bool whole_ref = ps == 0 && pe == job.len;
-            if (!whole_ref && src.fetch_regions(ctx, gbam, tid(job.chrom), {ps}, {pe}, o.Q, &job.dec)) job.gpu_fed++;
-            else src.fetch(ctx, gbam, tid(job.chrom), ps, pe, o.Q, o.threads, 0, whole_ref, &job.dec, &job.gpu_fed);
+        for (long long ps = 0; ps < job.len; ps += o.pass) {
+            const long long pe = std::min(job.len, ps + o.pass);
+            src.fetch_pass(ctx, gbam, tid(job.chrom), ps, pe, job.len, o.Q, o.threads, &job.dec, &job.gpu_fed);
             const double tg = now_s();
             const bool dtext = !o.stats && job.chrom.size() <= 64;
             if (dtext && src.on_device) {                                      // segments already on the device (GPU feeder)
@@ -711,6 +826,7 @@ static int cmd_depth(int argc, char** argv) {
             jobs.emplace_back();
             jobs.back().chrom = c; jobs.back().len = len;
         }
+        if (!jobs.empty()) o.pass = pass_length(o.step, o.W, "goleft depth");
     }
 
     DepthShared sh;
@@ -718,18 +834,18 @@ static int cmd_depth(int argc, char** argv) {
     sh.bam_path = bam;
     std::vector<std::string> out_hd(regions.size()), out_ca(regions.size());
     sh.regions = &regions; sh.out_hd = &out_hd; sh.out_ca = &out_ca;
-    // an unindexed BAM cannot be seeked: decode it once, whole (the reference's `samtools depth -r` would refuse it)
+    // an unindexed BAM is decoded once, whole (the reference's `samtools depth -r` would refuse it)
     glhts::SegmentSet preload;
     {
         glhts::BamFile probe;
         std::string e = probe.open(bam);
         if (!e.empty()) fatal(1, "%s", e.c_str());
-        if (!index_usable(probe)) {
-            fprintf(stderr, "goleft depth: no usable index (.bai or .csi) next to %s: decoding the whole file (index it for -c / --bed to read only what they need)\n", bam.c_str());
-            int thr = o.threads > 0 ? o.threads : (int)std::max(1u, std::thread::hardware_concurrency());
-            int only = -1;
-            if (!chrom.empty()) for (size_t i = 0; i < probe.header.refs.size(); i++) if (probe.header.refs[i].name == chrom) only = (int)i;
-            e = glhts::bam_decode_segments(bam, o.Q, thr, only, preload);
+        const int thr = o.threads > 0 ? o.threads : (int)std::max(1u, std::thread::hardware_concurrency());
+        int only = -1;
+        if (!chrom.empty()) for (size_t i = 0; i < probe.header.refs.size(); i++) if (probe.header.refs[i].name == chrom) only = (int)i;
+        const std::string note = "goleft depth: no usable index (.bai or .csi) next to " + bam +
+                                 ": decoding the whole file (index it for -c / --bed to read only what they need)";
+        if (decode_unindexed(probe, bam, o.Q, thr, only, preload, e, note.c_str())) {
             if (!e.empty()) fatal(1, "%s", e.c_str());
             sh.preload = &preload;
         }
@@ -1872,18 +1988,11 @@ static int cmd_indexcov(int argc, char** argv) {
 // V1 + V2 (covstats.go:122-220): gl_bam_covstats samples the records and computes the reference's Stats on the device;
 // a file it cannot take (GL_ESTATE), or GL_GPU_FEED=0, goes through gl_bam_covstats_host, with the same tail.
 //
-// --gpus N: one worker per GPU claims BAMs in argument order from a shared counter (a BAM the device refuses costs several
-// times more on the host route, so the dealing is dynamic).  A worker holds at most one BAM claimed ahead: it opens it before
-// it samples the current one, and starts reading its first batch (gl_bam_covstats_prefetch) as soon as the current one's
-// sampling call has consumed its own prefetch, so that the read overlaps the rest of the current BAM's work (the --hist
-// tail, the .bai read for the mapped counts, the commit).  The main thread commits the
-// rows in argument order; the first BAM that fails, in that order, ends the run as the sequential loop would, after the
-// workers have finished their current call and been joined.
-struct CsJob {
-    gl_bam* bh = nullptr;
-    bool done = false;
-    int code = 0;                           // exit code of this BAM's failure (0: none) and its message
-    std::string msg;
+// --gpus N: the BAMs go through a BamQueue, dealt dynamically (a BAM the device refuses costs several times more on the host
+// route).  A worker starts reading the first batch of the BAM it opened ahead (gl_bam_covstats_prefetch) as soon as the
+// current one's sampling call has consumed its own prefetch, so that the read overlaps the rest of the current BAM's work
+// (the --hist tail, the .bai read for the mapped counts, the commit).  The main thread prints the rows as they commit.
+struct CsJob : BamJob {
     gl_covstats st;
     std::vector<double> H;
     std::string names, not_found;
@@ -1906,30 +2015,10 @@ static int cmd_covstats(int argc, char** argv) {
     const std::vector<std::string>& bams = ap.positional;
     const size_t S = bams.size();
     const GpuPlan gp = resolve_gpus(gpus, S, "goleft covstats");
-    std::vector<CsJob> jobs(S);
-    std::mutex mu;
-    std::condition_variable cv;
-    std::string ctx_err;                            // a worker that could not create its context
-    size_t next_claim = 0, fail_at = S;             // no BAM after the first known failure is claimed
-    auto claim = [&]() -> size_t {
-        std::lock_guard<std::mutex> lk(mu);
-        if (next_claim >= fail_at || !ctx_err.empty()) return S;
-        return next_claim++;
-    };
-    auto finish = [&](size_t i) {
-        std::lock_guard<std::mutex> lk(mu);
-        jobs[i].done = true;
-        if (jobs[i].code) fail_at = std::min(fail_at, i);
-        cv.notify_all();
-    };
-    auto open = [&](size_t i) {
-        char oerr[512] = {0};
-        if (gl_bam_open(bams[i].c_str(), &jobs[i].bh, oerr, sizeof oerr) != GL_OK) { jobs[i].code = 1; jobs[i].msg = oerr; jobs[i].bh = nullptr; }
-    };
+    BamQueue<CsJob> queue(bams);
     // BAM i on worker context c: everything but the output
     auto run = [&](gl_ctx* c, size_t i, gl_bam* ahead) {
-        CsJob& J = jobs[i];
-        if (J.code) return;
+        CsJob& J = queue.jobs[i];
         const std::string& bam = bams[i];
         gl_bam* bh = J.bh;
         gl_covstats& st = J.st;
@@ -1981,49 +2070,16 @@ static int cmd_covstats(int argc, char** argv) {
             }
         }
     };
-    std::vector<std::thread> th = start_workers(gp, [&](int g) {
+    queue.start(gp, [&](int g, std::string& err) {
         gl_ctx* c = nullptr;
-        if (gl_ctx_create(g % gp.n_dev, &c) != GL_OK) {
-            std::lock_guard<std::mutex> lk(mu);
-            if (ctx_err.empty()) ctx_err = gl_last_error(nullptr);
-            cv.notify_all();
-            return;
-        }
-        size_t cur = claim();
-        if (cur < S) open(cur);
-        while (cur < S) {
-            const size_t nxt = claim();
-            if (nxt < S) open(nxt);
-            run(c, cur, nxt < S ? jobs[nxt].bh : nullptr);
-            if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
-            jobs[cur].bh = nullptr;
-            finish(cur);
-            cur = nxt;
-            bool stop;
-            { std::lock_guard<std::mutex> lk(mu); stop = cur > fail_at || !ctx_err.empty(); }
-            if (stop && cur < S) {                 // a BAM before it failed: it will never be committed
-                if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
-                jobs[cur].bh = nullptr;
-                break;
-            }
-        }
-        gl_ctx_destroy(c);
-    });
-    // the commit: rows in argument order.  stop() ends the claiming and joins the workers before a message ends the run.
-    auto stop = [&]() {
-        { std::lock_guard<std::mutex> lk(mu); fail_at = 0; }
-        for (std::thread& t : th) t.join();
-        th.clear();
-    };
+        if (gl_ctx_create(g % gp.n_dev, &c) != GL_OK) err = std::string("goleft covstats: ") + gl_last_error(nullptr);
+        return c;
+    }, run, [](gl_ctx* c) { gl_ctx_destroy(c); });
+    // the commit: rows in argument order
     long long region_genome = -1;
     for (size_t i = 0; i < S; i++) {
-        {
-            std::unique_lock<std::mutex> lk(mu);
-            cv.wait(lk, [&] { return jobs[i].done || !ctx_err.empty(); });
-        }
-        CsJob& J = jobs[i];
-        if (!J.done) { stop(); fatal(1, "goleft covstats: %s", ctx_err.c_str()); }
-        if (J.code) { stop(); fatal(J.code, "%s", J.msg.c_str()); }
+        const CsJob& J = queue.wait(i);
+        if (J.code) { queue.stop(); fatal(J.code, "%s", J.msg.c_str()); }
         const std::string& bam = bams[i];
         const gl_covstats& st = J.st;
         const double pBad = st.proportion_bad, pDup = st.proportion_duplicate, pProper = st.proportion_properly_paired, pUnmapped = st.proportion_unmapped;
@@ -2032,7 +2088,7 @@ static int cmd_covstats(int argc, char** argv) {
         if (!hist.empty()) {                                                        // Stats.H (covstats.go:202-217), one line per entry
             const std::string hp = hist + "." + J.names + ".template_hist.tsv";
             FILE* hf = fopen(hp.c_str(), "w");
-            if (!hf) { const int e = errno; stop(); fatal(1, "open %s: %s", hp.c_str(), strerror(e)); }
+            if (!hf) { const int e = errno; queue.stop(); fatal(1, "open %s: %s", hp.c_str(), strerror(e)); }
             for (size_t j = 0; j < J.H.size(); j++) fprintf(hf, "%lld\t%s\n", (long long)maxRead + (long long)j, go_float("%.6g", J.H[j]).c_str());
             fclose(hf);
         }
@@ -2041,7 +2097,7 @@ static int cmd_covstats(int argc, char** argv) {
         if (!regions.empty()) {                                                     // covstats.go:36-55, read once
             if (region_genome < 0) {
                 gzFile f = gzopen(regions.c_str(), "rb");
-                if (!f) stop();                                                     // read_lines ends the run with the open error
+                if (!f) queue.stop();                                               // read_lines ends the run with the open error
                 else gzclose(f);
                 region_genome = 0;
                 for (const std::string& ln : read_lines(regions, true)) {
@@ -2057,7 +2113,6 @@ static int cmd_covstats(int argc, char** argv) {
         printf("%.2f\t%.2f\t%.2f\t%d\t%d\t%.2f\t%.2f\t%.2f\t%.1f\t%.1f\t%.1f\t%d\t%s\t%s\n", coverage, insMean, insSd, pct5, pct95, tMean, tSd,
                100 * pUnmapped, 100 * pBad, 100 * pDup, 100 * pProper, maxRead, bam.c_str(), J.names.c_str());
     }
-    stop();
     return 0;
 }
 
@@ -2109,18 +2164,14 @@ static void wed_write(FILE* f, int64_t G, size_t S, const std::vector<std::strin
 // depthwed from BAMs: the matrix `goleft depth --prefix <base> -w W -Q Q [-c chrom] -r ref.fa x.bam` for every BAM, then
 // `goleft depthwed -s SIZE <base>[.chrom].depth.bed ...` print, with no text in between.  The rows are the .fai windows
 // [iW, min((i+1)W, len)) of every contig (or -c); the groups come from gl_depthwed_plan once, with a device map from window
-// to group.  One worker per GPU claims the BAMs in argument order and opens the next while it reduces the current one: per
-// contig (in passes of at most 2^30 - 1 bases) fetch, gl_depth_reduce, gl_depthwed_add_column into the sample's int64
-// column on the device; the finished column comes home once, as int32 cells (int64 when a group sum does not fit).  The main
-// thread takes the BAMs' messages in argument order, and the first that failed ends the run before anything is printed.
+// to group.  The BAMs go through a BamQueue, one worker per GPU: per contig (in passes of at most 2^30 - 1 bases) fetch,
+// gl_depth_reduce, gl_depthwed_add_column into the sample's int64 column on the device; the finished column comes home once,
+// as int32 cells (int64 when a group sum does not fit).  The main thread takes the BAMs' messages in argument order, and the
+// first that failed ends the run before anything is printed.
 namespace {
 
-struct WedJob {
-    gl_bam* bh = nullptr;
-    bool whole = false;                     // no usable index: the file is decoded whole
-    bool done = false;
-    int code = 0;                           // exit code of this BAM's failure (0: none) and its message
-    std::string msg, note;                  // note: a line for stderr
+struct WedJob : BamJob {
+    std::string note;                       // a line for stderr
     std::vector<int64_t> wide;              // the column as int64 when a group sum does not fit int32
     glhts::DecodeStats dec;
     int gpu_fed = 0;
@@ -2140,8 +2191,7 @@ static int wed_bams(const ArgParser& ap, long long size, const std::string& w, c
     const int W = atoi(w.c_str()), Q = atoi(q.c_str()), threads = std::max(0, atoi(procs.c_str()));
     if (W <= 0) ap.fail("windowsize must be > 0");
     const long long step = std::max(1LL, 10000000LL / W) * W;                // depth.go:132
-    const long long kMaxPass = ((1LL << 30) - 1) / step * step;
-    if (kMaxPass == 0) fatal(1, "goleft depthwed: windowsize %d is above the 2^30 - 1 bases of one pass", W);
+    const long long pass = pass_length(step, W, "goleft depthwed");
 
     // rows: the .fai contigs goleft depth walks (cmd_depth), their windows numbered across the genome
     std::vector<WedContig> contigs;
@@ -2200,48 +2250,24 @@ static int wed_bams(const ArgParser& ap, long long size, const std::string& w, c
 
     const GpuPlan gp = resolve_gpus(gpus, S, "goleft depthwed");
     std::vector<int32_t> m32((size_t)S * (size_t)G);                          // sample-major: column s at [s * G, (s + 1) * G)
-    std::vector<WedJob> jobs(S);
-    std::mutex mu;
-    std::condition_variable cv;
-    std::string ctx_err;                            // a worker that could not create its context or its buffers
-    size_t next_claim = 0, fail_at = S;             // no BAM after the first known failure is claimed
-    auto claim = [&]() -> size_t {
-        std::lock_guard<std::mutex> lk(mu);
-        if (next_claim >= fail_at || !ctx_err.empty()) return S;
-        return next_claim++;
-    };
-    auto finish = [&](size_t i) {
-        std::lock_guard<std::mutex> lk(mu);
-        jobs[i].done = true;
-        if (jobs[i].code) fail_at = std::min(fail_at, i);
-        cv.notify_all();
-    };
-    auto open = [&](size_t i) {
-        WedJob& J = jobs[i];
-        char oerr[512] = {0};
-        if (gl_bam_open(bams[i].c_str(), &J.bh, oerr, sizeof oerr) != GL_OK) { J.code = 1; J.msg = oerr; J.bh = nullptr; return; }
-        if (!index_usable(J.bh->f)) {
-            J.whole = true;
-            J.note = "goleft depthwed: no usable index (.bai or .csi) next to " + bams[i] + ": decoding the whole file";
-        }
-    };
+    BamQueue<WedJob> queue(bams);
     struct Dev { gl_ctx* c = nullptr; int32_t* map = nullptr; int64_t* col = nullptr; int32_t* col32 = nullptr; int32_t* ovf = nullptr; };
     // BAM i on one worker's device: its column into m32 (or J.wide)
-    auto run = [&](Dev& d, size_t i) {
-        WedJob& J = jobs[i];
-        if (J.code) return;
+    auto run = [&](Dev& d, size_t i, gl_bam*) {
+        WedJob& J = queue.jobs[i];
         gl_ctx* c = d.c;
         gl_bam& bam = *J.bh;
         glhts::SegmentSet whole;
         SegSource src;
         std::map<std::string, int> tid_of;
         for (size_t r = 0; r < bam.f.header.refs.size(); r++) tid_of[bam.f.header.refs[r].name] = (int)r;
-        if (J.whole) {
-            const double t0 = now_s();
-            int only = -1;
-            if (!chrom.empty()) { auto it = tid_of.find(chrom); if (it != tid_of.end()) only = it->second; }
-            const int thr = threads > 0 ? threads : (int)std::max(1u, std::thread::hardware_concurrency());
-            const std::string e = glhts::bam_decode_segments(bams[i], Q, thr, only, whole);
+        int only = -1;
+        if (!chrom.empty()) { auto it = tid_of.find(chrom); if (it != tid_of.end()) only = it->second; }
+        const int thr = threads > 0 ? threads : (int)std::max(1u, std::thread::hardware_concurrency());
+        const double t0 = now_s();
+        std::string e;
+        if (decode_unindexed(bam.f, bams[i], Q, thr, only, whole, e)) {
+            J.note = "goleft depthwed: no usable index (.bai or .csi) next to " + bams[i] + ": decoding the whole file";
             if (!e.empty()) { J.code = 1; J.msg = e; return; }
             src.whole = &whole;
             J.dec.wall_s += now_s() - t0;
@@ -2250,12 +2276,9 @@ static int wed_bams(const ArgParser& ap, long long size, const std::string& w, c
         for (const WedContig& k : contigs) {
             auto it = tid_of.find(k.name);
             if (it == tid_of.end()) continue;                                 // not in the BAM: every window is 0
-            const int tid = it->second;
-            for (long long ps = 0; ps < k.len; ps += kMaxPass) {              // as goleft depth's run_contig
-                const long long pe = std::min(k.len, ps + kMaxPass);
-                const bool whole_ref = ps == 0 && pe == k.len;
-                if (!whole_ref && src.fetch_regions(c, bam, tid, {ps}, {pe}, Q, &J.dec)) J.gpu_fed++;
-                else src.fetch(c, bam, tid, ps, pe, Q, threads, 0, whole_ref, &J.dec, &J.gpu_fed);
+            for (long long ps = 0; ps < k.len; ps += pass) {
+                const long long pe = std::min(k.len, ps + pass);
+                src.fetch_pass(c, bam, it->second, ps, pe, k.len, Q, threads, &J.dec, &J.gpu_fed);
                 const double tg = now_s();
                 glck(c, gl_depth_begin(c, ps, pe), "gl_depth_begin");
                 src.add(c);
@@ -2264,7 +2287,7 @@ static int wed_bams(const ArgParser& ap, long long size, const std::string& w, c
                 J.gpu_s += now_s() - tg;
             }
         }
-        const double t0 = now_s();
+        const double t1 = now_s();
         glck(c, gl_depthwed_column_i32(c, d.col, G, d.col32, d.ovf), "gl_depthwed_column_i32");
         int32_t ovf = 0;
         if (G) glck(c, gl_memcpy_d2h(c, m32.data() + i * (size_t)G, d.col32, G * 4), "gl_memcpy_d2h");
@@ -2273,71 +2296,38 @@ static int wed_bams(const ArgParser& ap, long long size, const std::string& w, c
             J.wide.resize((size_t)G);
             glck(c, gl_memcpy_d2h(c, J.wide.data(), d.col, G * 8), "gl_memcpy_d2h");
         }
-        J.d2h_s = now_s() - t0;
+        J.d2h_s = now_s() - t1;
     };
-    std::vector<std::thread> th = start_workers(gp, [&](int g) {
+    queue.start(gp, [&](int g, std::string& err) {
         Dev d;
-        auto dev_fail = [&](const char* what) {
-            std::lock_guard<std::mutex> lk(mu);
-            if (ctx_err.empty()) ctx_err = std::string(what) + ": " + gl_last_error(d.c);
-            cv.notify_all();
-        };
-        if (gl_ctx_create(g % gp.n_dev, &d.c) != GL_OK) { dev_fail("gl_ctx_create"); return; }
+        if (gl_ctx_create(g % gp.n_dev, &d.c) != GL_OK) { err = std::string("goleft depthwed: gl_ctx_create: ") + gl_last_error(nullptr); return d; }
         void *pm = nullptr, *pc = nullptr, *p32 = nullptr, *po = nullptr;
         if (gl_dev_alloc(d.c, std::max<int64_t>(R, 1) * 4, &pm) != GL_OK || gl_dev_alloc(d.c, std::max<int64_t>(G, 1) * 8, &pc) != GL_OK ||
             gl_dev_alloc(d.c, std::max<int64_t>(G, 1) * 4, &p32) != GL_OK || gl_dev_alloc(d.c, 16, &po) != GL_OK ||
-            (R > 0 && gl_memcpy_h2d(d.c, pm, grp_of.data(), R * 4) != GL_OK)) {
-            dev_fail("goleft depthwed");
-        } else {
-            d.map = static_cast<int32_t*>(pm); d.col = static_cast<int64_t*>(pc); d.col32 = static_cast<int32_t*>(p32); d.ovf = static_cast<int32_t*>(po);
-            size_t cur = claim();
-            if (cur < S) open(cur);
-            while (cur < S) {
-                const size_t nxt = claim();
-                if (nxt < S) open(nxt);
-                run(d, cur);
-                if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
-                jobs[cur].bh = nullptr;
-                finish(cur);
-                cur = nxt;
-                bool stop;
-                { std::lock_guard<std::mutex> lk(mu); stop = cur > fail_at || !ctx_err.empty(); }
-                if (stop && cur < S) {                 // a BAM before it failed: it will never be committed
-                    if (jobs[cur].bh) gl_bam_close(jobs[cur].bh);
-                    jobs[cur].bh = nullptr;
-                    break;
-                }
-            }
-        }
-        for (void* p : {pm, pc, p32, po}) if (p) gl_dev_free(d.c, p);
+            (R > 0 && gl_memcpy_h2d(d.c, pm, grp_of.data(), R * 4) != GL_OK))
+            err = std::string("goleft depthwed: goleft depthwed: ") + gl_last_error(d.c);
+        d.map = static_cast<int32_t*>(pm); d.col = static_cast<int64_t*>(pc); d.col32 = static_cast<int32_t*>(p32); d.ovf = static_cast<int32_t*>(po);
+        return d;
+    }, run, [](Dev& d) {
+        for (void* p : std::initializer_list<void*>{d.map, d.col, d.col32, d.ovf}) if (p) gl_dev_free(d.c, p);
         gl_ctx_destroy(d.c);
     });
-    auto stop = [&]() {
-        { std::lock_guard<std::mutex> lk(mu); fail_at = 0; }
-        for (std::thread& t : th) t.join();
-        th.clear();
-    };
     for (size_t i = 0; i < S; i++) {
-        {
-            std::unique_lock<std::mutex> lk(mu);
-            cv.wait(lk, [&] { return jobs[i].done || !ctx_err.empty(); });
-        }
-        WedJob& J = jobs[i];
-        if (!J.done) { stop(); fatal(1, "goleft depthwed: %s", ctx_err.c_str()); }
+        const WedJob& J = queue.wait(i);
         if (!J.note.empty()) fprintf(stderr, "%s\n", J.note.c_str());
-        if (J.code) { stop(); fatal(J.code, "%s", J.msg.c_str()); }
+        if (J.code) { queue.stop(); fatal(J.code, "%s", J.msg.c_str()); }
     }
-    stop();
+    queue.stop();
     const double t_fmt = now_s();
     printf("%s\n", header.c_str());
     wed_write(stdout, G, S, names, oc.data(), os.data(), oe.data(), [&](int64_t g, size_t s) -> long long {
-        const WedJob& J = jobs[s];
+        const WedJob& J = queue.jobs[s];
         return J.wide.empty() ? (long long)m32[s * (size_t)G + (size_t)g] : (long long)J.wide[(size_t)g];
     });
     fflush(stdout);
     if (timing) {
         double dec = 0, gpu = 0, d2h = 0; long long rec = 0, bin = 0; int fed = 0;
-        for (const WedJob& J : jobs) { dec += J.dec.wall_s; gpu += J.gpu_s; d2h += J.d2h_s; rec += J.dec.n_records; bin += J.dec.bytes_in; fed += J.gpu_fed; }
+        for (const WedJob& J : queue.jobs) { dec += J.dec.wall_s; gpu += J.gpu_s; d2h += J.d2h_s; rec += J.dec.n_records; bin += J.dec.bytes_in; fed += J.gpu_fed; }
         fprintf(stderr, "{\"goleft_depthwed_timing\": {\"wall_s\": %.4f, \"gpus\": %d, \"samples\": %zu, \"windows\": %lld, \"rows\": %lld, "
                         "\"decode_wall_s_sum\": %.4f, \"reduce_column_s_sum\": %.4f, \"d2h_s_sum\": %.4f, \"format_s\": %.4f, "
                         "\"records\": %lld, \"bgzf_bytes_in\": %lld, \"gpu_fed_passes\": %d}}\n",
@@ -2585,11 +2575,11 @@ static int cmd_multidepth(int argc, char** argv) {
     // sample i's segments of the contig: without an index, a whole-file decode of that one reference; otherwise the GPU feeder
     // when it can, else the host feeder.  A sample that stays on the host is decoded on a helper thread beside the GPU work
     // of sample i-1.
-    auto stays_on_host = [&](int i) { return !(SegSource::gpu_feed() && bam[(size_t)i].f.has_index); };
+    auto stays_on_host = [&](int i) { return !(SegSource::gpu_feed() && index_usable(bam[(size_t)i].f)); };
     auto fetch = [&](gl_ctx* c, int i) {
         const size_t k = (size_t)i;
-        if (!bam[k].f.has_index) {
-            std::string e = glhts::bam_decode_segments(bams[k], Q, threads > 0 ? threads : 8, tid[k], whole[k]);
+        std::string e;
+        if (decode_unindexed(bam[k].f, bams[k], Q, threads > 0 ? threads : 8, tid[k], whole[k], e)) {
             if (!e.empty()) fatal(1, "%s", e.c_str());
             smp[k].whole = &whole[k];
         }
